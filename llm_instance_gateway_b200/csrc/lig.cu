@@ -167,6 +167,14 @@ struct lig_ctx {
   QueueItem* h_items[kItemSlots] = {};
   cudaEvent_t items_free[kItemSlots] = {};
   int item_slot = 0;
+  // tile-claim counters of the persistent kernels (TileClaim): launches on different streams may
+  // run at once, so each takes the next counter of a ring; claim_free[i] is recorded after the
+  // kernel that last used counter i, and claim_base[i] is that counter's value once it has finished
+  static constexpr int kClaimSlots = 16;
+  uint32_t* d_claims = nullptr;
+  uint32_t claim_base[kClaimSlots] = {};
+  cudaEvent_t claim_free[kClaimSlots] = {};
+  int claim_slot = 0;
 
   // ---- streaming doorbell (lig_stream_open): a persistent kernel polling a host mailbox ----
   Mailbox* mailbox = nullptr;       // pinned, device-mapped
@@ -382,6 +390,21 @@ bool tables_fit_smem(const lig_ctx* c, const Slot& s, bool with_models) {
   return need <= kTabBudget;
 }
 
+// Launch persistent kernel v (its last argument, *tc, is filled in here) with the next tile-claim
+// counter of the ring.  On the device the launch first waits for the counter's previous kernel,
+// whose claims the counter's base already counts.  Caller holds c->mu.
+int launch_claimed(lig_ctx* c, const PersistVariant& v, int grid, int total_tiles, void** args, TileClaim* tc,
+                   cudaStream_t st) {
+  const int k = c->claim_slot;
+  c->claim_slot = (k + 1) % lig_ctx::kClaimSlots;
+  CUDA_TRY(cudaStreamWaitEvent(st, c->claim_free[k], 0));   // no-op unless the ring wrapped onto a live launch
+  *tc = TileClaim{c->d_claims + k, c->claim_base[k]};
+  CUDA_TRY(cudaLaunchKernel(v.fn, dim3((unsigned)grid), dim3((unsigned)v.threads), args, v.smem, st));
+  c->claim_base[k] += (uint32_t)total_tiles + (uint32_t)grid;   // every CTA's producer fails one claim
+  CUDA_TRY(cudaEventRecord(c->claim_free[k], st));
+  return 0;
+}
+
 // The persistent TMA-pipelined pick over a queue of n batches of R requests (one launch per
 // <= 2^30 tiles).  Caller holds c->mu.
 int launch_persistent(lig_ctx* c, const Slot& s, uint64_t seed, const lig_req* const* reqs, int R,
@@ -427,7 +450,8 @@ int launch_persistent(lig_ctx* c, const Slot& s, uint64_t seed, const lig_req* c
     int A = s.A;
     const unsigned char* ctab = s.d_ctab;
     uint32_t ctab_bytes = tab ? s.h_hdr->bytes : 0u;
-    void* args[6] = {&qp, &cls, &lists, &A, &ctab, &ctab_bytes};
+    TileClaim tc{};
+    void* args[7] = {&qp, &cls, &lists, &A, &ctab, &ctab_bytes, &tc};
     if (c->pick_kernel == 1) {
       const PersistVariant v = loop_variant(tab);
       const int cap = c->loop_grid[tab ? 1 : 0];
@@ -438,7 +462,7 @@ int launch_persistent(lig_ctx* c, const Slot& s, uint64_t seed, const lig_req* c
       const PersistVariant v = persist_variant(c->tma_groups, c->tma_stages, bulk, tab);
       const int cap = c->persist_grid[bulk ? 1 : 0][tab ? 1 : 0];
       const int grid = qp.total_tiles < cap ? qp.total_tiles : cap;
-      CUDA_TRY(cudaLaunchKernel(v.fn, dim3((unsigned)grid), dim3((unsigned)v.threads), args, v.smem, st));
+      if (int rc = launch_claimed(c, v, grid, qp.total_tiles, args, &tc, st)) return rc;
     }
     c->launches++;
     if (slot >= 0) CUDA_TRY(cudaEventRecord(c->items_free[slot], st));   // after the kernel that reads the table
@@ -504,11 +528,12 @@ int launch_models(lig_ctx* c, const Slot& s, uint64_t seed, uint64_t first_index
     uint32_t ctab_bytes = tab ? s.h_hdr->bytes : 0u;
     const unsigned char* mtab = s.d_mtab;
     uint32_t mtab_bytes = s.mtab_bytes, n_models = s.n_models;
-    void* args[9] = {&qp, &cls, &lists, &A, &ctab, &ctab_bytes, &mtab, &mtab_bytes, &n_models};
+    TileClaim tc{};
+    void* args[10] = {&qp, &cls, &lists, &A, &ctab, &ctab_bytes, &mtab, &mtab_bytes, &n_models, &tc};
     const PersistVariant v = models_variant(c->models_groups, c->models_stages, tab);
     const int cap = c->models_grid[tab ? 1 : 0];
     const int grid = qp.total_tiles < cap ? qp.total_tiles : cap;
-    CUDA_TRY(cudaLaunchKernel(v.fn, dim3((unsigned)grid), dim3((unsigned)v.threads), args, v.smem, st));
+    if (int rc = launch_claimed(c, v, grid, qp.total_tiles, args, &tc, st)) return rc;
     c->launches++;
   }
   return 0;
@@ -969,9 +994,13 @@ static int create_impl(lig_ctx* c, int device, int max_pods, int max_adapters, i
     CUDA_TRY(cudaHostAlloc(&c->h_items[i], sizeof(QueueItem) * lig_ctx::kMaxItems, cudaHostAllocDefault));
     CUDA_TRY(cudaEventCreateWithFlags(&c->items_free[i], cudaEventDisableTiming));
   }
+  for (auto& ev : c->claim_free) CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
   CUDA_TRY(cudaEventCreateWithFlags(&c->fork, cudaEventDisableTiming));
   for (auto& ev : c->join) CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
   CUDA_TRY(cudaStreamCreateWithFlags(&c->s_up, cudaStreamNonBlocking));
+  CUDA_TRY(cudaMalloc(&c->d_claims, sizeof(uint32_t) * lig_ctx::kClaimSlots));
+  CUDA_TRY(cudaMemsetAsync(c->d_claims, 0, sizeof(uint32_t) * lig_ctx::kClaimSlots, c->s_up));
+  CUDA_TRY(cudaStreamSynchronize(c->s_up));   // the counters are zero before any launch reads one
   for (auto& s : c->s_lane) CUDA_TRY(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
   c->free_tickets.reserve(LIG_MAX_TICKETS);
   for (int i = LIG_MAX_TICKETS - 1; i >= 0; --i) {
@@ -1059,6 +1088,9 @@ void lig_destroy(lig_ctx* c) {
     cudaFreeHost(c->h_items[i]);
     if (c->items_free[i]) cudaEventDestroy(c->items_free[i]);
   }
+  cudaFree(c->d_claims);
+  for (auto& ev : c->claim_free)
+    if (ev) cudaEventDestroy(ev);
   for (auto& ev : c->ticket_ev)
     if (ev) cudaEventDestroy(ev);
   if (c->fork) cudaEventDestroy(c->fork);

@@ -1425,12 +1425,12 @@ lig_pick_queue_kernel(const QueueItem* __restrict__ items, int R, const uint4* _
 }
 
 // ---- K2c: the persistent, TMA-pipelined pick (default for HBM-resident batches) -----------------
-// One launch serves a whole queue of batches with a FIXED grid of resident CTAs.  Every CTA walks
-// the queue's 1024-request tiles (CTA-local tile j = global tile blockIdx.x + j * gridDim.x):
+// One launch serves a whole queue of batches with a FIXED grid of resident CTAs.  The CTAs claim
+// the queue's 1024-request tiles from a shared counter (see produce_claimed_tiles):
 //   * a producer warp streams each tile's 16 KB of descriptors global -> shared with one TMA bulk
 //     copy (cp.async.bulk, SASS UBLKCP.S.G) into a kStages-deep ring, completion signalled on an
 //     mbarrier (expect_tx), so HBM reads never wait for the compute of an earlier tile;
-//   * kGroups consumer groups of 8 warps take the CTA's tiles in turn (group g: tiles g,
+//   * kGroups consumer groups of 8 warps take the CTA's tiles in turn (group g: ring positions g,
 //     g + kGroups, ...).  A group waits for its tile, takes 4 descriptors per thread out of shared
 //     memory (conflict-free LDS.128) and hands the stage straight back (mbarrier arrive): the ring
 //     only holds bytes in flight, never bytes being worked on, so a few 16 KB stages feed many
@@ -1459,6 +1459,8 @@ struct QueueParams {
 constexpr uint32_t kTabBudget = 72 * 1024;
 
 __host__ __device__ constexpr int persist_threads(int groups) { return groups * kGroupThreads + 32; }
+// Ring, [bulk-store staging,] full[] and empty[] barriers, then 64 bytes for the table barrier and
+// tile_of[stages] (8 + 4 * 8 bytes at most: both kernels have <= 8 stages).
 __host__ __device__ constexpr size_t persist_smem_bytes(int groups, int stages, bool bulk_store, bool tab_smem) {
   return (tab_smem ? (size_t)kTabBudget : 0) + (size_t)stages * kTile * 16 +
          (bulk_store ? (size_t)groups * kTile * 8 : 0) + 2u * (size_t)stages * 8 + 64;
@@ -1517,6 +1519,74 @@ __device__ __forceinline__ QueueItem queue_item(const QueueParams& qp, int b) {
   return it;
 }
 
+// ---- dynamic tile claiming (both persistent kernels) ----------------------------------------------
+// The producer lane of every CTA claims the launch's tiles one at a time, in global tile order, from
+// one counter, so a CTA whose tiles land early takes more of them and all CTAs finish within about a
+// tile of each other.  (With a fixed split every group owned ~39 tiles at C4, K = 20, and the launch
+// waited for the slowest group while the others sat idle and HBM ran below bandwidth.)  Which CTA
+// computes a tile does not change its picks: they depend on (batch, tile, seed) only.
+//
+// The counter is never reset: the host passes its value before the launch as `base` and then
+// advances its copy by total_tiles + gridDim.x, the exact number of claims of a launch (every
+// producer claims until its first failed claim, and fails exactly once).  Unsigned 32-bit
+// arithmetic, so wrapping is harmless (total_tiles + gridDim.x < 2^31).
+struct TileClaim {
+  uint32_t* counter;
+  uint32_t base;
+};
+
+__device__ __forceinline__ uint32_t claim_tile(const TileClaim& tc) {
+  return atomicAdd(tc.counter, 1u) - tc.base;
+}
+
+// The producer lane: ring position p (stage p % kStages) goes to consumer group p % kGroups, as with
+// a fixed split; what is dynamic is which tile a position carries.  For every claimed tile g it
+// finds the tile's source and byte count (src_of(g, &bytes)), waits for the stage to be free,
+// writes g into tile_of[stage], arrives on full[stage] with expect_tx and starts the bulk copy.
+// The next claim and the source lookup go out before that wait, so neither the atomic's round trip
+// nor the lookup delays the copy once the stage frees: in steady state the ring is HBM-latency
+// bound, and every cycle between a stage's release and its next copy is bytes not in flight.
+//
+// Termination.  After the first failed claim the producer posts the end marker -1, with a plain
+// arrive (no transaction bytes, so the phase completes at once), into the next kGroups ring
+// positions n .. n + kGroups - 1, where n is the number of tiles it loaded: exactly one position
+// of every group, and every earlier position of that group carried a tile.  So each group
+// consumes its tiles, then meets one marker and leaves; no group waits on a position nobody
+// fills.  The producer's own waits all pass: position p >= kStages waits for position p - kStages
+// to be freed, which the same group (kStages is a multiple of kGroups) consumed, and every such
+// position carried a tile (p - kStages < n because kGroups <= kStages), so the group freed it
+// right after its full wait.  This covers
+//   * a CTA whose first claim fails (fewer tiles than CTAs, a queue of one, or a late CTA): n = 0,
+//     the markers go into stages 0 .. kGroups - 1 on the first lap, whose empty waits pass at once;
+//   * ragged last tiles: only the byte count differs, never the handshake;
+//   * the bulk-store path: all 256 threads of a group read the same tile_of word, so they take
+//     the same branches to the group's named barriers and leave the loop together;
+//   * 1 group (markers: position n) and 3 groups (kStages 3 or 6: positions n, n + 1, n + 2).
+template <int kGroups, int kStages, typename TileSrc>
+__device__ __forceinline__ void produce_claimed_tiles(const TileClaim& tc, uint32_t total, unsigned char* ring,
+                                                      uint32_t stage_bytes, uint64_t* full, uint64_t* empty,
+                                                      int* tile_of, TileSrc src_of) {
+  int stage = 0;                                     // (the host only launches kStages % kGroups == 0)
+  uint32_t phase = 0;
+  for (uint32_t g = claim_tile(tc); g < total;) {
+    const uint32_t next = claim_tile(tc);
+    uint32_t bytes;
+    const void* src = src_of((int)g, &bytes);
+    mbar_wait(empty + stage, phase ^ 1u);            // free (passes at once on the first lap)
+    tile_of[stage] = (int)g;
+    mbar_arrive_expect_tx(full + stage, bytes);
+    bulk_load(ring + (size_t)stage * stage_bytes, src, bytes, full + stage);
+    if (++stage == kStages) { stage = 0; phase ^= 1u; }
+    g = next;
+  }
+  for (int k = 0; k < kGroups; ++k) {
+    mbar_wait(empty + stage, phase ^ 1u);
+    tile_of[stage] = -1;
+    mbar_arrive(full + stage);
+    if (++stage == kStages) { stage = 0; phase ^= 1u; }
+  }
+}
+
 // kTabSmem: the compact tables (ctab, ctab_bytes <= kTabBudget) are pulled into shared memory by
 // one TMA bulk copy at CTA start and every lookup is an LDS; otherwise lookups go to the strided
 // tables (cls, lists) through L1.  The host picks the variant (see launch_persistent).
@@ -1524,7 +1594,7 @@ template <int kGroups, int kStages, bool kBulkStore, bool kTabSmem>
 __global__ void __launch_bounds__(persist_threads(kGroups), (kTabSmem ? 2 : 6) / kGroups > 0 ? (kTabSmem ? 2 : 6) / kGroups : 1)
 lig_pick_persistent_kernel(const __grid_constant__ QueueParams qp, const uint4* __restrict__ cls,
                            const uint16_t* __restrict__ lists, int A,
-                           const unsigned char* __restrict__ ctab, uint32_t ctab_bytes) {
+                           const unsigned char* __restrict__ ctab, uint32_t ctab_bytes, TileClaim tc) {
   extern __shared__ __align__(16) unsigned char smem[];
   unsigned char* base = smem + (kTabSmem ? kTabBudget : 0u);
   int4* in_ring = reinterpret_cast<int4*>(base);                                   // [kStages][kTile]
@@ -1533,6 +1603,7 @@ lig_pick_persistent_kernel(const __grid_constant__ QueueParams qp, const uint4* 
                                                (kBulkStore ? (size_t)kGroups * kTile * 8 : 0));
   uint64_t* empty = full + kStages;
   uint64_t* tab_bar = empty + kStages;
+  int* tile_of = reinterpret_cast<int*>(tab_bar + 1);  // [kStages] the tile each stage holds, -1 = end
   const uint4* tab = reinterpret_cast<const uint4*>(smem + sizeof(CompactHeader));
   const uint16_t* pool = reinterpret_cast<const uint16_t*>(smem + sizeof(CompactHeader) +
                                                            (size_t)2 * ((size_t)A + 1) * sizeof(ClassEntry));
@@ -1547,50 +1618,40 @@ lig_pick_persistent_kernel(const __grid_constant__ QueueParams qp, const uint4* 
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  const int tpb = qp.tiles_per_batch, total = qp.total_tiles, R = qp.R;
+  const int tpb = qp.tiles_per_batch, R = qp.R;
 
   if (warp == kGroups * (kGroupThreads / 32)) {
-    // ---- producer: one lane feeds the ring, CTA-local tiles in order ----
+    // ---- producer: one lane feeds the ring with the tiles it claims ----
     if (lane == 0) {
       if (kTabSmem) {                                  // the tables first: one bulk copy, L2-resident
         mbar_arrive_expect_tx(tab_bar, ctab_bytes);
         bulk_load(smem, ctab, ctab_bytes, tab_bar);
       }
-      const int step = (int)gridDim.x;
-      int b = (int)blockIdx.x / tpb;
-      int t = (int)blockIdx.x - b * tpb;
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int g = (int)blockIdx.x; g < total; g += step) {
-        mbar_wait(empty + stage, phase ^ 1u);          // free (passes at once on the first lap)
-        const QueueItem it = queue_item(qp, b);
-        const uint32_t n = (uint32_t)min(kTile, R - t * kTile);
-        mbar_arrive_expect_tx(full + stage, n * 16u);
-        bulk_load(in_ring + (size_t)stage * kTile, it.reqs + (size_t)t * kTile, n * 16u, full + stage);
-        if (++stage == kStages) { stage = 0; phase ^= 1u; }
-        t += step;
-        while (t >= tpb) { t -= tpb; ++b; }
-      }
+      produce_claimed_tiles<kGroups, kStages>(tc, (uint32_t)qp.total_tiles, base, kTile * 16u, full, empty,
+                                              tile_of, [&](int g, uint32_t* bytes) {
+        const int b = g / tpb, t = g - b * tpb;
+        *bytes = (uint32_t)min(kTile, R - t * kTile) * 16u;
+        return static_cast<const void*>(queue_item(qp, b).reqs + (size_t)t * kTile);
+      });
     }
     return;
   }
 
-  // ---- consumer group `grp`: CTA-local tiles grp, grp + kGroups, ... ----
+  // ---- consumer group `grp`: ring positions grp, grp + kGroups, ... until the end marker ----
   const int grp = warp / (kGroupThreads / 32);
   const int tid = (int)threadIdx.x - grp * kGroupThreads;
-  const int step = (int)gridDim.x * kGroups;
-  int g = (int)blockIdx.x + grp * (int)gridDim.x;
-  int b = g / tpb;
-  int t = g - b * tpb;
   int stage = grp % kStages;
   uint32_t phase = (uint32_t)(grp / kStages) & 1u;
-  if (kTabSmem) mbar_wait(tab_bar, 0);                 // the tables have landed
-  for (; g < total; g += step) {
+  bool tab_ready = !kTabSmem;
+  for (;;) {
+    mbar_wait(full + stage, phase);                    // the tile's bytes (or the end marker) have landed
+    const int g = tile_of[stage];
+    if (g < 0) break;
+    const int b = g / tpb, t = g - b * tpb;
     const QueueItem it = queue_item(qp, b);
     const int n = min(kTile, R - t * kTile);
     const int4* tile = in_ring + (size_t)stage * kTile + tid;
     int4 r[4];
-    mbar_wait(full + stage, phase);                    // the tile's bytes have landed
     if (n == kTile) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) r[j] = tile[j * kGroupThreads];
@@ -1604,6 +1665,9 @@ lig_pick_persistent_kernel(const __grid_constant__ QueueParams qp, const uint4* 
     // this group's next tile is kGroups ring positions further
     stage += kGroups;
     while (stage >= kStages) { stage -= kStages; phase ^= 1u; }
+    // the first tile's stage is free before the wait for the tables, so the producer refills the
+    // ring while they are still landing
+    if (!tab_ready) { mbar_wait(tab_bar, 0); tab_ready = true; }
     int2 p[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j)
@@ -1625,10 +1689,11 @@ lig_pick_persistent_kernel(const __grid_constant__ QueueParams qp, const uint4* 
       for (int j = 0; j < 4; ++j)
         if (tid + j * kGroupThreads < n) st_stream_int2(dst + j * kGroupThreads, p[j]);
     }
-    t += step;
-    while (t >= tpb) { t -= tpb; ++b; }
   }
-  if (kBulkStore && tid == 0) bulk_store_wait_read_all();   // shared memory must outlive the reads
+  // shared memory must outlive the bulk copies: the table pull of a CTA that got no tile, the
+  // bulk stores' reads
+  if (!tab_ready) mbar_wait(tab_bar, 0);
+  if (kBulkStore && tid == 0) bulk_store_wait_read_all();
 }
 
 // ---- K2d: persistent grid-stride pick with register prefetch (no shared memory) ------------------
@@ -1827,20 +1892,22 @@ __host__ __device__ constexpr size_t mpersist_smem_bytes(int stages, bool tab_sm
 }
 
 // Persistent kernel for HBM-resident model-id batches: same structure as K2c (TMA ring, consumer
-// groups, tables in shared memory), 4 KB tiles, every thread takes 4 consecutive requests
+// groups, claimed tiles, tables in shared memory), 4 KB tiles, every thread takes 4 consecutive requests
 // (one LDS.128 in, one 16-byte store out).
 template <int kGroups, int kStages, bool kTabSmem>
 __global__ void __launch_bounds__(persist_threads(kGroups), kGroups == 1 ? 3 : 2)
 lig_pick_models_kernel(const __grid_constant__ MQueueParams qp, const uint4* __restrict__ cls,
                        const uint16_t* __restrict__ lists, int A,
                        const unsigned char* __restrict__ ctab, uint32_t ctab_bytes,
-                       const unsigned char* __restrict__ mtab, uint32_t mtab_bytes, uint32_t n_models) {
+                       const unsigned char* __restrict__ mtab, uint32_t mtab_bytes, uint32_t n_models,
+                       TileClaim tc) {
   extern __shared__ __align__(16) unsigned char smem[];
   unsigned char* base = smem + (kTabSmem ? kTabBudget : 0u);
   uint4* in_ring = reinterpret_cast<uint4*>(base);                                  // [kStages][kTile / 4]
   uint64_t* full = reinterpret_cast<uint64_t*>(base + (size_t)kStages * kTile * 4);
   uint64_t* empty = full + kStages;
   uint64_t* tab_bar = empty + kStages;
+  int* tile_of = reinterpret_cast<int*>(tab_bar + 1);  // [kStages] the tile each stage holds, -1 = end
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
 #pragma unroll
@@ -1852,7 +1919,7 @@ lig_pick_models_kernel(const __grid_constant__ MQueueParams qp, const uint4* __r
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  const int tpb = qp.tiles_per_batch, total = qp.total_tiles, R = qp.R;
+  const int tpb = qp.tiles_per_batch, R = qp.R;
 
   if (warp == kGroups * (kGroupThreads / 32)) {
     if (lane == 0) {
@@ -1861,32 +1928,19 @@ lig_pick_models_kernel(const __grid_constant__ MQueueParams qp, const uint4* __r
         bulk_load(smem, ctab, ctab_bytes, tab_bar);
         bulk_load(smem + ctab_bytes, mtab, mtab_bytes, tab_bar);
       }
-      const int step = (int)gridDim.x;
-      int b = (int)blockIdx.x / tpb;
-      int t = (int)blockIdx.x - b * tpb;
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int g = (int)blockIdx.x; g < total; g += step) {
-        mbar_wait(empty + stage, phase ^ 1u);
-        const MQueueItem it = mqueue_item(qp, b);
+      produce_claimed_tiles<kGroups, kStages>(tc, (uint32_t)qp.total_tiles, base, kTile * 4u, full, empty,
+                                              tile_of, [&](int g, uint32_t* bytes) {
+        const int b = g / tpb, t = g - b * tpb;
         const uint32_t n = (uint32_t)min(kTile, R - t * kTile);
-        const uint32_t bytes = (n * 4u + 15u) & ~15u;   // the buffers are padded to 16 bytes by the ABI
-        mbar_arrive_expect_tx(full + stage, bytes);
-        bulk_load(in_ring + (size_t)stage * (kTile / 4), it.ids + (size_t)t * kTile, bytes, full + stage);
-        if (++stage == kStages) { stage = 0; phase ^= 1u; }
-        t += step;
-        while (t >= tpb) { t -= tpb; ++b; }
-      }
+        *bytes = (n * 4u + 15u) & ~15u;   // the buffers are padded to 16 bytes by the ABI
+        return static_cast<const void*>(mqueue_item(qp, b).ids + (size_t)t * kTile);
+      });
     }
     return;
   }
 
   const int grp = warp / (kGroupThreads / 32);
   const int tid = (int)threadIdx.x - grp * kGroupThreads;
-  const int step = (int)gridDim.x * kGroups;
-  int g = (int)blockIdx.x + grp * (int)gridDim.x;
-  int b = g / tpb;
-  int t = g - b * tpb;
   int stage = grp % kStages;
   uint32_t phase = (uint32_t)(grp / kStages) & 1u;
   ModelTables mt;
@@ -1901,16 +1955,20 @@ lig_pick_models_kernel(const __grid_constant__ MQueueParams qp, const uint4* __r
   }
   mt.targets = reinterpret_cast<const uint2*>(mt.entries + n_models);
   mt.n_models = n_models;
-  if (kTabSmem) mbar_wait(tab_bar, 0);
-  for (; g < total; g += step) {
+  bool tab_ready = !kTabSmem;
+  for (;;) {
+    mbar_wait(full + stage, phase);
+    const int g = tile_of[stage];
+    if (g < 0) break;
+    const int b = g / tpb, t = g - b * tpb;
     const MQueueItem it = mqueue_item(qp, b);
     const int n = min(kTile, R - t * kTile);
-    mbar_wait(full + stage, phase);
     const uint4 ids = in_ring[(size_t)stage * (kTile / 4) + tid];
     __syncwarp();
     if (lane == 0) mbar_arrive(empty + stage);
     stage += kGroups;
     while (stage >= kStages) { stage -= kStages; phase ^= 1u; }
+    if (!tab_ready) { mbar_wait(tab_bar, 0); tab_ready = true; }   // after freeing the first stage
     const int i0 = tid * 4;
     const uint64_t key0 = it.first_index + (uint64_t)t * kTile + (uint64_t)i0;
     // The thread's 4 requests in three passes.  (1) entry lookups; models with at most one target
@@ -1962,9 +2020,8 @@ lig_pick_models_kernel(const __grid_constant__ MQueueParams qp, const uint4* __r
       if (i0 + 1 < n) dst[1] = o.y;
       if (i0 + 2 < n) dst[2] = o.z;
     }
-    t += step;
-    while (t >= tpb) { t -= tpb; ++b; }
   }
+  if (!tab_ready) mbar_wait(tab_bar, 0);   // a CTA that got no tile: its table pull must land before exit
 }
 
 // The plain form: one short-lived CTA per 1024 requests, LDG/STG only.  Host-buffer path (`ids` /
