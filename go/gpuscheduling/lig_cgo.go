@@ -80,6 +80,18 @@ func (c *ctx) setThresholds(kv float64, qCritical, qLoRA int64) error {
 	return ligError("lig_set_thresholds", C.lig_set_thresholds(c.p, &t))
 }
 
+// setFilterTree hands a caller flow chart to lig_set_filter_tree.  The node table is a Go slice of
+// C structs without Go pointers, which cgo may pass for the duration of the call.
+func (c *ctx) setFilterTree(nodes []FilterNode) error {
+	cn := make([]C.lig_filter_node, len(nodes))
+	for i, n := range nodes {
+		cn[i] = C.lig_filter_node{kind: C.int32_t(n.Kind), next_on_success: C.int32_t(n.NextOnSuccess),
+			next_on_failure: C.int32_t(n.NextOnFailure), next_on_success_or_failure: C.int32_t(n.NextOnSuccessOrFailure),
+			queue_threshold: C.int64_t(n.QueueThreshold), kv_threshold: C.double(n.KVThreshold)}
+	}
+	return ligError("lig_set_filter_tree", C.lig_set_filter_tree(c.p, &cn[0], C.int(len(cn))))
+}
+
 // uploadSnapshot copies the packed columns into C memory for the duration of the call only
 // (the library stages them into its own pinned blob before returning).
 func (c *ctx) uploadSnapshot(epoch uint64, s *packedSnapshot) error {

@@ -32,6 +32,36 @@ type Options struct {
 	KVCacheThreshold       float64
 	QueueThresholdCritical int64
 	QueueingThresholdLoRA  int64
+	// FilterTree replaces defaultFilter (scheduler.go:26-91) by a caller flow chart of the
+	// reference's filter nodes (filter.go:17-73); nil = defaultFilter.  Its nodes carry their own
+	// thresholds, so the three above then do not apply.  See lig_set_filter_tree in include/lig.h.
+	FilterTree []FilterNode
+}
+
+// FilterKind names the filter functions of filter.go / scheduler.go a FilterNode runs.
+type FilterKind int32
+
+const (
+	FilterCriticalRequest  FilterKind = iota // criticalRequestPredicate             filter.go:179-181
+	FilterLowQueueing                        // WaitingQueueSize < QueueThreshold     filter.go:124-126
+	FilterLoRAAffinity                       // loRAAffinityPredicate                filter.go:169-172
+	FilterCanAcceptNewLoRA                   // canAcceptNewLoraPredicate            filter.go:175-177
+	FilterLowLoRACost                        // lowLoRACostPredicate                 filter.go:163-166
+	FilterNoQueueAndLowKV                    // noQueueAndLessThanKVCacheThresholdPredicate  filter.go:183-187
+	FilterLeastQueuing                       // leastQueuingFilterFunc               filter.go:102-122
+	FilterLeastKVCache                       // leastKVCacheFilterFunc               filter.go:134-154
+	FilterDrop                               // the "drop request" func              scheduler.go:83-89
+)
+
+// FilterNode is one node of a caller flow chart (include/lig.h lig_filter_node).  Node 0 is the
+// root; successors are indices of later nodes, -1 = nil, and a node may have several parents.
+type FilterNode struct {
+	Kind                   FilterKind
+	NextOnSuccess          int32
+	NextOnFailure          int32
+	NextOnSuccessOrFailure int32
+	QueueThreshold         int64   // FilterLowQueueing, FilterNoQueueAndLowKV
+	KVThreshold            float64 // FilterNoQueueAndLowKV
 }
 
 func DefaultOptions() Options {
@@ -83,6 +113,12 @@ func NewGPUScheduler(pmp scheduling.PodMetricsProvider, opt Options) (*GPUSchedu
 	if err := c.setThresholds(opt.KVCacheThreshold, opt.QueueThresholdCritical, opt.QueueingThresholdLoRA); err != nil {
 		c.close()
 		return nil, err
+	}
+	if len(opt.FilterTree) > 0 { // before the first snapshot upload: every table is built with it
+		if err := c.setFilterTree(opt.FilterTree); err != nil {
+			c.close()
+			return nil, err
+		}
 	}
 	in, err := allocPinned(opt.MaxBatch * 16)
 	if err != nil {
@@ -254,6 +290,10 @@ func (g *GPUScheduler) flush(batch []*waiter) {
 			// after request.go:74 wraps it again and server.go:97-109 answers 429.
 			inner := status.Errorf(codes.ResourceExhausted, "dropping request due to limited backend resources")
 			w.done <- result{err: fmt.Errorf("failed to apply filter, resulted %v pods, this should never happen: %w", 0, inner)}
+		case C.LIG_NO_PODS_LEFT:
+			// a FilterTree ended on a predicate node that kept no pod: toFilterFunc's error
+			// (filter.go:88-90) wrapped like scheduler.go:117; status.Code(err) is Unknown
+			w.done <- result{err: fmt.Errorf("failed to apply filter, resulted %v pods, this should never happen: %w", 0, fmt.Errorf("no pods left"))}
 		default:
 			var nilErr error
 			w.done <- result{err: fmt.Errorf("failed to apply filter, resulted %v pods, this should never happen: %w", 0, nilErr)}

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define LIG_ABI_VERSION 2
+#define LIG_ABI_VERSION 3
 
 /* ---- per-request status (lig_pick.status) ------------------------------------------------------
  * LIG_OK    Schedule returned a pod, nil                      pkg/ext-proc/scheduling/scheduler.go:120-121
@@ -34,11 +34,17 @@ extern "C" {
  *           resources") wrapped like scheduler.go:117         scheduler.go:83-89  -> 429 at handlers/server.go:97-109
  * LIG_EMPTY the tree returned ([], nil): "failed to apply filter, resulted 0 pods, this should
  *           never happen"                                      scheduler.go:116-118
+ * LIG_NO_PODS_LEFT  (caller filter trees only, see lig_set_filter_tree) the tree ended on a
+ *           predicate node that kept no pod: toFilterFunc's fmt.Errorf("no pods left")
+ *           (filter.go:88-90) wrapped by Schedule: "failed to apply filter, resulted 0 pods, this
+ *           should never happen: no pods left" (scheduler.go:116-118).  The built-in tree never
+ *           ends this way: every predicate node in it has a failure successor.
  */
 enum { LIG_OK = 0, LIG_DROP = 1, LIG_EMPTY = 2,
        /* only from the model entry points (lig_schedule_models_*): FetchModelData returned nil,
         * "error finding a model object in InferenceModel for input ..."  handlers/request.go:42-45 */
-       LIG_NO_MODEL = 3 };
+       LIG_NO_MODEL = 3,
+       LIG_NO_PODS_LEFT = 4 };
 
 /* ---- batch-level error codes (negative return values) ---------------------------------------- */
 enum {
@@ -100,8 +106,55 @@ typedef struct lig_ctx lig_ctx; /* opaque; one per (process, device) */
 int  lig_create(lig_ctx** out, int device, int max_pods, int max_adapters, int max_batch);
 void lig_destroy(lig_ctx* ctx);
 
+/* With a caller filter tree set (lig_set_filter_tree) the thresholds are still stored but do not
+ * affect the class-table build: every node of a caller tree carries its own thresholds. */
 int  lig_set_thresholds(lig_ctx* ctx, const lig_thresholds* t);   /* scheduler.go:15-24 */
 int  lig_get_thresholds(const lig_ctx* ctx, lig_thresholds* t);
+
+/* ---- caller-defined filter trees ----------------------------------------------------------------
+ * The reference's scheduler is a flow chart of `filter` nodes linked by nextOnSuccess,
+ * nextOnFailure and nextOnSuccessOrFailure (filter.go:17-73); Scheduler holds it as a Filter field
+ * (scheduler.go:101-104) and defaultFilter (scheduler.go:26-91) is one such chart.  A caller tree
+ * is any chart of the node kinds below, given as a table whose node 0 is the root.  Routing is
+ * (*filter).Filter (filter.go:44-73): success = no error AND a non-empty result; on success the
+ * node's result goes to next_on_success if set, else next_on_success_or_failure; on failure the
+ * node's INPUT goes to next_on_failure if set, else next_on_success_or_failure; when the chosen
+ * field is -1 (nil) the node's own (result, error) is the tree's result.  Every kind depends on the
+ * request only through (Critical, ResolvedTargetModel), so any tree still yields one survivor set
+ * per request class and runs on the class tables of every entry point above and below. */
+enum {                                   /* filter.go / scheduler.go names                         */
+  LIG_F_CRITICAL_REQUEST = 0,            /* criticalRequestPredicate             filter.go:179-181 */
+  LIG_F_LOW_QUEUEING,                    /* WaitingQueueSize < queue_threshold   filter.go:124-126 */
+  LIG_F_LORA_AFFINITY,                   /* loRAAffinityPredicate                filter.go:169-172 */
+  LIG_F_CAN_ACCEPT_NEW_LORA,             /* canAcceptNewLoraPredicate            filter.go:175-177 */
+  LIG_F_LOW_LORA_COST,                   /* lowLoRACostPredicate                 filter.go:163-166 */
+  LIG_F_NO_QUEUE_AND_LOW_KV,             /* q <= queue_threshold && kv <= kv_threshold
+                                            noQueueAndLessThanKVCacheThresholdPredicate filter.go:183-187 */
+  LIG_F_LEAST_QUEUING,                   /* leastQueuingFilterFunc               filter.go:102-122 */
+  LIG_F_LEAST_KV_CACHE,                  /* leastKVCacheFilterFunc               filter.go:134-154 */
+  LIG_F_DROP                             /* the "drop request" func: ([], ResourceExhausted)
+                                                                                 scheduler.go:83-89 */
+};
+/* Predicate kinds (the first six) fail with "no pods left" when they keep no pod (toFilterFunc,
+ * filter.go:79-93); the two range kinds never err, they fail only on an empty result. */
+typedef struct lig_filter_node {         /* 32 bytes */
+  int32_t kind;                          /* LIG_F_* */
+  int32_t next_on_success, next_on_failure, next_on_success_or_failure;  /* node index, -1 = nil */
+  int64_t queue_threshold;               /* LOW_QUEUEING, NO_QUEUE_AND_LOW_KV; ignored otherwise   */
+  double  kv_threshold;                  /* NO_QUEUE_AND_LOW_KV; ignored otherwise                 */
+} lig_filter_node;
+#define LIG_MAX_FILTER_NODES 32
+/* Use `nodes` for every class-table build enqueued after the call returns: lig_upload_snapshot
+ * and its _async / _device forms, lig_update_snapshot, the lig_comm_* uploads and the per-window
+ * rebuilds of lig_schedule_batch_feedback_device.  Resident epochs keep the tables they were built
+ * with.  nodes == NULL with n_nodes == 0 restores the built-in tree (defaultFilter with the
+ * lig_set_thresholds values).  LIG_ERR_INVALID, and the previous tree stays in force, when n_nodes
+ * is outside [1, LIG_MAX_FILTER_NODES], a kind is unknown, or a successor of node i is neither -1
+ * nor in (i, n_nodes): edges only point forward, so every table is acyclic, and a node may have
+ * several parents (defaultFilter shares queueAndKVCacheFilter).  The direct scan
+ * (lig_schedule_scan[_device]) restates the built-in tree only: it returns LIG_ERR_INVALID for an
+ * epoch whose tables a caller tree built; lig_read_class reads a caller tree's survivor sets. */
+int  lig_set_filter_tree(lig_ctx* ctx, const lig_filter_node* nodes, int n_nodes);
 
 /* ---- snapshot = the value of PodMetricsProvider.AllPodMetrics() (scheduler.go:108-115,
  * backend/provider.go:38-46) frozen at one refresh tick, in device layout -----------------------
@@ -286,7 +339,7 @@ int lig_read_class(lig_ctx* ctx, uint64_t epoch, int critical, int adapter_id, i
 #define LIG_DRAW_DOMAIN 0xA0761D6478BD642Full
 typedef struct lig_mpick {
   int16_t pod_idx;     /* as lig_pick.pod_idx (-1 unless LIG_OK)                                  */
-  uint8_t status;      /* LIG_OK / LIG_DROP / LIG_EMPTY / LIG_NO_MODEL                            */
+  uint8_t status;      /* LIG_OK / LIG_DROP / LIG_EMPTY / LIG_NO_MODEL / LIG_NO_PODS_LEFT         */
   uint8_t target_idx;  /* index of the drawn Spec.TargetModels entry (the body's "model" rewrite,
                           request.go:61-69); 255 = TargetModels empty, the model name passes through */
 } lig_mpick;
@@ -343,6 +396,8 @@ void lig_group_destroy(lig_group* g);
 int  lig_group_size(const lig_group* g);
 lig_ctx* lig_group_ctx(lig_group* g, int member);   /* member ctx, e.g. for the device-pointer API */
 int  lig_group_set_thresholds(lig_group* g, const lig_thresholds* t);
+/* lig_set_filter_tree on every member (validated once: an invalid table changes no member). */
+int  lig_group_set_filter_tree(lig_group* g, const lig_filter_node* nodes, int n_nodes);
 /* lig_upload_snapshot for the whole group: one pack, one H2D to member 0, one ncclBroadcast over
  * NVLink, one class-table build per member.  Resident on every member when it returns. */
 int  lig_group_upload_snapshot(lig_group* g, uint64_t epoch, int P, int A, const double* kv,

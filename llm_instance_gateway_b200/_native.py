@@ -11,12 +11,16 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "liblig.so")
 
-LIG_OK, LIG_DROP, LIG_EMPTY, LIG_NO_MODEL = 0, 1, 2, 3
+LIG_OK, LIG_DROP, LIG_EMPTY, LIG_NO_MODEL, LIG_NO_PODS_LEFT = 0, 1, 2, 3, 4
 LIG_DRAW_DOMAIN = 0xA0761D6478BD642F
 LIG_ERR_INVALID, LIG_ERR_CUDA, LIG_ERR_STALE_EPOCH, LIG_ERR_NO_SNAPSHOT, LIG_ERR_RANGE = -1, -2, -3, -4, -5
 LIG_ERR_BUSY, LIG_ERR_NCCL = -6, -7
 LIG_MAX_TICKETS, LIG_COMM_ID_BYTES = 256, 128
-LIG_ABI_VERSION = 2
+LIG_ABI_VERSION = 3
+# filter node kinds of a caller filter tree (lig_set_filter_tree)
+(LIG_F_CRITICAL_REQUEST, LIG_F_LOW_QUEUEING, LIG_F_LORA_AFFINITY, LIG_F_CAN_ACCEPT_NEW_LORA, LIG_F_LOW_LORA_COST,
+ LIG_F_NO_QUEUE_AND_LOW_KV, LIG_F_LEAST_QUEUING, LIG_F_LEAST_KV_CACHE, LIG_F_DROP) = range(9)
+LIG_MAX_FILTER_NODES = 32
 LIG_REQ_CRITICAL = 1
 LIG_MAX_PODS, LIG_MAX_ADAPTERS = 32768, 65534
 
@@ -35,7 +39,7 @@ EXPORTED_SYMBOLS = (
     "lig_comm_allreduce_i32",
     "lig_upload_models", "lig_schedule_models_batch", "lig_schedule_models_batches_device", "lig_resolve_models",
     "lig_pick_kernel_info", "lig_schedule_batch_feedback_device", "lig_update_snapshot",
-    "lig_upload_snapshot_async", "lig_upload_models_async",
+    "lig_upload_snapshot_async", "lig_upload_models_async", "lig_set_filter_tree", "lig_group_set_filter_tree",
 )
 
 
@@ -50,6 +54,12 @@ class LigPick(C.Structure):
 class LigThresholds(C.Structure):
     _fields_ = [("kv_cache_threshold", C.c_double), ("queue_threshold_critical", C.c_int64),
                 ("queueing_threshold_lora", C.c_int64)]
+
+
+class LigFilterNode(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("next_on_success", C.c_int32), ("next_on_failure", C.c_int32),
+                ("next_on_success_or_failure", C.c_int32), ("queue_threshold", C.c_int64),
+                ("kv_threshold", C.c_double)]
 
 
 class LigError(RuntimeError):
@@ -78,6 +88,8 @@ def load() -> C.CDLL:
     lib.lig_destroy.restype = None
     lib.lig_set_thresholds.argtypes = [vp, C.POINTER(LigThresholds)]
     lib.lig_get_thresholds.argtypes = [vp, C.POINTER(LigThresholds)]
+    lib.lig_set_filter_tree.argtypes = [vp, C.POINTER(LigFilterNode), i32]
+    lib.lig_group_set_filter_tree.argtypes = [vp, C.POINTER(LigFilterNode), i32]
     lib.lig_snapshot_bytes.argtypes = [i32, i32]
     lib.lig_snapshot_bytes.restype = C.c_size_t
     lib.lig_pack_pods.argtypes = [i32, vp, vp, vp, vp, vp, vp]

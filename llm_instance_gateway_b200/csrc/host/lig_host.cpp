@@ -47,11 +47,15 @@ Status NewScheduler(std::shared_ptr<PodMetricsProvider> pmp, const Options& opt,
                          opt.max_batch) != 0)
       return LigFailure("lig_group_create");
     if (lig_group_set_thresholds(s->group_, &t) != 0) return LigFailure("lig_group_set_thresholds");
+    if (!opt.filter.empty() && lig_group_set_filter_tree(s->group_, opt.filter.data(), (int)opt.filter.size()) != 0)
+      return LigFailure("lig_group_set_filter_tree");
   } else {
     const int dev = opt.devices.size() == 1 ? opt.devices[0] : opt.device;
     if (lig_create(&s->ctx_, dev, opt.max_pods, opt.max_adapters, opt.max_batch) != 0)
       return LigFailure("lig_create");
     if (lig_set_thresholds(s->ctx_, &t) != 0) return LigFailure("lig_set_thresholds");
+    if (!opt.filter.empty() && lig_set_filter_tree(s->ctx_, opt.filter.data(), (int)opt.filter.size()) != 0)
+      return LigFailure("lig_set_filter_tree");
   }
   s->h_reqs_ = static_cast<lig_req*>(lig_host_alloc((size_t)opt.max_batch * sizeof(lig_req)));
   s->h_picks_ = static_cast<lig_pick*>(lig_host_alloc((size_t)opt.max_batch * sizeof(lig_pick)));
@@ -379,6 +383,9 @@ void Scheduler::Flush(std::vector<Waiter*>& batch) {
         w->status = Errorf(ResourceExhausted,                         // scheduler.go:117
                            std::string("failed to apply filter, resulted 0 pods, this should never "
                                        "happen: ") + kDropInner);
+      } else if (h_picks_[i].status == LIG_NO_PODS_LEFT) {   // a caller tree's predicate leaf kept no pod
+        w->status = Errorf(Unknown, "failed to apply filter, resulted 0 pods, this should never "
+                                    "happen: no pods left");   // filter.go:88-90
       } else {
         w->status = Errorf(Unknown, "failed to apply filter, resulted 0 pods, this should never "
                                     "happen: %!w(<nil>)");

@@ -27,6 +27,8 @@
 #include <unordered_map>
 #include <vector>
 
+#include "../../../include/lig.h"
+
 struct lig_ctx;
 struct lig_group;
 struct lig_req;
@@ -136,6 +138,9 @@ struct Options {
   double kv_cache_threshold = 0.8;   // scheduler.go:15-24
   int64_t queue_threshold_critical = 5;
   int64_t queueing_threshold_lora = 50;
+  // A caller flow chart of the reference's filter nodes (lig_set_filter_tree, node 0 = root)
+  // instead of defaultFilter; empty = the built-in tree.  Its nodes carry their own thresholds.
+  std::vector<lig_filter_node> filter;
 };
 
 struct Stats {

@@ -163,6 +163,36 @@ ligh_scheduler* ligh_scheduler_new(ligh_provider* p, int device, int max_pods, i
                              refresh_ms, seed, 0, 0, 0, err, err_cap);
 }
 
+ligh_scheduler* ligh_scheduler_new_tree(ligh_provider* p, int device, const int* devices, int n_devices,
+                                        int max_pods, int max_adapters, int max_batch, int flush_size,
+                                        int window_us, int refresh_ms, uint64_t seed, int busy_poll,
+                                        int caller_spin_us, int use_doorbell, const lig_filter_node* nodes,
+                                        int n_nodes, char* err, int err_cap) {
+  scheduling::Options o;
+  o.device = device;
+  if (devices && n_devices > 1) o.devices.assign(devices, devices + n_devices);
+  o.busy_poll = busy_poll != 0;
+  o.caller_spin = std::chrono::microseconds(caller_spin_us);
+  o.use_doorbell = use_doorbell != 0;
+  o.max_pods = max_pods;
+  o.max_adapters = max_adapters;
+  o.max_batch = max_batch;
+  o.flush_size = flush_size;
+  o.batch_window = std::chrono::microseconds(window_us);
+  o.refresh_interval = std::chrono::milliseconds(refresh_ms);
+  o.seed = seed;
+  if (nodes && n_nodes > 0) o.filter.assign(nodes, nodes + n_nodes);
+  auto* s = new ligh_scheduler();
+  s->provider = share(p);
+  scheduling::Status st = scheduling::NewScheduler(s->provider, o, &s->sched);
+  if (!st.ok()) {
+    put(err, err_cap, st.message);
+    delete s;
+    return nullptr;
+  }
+  return s;
+}
+
 void ligh_scheduler_free(ligh_scheduler* s) { delete s; }
 
 int ligh_schedule(ligh_scheduler* s, const char* model, const char* resolved, int critical,

@@ -3,6 +3,8 @@
 #ifndef LIG_HOST_C_H_
 #define LIG_HOST_C_H_
 #include <stdint.h>
+
+#include "../../../include/lig.h"
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -28,6 +30,13 @@ ligh_scheduler* ligh_scheduler_new2(ligh_provider*, int device, int max_pods, in
                                     int max_batch, int flush_size, int batch_window_us,
                                     int refresh_interval_ms, uint64_t seed, int busy_poll,
                                     int caller_spin_us, int use_doorbell, char* err, int err_cap);
+/* ligh_scheduler_new2 / _new_devices with a caller filter tree (Options::filter; see
+ * lig_set_filter_tree): n_devices > 1 lists the GPUs of one scheduler (then `device` is ignored). */
+ligh_scheduler* ligh_scheduler_new_tree(ligh_provider*, int device, const int* devices, int n_devices,
+                                        int max_pods, int max_adapters, int max_batch, int flush_size,
+                                        int batch_window_us, int refresh_interval_ms, uint64_t seed,
+                                        int busy_poll, int caller_spin_us, int use_doorbell,
+                                        const lig_filter_node* nodes, int n_nodes, char* err, int err_cap);
 void ligh_scheduler_free(ligh_scheduler*);
 /* Scheduler.Schedule: returns the gRPC code (0 OK, 8 ResourceExhausted, 2 Unknown, 13 Internal). */
 int ligh_schedule(ligh_scheduler*, const char* model, const char* resolved_target_model, int critical,

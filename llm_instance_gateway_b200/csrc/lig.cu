@@ -107,6 +107,7 @@ struct Slot {
   cudaEvent_t readers[kReaders] = {};
   int next_reader = 0;
   uint64_t stamp = 0;               // upload order, to pick the slot to overwrite
+  bool caller_tree = false;         // tables built with a caller filter tree (thresholds do not apply)
 };
 
 constexpr int kLanes = 8;   // streams of the host-buffer path; also the queue streams
@@ -119,6 +120,9 @@ struct lig_ctx {
   int sm_count = 0;
   size_t smem_optin = 0;
   lig_thresholds thr{0.8, 5, 50};
+  // caller filter tree (lig_set_filter_tree), guarded by upload_mu like every snapshot writer
+  FilterTree tree{};
+  bool has_tree = false;
   // mu guards the slot metadata, the reader rings, lanes/tickets and the item ring.  It is held
   // only while work is ENQUEUED, never across a host-device synchronisation.  upload_mu serialises
   // snapshot writers (uploads, threshold rebuilds) and is taken BEFORE mu.  bounce_mu serialises
@@ -255,6 +259,15 @@ int note_reader(Slot& s, cudaStream_t st) {
   return 0;
 }
 
+// The direct scan restates the built-in tree only: it refuses an epoch whose class tables a caller
+// filter tree built (lig_read_class reads those survivor sets).
+int check_scannable(const Slot& s, uint64_t epoch) {
+  if (s.caller_tree)
+    return fail(LIG_ERR_INVALID, "direct scan: epoch %llu was built with a caller filter tree; the scan "
+                                 "walks the built-in tree only", (unsigned long long)epoch);
+  return 0;
+}
+
 // `writer` must not touch slot s before every recorded reader has finished.
 int wait_readers(Slot& s, cudaStream_t writer) {
   for (cudaEvent_t ev : s.readers) CUDA_TRY(cudaStreamWaitEvent(writer, ev, 0));
@@ -266,11 +279,32 @@ bool staged_fits(const lig_ctx* c, int W) {
   return scratch_bytes(W) + staged_bytes(W) <= c->smem_optin;
 }
 
-// Enqueue the class-table build for slot s on `stream`.
-int launch_class_build(lig_ctx* c, Slot& s, cudaStream_t stream) {
+// Enqueue the class-table build for slot s on `stream`: the caller's filter tree when `tree` is not
+// null, else the built-in tree.
+int launch_class_build(lig_ctx* c, Slot& s, cudaStream_t stream, const FilterTree* tree) {
   const SnapView v = view_of(s);
   const int n_classes = 2 * (s.A + 1);
   const int W = s.W > 0 ? s.W : 1;
+  s.caller_tree = tree != nullptr;
+  if (tree) {
+    // one warp per class; the pod columns go to shared memory when they fit (P up to ~12 K pods)
+    const bool staged = s.P > 0 && tree_fixed_bytes(W) + staged_bytes(W) <= c->smem_optin;
+    const size_t smem = tree_fixed_bytes(W) + (staged ? staged_bytes(W) : 0);
+    int per_sm = 0;
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(
+        &per_sm, staged ? lig_class_build_tree_kernel<true> : lig_class_build_tree_kernel<false>, kCtaThreads, smem));
+    int grid = (n_classes + kWarpsPerCta - 1) / kWarpsPerCta;
+    if (grid > c->sm_count * (per_sm > 0 ? per_sm : 1)) grid = c->sm_count * (per_sm > 0 ? per_sm : 1);
+    const CompactOut co{s.d_ctab, s.d_counters, s.ctab_pool_capacity, s.d_hdr_alias, nullptr};
+    const int stride = s.P > 0 ? s.P : 1;
+    if (staged)
+      lig_class_build_tree_kernel<true><<<grid, kCtaThreads, smem, stream>>>(v, *tree, s.d_cls, s.d_lists, stride, co);
+    else
+      lig_class_build_tree_kernel<false><<<grid, kCtaThreads, smem, stream>>>(v, *tree, s.d_cls, s.d_lists, stride, co);
+    CUDA_TRY(cudaGetLastError());
+    c->launches++;
+    return 0;
+  }
   const bool staged = s.P > 0 && build_fixed_bytes(W) + staged_bytes(W) <= c->smem_optin;
   const size_t smem = build_fixed_bytes(W) + (staged ? staged_bytes(W) : 0);
   // every CTA repeats the shared stages, so no more CTAs than needed to give each warp a couple
@@ -699,6 +733,24 @@ void set_comm_destructor(void (*fn)(void*)) { g_comm_destructor = fn; }
 static allreduce_fn g_allreduce = nullptr;
 void set_allreduce(allreduce_fn fn) { g_allreduce = fn; }
 
+int check_filter_tree(const lig_filter_node* nodes, int n_nodes) {
+  if (!nodes && n_nodes == 0) return 0;   // back to the built-in tree
+  if (!nodes || n_nodes < 1 || n_nodes > LIG_MAX_FILTER_NODES)
+    return fail(LIG_ERR_INVALID, "filter tree: %d nodes (1..%d, or NULL and 0 for the built-in tree)",
+                n_nodes, LIG_MAX_FILTER_NODES);
+  for (int i = 0; i < n_nodes; ++i) {
+    const lig_filter_node& nd = nodes[i];
+    if (nd.kind < LIG_F_CRITICAL_REQUEST || nd.kind > LIG_F_DROP)
+      return fail(LIG_ERR_INVALID, "filter tree: node %d has unknown kind %d", i, nd.kind);
+    const int32_t next[3] = {nd.next_on_success, nd.next_on_failure, nd.next_on_success_or_failure};
+    for (int32_t j : next)
+      if (j != -1 && (j <= i || j >= n_nodes))
+        return fail(LIG_ERR_INVALID, "filter tree: node %d links to %d (successors are -1 or in (%d, %d))",
+                    i, j, i, n_nodes);
+  }
+  return 0;
+}
+
 int begin_write(lig_ctx* c, uint64_t epoch, int P, int A, cudaStream_t stream, bool own_stream,
                 SnapshotWrite* w) {
   if (int rc = check_shape(c, P, A)) return rc;
@@ -747,7 +799,7 @@ int begin_write(lig_ctx* c, uint64_t epoch, int P, int A, cudaStream_t stream, b
 int enqueue_build(lig_ctx* c, SnapshotWrite* w) {
   Slot& s = *static_cast<Slot*>(w->slot);
   CUDA_TRY(cudaSetDevice(c->device));
-  if (int rc = launch_class_build(c, s, w->stream)) return rc;
+  if (int rc = launch_class_build(c, s, w->stream, c->has_tree ? &c->tree : nullptr)) return rc;
   CUDA_TRY(cudaEventRecord(s.ready, w->stream));
   return 0;
 }
@@ -907,6 +959,8 @@ static int create_impl(lig_ctx* c, int device, int max_pods, int max_adapters, i
   CUDA_TRY(cudaFuncSetAttribute(lig_class_build_kernel<false>,
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_class_build_fast_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_class_build_tree_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_class_build_tree_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_scan_kernel<true>,
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_scan_kernel<false>,
@@ -1116,16 +1170,30 @@ int lig_set_thresholds(lig_ctx* c, const lig_thresholds* t) {
   {
     std::lock_guard<std::mutex> lk(c->mu);
     c->thr = *t;
-    // resident class tables were built with the old thresholds: rebuild them
+    // resident class tables built by the built-in tree used the old thresholds: rebuild them
+    // (tables of a caller tree do not depend on them)
     for (auto& s : c->slot) {
-      if (!s.valid) continue;
+      if (!s.valid || s.caller_tree) continue;
       if (int rc = wait_readers(s, c->s_up)) return rc;
       CUDA_TRY(cudaStreamWaitEvent(c->s_up, s.ready, 0));
-      if (int rc = launch_class_build(c, s, c->s_up)) return rc;
+      if (int rc = launch_class_build(c, s, c->s_up, nullptr)) return rc;
       CUDA_TRY(cudaEventRecord(s.ready, c->s_up));
     }
   }
   CUDA_TRY(cudaStreamSynchronize(c->s_up));
+  return 0;
+}
+
+int lig_set_filter_tree(lig_ctx* c, const lig_filter_node* nodes, int n_nodes) {
+  if (!c) return fail(LIG_ERR_INVALID, "lig_set_filter_tree: null ctx");
+  if (int rc = ligi::check_filter_tree(nodes, n_nodes)) return rc;
+  std::lock_guard<std::mutex> uk(c->upload_mu);
+  if (nodes) {
+    c->tree = FilterTree{};
+    memcpy(c->tree.nodes, nodes, (size_t)n_nodes * sizeof(lig_filter_node));
+    c->tree.n_nodes = n_nodes;
+  }
+  c->has_tree = nodes != nullptr;
   return 0;
 }
 
@@ -1353,6 +1421,7 @@ int lig_schedule_scan_device(lig_ctx* c, uint64_t epoch, uint64_t seed, const li
   std::lock_guard<std::mutex> lk(c->mu);
   Slot* s = nullptr;
   if (int rc = resolve_slot(c, epoch, &s)) return rc;
+  if (int rc = check_scannable(*s, epoch)) return rc;
   if (R == 0) return 0;
   CUDA_TRY(cudaSetDevice(c->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1440,6 +1509,7 @@ int lig_schedule_scan(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* 
     std::lock_guard<std::mutex> lk(c->mu);
     Slot* s = nullptr;
     if (int rc = resolve_slot(c, epoch, &s)) return rc;
+    if (int rc = check_scannable(*s, epoch)) return rc;
     if (R == 0) return 0;
     CUDA_TRY(cudaSetDevice(c->device));
     mask_bytes = masks ? (size_t)R * (s->W > 0 ? s->W : 1) * sizeof(uint32_t) : 0;
@@ -1707,6 +1777,14 @@ int lig_schedule_batch_feedback_device(lig_ctx* c, uint64_t epoch, uint64_t seed
   if (n_windows <= 0) n_windows = (R + sub_batch - 1) / sub_batch;
   if ((long long)n_windows * sub_batch < R)
     return fail(LIG_ERR_INVALID, "n_windows=%d x sub_batch=%d does not cover R=%d", n_windows, sub_batch, R);
+  // the tree in force when the call starts rebuilds every window's tables
+  FilterTree tree;
+  bool has_tree;
+  {
+    std::lock_guard<std::mutex> uk(c->upload_mu);
+    has_tree = c->has_tree;
+    if (has_tree) tree = c->tree;
+  }
   std::lock_guard<std::mutex> fk(c->fb_mu);
   CUDA_TRY(cudaSetDevice(c->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1738,7 +1816,7 @@ int lig_schedule_batch_feedback_device(lig_ctx* c, uint64_t epoch, uint64_t seed
     const int n = lo >= R ? 0 : (int)((R - lo) < sub_batch ? (R - lo) : sub_batch);
     {
       std::lock_guard<std::mutex> lk(c->mu);                 // launch counters, item ring
-      if (int rc = launch_class_build(c, fs, st)) return rc;
+      if (int rc = launch_class_build(c, fs, st, has_tree ? &tree : nullptr)) return rc;
       if (n > 0) {
         // the tables of the scratch copy change every window: always the strided tables through
         // L1 (no host round trip for the compact header inside the loop)

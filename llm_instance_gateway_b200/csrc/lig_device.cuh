@@ -48,8 +48,9 @@ struct Thr {
 // (rows 2(A+1) and 2(A+1)+1 of the list pool); the others own row c.  List offsets are in list
 // entries and fit 32 bits: (2 * 65535 + 3) rows x 32768 entries < 2^32.
 //
-//   info    : bits 0-1 status | 4-8 shift | 16-31 n
-//             (info & 0xffff0003 is the second word of lig_pick as is: status | n_survivors << 16)
+//   info    : bits 0-2 status | 4-8 shift | 16-31 n   (bit 2 only for LIG_NO_PODS_LEFT, which only
+//             caller filter trees produce)
+//             (info & 0xffff0007 is the second word of lig_pick as is: status | n_survivors << 16)
 //   magic   : M = ceil(2^(32+shift) / n), shift = ceil(log2 n) - 1, so that for every v < 2^31
 //             floor(v / n) == umulhi(v, M) >> shift   (Granlund-Montgomery, N = 31 bits; n >= 2)
 //   q_limit : floor(2^31 / n).  With q = floor(v / n), Go's Int31n is k = v - q * n, resampling
@@ -66,7 +67,7 @@ struct ClassEntry {
 };
 
 __host__ __device__ inline uint32_t entry_n(uint32_t info) { return info >> 16; }
-__host__ __device__ inline uint32_t entry_status(uint32_t info) { return info & 3u; }
+__host__ __device__ inline uint32_t entry_status(uint32_t info) { return info & 7u; }
 // Entries of the list pool: one row per class, two shared default rows, then the sentinel.
 __host__ __device__ inline size_t list_pool_entries(size_t n_classes, size_t stride) {
   return (n_classes + 2) * stride + 8;
@@ -674,6 +675,34 @@ struct CompactOut {       // where the build writes the blob; counters[0] = pool
 };
 #define LIG_STAMP(k) do { if (co.dbg && blockIdx.x == 0 && threadIdx.x == 0) co.dbg[k] = clock64(); } while (0)
 
+// The last CTA of a build to finish seals the compact blob: total size, or 0 when the pool
+// overflowed (the pick kernels then keep to the strided tables).  Called by every thread.
+__device__ __forceinline__ void seal_compact(const CompactOut& co, int n_classes, uint32_t fixed_entries) {
+  CompactHeader* chdr = reinterpret_cast<CompactHeader*>(co.blob);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    if (atomicAdd(co.counters + 1, 1u) == gridDim.x - 1) {
+      __threadfence();
+      const uint32_t total = fixed_entries + *reinterpret_cast<volatile uint32_t*>(co.counters);
+      chdr->n_classes = (uint32_t)n_classes;
+      chdr->pool_entries = total;
+      chdr->reserved = 0;
+      chdr->bytes = total <= co.pool_capacity
+                        ? (uint32_t)((sizeof(CompactHeader) + (size_t)n_classes * sizeof(ClassEntry) +
+                                      (size_t)total * sizeof(uint16_t) + 15) & ~(size_t)15) : 0u;
+      if (co.host_hdr) {
+        co.host_hdr->n_classes = chdr->n_classes;
+        co.host_hdr->pool_entries = total;
+        co.host_hdr->reserved = 0;
+        co.host_hdr->bytes = chdr->bytes;
+      }
+      co.counters[0] = 0;   // ready for the next build of this slot
+      co.counters[1] = 0;
+    }
+  }
+}
+
 template <bool kStaged>
 __global__ void __launch_bounds__(kBuildThreads)
 lig_class_build_kernel(SnapView s, Thr thr, ClassEntry* __restrict__ cls,
@@ -701,34 +730,10 @@ lig_class_build_kernel(SnapView s, Thr thr, ClassEntry* __restrict__ cls,
   const uint32_t rs_row = rc_row + (uint32_t)list_stride;
   const uint32_t none = rs_row + (uint32_t)list_stride;                       // sentinel entry
   if (blockIdx.x == 0 && threadIdx.x == 0) lists[none] = 0xffffu;             // reads back as pod_idx -1
-  CompactHeader* chdr = reinterpret_cast<CompactHeader*>(co.blob);
   uint4* centries = reinterpret_cast<uint4*>(co.blob + sizeof(CompactHeader));
   uint16_t* cpool = reinterpret_cast<uint16_t*>(co.blob + sizeof(CompactHeader) + (size_t)n_classes * sizeof(ClassEntry));
   // the last CTA to finish seals the blob: total size, or 0 when the pool overflowed
-  auto seal = [&](uint32_t fixed_entries) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      __threadfence();
-      if (atomicAdd(co.counters + 1, 1u) == gridDim.x - 1) {
-        __threadfence();
-        const uint32_t total = fixed_entries + *reinterpret_cast<volatile uint32_t*>(co.counters);
-        chdr->n_classes = (uint32_t)n_classes;
-        chdr->pool_entries = total;
-        chdr->reserved = 0;
-        chdr->bytes = total <= co.pool_capacity
-                          ? (uint32_t)((sizeof(CompactHeader) + (size_t)n_classes * sizeof(ClassEntry) +
-                                        (size_t)total * sizeof(uint16_t) + 15) & ~(size_t)15) : 0u;
-        if (co.host_hdr) {
-          co.host_hdr->n_classes = chdr->n_classes;
-          co.host_hdr->pool_entries = total;
-          co.host_hdr->reserved = 0;
-          co.host_hdr->bytes = chdr->bytes;
-        }
-        co.counters[0] = 0;   // ready for the next build of this slot
-        co.counters[1] = 0;
-      }
-    }
-  };
+  auto seal = [&](uint32_t fixed_entries) { seal_compact(co, n_classes, fixed_entries); };
 
   if (P == 0) {   // critical: predicate node errs on an empty pool -> sheddable branch -> drop
     for (int c = blockIdx.x * kBuildThreads + threadIdx.x; c < n_classes; c += gridDim.x * kBuildThreads) {
@@ -974,7 +979,6 @@ lig_class_build_fast_kernel(SnapView s, Thr thr, ClassEntry* __restrict__ cls, u
   const uint32_t rc_row = (uint32_t)n_classes * (uint32_t)list_stride;
   const uint32_t rs_row = rc_row + (uint32_t)list_stride;
   const uint32_t none = rs_row + (uint32_t)list_stride;
-  CompactHeader* chdr = reinterpret_cast<CompactHeader*>(co.blob);
   uint4* centries = reinterpret_cast<uint4*>(co.blob + sizeof(CompactHeader));
   uint16_t* cpool = reinterpret_cast<uint16_t*>(co.blob + sizeof(CompactHeader) + (size_t)n_classes * sizeof(ClassEntry));
 
@@ -1034,30 +1038,7 @@ lig_class_build_fast_kernel(SnapView s, Thr thr, ClassEntry* __restrict__ cls, u
     }
     rb ^= 1;
   };
-  auto seal = [&](uint32_t fixed_entries) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      __threadfence();
-      if (atomicAdd(co.counters + 1, 1u) == gridDim.x - 1) {
-        __threadfence();
-        const uint32_t total = fixed_entries + *reinterpret_cast<volatile uint32_t*>(co.counters);
-        chdr->n_classes = (uint32_t)n_classes;
-        chdr->pool_entries = total;
-        chdr->reserved = 0;
-        chdr->bytes = total <= co.pool_capacity
-                          ? (uint32_t)((sizeof(CompactHeader) + (size_t)n_classes * sizeof(ClassEntry) +
-                                        (size_t)total * sizeof(uint16_t) + 15) & ~(size_t)15) : 0u;
-        if (co.host_hdr) {
-          co.host_hdr->n_classes = chdr->n_classes;
-          co.host_hdr->pool_entries = total;
-          co.host_hdr->reserved = 0;
-          co.host_hdr->bytes = chdr->bytes;
-        }
-        co.counters[0] = 0;   // ready for the next build of this slot
-        co.counters[1] = 0;
-      }
-    }
-  };
+  auto seal = [&](uint32_t fixed_entries) { seal_compact(co, n_classes, fixed_entries); };
 
   // ---- shared stages ----
   LIG_STAMP(2);
@@ -1255,6 +1236,147 @@ lig_class_build_fast_kernel(SnapView s, Thr thr, ClassEntry* __restrict__ cls, u
   LIG_STAMP(7);
 }
 
+// ---- K2a (caller filter trees): any chart of the reference's filter nodes ---------------------------
+// lig_set_filter_tree.  Only the class-table build knows the tree: every node kind depends on the
+// request only through (Critical, ResolvedTargetModel), so a caller tree still has one survivor set
+// per class and every pick kernel consumes its tables unchanged.
+//
+// One warp per class walks the table (filter.go:44-73) over all P pods with two W-word masks: `in`
+// is the node's input, `res` its result.  A failing node forwards its input (`in` stays), a
+// succeeding one its result (the masks swap), so the walk needs no stack; successors only point
+// forward, so it visits at most LIG_MAX_FILTER_NODES nodes.  Every class owns its strided row (no
+// shared default rows); the compact blob is packed and sealed as by the built-in builds.
+struct FilterTree {                      // passed by value: a __grid_constant__ kernel parameter
+  lig_filter_node nodes[LIG_MAX_FILTER_NODES];
+  int n_nodes;
+};
+constexpr size_t kTreeNodeBytes = sizeof(lig_filter_node) * LIG_MAX_FILTER_NODES;   // 1 KB
+static_assert(sizeof(lig_filter_node) == 32 && kTreeNodeBytes % 16 == 0, "node table layout");
+
+// Shared-memory carve-up of the tree build:
+//   [ node table ][ per-warp scratch: kWarpsPerCta x 3 x W words (H, in, res) ][ staged columns ]
+__host__ __device__ inline size_t tree_fixed_bytes(int W) { return kTreeNodeBytes + scratch_bytes(W); }
+
+// Does the predicate node `nd` keep pod w * 32 + lane?                          filter.go:163-187
+template <bool kStaged>
+__device__ __forceinline__ bool node_keeps(const lig_filter_node& nd, const Fields& f, const uint32_t* H,
+                                           bool critical, int w, int lane) {
+  const int p = w * 32 + lane;
+  switch (nd.kind) {
+    case LIG_F_CRITICAL_REQUEST: return critical;                                   // filter.go:179-181
+    case LIG_F_LOW_QUEUEING: return (long long)ld_q<kStaged>(f, p) < nd.queue_threshold;   // :124-126
+    case LIG_F_LORA_AFFINITY: return H && ((H[w] >> lane) & 1u);                     // filter.go:169-172
+    case LIG_F_CAN_ACCEPT_NEW_LORA: return has_room<kStaged>(f, p);                  // filter.go:175-177
+    case LIG_F_LOW_LORA_COST:                                                        // filter.go:163-166
+      return (H && ((H[w] >> lane) & 1u)) || has_room<kStaged>(f, p);
+    default:                             // LIG_F_NO_QUEUE_AND_LOW_KV                  filter.go:183-187
+      return (long long)ld_q<kStaged>(f, p) <= nd.queue_threshold && ld_kv<kStaged>(f, p) <= nd.kv_threshold;
+  }
+}
+
+// Walk the caller's tree for one (critical, adapter row), one warp.  H: the adapter's bitmap row in
+// shared memory, or nullptr for an adapter in no pod's ActiveModels (a Go map miss on every pod).
+template <bool kStaged>
+__device__ __forceinline__ EvalResult tree_walk_warp(const Fields& f, const lig_filter_node* nodes,
+                                                     const uint32_t* H, bool critical, int P, int W,
+                                                     uint32_t* in, uint32_t* res, int lane) {
+  for (int w = lane; w < W; w += 32) {   // the root's input: AllPodMetrics()    scheduler.go:115
+    const int rem = P - w * 32;
+    in[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
+  }
+  __syncwarp();
+  uint32_t n = (uint32_t)P;
+  int i = 0;
+  for (;;) {
+    const lig_filter_node nd = nodes[i];
+    uint32_t nr = 0, err = LIG_OK;
+    if (nd.kind == LIG_F_LEAST_QUEUING || nd.kind == LIG_F_LEAST_KV_CACHE) {
+      // the range filters work in place and a failure forwards the input: filter a copy
+      for (int w = lane; w < W; w += 32) res[w] = in[w];
+      __syncwarp();
+      nr = nd.kind == LIG_F_LEAST_QUEUING ? stage_least_queuing<kStaged>(f, res, W, lane, n)
+                                          : stage_least_kv<kStaged>(f, res, W, lane, n);
+    } else if (nd.kind == LIG_F_DROP) {
+      err = LIG_DROP;                    // ([], ResourceExhausted)                   scheduler.go:83-89
+    } else {                             // toFilterFunc(predicate)                    filter.go:79-93
+      for (int w = 0; w < W; ++w) {
+        const uint32_t word = in[w];
+        uint32_t nw = 0;
+        if (word != 0) nw = __ballot_sync(kFull, ((word >> lane) & 1u) && node_keeps<kStaged>(nd, f, H, critical, w, lane));
+        if (lane == 0) res[w] = nw;
+        nr += __popc(nw);
+      }
+      __syncwarp();
+      if (nr == 0) err = LIG_NO_PODS_LEFT;   // fmt.Errorf("no pods left")            filter.go:88-90
+    }
+    const bool ok = err == LIG_OK && nr > 0;                                        // filter.go:50
+    const int next = ok ? (nd.next_on_success >= 0 ? nd.next_on_success : nd.next_on_success_or_failure)
+                        : (nd.next_on_failure >= 0 ? nd.next_on_failure : nd.next_on_success_or_failure);
+    if (next < 0)                        // no successor: the node's own (filtered, err)  filter.go:52-54, 62-64
+      return {res, nr, err != LIG_OK ? err : (nr ? (uint32_t)LIG_OK : (uint32_t)LIG_EMPTY)};
+    if (ok) {                            // success passes the result on, failure the input  filter.go:60, 71
+      uint32_t* t = in; in = res; res = t;
+      n = nr;
+    }
+    i = next;
+  }
+}
+
+template <bool kStaged>
+__global__ void __launch_bounds__(kCtaThreads)
+lig_class_build_tree_kernel(SnapView s, const __grid_constant__ FilterTree tree, ClassEntry* __restrict__ cls,
+                            uint16_t* __restrict__ lists, int list_stride, CompactOut co) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int P = s.P, W = s.W, A = s.A;
+  lig_filter_node* nodes = reinterpret_cast<lig_filter_node*>(smem);
+  {
+    const uint32_t* src = reinterpret_cast<const uint32_t*>(tree.nodes);
+    uint32_t* dst = reinterpret_cast<uint32_t*>(smem);
+    const int words = tree.n_nodes * (int)(sizeof(lig_filter_node) / sizeof(uint32_t));
+    for (int i = threadIdx.x; i < words; i += blockDim.x) dst[i] = src[i];
+  }
+  uint32_t* H = reinterpret_cast<uint32_t*>(smem + kTreeNodeBytes) + (size_t)warp * 3 * W;
+  uint32_t* M0 = H + W;
+  uint32_t* M1 = H + 2 * W;
+  Fields f{s.kv, s.q, s.n_active, s.max_active};
+  if constexpr (kStaged) {
+    f = stage_fields(s, smem + tree_fixed_bytes(W));
+  }
+  __syncthreads();
+  const int n_classes = 2 * (A + 1);
+  const uint32_t none = (uint32_t)(n_classes + 2) * (uint32_t)list_stride;   // sentinel, as in the other builds
+  uint4* centries = reinterpret_cast<uint4*>(co.blob + sizeof(CompactHeader));
+  uint16_t* cpool = reinterpret_cast<uint16_t*>(co.blob + sizeof(CompactHeader) + (size_t)n_classes * sizeof(ClassEntry));
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    lists[none] = 0xffffu;               // reads back as pod_idx -1
+    cpool[0] = 0xffffu;
+  }
+  for (int c = blockIdx.x * kWarpsPerCta + warp; c < n_classes; c += gridDim.x * kWarpsPerCta) {
+    const bool critical = c >= A + 1;
+    const int a = critical ? c - (A + 1) : c;
+    const uint32_t* Hrow = stage_adapter_row(s, a, H, lane);     // nullptr for a == A
+    const EvalResult r = tree_walk_warp<kStaged>(f, nodes, Hrow, critical, P, W, M0, M1, lane);
+    const uint32_t off = (uint32_t)c * (uint32_t)list_stride;
+    uint32_t coff = 0;                   // the class's list in the compact pool (0 = the sentinel)
+    if (r.n) {
+      compact_mask_to_list(r.mask, W, lane, lists + off);
+      uint32_t at = 0;
+      if (lane == 0) at = atomicAdd(co.counters, r.n);             // pool space for this list
+      at = __shfl_sync(kFull, at, 0) + 1u;                          // behind the sentinel
+      if (at + r.n <= co.pool_capacity) compact_mask_to_list(r.mask, W, lane, cpool + at);
+      coff = at;
+    }
+    const ClassEntry e = make_entry(r.n, r.status, r.n ? off : none);
+    if (lane == 0) {
+      *reinterpret_cast<uint4*>(cls + c) = make_uint4(e.info, e.magic, e.q_limit, e.list_off);
+      centries[c] = make_uint4(e.info, e.magic, e.q_limit, coff);
+    }
+    __syncwarp();
+  }
+  seal_compact(co, n_classes, 1u);
+}
+
 // ---- snapshot delta ---------------------------------------------------------------------------------
 // One warp per dirty pod: overwrite its four column values, clear its bit in every adapter row,
 // set it again in the rows of its new ActiveModels.  Different pods may share a bitmap word, hence
@@ -1311,7 +1433,7 @@ __device__ __forceinline__ int2 pick_one(const int4 r, const uint4* __restrict__
   const uint32_t k = int31n_entry(seed ^ key, e);
   // n == 0: list_off is the pool's 0xffff sentinel -> -1
   const int pod = (int)(short)__ldg(lists + (e.w + k));
-  return make_int2(pod, (int)(e.x & 0xffff0003u));   // {pod_idx, status | n_survivors << 16}
+  return make_int2(pod, (int)(e.x & 0xffff0007u));   // {pod_idx, status | n_survivors << 16}
 }
 
 // The same pick against the compact tables in shared memory (entries + pool, see CompactHeader).
@@ -1324,7 +1446,7 @@ __device__ __forceinline__ int2 pick_one_smem(const int4 r, const uint4* tab, co
   const uint4 e = tab[c];
   const uint32_t k = int31n_entry(seed ^ key, e);
   const int pod = (int)(short)pool[e.w + k];
-  return make_int2(pod, (int)(e.x & 0xffff0003u));
+  return make_int2(pod, (int)(e.x & 0xffff0007u));
 }
 
 // One CTA's share of one batch: kPerThread requests per thread.
@@ -1857,7 +1979,7 @@ __device__ __forceinline__ uint32_t pick_model(uint32_t m, uint64_t key, const M
     return pack_mpick(-1, (uint32_t)LIG_NO_MODEL, 255u);
   const int4 r = make_int4((int)adapter, (int)critical, (int)(uint32_t)key, (int)(uint32_t)(key >> 32));
   const int2 p = kSmem ? pick_one_smem(r, cls, lists, A, seed) : pick_one(r, cls, lists, A, seed);
-  return pack_mpick(p.x, (uint32_t)p.y & 3u, target);
+  return pack_mpick(p.x, (uint32_t)p.y & 7u, target);
 }
 
 struct MQueueItem {
@@ -2008,7 +2130,7 @@ lig_pick_models_kernel(const __grid_constant__ MQueueParams qp, const uint4* __r
       const uint64_t key = key0 + (uint64_t)j;
       const int4 r = make_int4((int)adapter[j], (int)((crit >> j) & 1u), (int)(uint32_t)key, (int)(uint32_t)(key >> 32));
       const int2 p = kTabSmem ? pick_one_smem(r, tab, pool, (uint32_t)A, it.seed) : pick_one(r, tab, pool, (uint32_t)A, it.seed);
-      ov[j] = ((okm >> j) & 1u) ? pack_mpick(p.x, (uint32_t)p.y & 3u, tgt[j]) : pack_mpick(-1, (uint32_t)LIG_NO_MODEL, 255u);
+      ov[j] = ((okm >> j) & 1u) ? pack_mpick(p.x, (uint32_t)p.y & 7u, tgt[j]) : pack_mpick(-1, (uint32_t)LIG_NO_MODEL, 255u);
     }
     uint4 o = make_uint4(ov[0], ov[1], ov[2], ov[3]);
     uint32_t* dst = it.out + (size_t)t * kTile + i0;
@@ -2136,7 +2258,7 @@ __device__ __forceinline__ int2 doorbell_pick(const int4 r, const uint4* cls, co
   const uint4 e = ld_cg_uint4(cls + c);
   const uint32_t k = int31n_entry(seed ^ key, e);
   const int pod = (int)(short)ld_cg_u16(lists + (e.w + k));
-  return make_int2(pod, (int)(e.x & 0xffff0003u));
+  return make_int2(pod, (int)(e.x & 0xffff0007u));
 }
 
 __global__ void __launch_bounds__(kPickThreads)

@@ -38,6 +38,9 @@ int enqueue_build(lig_ctx* c, SnapshotWrite* w);
 int finish_write(lig_ctx* c, SnapshotWrite* w, bool synchronise);
 void abort_write(lig_ctx* c, SnapshotWrite* w);
 
+// Validate a caller filter tree table (see lig_set_filter_tree); 0 or LIG_ERR_INVALID.
+int check_filter_tree(const lig_filter_node* nodes, int n_nodes);
+
 int device_of(const lig_ctx* c);
 int max_batch_of(const lig_ctx* c);
 

@@ -193,6 +193,15 @@ int lig_group_set_thresholds(lig_group* g, const lig_thresholds* t) {
   return 0;
 }
 
+int lig_group_set_filter_tree(lig_group* g, const lig_filter_node* nodes, int n_nodes) {
+  if (!g) return fail(LIG_ERR_INVALID, "lig_group_set_filter_tree: group is null");
+  if (int rc = ligi::check_filter_tree(nodes, n_nodes)) return rc;   // all members or none
+  std::lock_guard<std::mutex> lk(g->mu);
+  for (lig_ctx* c : g->ctx)
+    if (int rc = lig_set_filter_tree(c, nodes, n_nodes)) return rc;
+  return 0;
+}
+
 int lig_group_upload_snapshot(lig_group* g, uint64_t epoch, int P, int A, const double* kv,
                               const int32_t* q, const uint16_t* na, const uint16_t* ma,
                               const uint32_t* bitmap) {

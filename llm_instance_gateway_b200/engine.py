@@ -10,6 +10,16 @@ from . import _native as N
 from .packer import MPICK_DTYPE, PICK_DTYPE, REQ_DTYPE, PackedModels, PackedSnapshot, _ptr
 
 
+def _node_table(nodes):
+    """(pointer, count) of a filter-tree table for lig_set_filter_tree (see Engine.set_filter_tree)."""
+    if nodes is None:
+        return None, 0
+    if hasattr(nodes, "flatten"):
+        nodes = nodes.flatten()
+    rows = [n if isinstance(n, N.LigFilterNode) else N.LigFilterNode(*n) for n in nodes]
+    return (N.LigFilterNode * len(rows))(*rows), len(rows)
+
+
 class Engine:
     def __init__(self, device: int = 0, max_pods: int = 4096, max_adapters: int = 1024,
                  max_batch: int = 1 << 20, _borrowed_ctx=None):
@@ -46,6 +56,14 @@ class Engine:
                        queueing_threshold_lora=50) -> None:
         t = N.LigThresholds(kv_cache_threshold, queue_threshold_critical, queueing_threshold_lora)
         N.check(self._lib.lig_set_thresholds(self._ctx, C.byref(t)))
+
+    # ---- caller filter trees ----
+    def set_filter_tree(self, nodes) -> None:
+        """Build the class tables of later uploads with a caller filter tree: a ``scheduling.Filter``
+        chart, a sequence of ``LigFilterNode`` / (kind, next_on_success, next_on_failure,
+        next_on_success_or_failure, queue_threshold, kv_threshold) rows (node 0 = root), or None for
+        the built-in tree.  Resident epochs keep their tables."""
+        N.check(self._lib.lig_set_filter_tree(self._ctx, *_node_table(nodes)))
 
     # ---- snapshots ----
     def upload_snapshot(self, epoch: int, snap: PackedSnapshot, block: bool = True) -> None:
@@ -267,6 +285,10 @@ class EngineGroup:
     def set_thresholds(self, kv_cache_threshold=0.8, queue_threshold_critical=5, queueing_threshold_lora=50) -> None:
         t = N.LigThresholds(kv_cache_threshold, queue_threshold_critical, queueing_threshold_lora)
         N.check(self._lib.lig_group_set_thresholds(self._g, C.byref(t)))
+
+    def set_filter_tree(self, nodes) -> None:
+        """Engine.set_filter_tree on every member (an invalid table changes none)."""
+        N.check(self._lib.lig_group_set_filter_tree(self._g, *_node_table(nodes)))
 
     def upload_snapshot(self, epoch: int, snap: PackedSnapshot) -> None:
         N.check(self._lib.lig_group_upload_snapshot(self._g, epoch, snap.P, snap.A, _ptr(snap.kv), _ptr(snap.q),

@@ -26,7 +26,7 @@ EXPORTED_SYMBOLS = (
     "ligh_scheduler_free", "ligh_schedule", "ligh_refresh", "ligh_stats",
     "ligh_schedule_concurrent", "ligh_stream_bench", "ligh_refresh_timing", "ligh_flush_timing",
     "ligh_scheduler_new_devices", "ligh_datastore_new", "ligh_datastore_free", "ligh_datastore_set_model",
-    "ligh_schedule_model",
+    "ligh_schedule_model", "ligh_scheduler_new_tree",
 )
 
 _lib = None
@@ -51,6 +51,9 @@ def load() -> C.CDLL:
     lib.ligh_scheduler_new2.restype = vp
     lib.ligh_scheduler_new_devices.argtypes = [vp, C.POINTER(i32), i32, i32, i32, i32, i32, i32, i32, u64, C.c_char_p, i32]
     lib.ligh_scheduler_new_devices.restype = vp
+    lib.ligh_scheduler_new_tree.argtypes = [vp, i32, C.POINTER(i32), i32, i32, i32, i32, i32, i32, i32, u64, i32, i32,
+                                            i32, vp, i32, C.c_char_p, i32]
+    lib.ligh_scheduler_new_tree.restype = vp
     lib.ligh_datastore_new.restype = vp
     lib.ligh_datastore_free.argtypes = [vp]
     lib.ligh_datastore_free.restype = None
@@ -123,11 +126,20 @@ class HostScheduler:
                  max_adapters: int = 1024, max_batch: int = 1 << 16, flush_size: int = 4096,
                  batch_window_us: int = 50, refresh_interval_ms: int = 0, seed: int = 1,
                  busy_poll: bool = False, caller_spin_us: int = 0, use_doorbell: bool = False,
-                 devices: Optional[Sequence[int]] = None):
+                 devices: Optional[Sequence[int]] = None, filter=None):
         self._lib = load()
         self.provider = provider
         err = C.create_string_buffer(512)
-        if devices is not None and len(devices) > 1:
+        if filter is not None:         # Options::filter: a scheduling.Filter chart or a node table
+            from .engine import _node_table
+            nodes, n = _node_table(filter)
+            devs = list(devices) if devices is not None else []
+            arr = (C.c_int * max(len(devs), 1))(*devs)
+            self._s = self._lib.ligh_scheduler_new_tree(provider._p, device, arr, len(devs), max_pods, max_adapters,
+                                                        max_batch, flush_size, batch_window_us, refresh_interval_ms,
+                                                        seed, int(busy_poll), caller_spin_us, int(use_doorbell),
+                                                        C.cast(nodes, C.c_void_p), n, err, 512)
+        elif devices is not None and len(devices) > 1:
             arr = (C.c_int * len(devices))(*devices)
             self._s = self._lib.ligh_scheduler_new_devices(provider._p, arr, len(devices), max_pods, max_adapters,
                                                            max_batch, flush_size, batch_window_us, refresh_interval_ms,

@@ -8,7 +8,9 @@ Same names, argument meaning and error behaviour as the reference so that it dro
 
 ``Schedule`` returns a ``backend.Pod`` or raises ``StatusError``; its ``.code`` is
 ``"ResourceExhausted"`` when the tree shed the request (scheduler.go:83-89), which the ext-proc
-server turns into HTTP 429 (handlers/server.go:97-109).  ``ScheduleBatch`` is the micro-batched
+server turns into HTTP 429 (handlers/server.go:97-109).  ``NewScheduler(pmp, filter=...)`` runs a
+caller-built flow chart of the reference's filter nodes (``Filter``, filter.go:17-73) instead of
+``defaultFilter``; ``DEFAULT_FILTER`` restates defaultFilter node for node.  ``ScheduleBatch`` is the micro-batched
 form the Go adapter uses under load (one C-ABI call per batch).  There is no CPU path here:
 without liblig.so or without a CUDA device construction fails.
 """
@@ -47,6 +49,94 @@ class StatusError(Exception):
 
 
 _DROP_DESC = "dropping request due to limited backend resources"          # scheduler.go:87
+_ERR_PREFIX = "failed to apply filter, resulted 0 pods, this should never happen: "   # scheduler.go:117
+
+# ---- caller filter trees (lig_set_filter_tree) --------------------------------------------------
+# Node kinds: the filter functions of filter.go / scheduler.go.
+CRITICAL_REQUEST = N.LIG_F_CRITICAL_REQUEST        # criticalRequestPredicate            filter.go:179-181
+LOW_QUEUEING = N.LIG_F_LOW_QUEUEING                # q < queue_threshold                 filter.go:124-126
+LORA_AFFINITY = N.LIG_F_LORA_AFFINITY              # loRAAffinityPredicate               filter.go:169-172
+CAN_ACCEPT_NEW_LORA = N.LIG_F_CAN_ACCEPT_NEW_LORA  # canAcceptNewLoraPredicate           filter.go:175-177
+LOW_LORA_COST = N.LIG_F_LOW_LORA_COST              # lowLoRACostPredicate                filter.go:163-166
+NO_QUEUE_AND_LOW_KV = N.LIG_F_NO_QUEUE_AND_LOW_KV  # q <= queue_threshold && kv <= kv_threshold  filter.go:183-187
+LEAST_QUEUING = N.LIG_F_LEAST_QUEUING              # leastQueuingFilterFunc              filter.go:102-122
+LEAST_KV_CACHE = N.LIG_F_LEAST_KV_CACHE            # leastKVCacheFilterFunc              filter.go:134-154
+DROP = N.LIG_F_DROP                                # the "drop request" func             scheduler.go:83-89
+
+
+class Filter:
+    """One node of a flow chart, as the reference's ``filter`` struct (filter.go:20-35).  Successors
+    are other ``Filter`` objects (or None); a node may be the successor of several parents."""
+
+    def __init__(self, name: str, kind: int, next_on_success: "Optional[Filter]" = None,
+                 next_on_failure: "Optional[Filter]" = None,
+                 next_on_success_or_failure: "Optional[Filter]" = None,
+                 queue_threshold: int = 0, kv_threshold: float = 0.0):
+        self.name, self.kind = name, kind
+        self.next_on_success, self.next_on_failure = next_on_success, next_on_failure
+        self.next_on_success_or_failure = next_on_success_or_failure
+        self.queue_threshold, self.kv_threshold = queue_threshold, kv_threshold
+
+    def Name(self) -> str:                                                    # filter.go:37-42
+        return self.name
+
+    def _successors(self):
+        return (self.next_on_success, self.next_on_failure, self.next_on_success_or_failure)
+
+    def flatten(self) -> List[N.LigFilterNode]:
+        """The chart as lig_set_filter_tree's table: this node first, every edge pointing forward
+        (a topological order), each node object once, so shared subtrees stay shared.  ValueError
+        for a cyclic chart or one of more than LIG_MAX_FILTER_NODES nodes."""
+        post: List[Filter] = []
+        state: Dict[int, int] = {}            # id -> 1 on the DFS path, 2 finished
+        stack = [(self, iter(self._successors()))]
+        state[id(self)] = 1
+        while stack:
+            node, it = stack[-1]
+            nxt = next(it, StopIteration)
+            if nxt is StopIteration:
+                state[id(node)] = 2
+                post.append(node)
+                stack.pop()
+            elif nxt is not None:
+                st = state.get(id(nxt))
+                if st == 1:
+                    raise ValueError(f"filter chart has a cycle through {nxt.name!r}")
+                if st is None:
+                    state[id(nxt)] = 1
+                    stack.append((nxt, iter(nxt._successors())))
+        order = post[::-1]                    # reverse post-order: parents before children
+        if len(order) > N.LIG_MAX_FILTER_NODES:
+            raise ValueError(f"filter chart has {len(order)} nodes (at most {N.LIG_MAX_FILTER_NODES})")
+        index = {id(n): i for i, n in enumerate(order)}
+        ix = lambda n: -1 if n is None else index[id(n)]
+        return [N.LigFilterNode(n.kind, ix(n.next_on_success), ix(n.next_on_failure),
+                                ix(n.next_on_success_or_failure), int(n.queue_threshold), float(n.kv_threshold))
+                for n in order]
+
+
+# defaultFilter, node for node                                                scheduler.go:26-91
+kvCacheThreshold, queueThresholdCritical, queueingThresholdLoRA = 0.8, 5, 50   # scheduler.go:15-24
+queueLoRAAndKVCacheFilter = Filter(
+    "least queuing", LEAST_QUEUING,
+    next_on_success_or_failure=Filter("low cost LoRA", LOW_LORA_COST,
+                                      next_on_success_or_failure=Filter("least KV cache percent", LEAST_KV_CACHE)))
+queueAndKVCacheFilter = Filter(
+    "least queuing", LEAST_QUEUING,
+    next_on_success_or_failure=Filter("least KV cache percent", LEAST_KV_CACHE))
+lowLatencyFilter = Filter(
+    "low queueing filter", LOW_QUEUEING, queue_threshold=queueingThresholdLoRA,
+    next_on_success=Filter("affinity LoRA", LORA_AFFINITY, next_on_success=queueAndKVCacheFilter,
+                           next_on_failure=Filter("can accept LoRA Adapter", CAN_ACCEPT_NEW_LORA,
+                                                  next_on_success_or_failure=queueAndKVCacheFilter)),
+    next_on_failure=queueLoRAAndKVCacheFilter)
+sheddableRequestFilter = Filter(
+    "has capacity for sheddable requests", NO_QUEUE_AND_LOW_KV,
+    queue_threshold=queueThresholdCritical, kv_threshold=kvCacheThreshold,
+    next_on_success=queueLoRAAndKVCacheFilter,
+    next_on_failure=Filter("drop request", DROP))
+DEFAULT_FILTER = Filter("critical request", CRITICAL_REQUEST,
+                        next_on_success=lowLatencyFilter, next_on_failure=sheddableRequestFilter)
 
 
 def _schedule_error(status: int) -> StatusError:
@@ -54,20 +144,23 @@ def _schedule_error(status: int) -> StatusError:
     #                                                                       scheduler.go:117
     if status == N.LIG_DROP:
         inner = f"rpc error: code = ResourceExhausted desc = {_DROP_DESC}"
-        return StatusError("ResourceExhausted",
-                           f"failed to apply filter, resulted 0 pods, this should never happen: {inner}")
+        return StatusError("ResourceExhausted", _ERR_PREFIX + inner)
+    if status == N.LIG_NO_PODS_LEFT:       # a caller tree ended on a predicate that kept no pod
+        return StatusError("Unknown", _ERR_PREFIX + "no pods left")           # filter.go:88-90
     # tree returned ([], nil): Go prints a nil error under %w as %!w(<nil>); status.Code(err) of a
     # plain fmt error is Unknown.
-    return StatusError("Unknown",
-                       "failed to apply filter, resulted 0 pods, this should never happen: %!w(<nil>)")
+    return StatusError("Unknown", _ERR_PREFIX + "%!w(<nil>)")
 
 
 class Scheduler:
     def __init__(self, podMetricsProvider: PodMetricsProvider, device: int = 0,
                  max_pods: int = 4096, max_adapters: int = 1024, max_batch: int = 1 << 16,
-                 seed: Optional[int] = None):
+                 seed: Optional[int] = None, filter: Optional[Filter] = None):
         self.podMetricsProvider = podMetricsProvider
         self._engine = Engine(device, max_pods, max_adapters, max_batch)
+        self._filter = filter                # None: the built-in defaultFilter
+        if filter is not None:
+            self._engine.set_filter_tree(filter)
         self._epoch = 0
         self._snap: Optional[PackedSnapshot] = None
         self._rng = random.Random(seed)      # the Go global source is auto-seeded (scheduler.go:120)
@@ -122,6 +215,14 @@ class Scheduler:
     # Filter-level view (the GPU analogue of Filter.Filter, filter.go:12-15): survivor slice.
     def Filter(self, req: LLMRequest) -> Tuple[List[Pod], Optional[StatusError]]:
         snap = self._current()
+        if self._filter is not None:         # the class table holds the caller tree's survivor set
+            st, _, lst = self._engine.read_class(self._epoch, req.Critical, snap.adapter_id(req.ResolvedTargetModel),
+                                                 snap.P)
+            if st == N.LIG_DROP:
+                return [], StatusError("ResourceExhausted", _DROP_DESC)
+            if st == N.LIG_NO_PODS_LEFT:
+                return [], StatusError("Unknown", "no pods left")
+            return [snap.pods[int(p)] for p in lst], None
         arr = np.zeros(1, dtype=REQ_DTYPE)
         arr[0] = (snap.adapter_id(req.ResolvedTargetModel), N.LIG_REQ_CRITICAL if req.Critical else 0, 0)
         picks, masks = self._engine.schedule_scan(self._epoch, self._seed, arr, True, snap.W)
@@ -132,5 +233,6 @@ class Scheduler:
         return survivors, None
 
 
-def NewScheduler(pmp: PodMetricsProvider, **kw) -> Scheduler:       # scheduler.go:93-99
-    return Scheduler(pmp, **kw)
+def NewScheduler(pmp: PodMetricsProvider, filter: Optional[Filter] = None, **kw) -> Scheduler:  # scheduler.go:93-99
+    """filter: a caller flow chart (None = defaultFilter, the reference's only tree)."""
+    return Scheduler(pmp, filter=filter, **kw)
