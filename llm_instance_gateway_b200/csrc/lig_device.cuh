@@ -44,9 +44,11 @@ struct Thr {
 };
 
 // One entry per request class c = critical * (A + 1) + min(adapter, A); 16 bytes (one LDG.128).
-// Classes whose survivor set does not depend on the adapter share one of two default lists
-// (rows 2(A+1) and 2(A+1)+1 of the list pool); the others own row c.  List offsets are in list
-// entries and fit 32 bits: (2 * 65535 + 3) rows x 32768 entries < 2^32.
+// Classes whose survivor set does not depend on the adapter share one of two default lists; the
+// others own row c.  Adapter id A has no bitmap row, so the built-in builds always give the classes
+// (sheddable, A) and (critical, A) the default lists, which therefore live in those classes' own
+// rows A and 2A+1.  The sentinel follows the 2(A+1) rows.  List offsets are in list entries and
+// fit 32 bits: 2 * 65535 rows x 32768 entries + 1 = 2^32 - 65535.
 //
 //   info    : bits 0-2 status | 4-8 shift | 16-31 n   (bit 2 only for LIG_NO_PODS_LEFT, which only
 //             caller filter trees produce)
@@ -68,9 +70,9 @@ struct ClassEntry {
 
 __host__ __device__ inline uint32_t entry_n(uint32_t info) { return info >> 16; }
 __host__ __device__ inline uint32_t entry_status(uint32_t info) { return info & 7u; }
-// Entries of the list pool: one row per class, two shared default rows, then the sentinel.
+// Entries of the list pool: one row per class, then the sentinel.
 __host__ __device__ inline size_t list_pool_entries(size_t n_classes, size_t stride) {
-  return (n_classes + 2) * stride + 8;
+  return n_classes * stride + 8;
 }
 
 // Pod metric columns as the tree walk reads them: either the snapshot in global memory (read
@@ -726,9 +728,9 @@ lig_class_build_kernel(SnapView s, Thr thr, ClassEntry* __restrict__ cls,
   }
   __syncthreads();
   const int n_classes = 2 * (A + 1);
-  const uint32_t rc_row = (uint32_t)n_classes * (uint32_t)list_stride;        // default list rows
-  const uint32_t rs_row = rc_row + (uint32_t)list_stride;
-  const uint32_t none = rs_row + (uint32_t)list_stride;                       // sentinel entry
+  const uint32_t rc_row = (uint32_t)(2 * A + 1) * (uint32_t)list_stride;     // default lists: the rows of
+  const uint32_t rs_row = (uint32_t)A * (uint32_t)list_stride;               // (critical, A), (sheddable, A)
+  const uint32_t none = (uint32_t)n_classes * (uint32_t)list_stride;         // sentinel entry
   if (blockIdx.x == 0 && threadIdx.x == 0) lists[none] = 0xffffu;             // reads back as pod_idx -1
   uint4* centries = reinterpret_cast<uint4*>(co.blob + sizeof(CompactHeader));
   uint16_t* cpool = reinterpret_cast<uint16_t*>(co.blob + sizeof(CompactHeader) + (size_t)n_classes * sizeof(ClassEntry));
@@ -976,9 +978,9 @@ lig_class_build_fast_kernel(SnapView s, Thr thr, ClassEntry* __restrict__ cls, u
   uint32_t* TMPS = masks + 6 * W;      // the default sheddable one
   uint32_t* X = masks + (size_t)(7 + warp) * W;   // per-warp scratch
   const int n_classes = 2 * (A + 1);
-  const uint32_t rc_row = (uint32_t)n_classes * (uint32_t)list_stride;
-  const uint32_t rs_row = rc_row + (uint32_t)list_stride;
-  const uint32_t none = rs_row + (uint32_t)list_stride;
+  const uint32_t rc_row = (uint32_t)(2 * A + 1) * (uint32_t)list_stride;     // as in lig_class_build_kernel
+  const uint32_t rs_row = (uint32_t)A * (uint32_t)list_stride;
+  const uint32_t none = (uint32_t)n_classes * (uint32_t)list_stride;
   uint4* centries = reinterpret_cast<uint4*>(co.blob + sizeof(CompactHeader));
   uint16_t* cpool = reinterpret_cast<uint16_t*>(co.blob + sizeof(CompactHeader) + (size_t)n_classes * sizeof(ClassEntry));
 
@@ -1345,7 +1347,7 @@ lig_class_build_tree_kernel(SnapView s, const __grid_constant__ FilterTree tree,
   }
   __syncthreads();
   const int n_classes = 2 * (A + 1);
-  const uint32_t none = (uint32_t)(n_classes + 2) * (uint32_t)list_stride;   // sentinel, as in the other builds
+  const uint32_t none = (uint32_t)n_classes * (uint32_t)list_stride;   // sentinel, as in the other builds
   uint4* centries = reinterpret_cast<uint4*>(co.blob + sizeof(CompactHeader));
   uint16_t* cpool = reinterpret_cast<uint16_t*>(co.blob + sizeof(CompactHeader) + (size_t)n_classes * sizeof(ClassEntry));
   if (blockIdx.x == 0 && threadIdx.x == 0) {
