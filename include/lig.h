@@ -208,7 +208,12 @@ int lig_upload_snapshot_async(lig_ctx* ctx, uint64_t epoch, int P, int A, const 
  * Only the delta crosses PCIe; the base blob is copied device-to-device, the dirty rows and
  * bitmap bits are patched by a kernel, and the class tables are rebuilt.  LIG_ERR_INVALID when
  * the base epoch is the slot the new epoch would have to overwrite (it is the older of the two
- * resident epochs): fall back to lig_upload_snapshot. */
+ * resident epochs): fall back to lig_upload_snapshot.  LIG_ERR_INVALID too, before anything is
+ * written (both resident epochs stay as they were), when the delta is malformed:
+ *   - a pod index is outside [0, P) or appears more than once in pod_idx;
+ *   - adapter_offsets[0] != 0, or adapter_offsets decreases anywhere;
+ *   - an adapter id is outside [0, A) of the base.
+ * The same id twice within one pod's list is allowed (it sets the same bit). */
 int lig_update_snapshot(lig_ctx* ctx, uint64_t new_epoch, uint64_t base_epoch, int n_dirty,
                         const int32_t* pod_idx, const double* kv, const int32_t* q,
                         const uint16_t* n_active, const uint16_t* max_active,

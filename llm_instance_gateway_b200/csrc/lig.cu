@@ -1253,8 +1253,23 @@ int lig_update_snapshot(lig_ctx* c, uint64_t new_epoch, uint64_t base_epoch, int
       return fail(LIG_ERR_INVALID, "base epoch %llu is the slot epoch %llu would overwrite: use lig_upload_snapshot",
                   (unsigned long long)base_epoch, (unsigned long long)new_epoch);
   }
-  for (int i = 0; i < n_dirty; ++i)
-    if (pod_idx[i] < 0 || pod_idx[i] >= P) return fail(LIG_ERR_INVALID, "dirty pod index %d outside [0, %d)", pod_idx[i], P);
+  // The delta kernel gives every entry its own warp, so a pod listed twice would be patched by two
+  // racing warps, and every adapter id is read between the offsets: reject such input here, before
+  // the writer lock, so a refused call leaves both resident epochs untouched.
+  if (n_dirty > 0) {
+    std::vector<unsigned char> seen((size_t)P, 0);
+    for (int i = 0; i < n_dirty; ++i) {
+      if (pod_idx[i] < 0 || pod_idx[i] >= P) return fail(LIG_ERR_INVALID, "dirty pod index %d outside [0, %d)", pod_idx[i], P);
+      if (seen[pod_idx[i]]) return fail(LIG_ERR_INVALID, "dirty pod index %d listed twice", pod_idx[i]);
+      seen[pod_idx[i]] = 1;
+    }
+    if (a_off[0] != 0) return fail(LIG_ERR_INVALID, "adapter_offsets[0] is %d, not 0", a_off[0]);
+    for (int i = 0; i < n_dirty; ++i)
+      if (a_off[i + 1] < a_off[i])
+        return fail(LIG_ERR_INVALID, "adapter_offsets decrease at entry %d (%d -> %d)", i + 1, a_off[i], a_off[i + 1]);
+    for (int k = 0; k < n_ids; ++k)
+      if (a_ids[k] < 0 || a_ids[k] >= A) return fail(LIG_ERR_INVALID, "adapter id %d outside [0, %d)", a_ids[k], A);
+  }
   ligi::SnapshotWrite w;
   if (int rc = ligi::begin_write(c, new_epoch, P, A, nullptr, true, &w)) return rc;
   // from here on failures must release the writer lock
