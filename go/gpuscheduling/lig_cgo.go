@@ -114,3 +114,10 @@ func (c *ctx) uploadSnapshot(epoch uint64, s *packedSnapshot) error {
 func (c *ctx) scheduleBatch(epoch, seed uint64, in, out *pinned, n int) C.int {
 	return C.lig_schedule_batch(c.p, C.uint64_t(epoch), C.uint64_t(seed), (*C.lig_req)(in.ptr), C.int(n), (*C.lig_pick)(out.ptr))
 }
+
+// scheduleBatchFeedbackChain is scheduleBatch through the load-feedback chain: windows of `window`
+// requests counted across calls against one epoch (include/lig.h).
+func (c *ctx) scheduleBatchFeedbackChain(epoch, seed uint64, in, out *pinned, n, window int) C.int {
+	return C.lig_schedule_batch_feedback_chain(c.p, C.uint64_t(epoch), C.uint64_t(seed), (*C.lig_req)(in.ptr), C.int(n),
+		(*C.lig_pick)(out.ptr), C.int(window), nil)
+}

@@ -36,6 +36,12 @@ type Options struct {
 	// reference's filter nodes (filter.go:17-73); nil = defaultFilter.  Its nodes carry their own
 	// thresholds, so the three above then do not apply.  See lig_set_filter_tree in include/lig.h.
 	FilterTree []FilterNode
+	// LoadFeedbackWindow > 0 carries load feedback across flushes (lig_schedule_batch_feedback_chain
+	// in include/lig.h): every window of this many requests, counted across flushes, adds its picks
+	// to the pods' WaitingQueueSize before the next request is scheduled, until the next Refresh
+	// uploads a new epoch.  The reference never writes pod metrics while scheduling
+	// (scheduler.go:113-122), so 0 (off) is the reference's behaviour.
+	LoadFeedbackWindow int
 }
 
 // FilterKind names the filter functions of filter.go / scheduler.go a FilterNode runs.
@@ -106,6 +112,9 @@ type GPUScheduler struct {
 
 // NewGPUScheduler mirrors scheduling.NewScheduler(pmp) (scheduler.go:93-99).
 func NewGPUScheduler(pmp scheduling.PodMetricsProvider, opt Options) (*GPUScheduler, error) {
+	if opt.LoadFeedbackWindow < 0 {
+		return nil, fmt.Errorf("gpu scheduler: LoadFeedbackWindow must be >= 0, got %d", opt.LoadFeedbackWindow)
+	}
 	c, err := newCtx(opt.Device, opt.MaxPods, opt.MaxAdapters, opt.MaxBatch)
 	if err != nil {
 		return nil, err // no CPU fallback: without the GPU the caller keeps the stock scheduler
@@ -267,7 +276,11 @@ func (g *GPUScheduler) flush(batch []*waiter) {
 			}
 			reqs[i].rand_key = C.uint64_t(g.rng.Uint64())
 		}
-		rc = g.c.scheduleBatch(snap.epoch, g.seed, g.in, g.out, n)
+		if g.opt.LoadFeedbackWindow > 0 {
+			rc = g.c.scheduleBatchFeedbackChain(snap.epoch, g.seed, g.in, g.out, n, g.opt.LoadFeedbackWindow)
+		} else {
+			rc = g.c.scheduleBatch(snap.epoch, g.seed, g.in, g.out, n)
+		}
 		if rc != C.LIG_ERR_STALE_EPOCH {
 			break
 		}

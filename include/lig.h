@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define LIG_ABI_VERSION 3
+#define LIG_ABI_VERSION 4
 
 /* ---- per-request status (lig_pick.status) ------------------------------------------------------
  * LIG_OK    Schedule returned a pod, nil                      pkg/ext-proc/scheduling/scheduler.go:120-121
@@ -382,10 +382,56 @@ int lig_resolve_models(lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64_t fir
  *   n_windows <= 0: ceil(R / sub_batch) windows; ranks of one communicator must pass the same
  *   n_windows (trailing windows may be empty).  d_hist (nullable): int32[P], receives the total
  *   picks per pod of this call (all ranks).  Resident epochs are not modified.  Enqueued on
- *   `stream`, not synchronised.  Defined sequentially in oracle/feedback.py. */
+ *   `stream`, not synchronised.  Ends any feedback chain of the ctx (see below).  Defined
+ *   sequentially in oracle/feedback.py. */
 int lig_schedule_batch_feedback_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* d_reqs,
                                        int R, lig_pick* d_out, int sub_batch, int n_windows,
                                        int32_t* d_hist, void* stream);
+
+/* ---- load feedback across calls: the feedback chain (opt-in) ------------------------------------
+ * A deployed scheduler sends a stream of small micro-batches, one per flush, against one scraped
+ * epoch (refreshMetricsInterval = 50 ms, main.go:39); the herd of scheduler.go:113-122 forms
+ * ACROSS those calls, where the in-batch call above cannot see it.  A chain carries the feedback
+ * from call to call until the next metrics refresh replaces the epoch.
+ *
+ * A ctx holds at most one chain: a resident epoch E, a window size W >= 1, a private copy of E's
+ * snapshot whose WaitingQueueSize column grows, and the requests counted so far.  Take the requests
+ * of all chain calls against E, in call order, as one sequence and cut it into windows of W
+ * requests; window boundaries ignore call boundaries.  Every request is scheduled against the
+ * private copy's current tables with its own call's seed and its own rand_key, exactly as
+ * lig_schedule_batch would on those tables.  When a window fills, its picks per pod are added to
+ * WaitingQueueSize (saturating at INT32_MAX) and the tables are rebuilt before the next request;
+ * DROP, EMPTY and NO_PODS_LEFT results count toward the window but add no pick.  So a chain of
+ * calls with one seed gives the same picks as ONE lig_schedule_batch_feedback_device call over
+ * their concatenation with sub_batch = W, however the requests are split into calls.
+ *
+ * A call starts a new chain (copies E afresh, zero loads) when its epoch differs from the chain's
+ * or E was uploaded again since (the next scrape supersedes the estimate; lig_update_snapshot
+ * makes a new epoch too), when its window differs, after lig_feedback_chain_reset, and after an
+ * in-batch feedback call on the ctx (the two share one private copy).  The filter tree and the
+ * thresholds in force when a chain starts rebuild all of its windows: a later lig_set_filter_tree
+ * or lig_set_thresholds takes effect at the next chain start.  Resident epochs are never written.
+ *
+ * `window` is W; `loads` (nullable, int32[P]) receives the picks per pod since the chain began,
+ * closed windows plus the open one; R = 0 with `loads` reads them without scheduling.  A call that
+ * returns LIG_ERR_* for a bad argument (window < 1, R < 0, a null buffer, R > max_batch on the host
+ * form), a stale epoch (E must be resident at every call), a ctx with a communicator, or a doorbell
+ * stream open before the first feedback call allocated the private copy, leaves the chain exactly
+ * as it was; after LIG_ERR_CUDA the next call starts a new chain.  Calls are serialised on the
+ * chain; the order in which they take its lock is the sequence, so a reproducible sequence needs
+ * one calling thread.  Calls may alternate between the two forms and between streams: each is
+ * ordered behind the previous one on the device.  A ctx with a communicator (lig_comm_init_rank)
+ * returns LIG_ERR_INVALID: per-rank micro-batch streams share no window boundaries.  Defined
+ * sequentially in the tests' chain oracle (tests/feedback_chain_ref.py). */
+/* host buffers (page-locked ones are used in place, pageable ones bounce like lig_schedule_batch);
+ * blocks until `out` and `loads` are complete */
+int lig_schedule_batch_feedback_chain(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* reqs,
+                                      int R, lig_pick* out, int window, int32_t* loads);
+/* device pointers, enqueued on `stream`, not synchronised */
+int lig_schedule_batch_feedback_chain_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* d_reqs,
+                                             int R, lig_pick* d_out, int window, int32_t* d_loads, void* stream);
+/* The next chain call starts a new chain. */
+int lig_feedback_chain_reset(lig_ctx* ctx);
 
 /* ---- several GPUs, one process (the reference runs ONE scheduler per process, main.go:137) ------
  * A lig_group owns one lig_ctx per listed CUDA device and an NCCL communicator over them

@@ -41,6 +41,13 @@ Status NewScheduler(std::shared_ptr<PodMetricsProvider> pmp, const Options& opt,
   s->pmp_ = std::move(pmp);
   s->opt_ = opt;
   lig_thresholds t{opt.kv_cache_threshold, opt.queue_threshold_critical, opt.queueing_threshold_lora};
+  if (opt.load_feedback_window < 0) return Errorf(Internal, "NewScheduler: load_feedback_window must be >= 0");
+  if (opt.load_feedback_window > 0 && opt.devices.size() > 1)
+    return Errorf(Internal, "NewScheduler: load_feedback_window needs a single device (the feedback chain has no "
+                            "cross-device windows)");
+  if (opt.load_feedback_window > 0 && opt.use_doorbell)
+    return Errorf(Internal, "NewScheduler: load_feedback_window cannot be combined with use_doorbell (the doorbell "
+                            "kernel schedules against the resident epoch only)");
   if (opt.devices.size() > 1) {
     if (opt.use_doorbell) return Errorf(Internal, "the doorbell stream is a single-device mode");
     if (lig_group_create(&s->group_, opt.devices.data(), (int)opt.devices.size(), opt.max_pods, opt.max_adapters,
@@ -359,10 +366,24 @@ void Scheduler::Flush(std::vector<Waiter*>& batch) {
       }
       const auto call_t0 = std::chrono::steady_clock::now();
       const double cpu_t0 = thread_cpu_us();
+      const int W = opt_.load_feedback_window;
       rc = group_ ? lig_group_schedule_batch(group_, snap->epoch, seed_, h_reqs_, n, h_picks_)
+           : W > 0 ? lig_schedule_batch_feedback_chain(ctx_, snap->epoch, seed_, h_reqs_, n, h_picks_, W, nullptr)
            : (opt_.use_doorbell && n <= lig_stream_capacity())
                ? lig_stream_submit(ctx_, snap->epoch, seed_, h_reqs_, n, h_picks_)
                : lig_schedule_batch(ctx_, snap->epoch, seed_, h_reqs_, n, h_picks_);
+      if (rc == 0 && W > 0) {
+        // the chain restarts on every new epoch: "until the next metrics refresh" (Refresh never
+        // reuses an epoch number)
+        std::lock_guard<std::mutex> sk(stats_mu_);
+        if (snap->epoch != fb_epoch_) {
+          if (fb_epoch_ != 0) stats_.feedback_restarts++;
+          fb_epoch_ = snap->epoch;
+          fb_filled_ = 0;
+        }
+        stats_.feedback_windows += (uint64_t)((fb_filled_ + (int64_t)n) / W);
+        fb_filled_ = (int)((fb_filled_ + (int64_t)n) % W);
+      }
       const double call_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - call_t0).count();
       if (call_us > device_us) {
         device_us = call_us;
@@ -372,7 +393,8 @@ void Scheduler::Flush(std::vector<Waiter*>& batch) {
       std::lock_guard<std::mutex> sk(stats_mu_);
       stats_.stale_retries++;
     }
-    if (rc != 0) failure = LigFailure("lig_schedule_batch");
+    if (rc != 0)
+      failure = LigFailure(opt_.load_feedback_window > 0 ? "lig_schedule_batch_feedback_chain" : "lig_schedule_batch");
     for (int i = 0; i < n; ++i) {
       Waiter* w = batch[done + i];
       if (rc != 0) {

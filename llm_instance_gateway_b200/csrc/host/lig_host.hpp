@@ -141,6 +141,11 @@ struct Options {
   // A caller flow chart of the reference's filter nodes (lig_set_filter_tree, node 0 = root)
   // instead of defaultFilter; empty = the built-in tree.  Its nodes carry their own thresholds.
   std::vector<lig_filter_node> filter;
+  // >0: in-batch load feedback carried across flushes (lig_schedule_batch_feedback_chain): every
+  // window of this many requests adds its picks to the pods' WaitingQueueSize before the next
+  // request is scheduled, until the next refresh replaces the snapshot (each refresh restarts the
+  // chain on the new epoch).  0 = off, the reference's behaviour.  Single device, no doorbell.
+  int load_feedback_window = 0;
 };
 
 struct Stats {
@@ -153,6 +158,8 @@ struct Stats {
   uint64_t last_dirty_pods = 0;    // pods whose metrics changed at the last refresh
   uint64_t failed_refreshes = 0;   // Refresh() calls that kept the previous snapshot (see last_refresh_error)
   uint64_t excluded_pods = 0;      // pods left out of the last snapshot: a metric did not fit the device record
+  uint64_t feedback_windows = 0;   // load-feedback windows closed (Options::load_feedback_window)
+  uint64_t feedback_restarts = 0;  // feedback chains restarted on a new epoch after the first one
   double last_pack_us = 0;     // last Refresh: provider slice -> columns + bitmap (host)
   double last_upload_us = 0;   // last Refresh: lig_upload_snapshot (H2D + class tables)
   double max_device_call_us = 0;   // slowest single lig_schedule_batch call (launch + kernel + synchronise)
@@ -241,6 +248,9 @@ class Scheduler {
   lig_pick* h_picks_ = nullptr;
   uint64_t seed_ = 0;
   uint64_t rng_state_ = 0;
+  // the feedback chain as the batcher thread sees it (the library's window count is deterministic)
+  uint64_t fb_epoch_ = 0;
+  int fb_filled_ = 0;
 
   mutable std::mutex snap_mu_;
   std::shared_ptr<const Snapshot> snap_;

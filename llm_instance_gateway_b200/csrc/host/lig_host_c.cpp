@@ -168,7 +168,18 @@ ligh_scheduler* ligh_scheduler_new_tree(ligh_provider* p, int device, const int*
                                         int window_us, int refresh_ms, uint64_t seed, int busy_poll,
                                         int caller_spin_us, int use_doorbell, const lig_filter_node* nodes,
                                         int n_nodes, char* err, int err_cap) {
+  return ligh_scheduler_new_feedback(p, device, devices, n_devices, max_pods, max_adapters, max_batch, flush_size,
+                                     window_us, refresh_ms, seed, busy_poll, caller_spin_us, use_doorbell, nodes,
+                                     n_nodes, 0, err, err_cap);
+}
+
+ligh_scheduler* ligh_scheduler_new_feedback(ligh_provider* p, int device, const int* devices, int n_devices,
+                                            int max_pods, int max_adapters, int max_batch, int flush_size,
+                                            int window_us, int refresh_ms, uint64_t seed, int busy_poll,
+                                            int caller_spin_us, int use_doorbell, const lig_filter_node* nodes,
+                                            int n_nodes, int load_feedback_window, char* err, int err_cap) {
   scheduling::Options o;
+  o.load_feedback_window = load_feedback_window;
   o.device = device;
   if (devices && n_devices > 1) o.devices.assign(devices, devices + n_devices);
   o.busy_poll = busy_poll != 0;
@@ -223,6 +234,12 @@ void ligh_stats(ligh_scheduler* s, uint64_t out[9]) {
   out[0] = st.scheduled; out[1] = st.batches; out[2] = st.max_batch; out[3] = st.refreshes;
   out[4] = st.stale_retries; out[5] = st.failed_refreshes; out[6] = st.excluded_pods;
   out[7] = st.delta_refreshes; out[8] = st.last_dirty_pods;
+}
+
+void ligh_feedback_stats(ligh_scheduler* s, uint64_t out[2]) {
+  scheduling::Stats st = s->sched->stats();
+  out[0] = st.feedback_windows;
+  out[1] = st.feedback_restarts;
 }
 
 void ligh_refresh_timing(ligh_scheduler* s, double out[2]) {

@@ -37,6 +37,14 @@ ligh_scheduler* ligh_scheduler_new_tree(ligh_provider*, int device, const int* d
                                         int batch_window_us, int refresh_interval_ms, uint64_t seed,
                                         int busy_poll, int caller_spin_us, int use_doorbell,
                                         const lig_filter_node* nodes, int n_nodes, char* err, int err_cap);
+/* ligh_scheduler_new_tree plus Options::load_feedback_window (0 = off; > 0 flushes through
+ * lig_schedule_batch_feedback_chain; refused with several devices or use_doorbell). */
+ligh_scheduler* ligh_scheduler_new_feedback(ligh_provider*, int device, const int* devices, int n_devices,
+                                            int max_pods, int max_adapters, int max_batch, int flush_size,
+                                            int batch_window_us, int refresh_interval_ms, uint64_t seed,
+                                            int busy_poll, int caller_spin_us, int use_doorbell,
+                                            const lig_filter_node* nodes, int n_nodes, int load_feedback_window,
+                                            char* err, int err_cap);
 void ligh_scheduler_free(ligh_scheduler*);
 /* Scheduler.Schedule: returns the gRPC code (0 OK, 8 ResourceExhausted, 2 Unknown, 13 Internal). */
 int ligh_schedule(ligh_scheduler*, const char* model, const char* resolved_target_model, int critical,
@@ -55,6 +63,7 @@ int ligh_datastore_set_model(ligh_datastore*, const char* model_name, int critic
 int ligh_schedule_model(ligh_scheduler*, ligh_datastore*, const char* model, char* resolved, int resolved_cap,
                         char* name, int name_cap, char* addr, int addr_cap, char* err, int err_cap);
 void ligh_stats(ligh_scheduler*, uint64_t out[9]); /* scheduled, batches, max_batch, refreshes, stale_retries */
+void ligh_feedback_stats(ligh_scheduler*, uint64_t out[2]); /* feedback_windows, feedback_restarts */
 void ligh_refresh_timing(ligh_scheduler*, double out[2]); /* last Refresh: host pack us, lig_upload_snapshot us */
 void ligh_flush_timing(ligh_scheduler*, double out[4]);   /* slowest device call us, slowest Flush us, index of that call, thread CPU us inside it */
 

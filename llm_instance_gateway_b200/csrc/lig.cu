@@ -142,7 +142,21 @@ struct lig_ctx {
   std::mutex fb_mu;
   Slot fb_scratch;                            // allocated at first use
   int32_t* d_fb_hist = nullptr;               // picks per pod of the current window
+  int32_t* d_fb_total = nullptr;              // picks per pod of the chain's closed windows
+  int32_t* h_fb_loads = nullptr;              // pinned, mapped: the chain's loads for pageable callers
+  cudaStream_t s_fb = nullptr;                // host-buffer chain calls
   cudaEvent_t fb_free = nullptr;              // the previous feedback call has finished with the scratch
+  // The feedback chain (lig_schedule_batch_feedback_chain) the scratch holds between calls; all
+  // of it guarded by fb_mu.  chain_live is false before the first chain call, after
+  // lig_feedback_chain_reset, an in-batch feedback call or a failed chain call.
+  bool chain_live = false;
+  uint64_t chain_epoch = 0, chain_stamp = 0;  // the epoch copied, and its upload (Slot::stamp)
+  int chain_window = 0;
+  int chain_filled = 0;                       // requests in the open window
+  bool chain_stale = true;                    // a window closed since the scratch's tables were built
+  bool chain_has_tree = false;                // the filter tree and thresholds of the chain's start
+  FilterTree chain_tree{};
+  Thr chain_thr{};
 
   // ---- snapshots: two resident epochs ----
   Slot slot[2];
@@ -280,9 +294,11 @@ bool staged_fits(const lig_ctx* c, int W) {
 }
 
 // Enqueue the class-table build for slot s on `stream`: the caller's filter tree when `tree` is not
-// null, else the built-in tree.
-int launch_class_build(lig_ctx* c, Slot& s, cudaStream_t stream, const FilterTree* tree) {
+// null, else the built-in tree with the thresholds *thr (null: the ctx's current ones).
+int launch_class_build(lig_ctx* c, Slot& s, cudaStream_t stream, const FilterTree* tree,
+                       const Thr* thr = nullptr) {
   const SnapView v = view_of(s);
+  const Thr th = thr ? *thr : thr_of(c);
   const int n_classes = 2 * (s.A + 1);
   const int W = s.W > 0 ? s.W : 1;
   s.caller_tree = tree != nullptr;
@@ -333,11 +349,11 @@ int launch_class_build(lig_ctx* c, Slot& s, cudaStream_t stream, const FilterTre
     int fgrid = (n_classes + kBuildWarps - 1) / kBuildWarps;
     if (fgrid > c->sm_count) fgrid = c->sm_count;
     lig_class_build_fast_kernel<<<fgrid, kBuildThreads, fast_fixed_bytes(W) + staged_bytes(W), stream>>>(
-        v, thr_of(c), s.d_cls, s.d_lists, stride, co);
+        v, th, s.d_cls, s.d_lists, stride, co);
   } else if (staged) {
-    lig_class_build_kernel<true><<<grid, kBuildThreads, smem, stream>>>(v, thr_of(c), s.d_cls, s.d_lists, stride, co);
+    lig_class_build_kernel<true><<<grid, kBuildThreads, smem, stream>>>(v, th, s.d_cls, s.d_lists, stride, co);
   } else {
-    lig_class_build_kernel<false><<<grid, kBuildThreads, smem, stream>>>(v, thr_of(c), s.d_cls, s.d_lists, stride, co);
+    lig_class_build_kernel<false><<<grid, kBuildThreads, smem, stream>>>(v, th, s.d_cls, s.d_lists, stride, co);
   }
   CUDA_TRY(cudaGetLastError());
   c->launches++;
@@ -1087,7 +1103,8 @@ static int create_impl(lig_ctx* c, int device, int max_pods, int max_adapters, i
         (const void*)lig_pick_queue_kernel<2>,   (const void*)lig_pick_queue_kernel<4>,
         (const void*)lig_pick_queue_kernel<8>,   (const void*)lig_pick_queue_kernel<16>,
         (const void*)lig_pick_models_stream_kernel, (const void*)lig_apply_delta_kernel,
-        (const void*)lig_pick_hist_kernel,       (const void*)lig_apply_feedback_kernel,
+        (const void*)lig_pick_count_kernel,      (const void*)lig_apply_feedback_kernel,
+        (const void*)lig_feedback_loads_kernel,
     };
     for (const void* fn : fns) CUDA_TRY(cudaFuncGetAttributes(&fa, fn));
   }
@@ -1134,6 +1151,9 @@ void lig_destroy(lig_ctx* c) {
   cudaFree(c->d_delta);
   if (c->fb_scratch.d_blob) free_slot(c->fb_scratch);
   cudaFree(c->d_fb_hist);
+  cudaFree(c->d_fb_total);
+  if (c->h_fb_loads) cudaFreeHost(c->h_fb_loads);
+  if (c->s_fb) cudaStreamDestroy(c->s_fb);
   if (c->fb_free) cudaEventDestroy(c->fb_free);
   if (c->mailbox) cudaFreeHost(c->mailbox);
   if (c->s_doorbell) cudaStreamDestroy(c->s_doorbell);
@@ -1784,6 +1804,98 @@ int lig_pick_kernel_info(lig_ctx* c, uint64_t epoch, char* name, int name_len, i
   return 0;
 }
 
+// ---- load feedback: the private scratch copy, its window loop, the in-batch call and the chain ----
+// Both entry points schedule against fb_scratch, count the open window's picks in d_fb_hist and
+// close a window by adding it to the scratch's WaitingQueueSize column; the in-batch call is a
+// chain that starts and ends inside one call.  Everything below runs under c->fb_mu.
+struct FbRun {
+  int window = 1;                 // W
+  int filled = 0;                 // requests in the open window
+  bool stale = true;              // the scratch's tables predate the last closed window
+  const FilterTree* tree = nullptr;
+  Thr thr{};
+  int32_t* d_total = nullptr;     // += every closed window (nullable)
+  long long closed = 0;           // windows closed
+};
+
+static int fb_alloc_scratch(lig_ctx* c) {
+  if (c->fb_scratch.d_blob) return 0;
+  if (c->stream_open) return fail(LIG_ERR_INVALID, "cannot allocate the feedback scratch while a doorbell stream is open");
+  if (int rc = alloc_slot(c, c->fb_scratch)) return rc;
+  CUDA_TRY(cudaMalloc(&c->d_fb_hist, (size_t)c->max_pods * sizeof(int32_t)));
+  CUDA_TRY(cudaMalloc(&c->d_fb_total, (size_t)c->max_pods * sizeof(int32_t)));
+  CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&c->h_fb_loads), (size_t)c->max_pods * sizeof(int32_t),
+                         cudaHostAllocMapped));
+  CUDA_TRY(cudaStreamCreateWithFlags(&c->s_fb, cudaStreamNonBlocking));
+  CUDA_TRY(cudaEventCreateWithFlags(&c->fb_free, cudaEventDisableTiming));
+  return 0;
+}
+
+// Copy resident slot s into the scratch on `st` (after the previous feedback call) and zero the
+// open window.  Caller holds c->mu.
+static int fb_copy_epoch(lig_ctx* c, Slot* s, cudaStream_t st) {
+  Slot& fs = c->fb_scratch;
+  CUDA_TRY(cudaStreamWaitEvent(st, c->fb_free, 0));         // an earlier feedback call on another stream
+  CUDA_TRY(cudaStreamWaitEvent(st, s->ready, 0));
+  fs.P = s->P;
+  fs.A = s->A;
+  fs.W = s->W;
+  CUDA_TRY(cudaMemcpyAsync(fs.d_blob, s->d_blob, layout_for(s->P, s->A).total, cudaMemcpyDeviceToDevice, st));
+  if (fs.P > 0) CUDA_TRY(cudaMemsetAsync(c->d_fb_hist, 0, (size_t)fs.P * sizeof(int32_t), st));
+  return note_reader(*s, st);
+}
+
+// Close the open window: sum it over the ranks (communicator ctxs), add it to WaitingQueueSize
+// (saturating) and to run.d_total, zero it.
+static int fb_close_window(lig_ctx* c, FbRun& run, cudaStream_t st) {
+  Slot& fs = c->fb_scratch;
+  const int P = fs.P;
+  if (P > 0) {
+    if (c->comm && ligi::g_allreduce)                        // picks of this window on every rank
+      if (int rc = ligi::g_allreduce(c, c->d_fb_hist, P, st)) return rc;
+    int* q = reinterpret_cast<int*>(fs.d_blob + layout_for(fs.P, fs.A).q);
+    lig_apply_feedback_kernel<<<(P + 255) / 256, 256, 0, st>>>(q, c->d_fb_hist, run.d_total, P);
+    CUDA_TRY(cudaGetLastError());
+    c->launches++;
+  }
+  run.filled = 0;
+  run.stale = true;
+  run.closed++;
+  return 0;
+}
+
+// Schedule R requests (device-visible pointers) through the window sequence: each segment is the
+// rest of the open window or of the call, whichever is shorter; one fused pick + count launch per
+// segment; a filled window is closed at once, its tables are rebuilt only when the next segment
+// needs them.
+static int fb_schedule(lig_ctx* c, FbRun& run, uint64_t seed, const lig_req* d_reqs, int R, lig_pick* d_out,
+                       cudaStream_t st) {
+  Slot& fs = c->fb_scratch;
+  for (int pos = 0; pos < R;) {
+    const int n = (R - pos) < (run.window - run.filled) ? (R - pos) : (run.window - run.filled);
+    {
+      std::lock_guard<std::mutex> lk(c->mu);                 // launch counters, build debug stamps
+      if (run.stale) {
+        if (int rc = launch_class_build(c, fs, st, run.tree, &run.thr)) return rc;
+        run.stale = false;
+      }
+    }
+    // the scratch's tables change every window: always the strided tables through L1 (no host
+    // round trip for the compact header)
+    lig_pick_count_kernel<<<(n + kPickThreads * kCountPerThread - 1) / (kPickThreads * kCountPerThread),
+                            kPickThreads, 0, st>>>(
+        reinterpret_cast<const int4*>(d_reqs + pos), reinterpret_cast<int2*>(d_out + pos), n,
+        reinterpret_cast<const uint4*>(fs.d_cls), fs.d_lists, fs.A, seed, c->d_fb_hist);
+    CUDA_TRY(cudaGetLastError());
+    c->launches++;
+    pos += n;
+    run.filled += n;
+    if (run.filled == run.window)
+      if (int rc = fb_close_window(c, run, st)) return rc;
+  }
+  return 0;
+}
+
 int lig_schedule_batch_feedback_device(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* d_reqs,
                                        int R, lig_pick* d_out, int sub_batch, int n_windows,
                                        int32_t* d_hist, void* stream) {
@@ -1792,67 +1904,174 @@ int lig_schedule_batch_feedback_device(lig_ctx* c, uint64_t epoch, uint64_t seed
   if (n_windows <= 0) n_windows = (R + sub_batch - 1) / sub_batch;
   if ((long long)n_windows * sub_batch < R)
     return fail(LIG_ERR_INVALID, "n_windows=%d x sub_batch=%d does not cover R=%d", n_windows, sub_batch, R);
-  // the tree in force when the call starts rebuilds every window's tables
+  // the tree and thresholds in force when the call starts rebuild every window's tables
+  FbRun run;
   FilterTree tree;
-  bool has_tree;
   {
     std::lock_guard<std::mutex> uk(c->upload_mu);
-    has_tree = c->has_tree;
-    if (has_tree) tree = c->tree;
+    if (c->has_tree) {
+      tree = c->tree;
+      run.tree = &tree;
+    }
+    run.thr = thr_of(c);
   }
+  run.window = sub_batch;
+  run.d_total = d_hist;
   std::lock_guard<std::mutex> fk(c->fb_mu);
   CUDA_TRY(cudaSetDevice(c->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (!c->fb_scratch.d_blob) {
-    if (c->stream_open) return fail(LIG_ERR_INVALID, "cannot allocate the feedback scratch while a doorbell stream is open");
-    if (int rc = alloc_slot(c, c->fb_scratch)) return rc;
-    CUDA_TRY(cudaMalloc(&c->d_fb_hist, (size_t)c->max_pods * sizeof(int32_t)));
-    CUDA_TRY(cudaEventCreateWithFlags(&c->fb_free, cudaEventDisableTiming));
-  }
-  Slot& fs = c->fb_scratch;
+  if (int rc = fb_alloc_scratch(c)) return rc;
   {
     std::lock_guard<std::mutex> lk(c->mu);
     Slot* s = nullptr;
     if (int rc = resolve_slot(c, epoch, &s)) return rc;
-    CUDA_TRY(cudaStreamWaitEvent(st, c->fb_free, 0));       // an earlier feedback call on another stream
-    CUDA_TRY(cudaStreamWaitEvent(st, s->ready, 0));
-    fs.P = s->P;
-    fs.A = s->A;
-    fs.W = s->W;
-    CUDA_TRY(cudaMemcpyAsync(fs.d_blob, s->d_blob, layout_for(s->P, s->A).total, cudaMemcpyDeviceToDevice, st));
-    if (int rc = note_reader(*s, st)) return rc;
+    c->chain_live = false;                                    // the scratch is reused: any chain ends
+    if (int rc = fb_copy_epoch(c, s, st)) return rc;
   }
-  const int P = fs.P;
-  int* q = reinterpret_cast<int*>(fs.d_blob + layout_for(fs.P, fs.A).q);
-  if (P > 0) CUDA_TRY(cudaMemsetAsync(c->d_fb_hist, 0, (size_t)P * sizeof(int32_t), st));
+  const int P = c->fb_scratch.P;
   if (d_hist && P > 0) CUDA_TRY(cudaMemsetAsync(d_hist, 0, (size_t)P * sizeof(int32_t), st));
-  for (int w = 0; w < n_windows; ++w) {
-    const long long lo = (long long)w * sub_batch;
-    const int n = lo >= R ? 0 : (int)((R - lo) < sub_batch ? (R - lo) : sub_batch);
+  if (int rc = fb_schedule(c, run, seed, d_reqs, R, d_out, st)) return rc;
+  // the last, partial window, then the trailing empty ones (their all-reduce still carries the
+  // picks of the other ranks)
+  if (run.filled > 0)
+    if (int rc = fb_close_window(c, run, st)) return rc;
+  while (run.closed < n_windows)
+    if (int rc = fb_close_window(c, run, st)) return rc;
+  CUDA_TRY(cudaEventRecord(c->fb_free, st));
+  return 0;
+}
+
+// One chain call (device-visible buffers, enqueued on `st`).  `d_loads` (nullable) receives the
+// chain's loads on the device.  Caller holds c->fb_mu, so no other call changes the chain meanwhile.
+static int chain_call(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* d_reqs, int R, lig_pick* d_out,
+                      int window, int32_t* d_loads, cudaStream_t st) {
+  // A chain (re)starts when it is not live, on another epoch or another upload of it (the next
+  // scrape supersedes the estimate), or with another window size.  The tree and thresholds in
+  // force at the start rebuild every window of the chain.  The tree is read under upload_mu, which
+  // is taken before mu: a start reads it first, then checks that the upload it copies is still the
+  // one it read the tree for.
+  FilterTree tree;
+  bool has_tree = false, have_tree = false;
+  Thr thr{};
+  uint64_t tree_stamp = 0;
+  for (;;) {
+    uint64_t stamp = 0;
     {
-      std::lock_guard<std::mutex> lk(c->mu);                 // launch counters, item ring
-      if (int rc = launch_class_build(c, fs, st, has_tree ? &tree : nullptr)) return rc;
-      if (n > 0) {
-        // the tables of the scratch copy change every window: always the strided tables through
-        // L1 (no host round trip for the compact header inside the loop)
-        if (int rc = launch_pick(c, fs, seed, d_reqs + lo, n, d_out + lo, st)) return rc;
+      std::lock_guard<std::mutex> lk(c->mu);
+      Slot* s = nullptr;
+      if (int rc = resolve_slot(c, epoch, &s)) return rc;    // refused: the chain is untouched
+      const bool restart = !c->chain_live || c->chain_epoch != epoch || c->chain_stamp != s->stamp ||
+                           c->chain_window != window;
+      if (!restart) {
+        c->chain_live = false;                                // until this call is enqueued
+        CUDA_TRY(cudaStreamWaitEvent(st, c->fb_free, 0));     // the chain's previous call, any stream
+        break;
       }
+      if (have_tree && tree_stamp == s->stamp) {
+        c->chain_live = false;
+        c->chain_has_tree = has_tree;
+        if (has_tree) c->chain_tree = tree;
+        c->chain_thr = thr;
+        c->chain_epoch = epoch;
+        c->chain_stamp = s->stamp;
+        c->chain_window = window;
+        c->chain_filled = 0;
+        c->chain_stale = true;
+        if (int rc = fb_copy_epoch(c, s, st)) return rc;
+        if (s->P > 0) CUDA_TRY(cudaMemsetAsync(c->d_fb_total, 0, (size_t)s->P * sizeof(int32_t), st));
+        break;
+      }
+      stamp = s->stamp;
     }
-    if (n > 0 && P > 0) {
-      lig_pick_hist_kernel<<<(n + 255) / 256 < 2048 ? (n + 255) / 256 : 2048, 256, 0, st>>>(
-          reinterpret_cast<const int2*>(d_out + lo), n, c->d_fb_hist);
-      CUDA_TRY(cudaGetLastError());
-      c->launches++;
+    {
+      std::lock_guard<std::mutex> uk(c->upload_mu);
+      has_tree = c->has_tree;
+      if (has_tree) tree = c->tree;
+      thr = thr_of(c);
     }
-    if (P > 0) {
-      if (c->comm && ligi::g_allreduce)                      // picks of this window on every rank
-        if (int rc = ligi::g_allreduce(c, c->d_fb_hist, P, st)) return rc;
-      lig_apply_feedback_kernel<<<(P + 255) / 256, 256, 0, st>>>(q, c->d_fb_hist, d_hist, P);
-      CUDA_TRY(cudaGetLastError());
-      c->launches++;
-    }
+    have_tree = true;
+    tree_stamp = stamp;
+  }
+  FbRun run;
+  run.window = window;
+  run.filled = c->chain_filled;
+  run.stale = c->chain_stale;
+  run.tree = c->chain_has_tree ? &c->chain_tree : nullptr;
+  run.thr = c->chain_thr;
+  run.d_total = c->d_fb_total;
+  if (int rc = fb_schedule(c, run, seed, d_reqs, R, d_out, st)) return rc;
+  const int P = c->fb_scratch.P;
+  if (d_loads && P > 0) {
+    lig_feedback_loads_kernel<<<(P + 255) / 256, 256, 0, st>>>(c->d_fb_total, c->d_fb_hist, d_loads, P);
+    CUDA_TRY(cudaGetLastError());
+    c->launches++;
   }
   CUDA_TRY(cudaEventRecord(c->fb_free, st));
+  c->chain_filled = run.filled;
+  c->chain_stale = run.stale;
+  c->chain_live = true;
+  return 0;
+}
+
+// Checks shared by both chain forms, before anything is touched.  Caller holds c->fb_mu.
+static int chain_admit(lig_ctx* c, const char* fn) {
+  if (c->comm)
+    return fail(LIG_ERR_INVALID, "%s: a ctx with a communicator has no feedback chain (per-rank micro-batch "
+                                 "streams share no window boundaries)", fn);
+  return fb_alloc_scratch(c);
+}
+
+int lig_schedule_batch_feedback_chain_device(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* d_reqs,
+                                             int R, lig_pick* d_out, int window, int32_t* d_loads, void* stream) {
+  if (!c || R < 0 || window < 1 || (R > 0 && (!d_reqs || !d_out)))
+    return fail(LIG_ERR_INVALID, "lig_schedule_batch_feedback_chain_device: bad argument");
+  std::lock_guard<std::mutex> fk(c->fb_mu);
+  CUDA_TRY(cudaSetDevice(c->device));
+  if (int rc = chain_admit(c, "lig_schedule_batch_feedback_chain_device")) return rc;
+  return chain_call(c, epoch, seed, d_reqs, R, d_out, window, d_loads, static_cast<cudaStream_t>(stream));
+}
+
+int lig_schedule_batch_feedback_chain(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
+                                      lig_pick* out, int window, int32_t* loads) {
+  if (!c || R < 0 || window < 1 || (R > 0 && (!reqs || !out)))
+    return fail(LIG_ERR_INVALID, "lig_schedule_batch_feedback_chain: bad argument");
+  if (R > c->max_batch) return fail(LIG_ERR_INVALID, "R=%d exceeds max_batch=%d", R, c->max_batch);
+  // as lig_schedule_batch: page-locked buffers are read and written in place, pageable ones bounce
+  const lig_req* dev_in = R ? mapped_device_pointer(reqs) : nullptr;
+  lig_pick* dev_out = R ? mapped_device_pointer(out) : nullptr;
+  const bool bounce = R > 0 && !(dev_in && dev_out);
+  std::unique_lock<std::mutex> bk(c->bounce_mu, std::defer_lock);
+  if (bounce) {
+    bk.lock();
+    dev_in = mapped_device_pointer(c->h_reqs);
+    dev_out = mapped_device_pointer(c->h_out);
+    if (!dev_in || !dev_out)
+      return fail(LIG_ERR_CUDA, "pinned staging buffers are not device-mapped on this platform");
+    memcpy(c->h_reqs, reqs, (size_t)R * sizeof(lig_req));
+  }
+  std::lock_guard<std::mutex> fk(c->fb_mu);
+  CUDA_TRY(cudaSetDevice(c->device));
+  if (int rc = chain_admit(c, "lig_schedule_batch_feedback_chain")) return rc;
+  int32_t* dev_loads = loads ? mapped_device_pointer(loads) : nullptr;
+  const bool loads_bounce = loads && !dev_loads;
+  if (loads_bounce && !(dev_loads = mapped_device_pointer(c->h_fb_loads)))
+    return fail(LIG_ERR_CUDA, "pinned staging buffers are not device-mapped on this platform");
+  if (int rc = chain_call(c, epoch, seed, dev_in, R, dev_out, window, dev_loads, c->s_fb)) return rc;
+  const cudaError_t e = cudaStreamSynchronize(c->s_fb);
+  if (e != cudaSuccess) {
+    c->chain_live = false;
+    return fail(LIG_ERR_CUDA, "feedback chain call failed on the device: %s", cudaGetErrorString(e));
+  }
+  if (bounce) memcpy(out, c->h_out, (size_t)R * sizeof(lig_pick));
+  if (loads_bounce && c->fb_scratch.P > 0)
+    memcpy(loads, c->h_fb_loads, (size_t)c->fb_scratch.P * sizeof(int32_t));
+  return 0;
+}
+
+int lig_feedback_chain_reset(lig_ctx* c) {
+  if (!c) return fail(LIG_ERR_INVALID, "lig_feedback_chain_reset: ctx is null");
+  std::lock_guard<std::mutex> fk(c->fb_mu);
+  c->chain_live = false;
   return 0;
 }
 

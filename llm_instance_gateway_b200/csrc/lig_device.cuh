@@ -2178,14 +2178,7 @@ lig_pick_models_stream_kernel(const uint32_t* __restrict__ ids, uint32_t* __rest
   }
 }
 
-// ---- K2f: load feedback between the windows of a batch (opt-in) -----------------------------------
-// hist[pod] += 1 for every pick of the window that chose a pod.
-__global__ void lig_pick_hist_kernel(const int2* __restrict__ picks, int n, int* __restrict__ hist) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const int pod = picks[i].x;
-    if (pod >= 0) atomicAdd(hist + pod, 1);
-  }
-}
+// ---- K2f: load feedback between the windows of a batch or of a chain of calls (opt-in) ------------
 // WaitingQueueSize += picks of the window (all ranks); total += window; window = 0.
 __global__ void lig_apply_feedback_kernel(int* __restrict__ q, int* __restrict__ hist_window,
                                           int* __restrict__ hist_total, int P) {
@@ -2197,6 +2190,47 @@ __global__ void lig_apply_feedback_kernel(int* __restrict__ q, int* __restrict__
   q[p] = nq > 0x7fffffffLL ? 0x7fffffff : (int)nq;
   if (hist_total) hist_total[p] += h;
   hist_window[p] = 0;
+}
+
+// The pick of lig_pick_stream_kernel (same pick_one, so the picks are byte-identical) that also
+// counts the picks per pod into the open window's histogram, for the load-feedback chain
+// (lig_schedule_batch_feedback_chain).  `reqs` / `out` may be mapped host memory.  A herd puts
+// most picks of a warp on a few pods, so the count is warp-aggregated: lanes that picked the same
+// pod find each other with __match_any_sync and the lowest of them adds the group's size with one
+// atomic; pod -1 (DROP, EMPTY, NO_PODS_LEFT) adds nothing.  Every lane of a CTA runs every round,
+// ragged ones with pod -1, so the full-warp match is always legal.
+constexpr int kCountPerThread = 4;
+__global__ void __launch_bounds__(kPickThreads, 8)
+lig_pick_count_kernel(const int4* __restrict__ reqs, int2* __restrict__ out, int R,
+                      const uint4* __restrict__ cls, const uint16_t* __restrict__ lists, int A,
+                      uint64_t seed, int* __restrict__ hist) {
+  const int first = blockIdx.x * (kPickThreads * kCountPerThread) + threadIdx.x;
+  const int lane = threadIdx.x & 31;
+  int4 r[kCountPerThread];
+#pragma unroll
+  for (int j = 0; j < kCountPerThread; ++j) {      // every load in flight before the first use
+    const int i = first + j * kPickThreads;
+    r[j] = i < R ? ld_stream_int4(reqs + i) : make_int4(0, 0, 0, 0);
+  }
+#pragma unroll
+  for (int j = 0; j < kCountPerThread; ++j) {
+    const int i = first + j * kPickThreads;
+    int pod = -1;
+    if (i < R) {
+      const int2 p = pick_one(r[j], cls, lists, (uint32_t)A, seed);
+      st_stream_int2(out + i, p);
+      pod = p.x;
+    }
+    const unsigned same = __match_any_sync(kFull, pod);
+    if (pod >= 0 && lane == __ffs(same) - 1) atomicAdd(hist + pod, __popc(same));
+  }
+}
+
+// loads[p] = picks of the closed windows + picks of the open one (the chain's per-pod loads).
+__global__ void lig_feedback_loads_kernel(const int* __restrict__ total, const int* __restrict__ window,
+                                          int* __restrict__ loads, int P) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p < P) loads[p] = total[p] + window[p];
 }
 
 // ---- K3: persistent doorbell kernel (streaming micro-batches) ------------------------------------

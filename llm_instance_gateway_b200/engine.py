@@ -149,6 +149,38 @@ class Engine:
         N.check(self._lib.lig_schedule_batch_feedback_device(self._ctx, epoch, seed, d_reqs, R, d_out, sub_batch,
                                                              n_windows, d_hist or None, stream or None))
 
+    def schedule_batch_feedback_chain(self, epoch: int, seed: int, reqs: np.ndarray, window: int,
+                                      loads: Optional[np.ndarray] = None,
+                                      out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Load feedback carried across calls against one epoch (include/lig.h, the feedback chain):
+        windows of `window` requests over the sequence of all chain calls, cut regardless of call
+        boundaries.  `loads` (int32[P], optional) receives the picks per pod since the chain began."""
+        assert reqs.dtype == REQ_DTYPE and reqs.flags.c_contiguous
+        R = int(reqs.shape[0])
+        if out is None:
+            out = np.empty(R, dtype=PICK_DTYPE)
+        if loads is not None:
+            assert loads.dtype == np.int32 and loads.flags.c_contiguous
+        N.check(self._lib.lig_schedule_batch_feedback_chain(self._ctx, epoch, seed, _ptr(reqs), R, _ptr(out), window,
+                                                            _ptr(loads) if loads is not None else None))
+        return out
+
+    def schedule_batch_feedback_chain_ptr(self, epoch: int, seed: int, h_reqs: int, R: int, h_out: int, window: int,
+                                          h_loads: int = 0) -> None:
+        N.check(self._lib.lig_schedule_batch_feedback_chain(self._ctx, epoch, seed, h_reqs, R, h_out, window,
+                                                            h_loads or None))
+
+    def schedule_batch_feedback_chain_device(self, epoch: int, seed: int, d_reqs: int, R: int, d_out: int,
+                                             window: int, d_loads: int = 0, stream: int = 0) -> None:
+        """The chain with device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_batch_feedback_chain_device(self._ctx, epoch, seed, d_reqs or None, R,
+                                                                   d_out or None, window, d_loads or None,
+                                                                   stream or None))
+
+    def feedback_chain_reset(self) -> None:
+        """The next feedback-chain call starts a new chain from its epoch's scrape."""
+        N.check(self._lib.lig_feedback_chain_reset(self._ctx))
+
     def pick_kernel_info(self, epoch: int) -> dict:
         name = C.create_string_buffer(64)
         grid, threads, tb, in_smem = C.c_int(), C.c_int(), C.c_int(), C.c_int()

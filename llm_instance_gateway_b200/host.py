@@ -26,7 +26,7 @@ EXPORTED_SYMBOLS = (
     "ligh_scheduler_free", "ligh_schedule", "ligh_refresh", "ligh_stats",
     "ligh_schedule_concurrent", "ligh_stream_bench", "ligh_refresh_timing", "ligh_flush_timing",
     "ligh_scheduler_new_devices", "ligh_datastore_new", "ligh_datastore_free", "ligh_datastore_set_model",
-    "ligh_schedule_model", "ligh_scheduler_new_tree",
+    "ligh_schedule_model", "ligh_scheduler_new_tree", "ligh_scheduler_new_feedback", "ligh_feedback_stats",
 )
 
 _lib = None
@@ -54,6 +54,11 @@ def load() -> C.CDLL:
     lib.ligh_scheduler_new_tree.argtypes = [vp, i32, C.POINTER(i32), i32, i32, i32, i32, i32, i32, i32, u64, i32, i32,
                                             i32, vp, i32, C.c_char_p, i32]
     lib.ligh_scheduler_new_tree.restype = vp
+    lib.ligh_scheduler_new_feedback.argtypes = [vp, i32, C.POINTER(i32), i32, i32, i32, i32, i32, i32, i32, u64, i32,
+                                                i32, i32, vp, i32, i32, C.c_char_p, i32]
+    lib.ligh_scheduler_new_feedback.restype = vp
+    lib.ligh_feedback_stats.argtypes = [vp, vp]
+    lib.ligh_feedback_stats.restype = None
     lib.ligh_datastore_new.restype = vp
     lib.ligh_datastore_free.argtypes = [vp]
     lib.ligh_datastore_free.restype = None
@@ -126,19 +131,22 @@ class HostScheduler:
                  max_adapters: int = 1024, max_batch: int = 1 << 16, flush_size: int = 4096,
                  batch_window_us: int = 50, refresh_interval_ms: int = 0, seed: int = 1,
                  busy_poll: bool = False, caller_spin_us: int = 0, use_doorbell: bool = False,
-                 devices: Optional[Sequence[int]] = None, filter=None):
+                 devices: Optional[Sequence[int]] = None, filter=None, load_feedback_window: int = 0):
         self._lib = load()
         self.provider = provider
         err = C.create_string_buffer(512)
-        if filter is not None:         # Options::filter: a scheduling.Filter chart or a node table
+        if filter is not None or load_feedback_window:
+            # Options::filter (a scheduling.Filter chart or a node table) and
+            # Options::load_feedback_window (load feedback carried across flushes, 0 = off)
             from .engine import _node_table
             nodes, n = _node_table(filter)
             devs = list(devices) if devices is not None else []
             arr = (C.c_int * max(len(devs), 1))(*devs)
-            self._s = self._lib.ligh_scheduler_new_tree(provider._p, device, arr, len(devs), max_pods, max_adapters,
-                                                        max_batch, flush_size, batch_window_us, refresh_interval_ms,
-                                                        seed, int(busy_poll), caller_spin_us, int(use_doorbell),
-                                                        C.cast(nodes, C.c_void_p), n, err, 512)
+            self._s = self._lib.ligh_scheduler_new_feedback(provider._p, device, arr, len(devs), max_pods,
+                                                            max_adapters, max_batch, flush_size, batch_window_us,
+                                                            refresh_interval_ms, seed, int(busy_poll), caller_spin_us,
+                                                            int(use_doorbell), C.cast(nodes, C.c_void_p), n,
+                                                            load_feedback_window, err, 512)
         elif devices is not None and len(devices) > 1:
             arr = (C.c_int * len(devices))(*devices)
             self._s = self._lib.ligh_scheduler_new_devices(provider._p, arr, len(devices), max_pods, max_adapters,
@@ -173,8 +181,11 @@ class HostScheduler:
     def stats(self) -> dict:
         out = (C.c_uint64 * 9)()
         self._lib.ligh_stats(self._s, out)
+        fb = (C.c_uint64 * 2)()
+        self._lib.ligh_feedback_stats(self._s, fb)
         return dict(zip(("scheduled", "batches", "max_batch", "refreshes", "stale_retries", "failed_refreshes",
-                         "excluded_pods", "delta_refreshes", "last_dirty_pods"), map(int, out)))
+                         "excluded_pods", "delta_refreshes", "last_dirty_pods", "feedback_windows",
+                         "feedback_restarts"), map(int, list(out) + list(fb))))
 
     def ScheduleModel(self, datastore: "HostDataStore", model: str):  # noqa: N802
         """resolve (FetchModelData + RandomWeightedDraw + IsCritical) + Schedule: (code, resolved, pod, err)."""

@@ -11,7 +11,8 @@ Same names, argument meaning and error behaviour as the reference so that it dro
 server turns into HTTP 429 (handlers/server.go:97-109).  ``NewScheduler(pmp, filter=...)`` runs a
 caller-built flow chart of the reference's filter nodes (``Filter``, filter.go:17-73) instead of
 ``defaultFilter``; ``DEFAULT_FILTER`` restates defaultFilter node for node.  ``ScheduleBatch`` is the micro-batched
-form the Go adapter uses under load (one C-ABI call per batch).  There is no CPU path here:
+form the Go adapter uses under load (one C-ABI call per batch); ``NewScheduler(pmp, load_feedback_window=W)``
+carries load feedback across those calls until the next refresh (off by default).  There is no CPU path here:
 without liblig.so or without a CUDA device construction fails.
 """
 from __future__ import annotations
@@ -155,8 +156,11 @@ def _schedule_error(status: int) -> StatusError:
 class Scheduler:
     def __init__(self, podMetricsProvider: PodMetricsProvider, device: int = 0,
                  max_pods: int = 4096, max_adapters: int = 1024, max_batch: int = 1 << 16,
-                 seed: Optional[int] = None, filter: Optional[Filter] = None):
+                 seed: Optional[int] = None, filter: Optional[Filter] = None, load_feedback_window: int = 0):
+        if load_feedback_window < 0:
+            raise ValueError(f"load_feedback_window must be >= 0, got {load_feedback_window}")
         self.podMetricsProvider = podMetricsProvider
+        self._window = load_feedback_window  # 0: the reference's behaviour (no load feedback)
         self._engine = Engine(device, max_pods, max_adapters, max_batch)
         self._filter = filter                # None: the built-in defaultFilter
         if filter is not None:
@@ -197,7 +201,12 @@ class Scheduler:
         for i, r in enumerate(reqs):
             arr[i] = (snap.adapter_id(r.ResolvedTargetModel), N.LIG_REQ_CRITICAL if r.Critical else 0,
                       self._rng.getrandbits(64))
-        picks = self._engine.schedule_batch(self._epoch, self._seed, arr)
+        if self._window:
+            # the feedback chain: each window of `_window` requests, across calls, adds its picks to
+            # the pods' WaitingQueueSize until the next refresh uploads a new epoch
+            picks = self._engine.schedule_batch_feedback_chain(self._epoch, self._seed, arr, self._window)
+        else:
+            picks = self._engine.schedule_batch(self._epoch, self._seed, arr)
         out = []
         for pk in picks:
             if pk["status"] == N.LIG_OK:
@@ -214,6 +223,8 @@ class Scheduler:
 
     # Filter-level view (the GPU analogue of Filter.Filter, filter.go:12-15): survivor slice.
     def Filter(self, req: LLMRequest) -> Tuple[List[Pod], Optional[StatusError]]:
+        """The survivors of `req` against the scraped snapshot.  With load_feedback_window set this
+        is still the scraped epoch: the queue sizes the feedback chain has added are not in it."""
         snap = self._current()
         if self._filter is not None:         # the class table holds the caller tree's survivor set
             st, _, lst = self._engine.read_class(self._epoch, req.Critical, snap.adapter_id(req.ResolvedTargetModel),
@@ -233,6 +244,10 @@ class Scheduler:
         return survivors, None
 
 
-def NewScheduler(pmp: PodMetricsProvider, filter: Optional[Filter] = None, **kw) -> Scheduler:  # scheduler.go:93-99
-    """filter: a caller flow chart (None = defaultFilter, the reference's only tree)."""
-    return Scheduler(pmp, filter=filter, **kw)
+def NewScheduler(pmp: PodMetricsProvider, filter: Optional[Filter] = None, load_feedback_window: int = 0,
+                 **kw) -> Scheduler:  # scheduler.go:93-99
+    """filter: a caller flow chart (None = defaultFilter, the reference's only tree).
+    load_feedback_window > 0: ScheduleBatch goes through the load-feedback chain (include/lig.h,
+    lig_schedule_batch_feedback_chain): every window of that many requests, counted across calls,
+    adds its picks to the pods' WaitingQueueSize until the next refresh.  0 = off."""
+    return Scheduler(pmp, filter=filter, load_feedback_window=load_feedback_window, **kw)
