@@ -345,7 +345,8 @@ int launch_class_build(lig_ctx* c, Slot& s, cudaStream_t stream, const FilterTre
   const bool fast = c->fast_build && s.P > 0 && W <= kFastMaxWords &&
                     fast_fixed_bytes(W) + staged_bytes(W) <= c->smem_optin;
   if (fast) {
-    // pools of up to 4096 pods: register-resident shared stages, one class per warp
+    // pools of up to 4096 pods: register-resident shared stages, one class per warp up to
+    // 8 * SMs adapters, several per warp (round-robin) beyond
     int fgrid = (n_classes + kBuildWarps - 1) / kBuildWarps;
     if (fgrid > c->sm_count) fgrid = c->sm_count;
     lig_class_build_fast_kernel<<<fgrid, kBuildThreads, fast_fixed_bytes(W) + staged_bytes(W), stream>>>(

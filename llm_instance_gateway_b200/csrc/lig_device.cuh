@@ -914,9 +914,12 @@ lig_class_build_kernel(SnapView s, Thr thr, ClassEntry* __restrict__ cls,
 //   * the shared stages keep each thread's 8 pods (word warp + 16 j, bit lane) in REGISTERS, sets
 //     are 8-bit masks per thread, a stage is a few compares + one warp reduction + ONE
 //     __syncthreads (double-buffered scratch) instead of ballot passes over shared-memory masks;
-//   * one class per warp (twice the CTAs), its bitmap row requested from HBM/L2 before the shared
-//     stages start, pool space reserved (atomic) before the compaction, one compaction pass that
-//     writes the strided row and the pool entry together, lanes owning contiguous words.
+//   * one class per warp (twice the CTAs, up to one per SM), its bitmap row requested from HBM/L2
+//     before the shared stages start, pool space reserved (atomic) before the compaction, one
+//     compaction pass that writes the strided row and the pool entry together, lanes owning
+//     contiguous words.  From 8 * SMs adapters on (2(A+1) > 16 * SMs classes), each warp takes
+//     several classes round-robin (c, c + 16 * gridDim.x, ...) and fetches each later one's row
+//     when it gets to it.
 constexpr int kOwn = 8;                                 // words per warp: W <= kBuildWarps * kOwn
 constexpr int kFastMaxWords = kBuildWarps * kOwn;       // 128 words = 4096 pods
 
@@ -1181,7 +1184,7 @@ lig_class_build_fast_kernel(SnapView s, Thr thr, ClassEntry* __restrict__ cls, u
       const uint32_t* Zm = critical ? (n_low > 0 ? nullptr : CZ) : SZ;
       uint32_t hit = 0;
       if (a < A) {
-        if (c != c0) {   // later classes of this warp (A > 1183): fetch the row now
+        if (c != c0) {   // later classes of this warp (A >= 8 * SMs): fetch the row now
           const uint32_t* row = s.bitmap + (size_t)a * W;
 #pragma unroll
           for (int i = 0; i < kFastMaxWords / 32; ++i) rowreg[i] = (lane + 32 * i < W) ? __ldg(row + lane + 32 * i) : 0u;
