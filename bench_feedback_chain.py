@@ -5,6 +5,8 @@ one GPU, in one process.  Prints the card and its power limit first, then one JS
   of 1, 16, 256 and 4096 requests: lig_schedule_batch, chain calls that close no window (W = 2^30)
   and chain calls that close one window each (W = the micro-batch: a pick, a window apply and one
   class build per call).  Median and p99 wall time per call over --reps calls;
+* models: the same for model-id requests at C4 with WL.make_models: lig_schedule_models_batch and
+  lig_schedule_models_batch_feedback_chain with no window closing and with one window per call;
 * herd: 5000 C4-distributed requests in micro-batches of 8 against one epoch: the most picks one
   pod received and the number of pods used, without feedback and with W in {1, 8, 64, 512};
 * stream: the C5 stream (100 K req/s Poisson) through the C++ runtime, p50 / p99 service latency
@@ -28,7 +30,7 @@ from llm_instance_gateway_b200 import host as H
 from llm_instance_gateway_b200 import workload as WL
 from llm_instance_gateway_b200.backend import Metrics, Pod, PodMetrics
 from llm_instance_gateway_b200.engine import Engine
-from llm_instance_gateway_b200.packer import PICK_DTYPE, REQ_DTYPE
+from llm_instance_gateway_b200.packer import MPICK_DTYPE, PICK_DTYPE, REQ_DTYPE, pack_models
 
 
 def card():
@@ -81,6 +83,40 @@ def latency(reps):
             lib.lig_host_free(rp)
             lib.lig_host_free(op)
     return {"part": "latency", "config": "C4 host-buffer calls, page-locked buffers", **out}
+
+
+def models(reps):
+    lib = N.load()
+    c = WL.CONFIGS["C4"]
+    snap = WL.make_snapshot(c["P"], c["A"])
+    out = {}
+    with Engine(0, max_pods=c["P"], max_adapters=c["A"], max_batch=4096) as e:
+        e.upload_snapshot(1, snap.packed)
+        e.upload_models(1, pack_models(WL.make_models(c["A"]), snap.packed))
+        for m in (1, 16, 256, 4096):
+            ip, ia = pinned(lib, m, np.uint32)
+            op, _ = pinned(lib, m, MPICK_DTYPE)
+            ia[:] = WL.make_model_requests(m, c["A"], seed=m)
+            row = {}
+            for name, call in (
+                    ("schedule_models_batch", lambda s: e.schedule_models_batch_ptr(1, s, s * m, ip, m, op)),
+                    ("chain_no_window",
+                     lambda s: e.schedule_models_batch_feedback_chain_ptr(1, s, s * m, ip, m, op, 1 << 30)),
+                    ("chain_one_window",
+                     lambda s: e.schedule_models_batch_feedback_chain_ptr(1, s, s * m, ip, m, op, m))):
+                e.feedback_chain_reset()
+                for s in range(20):                          # warm-up
+                    call(s)
+                ts = []
+                for s in range(reps):
+                    t0 = time.perf_counter()
+                    call(s)
+                    ts.append(time.perf_counter() - t0)
+                row[name] = stats_us(ts)
+            out[f"R={m}"] = row
+            lib.lig_host_free(ip)
+            lib.lig_host_free(op)
+    return {"part": "models", "config": "C4 model-id host-buffer calls, page-locked buffers", **out}
 
 
 def herd():
@@ -145,6 +181,7 @@ def main():
     a = ap.parse_args()
     print(json.dumps({"card": card()}), flush=True)
     print(json.dumps(latency(a.reps)), flush=True)
+    print(json.dumps(models(a.reps)), flush=True)
     print(json.dumps(herd()), flush=True)
     print(json.dumps(stream(a.seconds, a.stream_window)), flush=True)
 

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define LIG_ABI_VERSION 4
+#define LIG_ABI_VERSION 5
 
 /* ---- per-request status (lig_pick.status) ------------------------------------------------------
  * LIG_OK    Schedule returned a pod, nil                      pkg/ext-proc/scheduling/scheduler.go:120-121
@@ -430,6 +430,27 @@ int lig_schedule_batch_feedback_chain(lig_ctx* ctx, uint64_t epoch, uint64_t see
 /* device pointers, enqueued on `stream`, not synchronised */
 int lig_schedule_batch_feedback_chain_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* d_reqs,
                                              int R, lig_pick* d_out, int window, int32_t* d_loads, void* stream);
+/* The same chain for model-id requests (see lig_schedule_models_batch).  A model-id call is one more
+ * chain call: its R requests join the same sequence and the same windows as descriptor calls, and
+ * the two kinds of call may alternate without restarting the chain; the restart rules above are
+ * unchanged.  Request i of the call has rand_key = first_index + i; it is resolved against E's
+ * model table as that table stands at the call, then picked on the chain's current private tables
+ * with the call's seed.  So while no window has closed the picks equal lig_schedule_models_batch
+ * byte for byte.  The model table is read from E's resident slot, never copied into the chain: a
+ * lig_upload_models[_async] for E does not restart the chain (loads belong to pods, not to
+ * models) and the next chain call resolves against the new table.  A call is ordered on the device
+ * behind the table's upload, and a later model upload waits on the device for the calls that read
+ * the table before it overwrites it, whatever their stream.  LIG_NO_MODEL, LIG_DROP, LIG_EMPTY and
+ * LIG_NO_PODS_LEFT count toward the window and add no pick.  A call is refused, leaving the chain
+ * exactly as it was, for the reasons above and with LIG_ERR_NO_SNAPSHOT when E has no model table. */
+/* host buffers (page-locked ones used in place, pageable ones bounce); blocks */
+int lig_schedule_models_batch_feedback_chain(lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                                             const uint32_t* model_ids, int R, lig_mpick* out,
+                                             int window, int32_t* loads);
+/* device pointers, enqueued on `stream`, not synchronised */
+int lig_schedule_models_batch_feedback_chain_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed,
+                                                    uint64_t first_index, const uint32_t* d_model_ids, int R,
+                                                    lig_mpick* d_out, int window, int32_t* d_loads, void* stream);
 /* The next chain call starts a new chain. */
 int lig_feedback_chain_reset(lig_ctx* ctx);
 

@@ -1105,7 +1105,7 @@ static int create_impl(lig_ctx* c, int device, int max_pods, int max_adapters, i
         (const void*)lig_pick_queue_kernel<8>,   (const void*)lig_pick_queue_kernel<16>,
         (const void*)lig_pick_models_stream_kernel, (const void*)lig_apply_delta_kernel,
         (const void*)lig_pick_count_kernel,      (const void*)lig_apply_feedback_kernel,
-        (const void*)lig_feedback_loads_kernel,
+        (const void*)lig_feedback_loads_kernel,  (const void*)lig_pick_models_count_kernel,
     };
     for (const void* fn : fns) CUDA_TRY(cudaFuncGetAttributes(&fa, fn));
   }
@@ -1865,12 +1865,24 @@ static int fb_close_window(lig_ctx* c, FbRun& run, cudaStream_t st) {
   return 0;
 }
 
-// Schedule R requests (device-visible pointers) through the window sequence: each segment is the
-// rest of the open window or of the call, whichever is shorter; one fused pick + count launch per
-// segment; a filled window is closed at once, its tables are rebuilt only when the next segment
-// needs them.
-static int fb_schedule(lig_ctx* c, FbRun& run, uint64_t seed, const lig_req* d_reqs, int R, lig_pick* d_out,
-                       cudaStream_t st) {
+// The requests of one feedback call (device-visible pointers): 16-byte descriptors in, lig_pick
+// out; or 4-byte model ids in, lig_mpick out, request i with rand_key = first_index + i, resolved
+// against a resident epoch's model table.
+struct FbReqs {
+  const void* in = nullptr;              // lig_req[R] or uint32_t[R]
+  void* out = nullptr;                   // lig_pick[R] or lig_mpick[R]
+  bool models = false;
+  uint64_t first_index = 0;              // model ids: rand_key of request 0
+  const unsigned char* mtab = nullptr;   // model ids: the model table (set by chain_call)
+  uint32_t n_models = 0;
+  size_t in_bytes() const { return models ? sizeof(uint32_t) : sizeof(lig_req); }
+  size_t out_bytes() const { return models ? sizeof(lig_mpick) : sizeof(lig_pick); }
+};
+
+// Schedule R requests through the window sequence: each segment is the rest of the open window or
+// of the call, whichever is shorter; one fused pick + count launch per segment; a filled window is
+// closed at once, its tables are rebuilt only when the next segment needs them.
+static int fb_schedule(lig_ctx* c, FbRun& run, uint64_t seed, const FbReqs& rq, int R, cudaStream_t st) {
   Slot& fs = c->fb_scratch;
   for (int pos = 0; pos < R;) {
     const int n = (R - pos) < (run.window - run.filled) ? (R - pos) : (run.window - run.filled);
@@ -1883,10 +1895,17 @@ static int fb_schedule(lig_ctx* c, FbRun& run, uint64_t seed, const lig_req* d_r
     }
     // the scratch's tables change every window: always the strided tables through L1 (no host
     // round trip for the compact header)
-    lig_pick_count_kernel<<<(n + kPickThreads * kCountPerThread - 1) / (kPickThreads * kCountPerThread),
-                            kPickThreads, 0, st>>>(
-        reinterpret_cast<const int4*>(d_reqs + pos), reinterpret_cast<int2*>(d_out + pos), n,
-        reinterpret_cast<const uint4*>(fs.d_cls), fs.d_lists, fs.A, seed, c->d_fb_hist);
+    const void* in = static_cast<const unsigned char*>(rq.in) + (size_t)pos * rq.in_bytes();
+    void* out = static_cast<unsigned char*>(rq.out) + (size_t)pos * rq.out_bytes();
+    const int grid = (n + kPickThreads * kCountPerThread - 1) / (kPickThreads * kCountPerThread);
+    if (rq.models)
+      lig_pick_models_count_kernel<<<grid, kPickThreads, 0, st>>>(
+          static_cast<const uint32_t*>(in), static_cast<uint32_t*>(out), n, reinterpret_cast<const uint4*>(fs.d_cls),
+          fs.d_lists, fs.A, rq.mtab, rq.n_models, seed, rq.first_index + (uint64_t)pos, c->d_fb_hist);
+    else
+      lig_pick_count_kernel<<<grid, kPickThreads, 0, st>>>(
+          static_cast<const int4*>(in), static_cast<int2*>(out), n, reinterpret_cast<const uint4*>(fs.d_cls),
+          fs.d_lists, fs.A, seed, c->d_fb_hist);
     CUDA_TRY(cudaGetLastError());
     c->launches++;
     pos += n;
@@ -1931,7 +1950,10 @@ int lig_schedule_batch_feedback_device(lig_ctx* c, uint64_t epoch, uint64_t seed
   }
   const int P = c->fb_scratch.P;
   if (d_hist && P > 0) CUDA_TRY(cudaMemsetAsync(d_hist, 0, (size_t)P * sizeof(int32_t), st));
-  if (int rc = fb_schedule(c, run, seed, d_reqs, R, d_out, st)) return rc;
+  FbReqs rq;
+  rq.in = d_reqs;
+  rq.out = d_out;
+  if (int rc = fb_schedule(c, run, seed, rq, R, st)) return rc;
   // the last, partial window, then the trailing empty ones (their all-reduce still carries the
   // picks of the other ranks)
   if (run.filled > 0)
@@ -1944,8 +1966,14 @@ int lig_schedule_batch_feedback_device(lig_ctx* c, uint64_t epoch, uint64_t seed
 
 // One chain call (device-visible buffers, enqueued on `st`).  `d_loads` (nullable) receives the
 // chain's loads on the device.  Caller holds c->fb_mu, so no other call changes the chain meanwhile.
-static int chain_call(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* d_reqs, int R, lig_pick* d_out,
-                      int window, int32_t* d_loads, cudaStream_t st) {
+// Model ids are resolved against E's resident model table, which the chain never copies: a model
+// upload does not restart the chain.  The call holds upload_mu until it is enqueued, so that no
+// upload replaces the table between the resolve and the last launch, and registers as a reader of
+// E's slot, so that a later upload waits for the launches before it overwrites the table.
+static int chain_call(lig_ctx* c, uint64_t epoch, uint64_t seed, FbReqs rq, int R, int window, int32_t* d_loads,
+                      cudaStream_t st) {
+  std::unique_lock<std::mutex> held(c->upload_mu, std::defer_lock);
+  if (rq.models) held.lock();
   // A chain (re)starts when it is not live, on another epoch or another upload of it (the next
   // scrape supersedes the estimate), or with another window size.  The tree and thresholds in
   // force at the start rebuild every window of the chain.  The tree is read under upload_mu, which
@@ -1955,12 +1983,13 @@ static int chain_call(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* 
   bool has_tree = false, have_tree = false;
   Thr thr{};
   uint64_t tree_stamp = 0;
+  Slot* s = nullptr;
   for (;;) {
     uint64_t stamp = 0;
     {
       std::lock_guard<std::mutex> lk(c->mu);
-      Slot* s = nullptr;
-      if (int rc = resolve_slot(c, epoch, &s)) return rc;    // refused: the chain is untouched
+      // refused (stale epoch, no model table): the chain is untouched
+      if (int rc = rq.models ? resolve_models_slot(c, epoch, &s) : resolve_slot(c, epoch, &s)) return rc;
       const bool restart = !c->chain_live || c->chain_epoch != epoch || c->chain_stamp != s->stamp ||
                            c->chain_window != window;
       if (!restart) {
@@ -1985,13 +2014,20 @@ static int chain_call(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* 
       stamp = s->stamp;
     }
     {
-      std::lock_guard<std::mutex> uk(c->upload_mu);
+      std::unique_lock<std::mutex> uk(c->upload_mu, std::defer_lock);
+      if (!held) uk.lock();
       has_tree = c->has_tree;
       if (has_tree) tree = c->tree;
       thr = thr_of(c);
     }
     have_tree = true;
     tree_stamp = stamp;
+  }
+  if (rq.models) {
+    std::lock_guard<std::mutex> lk(c->mu);
+    CUDA_TRY(cudaStreamWaitEvent(st, s->models_ready, 0));
+    rq.mtab = s->d_mtab;
+    rq.n_models = s->n_models;
   }
   FbRun run;
   run.window = window;
@@ -2000,7 +2036,11 @@ static int chain_call(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* 
   run.tree = c->chain_has_tree ? &c->chain_tree : nullptr;
   run.thr = c->chain_thr;
   run.d_total = c->d_fb_total;
-  if (int rc = fb_schedule(c, run, seed, d_reqs, R, d_out, st)) return rc;
+  if (int rc = fb_schedule(c, run, seed, rq, R, st)) return rc;
+  if (rq.models) {
+    std::lock_guard<std::mutex> lk(c->mu);
+    if (int rc = note_reader(*s, st)) return rc;
+  }
   const int P = c->fb_scratch.P;
   if (d_loads && P > 0) {
     lig_feedback_loads_kernel<<<(P + 255) / 256, 256, 0, st>>>(c->d_fb_total, c->d_fb_hist, d_loads, P);
@@ -2022,51 +2062,96 @@ static int chain_admit(lig_ctx* c, const char* fn) {
   return fb_alloc_scratch(c);
 }
 
-int lig_schedule_batch_feedback_chain_device(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* d_reqs,
-                                             int R, lig_pick* d_out, int window, int32_t* d_loads, void* stream) {
-  if (!c || R < 0 || window < 1 || (R > 0 && (!d_reqs || !d_out)))
-    return fail(LIG_ERR_INVALID, "lig_schedule_batch_feedback_chain_device: bad argument");
+// The device form of both chain calls.
+static int chain_device(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t seed, const FbReqs& rq, int R,
+                        int window, int32_t* d_loads, void* stream) {
+  if (!c || R < 0 || window < 1 || (R > 0 && (!rq.in || !rq.out))) return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
   std::lock_guard<std::mutex> fk(c->fb_mu);
   CUDA_TRY(cudaSetDevice(c->device));
-  if (int rc = chain_admit(c, "lig_schedule_batch_feedback_chain_device")) return rc;
-  return chain_call(c, epoch, seed, d_reqs, R, d_out, window, d_loads, static_cast<cudaStream_t>(stream));
+  if (int rc = chain_admit(c, fn)) return rc;
+  return chain_call(c, epoch, seed, rq, R, window, d_loads, static_cast<cudaStream_t>(stream));
 }
 
-int lig_schedule_batch_feedback_chain(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
-                                      lig_pick* out, int window, int32_t* loads) {
-  if (!c || R < 0 || window < 1 || (R > 0 && (!reqs || !out)))
-    return fail(LIG_ERR_INVALID, "lig_schedule_batch_feedback_chain: bad argument");
+// The host form of both chain calls (rq holds the caller's host buffers); blocks.
+static int chain_host(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t seed, FbReqs rq, int R, int window,
+                      int32_t* loads) {
+  if (!c || R < 0 || window < 1 || (R > 0 && (!rq.in || !rq.out))) return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
   if (R > c->max_batch) return fail(LIG_ERR_INVALID, "R=%d exceeds max_batch=%d", R, c->max_batch);
   // as lig_schedule_batch: page-locked buffers are read and written in place, pageable ones bounce
-  const lig_req* dev_in = R ? mapped_device_pointer(reqs) : nullptr;
-  lig_pick* dev_out = R ? mapped_device_pointer(out) : nullptr;
-  const bool bounce = R > 0 && !(dev_in && dev_out);
+  // (4-byte model ids and picks fit the 16-byte / 8-byte bounce buffers)
+  const void* in = rq.in;
+  void* out = rq.out;
+  rq.in = R ? mapped_device_pointer(in) : nullptr;
+  rq.out = R ? mapped_device_pointer(out) : nullptr;
+  const bool bounce = R > 0 && !(rq.in && rq.out);
   std::unique_lock<std::mutex> bk(c->bounce_mu, std::defer_lock);
   if (bounce) {
     bk.lock();
-    dev_in = mapped_device_pointer(c->h_reqs);
-    dev_out = mapped_device_pointer(c->h_out);
-    if (!dev_in || !dev_out)
+    rq.in = mapped_device_pointer(c->h_reqs);
+    rq.out = mapped_device_pointer(c->h_out);
+    if (!rq.in || !rq.out)
       return fail(LIG_ERR_CUDA, "pinned staging buffers are not device-mapped on this platform");
-    memcpy(c->h_reqs, reqs, (size_t)R * sizeof(lig_req));
+    memcpy(c->h_reqs, in, (size_t)R * rq.in_bytes());
   }
   std::lock_guard<std::mutex> fk(c->fb_mu);
   CUDA_TRY(cudaSetDevice(c->device));
-  if (int rc = chain_admit(c, "lig_schedule_batch_feedback_chain")) return rc;
+  if (int rc = chain_admit(c, fn)) return rc;
   int32_t* dev_loads = loads ? mapped_device_pointer(loads) : nullptr;
   const bool loads_bounce = loads && !dev_loads;
   if (loads_bounce && !(dev_loads = mapped_device_pointer(c->h_fb_loads)))
     return fail(LIG_ERR_CUDA, "pinned staging buffers are not device-mapped on this platform");
-  if (int rc = chain_call(c, epoch, seed, dev_in, R, dev_out, window, dev_loads, c->s_fb)) return rc;
+  if (int rc = chain_call(c, epoch, seed, rq, R, window, dev_loads, c->s_fb)) return rc;
   const cudaError_t e = cudaStreamSynchronize(c->s_fb);
   if (e != cudaSuccess) {
     c->chain_live = false;
     return fail(LIG_ERR_CUDA, "feedback chain call failed on the device: %s", cudaGetErrorString(e));
   }
-  if (bounce) memcpy(out, c->h_out, (size_t)R * sizeof(lig_pick));
+  if (bounce) memcpy(out, c->h_out, (size_t)R * rq.out_bytes());
   if (loads_bounce && c->fb_scratch.P > 0)
     memcpy(loads, c->h_fb_loads, (size_t)c->fb_scratch.P * sizeof(int32_t));
   return 0;
+}
+
+static FbReqs descriptor_reqs(const lig_req* in, lig_pick* out) {
+  FbReqs rq;
+  rq.in = in;
+  rq.out = out;
+  return rq;
+}
+
+static FbReqs model_reqs(const uint32_t* ids, lig_mpick* out, uint64_t first_index) {
+  FbReqs rq;
+  rq.in = ids;
+  rq.out = out;
+  rq.models = true;
+  rq.first_index = first_index;
+  return rq;
+}
+
+int lig_schedule_batch_feedback_chain_device(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* d_reqs,
+                                             int R, lig_pick* d_out, int window, int32_t* d_loads, void* stream) {
+  return chain_device(c, "lig_schedule_batch_feedback_chain_device", epoch, seed, descriptor_reqs(d_reqs, d_out), R,
+                      window, d_loads, stream);
+}
+
+int lig_schedule_batch_feedback_chain(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
+                                      lig_pick* out, int window, int32_t* loads) {
+  return chain_host(c, "lig_schedule_batch_feedback_chain", epoch, seed, descriptor_reqs(reqs, out), R, window,
+                    loads);
+}
+
+int lig_schedule_models_batch_feedback_chain_device(lig_ctx* c, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                                                    const uint32_t* d_ids, int R, lig_mpick* d_out, int window,
+                                                    int32_t* d_loads, void* stream) {
+  return chain_device(c, "lig_schedule_models_batch_feedback_chain_device", epoch, seed,
+                      model_reqs(d_ids, d_out, first_index), R, window, d_loads, stream);
+}
+
+int lig_schedule_models_batch_feedback_chain(lig_ctx* c, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                                             const uint32_t* ids, int R, lig_mpick* out, int window,
+                                             int32_t* loads) {
+  return chain_host(c, "lig_schedule_models_batch_feedback_chain", epoch, seed, model_reqs(ids, out, first_index), R,
+                    window, loads);
 }
 
 int lig_feedback_chain_reset(lig_ctx* c) {

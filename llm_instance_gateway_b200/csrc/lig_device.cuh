@@ -2195,13 +2195,20 @@ __global__ void lig_apply_feedback_kernel(int* __restrict__ q, int* __restrict__
   hist_window[p] = 0;
 }
 
+// Adds one pick per lane to the open window's histogram.  A herd puts most picks of a warp on a
+// few pods, so the count is warp-aggregated: lanes that picked the same pod find each other with
+// __match_any_sync and the lowest of them adds the group's size with one atomic; pod -1 (DROP,
+// EMPTY, NO_MODEL, NO_PODS_LEFT, or a lane past the end) adds nothing.  Every lane of the warp
+// must call it.
+__device__ __forceinline__ void count_window_picks(int pod, int lane, int* __restrict__ hist) {
+  const unsigned same = __match_any_sync(kFull, pod);
+  if (pod >= 0 && lane == __ffs(same) - 1) atomicAdd(hist + pod, __popc(same));
+}
+
 // The pick of lig_pick_stream_kernel (same pick_one, so the picks are byte-identical) that also
 // counts the picks per pod into the open window's histogram, for the load-feedback chain
-// (lig_schedule_batch_feedback_chain).  `reqs` / `out` may be mapped host memory.  A herd puts
-// most picks of a warp on a few pods, so the count is warp-aggregated: lanes that picked the same
-// pod find each other with __match_any_sync and the lowest of them adds the group's size with one
-// atomic; pod -1 (DROP, EMPTY, NO_PODS_LEFT) adds nothing.  Every lane of a CTA runs every round,
-// ragged ones with pod -1, so the full-warp match is always legal.
+// (lig_schedule_batch_feedback_chain).  `reqs` / `out` may be mapped host memory.  Every lane of
+// a CTA runs every round, ragged ones with pod -1, so the full-warp match is always legal.
 constexpr int kCountPerThread = 4;
 __global__ void __launch_bounds__(kPickThreads, 8)
 lig_pick_count_kernel(const int4* __restrict__ reqs, int2* __restrict__ out, int R,
@@ -2224,8 +2231,42 @@ lig_pick_count_kernel(const int4* __restrict__ reqs, int2* __restrict__ out, int
       st_stream_int2(out + i, p);
       pod = p.x;
     }
-    const unsigned same = __match_any_sync(kFull, pod);
-    if (pod >= 0 && lane == __ffs(same) - 1) atomicAdd(hist + pod, __popc(same));
+    count_window_picks(pod, lane, hist);
+  }
+}
+
+// The same for model-id requests (lig_schedule_models_batch_feedback_chain): request i has
+// rand_key = first_index + i and goes through pick_model<false>, so the picks are byte-identical
+// to lig_pick_models_stream_kernel on the same tables.  `ids` / `out` may be mapped host memory;
+// the model table is a resident epoch's, the class tables are the chain's private copy.  The pod
+// is the 16-bit field of the packed pick (0xffff = -1: pods stay below LIG_MAX_PODS = 32768).
+__global__ void __launch_bounds__(kPickThreads, 8)
+lig_pick_models_count_kernel(const uint32_t* __restrict__ ids, uint32_t* __restrict__ out, int R,
+                             const uint4* __restrict__ cls, const uint16_t* __restrict__ lists, int A,
+                             const unsigned char* __restrict__ mtab, uint32_t n_models, uint64_t seed,
+                             uint64_t first_index, int* __restrict__ hist) {
+  ModelTables mt;
+  mt.entries = reinterpret_cast<const uint4*>(mtab + sizeof(ModelHeader));
+  mt.targets = reinterpret_cast<const uint2*>(mt.entries + n_models);
+  mt.n_models = n_models;
+  const int first = blockIdx.x * (kPickThreads * kCountPerThread) + threadIdx.x;
+  const int lane = threadIdx.x & 31;
+  uint32_t m[kCountPerThread];
+#pragma unroll
+  for (int j = 0; j < kCountPerThread; ++j) {      // every load in flight before the first use
+    const int i = first + j * kPickThreads;
+    m[j] = i < R ? __ldg(ids + i) : 0u;
+  }
+#pragma unroll
+  for (int j = 0; j < kCountPerThread; ++j) {
+    const int i = first + j * kPickThreads;
+    int pod = -1;
+    if (i < R) {
+      const uint32_t v = pick_model<false>(m[j], first_index + (uint64_t)i, mt, cls, lists, (uint32_t)A, seed);
+      out[i] = v;
+      pod = (int)(int16_t)(v & 0xffffu);
+    }
+    count_window_picks(pod, lane, hist);
   }
 }
 

@@ -177,6 +177,39 @@ class Engine:
                                                                    d_out or None, window, d_loads or None,
                                                                    stream or None))
 
+    def schedule_models_batch_feedback_chain(self, epoch: int, seed: int, model_ids: np.ndarray, window: int,
+                                             first_index: int = 0, loads=False,
+                                             out: Optional[np.ndarray] = None):
+        """Model-id requests in the feedback chain: one more chain call, in the same sequence and
+        windows as schedule_batch_feedback_chain, resolved against the epoch's resident model table
+        (rand_key of request i = first_index + i).  `loads` (an int32[P] array, or False) receives
+        the picks per pod since the chain began."""
+        assert model_ids.dtype == np.uint32 and model_ids.flags.c_contiguous
+        R = int(model_ids.shape[0])
+        if out is None:
+            out = np.empty(R, dtype=MPICK_DTYPE)
+        if loads is False or loads is None:
+            loads = None
+        else:
+            assert loads.dtype == np.int32 and loads.flags.c_contiguous
+        N.check(self._lib.lig_schedule_models_batch_feedback_chain(self._ctx, epoch, seed, first_index, _ptr(model_ids),
+                                                                   R, _ptr(out), window,
+                                                                   _ptr(loads) if loads is not None else None))
+        return out
+
+    def schedule_models_batch_feedback_chain_ptr(self, epoch: int, seed: int, first_index: int, h_ids: int, R: int,
+                                                 h_out: int, window: int, h_loads: int = 0) -> None:
+        N.check(self._lib.lig_schedule_models_batch_feedback_chain(self._ctx, epoch, seed, first_index, h_ids, R,
+                                                                   h_out, window, h_loads or None))
+
+    def schedule_models_batch_feedback_chain_device(self, epoch: int, seed: int, first_index: int, d_ids: int, R: int,
+                                                    d_out: int, window: int, d_loads: int = 0,
+                                                    stream: int = 0) -> None:
+        """The model-id chain call with device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_models_batch_feedback_chain_device(self._ctx, epoch, seed, first_index,
+                                                                          d_ids or None, R, d_out or None, window,
+                                                                          d_loads or None, stream or None))
+
     def feedback_chain_reset(self) -> None:
         """The next feedback-chain call starts a new chain from its epoch's scrape."""
         N.check(self._lib.lig_feedback_chain_reset(self._ctx))
