@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define LIG_ABI_VERSION 5
+#define LIG_ABI_VERSION 6
 
 /* ---- per-request status (lig_pick.status) ------------------------------------------------------
  * LIG_OK    Schedule returned a pod, nil                      pkg/ext-proc/scheduling/scheduler.go:120-121
@@ -289,11 +289,15 @@ int lig_schedule_batches_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed,
  * launch, no stream synchronisation (Scheduler.Schedule under a sustained request stream,
  * handlers/request.go:72).  Same results as lig_schedule_batch for the same (epoch, seed, reqs).
  * While a stream is open nothing in the process may synchronise the whole device
- * (cudaDeviceSynchronize, cudaFree): the resident kernel never finishes until lig_stream_close. */
+ * (cudaDeviceSynchronize, cudaFree): the resident kernel never finishes until lig_stream_close.
+ * A submit holds the ctx's upload lock for its whole round trip, and every snapshot and model
+ * upload takes that lock: no table the resident kernel reads can be overwritten during a submit,
+ * and submits of one ctx run one at a time. */
 int lig_stream_capacity(void);
 int lig_stream_open(lig_ctx* ctx);
 int lig_stream_submit(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* reqs, int n,
                       lig_pick* out);
+/* (lig_stream_submit_models, the model-id form, is declared with the model entry points below.) */
 int lig_stream_close(lig_ctx* ctx);
 
 /* Direct scan: every request walks the whole tree over all P pods itself (one warp per request,
@@ -368,6 +372,23 @@ int lig_schedule_models_batches_device(lig_ctx* ctx, uint64_t epoch, uint64_t se
  * and target index in `out`. */
 int lig_resolve_models(lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64_t first_index,
                        const uint32_t* model_ids, int R, lig_req* reqs_out, lig_mpick* out);
+/* The doorbell round trip (lig_stream_open / lig_stream_submit) for model-id requests: up to
+ * lig_stream_capacity() 4-byte ids in, as many 4-byte lig_mpicks out, byte for byte those of
+ * lig_schedule_models_batch(ctx, epoch, seed, first_index, model_ids, n) (rand_key = first_index + i),
+ * with the same contract as lig_stream_submit: it blocks, and one round trip of either kind runs
+ * at a time.  Resolved against the model table of `epoch` as it stands at the call; it waits for
+ * an enqueued upload of that table (lig_upload_models_async) as lig_stream_submit waits for the
+ * class tables.  The submit holds the ctx's upload lock for its whole round trip and every model
+ * upload takes that lock, so the table cannot be overwritten while the resident kernel reads it.
+ * Model tables may be uploaded before or after lig_stream_open.  An upload that has to allocate
+ * the slot's table (the first one for the slot, or one larger than the allocation, which is twice
+ * the table that caused it) stops the resident kernel, reallocates and relaunches it: the stream
+ * stays open, and no round trip is in flight meanwhile.
+ * LIG_ERR_NO_SNAPSHOT when `epoch` has no model table, LIG_ERR_STALE_EPOCH when it is not
+ * resident, LIG_ERR_INVALID before lig_stream_open, for n outside [0, capacity] or a null buffer.
+ * Submits of both kinds may alternate on one open stream. */
+int lig_stream_submit_models(lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                             const uint32_t* model_ids, int n, lig_mpick* out);
 
 /* ---- in-batch load feedback (opt-in; the default path never mutates the snapshot) ----------------
  * The reference schedules every request against the scraped metrics as they are

@@ -16,7 +16,7 @@ LIG_DRAW_DOMAIN = 0xA0761D6478BD642F
 LIG_ERR_INVALID, LIG_ERR_CUDA, LIG_ERR_STALE_EPOCH, LIG_ERR_NO_SNAPSHOT, LIG_ERR_RANGE = -1, -2, -3, -4, -5
 LIG_ERR_BUSY, LIG_ERR_NCCL = -6, -7
 LIG_MAX_TICKETS, LIG_COMM_ID_BYTES = 256, 128
-LIG_ABI_VERSION = 5
+LIG_ABI_VERSION = 6
 # filter node kinds of a caller filter tree (lig_set_filter_tree)
 (LIG_F_CRITICAL_REQUEST, LIG_F_LOW_QUEUEING, LIG_F_LORA_AFFINITY, LIG_F_CAN_ACCEPT_NEW_LORA, LIG_F_LOW_LORA_COST,
  LIG_F_NO_QUEUE_AND_LOW_KV, LIG_F_LEAST_QUEUING, LIG_F_LEAST_KV_CACHE, LIG_F_DROP) = range(9)
@@ -42,6 +42,7 @@ EXPORTED_SYMBOLS = (
     "lig_upload_snapshot_async", "lig_upload_models_async", "lig_set_filter_tree", "lig_group_set_filter_tree",
     "lig_schedule_batch_feedback_chain", "lig_schedule_batch_feedback_chain_device", "lig_feedback_chain_reset",
     "lig_schedule_models_batch_feedback_chain", "lig_schedule_models_batch_feedback_chain_device",
+    "lig_stream_submit_models",
 )
 
 
@@ -116,6 +117,7 @@ def load() -> C.CDLL:
     lib.lig_host_free.restype = None
     lib.lig_stream_open.argtypes = [vp]
     lib.lig_stream_submit.argtypes = [vp, u64, u64, vp, i32, vp]
+    lib.lig_stream_submit_models.argtypes = [vp, u64, u64, u64, vp, i32, vp]
     lib.lig_stream_close.argtypes = [vp]
     lib.lig_schedule_batch_async.argtypes = [vp, u64, u64, vp, i32, vp, C.POINTER(i32)]
     lib.lig_schedule_wait.argtypes = [vp, i32]

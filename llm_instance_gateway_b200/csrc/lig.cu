@@ -1573,6 +1573,26 @@ int lig_schedule_scan(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* 
   return 0;
 }
 
+// Launch the resident doorbell kernel on a fresh mailbox (tickets restart at 1).  Called with mu held.
+static int doorbell_launch(lig_ctx* c) {
+  memset(c->mailbox, 0, offsetof(Mailbox, reqs));
+  c->next_ticket = 1;
+  std::atomic_thread_fence(std::memory_order_seq_cst);
+  lig_doorbell_kernel<<<1, kPickThreads, 0, c->s_doorbell>>>(c->d_mailbox);
+  CUDA_TRY(cudaGetLastError());
+  c->launches++;
+  c->stream_open = true;
+  return 0;
+}
+
+// Make the resident doorbell kernel leave and wait for it.  Called with mu held.
+static int doorbell_stop(lig_ctx* c) {
+  reinterpret_cast<std::atomic<uint32_t>*>(&c->mailbox->ticket)->store(kMailboxQuit, std::memory_order_release);
+  CUDA_TRY(cudaStreamSynchronize(c->s_doorbell));
+  c->stream_open = false;
+  return 0;
+}
+
 static int upload_models_impl(lig_ctx* c, uint64_t epoch, int n_models, const int32_t* off,
                               const int32_t* tgt_ids, const int32_t* tgt_w, const uint8_t* critical,
                               const int32_t* self_ids, const uint8_t* present, bool synchronise) {
@@ -1632,8 +1652,14 @@ static int upload_models_impl(lig_ctx* c, uint64_t epoch, int n_models, const in
     if (int rc = wait_readers(*s, c->s_up)) return rc;      // batches still reading the old table
   }
   if (bytes > s->mtab_capacity) {
-    if (c->stream_open)
-      return fail(LIG_ERR_INVALID, "cannot grow the model table while a doorbell stream is open");
+    // cudaFree waits for every kernel on the device, the resident doorbell kernel included.  No
+    // doorbell round trip is in flight (submits hold upload_mu too), so an open stream is stopped
+    // around the reallocation and relaunched: to its callers it stays open.  mu keeps
+    // lig_stream_open / lig_stream_close out meanwhile.
+    std::lock_guard<std::mutex> lk(c->mu);
+    const bool restart = c->stream_open;
+    if (restart)
+      if (int rc = doorbell_stop(c)) return rc;
     CUDA_TRY(cudaStreamSynchronize(c->s_up));                 // the readers are done: safe to free
     cudaFree(s->d_mtab);
     if (s->h_mtab) cudaFreeHost(s->h_mtab);
@@ -1644,6 +1670,8 @@ static int upload_models_impl(lig_ctx* c, uint64_t epoch, int n_models, const in
     CUDA_TRY(cudaMalloc(&s->d_mtab, cap));
     CUDA_TRY(cudaHostAlloc(&s->h_mtab, cap, cudaHostAllocDefault));
     s->mtab_capacity = cap;
+    if (restart)
+      if (int rc = doorbell_launch(c)) return rc;
   }
   CUDA_TRY(cudaEventSynchronize(s->models_ready));   // an earlier _async upload may still read the staging copy
   memset(s->h_mtab, 0, bytes);
@@ -2216,14 +2244,7 @@ int lig_stream_open(lig_ctx* c) {
     CUDA_TRY(cudaHostGetDevicePointer(reinterpret_cast<void**>(&c->d_mailbox), c->mailbox, 0));
     CUDA_TRY(cudaStreamCreateWithFlags(&c->s_doorbell, cudaStreamNonBlocking));
   }
-  memset(c->mailbox, 0, offsetof(Mailbox, reqs));
-  c->next_ticket = 1;
-  std::atomic_thread_fence(std::memory_order_seq_cst);
-  lig_doorbell_kernel<<<1, kPickThreads, 0, c->s_doorbell>>>(c->d_mailbox);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  c->stream_open = true;
-  return 0;
+  return doorbell_launch(c);
 }
 
 int lig_stream_close(lig_ctx* c) {
@@ -2231,9 +2252,26 @@ int lig_stream_close(lig_ctx* c) {
   std::lock_guard<std::mutex> lk(c->mu);
   if (!c->stream_open) return 0;
   CUDA_TRY(cudaSetDevice(c->device));
-  reinterpret_cast<std::atomic<uint32_t>*>(&c->mailbox->ticket)->store(kMailboxQuit, std::memory_order_release);
-  CUDA_TRY(cudaStreamSynchronize(c->s_doorbell));
-  c->stream_open = false;
+  return doorbell_stop(c);
+}
+
+// Ring the doorbell for the micro-batch the caller wrote into the mailbox and spin until the
+// resident kernel has answered.  Called with upload_mu and mu held.
+static int doorbell_round_trip(lig_ctx* c) {
+  Mailbox* mb = c->mailbox;
+  const uint32_t ticket = c->next_ticket++;
+  reinterpret_cast<std::atomic<uint32_t>*>(&mb->ticket)->store(ticket, std::memory_order_release);
+  auto* done = reinterpret_cast<std::atomic<uint32_t>*>(&mb->done);
+  uint64_t spins = 0;
+  while (done->load(std::memory_order_acquire) != ticket) {
+#if defined(__x86_64__)
+    __builtin_ia32_pause();
+#endif
+    if ((++spins & 0xfffff) == 0 && cudaStreamQuery(c->s_doorbell) != cudaErrorNotReady) {
+      c->stream_open = false;   // the resident kernel is gone (error or device reset)
+      return fail(LIG_ERR_CUDA, "doorbell kernel is not running: %s", cudaGetErrorString(cudaGetLastError()));
+    }
+  }
   return 0;
 }
 
@@ -2259,24 +2297,45 @@ int lig_stream_submit(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* 
   memcpy(mb->reqs, reqs, (size_t)n * sizeof(lig_req));
   mb->count = (uint32_t)n;
   mb->A = (uint32_t)s->A;
-  mb->reserved0 = 0;
+  mb->mode = kMailboxDescriptors;
   mb->seed = seed;
   mb->cls = reinterpret_cast<const uint4*>(s->d_cls);
   mb->lists = s->d_lists;
-  const uint32_t ticket = c->next_ticket++;
-  reinterpret_cast<std::atomic<uint32_t>*>(&mb->ticket)->store(ticket, std::memory_order_release);
-  auto* done = reinterpret_cast<std::atomic<uint32_t>*>(&mb->done);
-  uint64_t spins = 0;
-  while (done->load(std::memory_order_acquire) != ticket) {
-#if defined(__x86_64__)
-    __builtin_ia32_pause();
-#endif
-    if ((++spins & 0xfffff) == 0 && cudaStreamQuery(c->s_doorbell) != cudaErrorNotReady) {
-      c->stream_open = false;   // the resident kernel is gone (error or device reset)
-      return fail(LIG_ERR_CUDA, "doorbell kernel is not running: %s", cudaGetErrorString(cudaGetLastError()));
-    }
-  }
+  if (int rc = doorbell_round_trip(c)) return rc;
   memcpy(out, mb->picks, (size_t)n * sizeof(lig_pick));
+  return 0;
+}
+
+int lig_stream_submit_models(lig_ctx* c, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                             const uint32_t* ids, int n, lig_mpick* out) {
+  if (!c || n < 0 || (n > 0 && (!ids || !out)))
+    return fail(LIG_ERR_INVALID, "lig_stream_submit_models: bad argument");
+  if (n > kMailboxCapacity)
+    return fail(LIG_ERR_INVALID, "n=%d exceeds the doorbell capacity %d", n, kMailboxCapacity);
+  // upload_mu for the whole round trip, as above: lig_upload_models takes it too, so the model
+  // table cannot be rewritten while the resident kernel reads it
+  std::lock_guard<std::mutex> uk(c->upload_mu);
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (!c->stream_open) return fail(LIG_ERR_INVALID, "lig_stream_submit_models: call lig_stream_open first");
+  Slot* s = nullptr;
+  if (int rc = resolve_models_slot(c, epoch, &s)) return rc;
+  if (n == 0) return 0;
+  CUDA_TRY(cudaSetDevice(c->device));
+  CUDA_TRY(cudaEventSynchronize(s->ready));
+  CUDA_TRY(cudaEventSynchronize(s->models_ready));   // an _async model upload may still be in flight
+  Mailbox* mb = c->mailbox;
+  memcpy(mb->reqs, ids, (size_t)n * sizeof(uint32_t));
+  mb->count = (uint32_t)n;
+  mb->A = (uint32_t)s->A;
+  mb->mode = kMailboxModels;
+  mb->seed = seed;
+  mb->cls = reinterpret_cast<const uint4*>(s->d_cls);
+  mb->lists = s->d_lists;
+  mb->mtab = s->d_mtab;
+  mb->first_index = first_index;
+  mb->n_models = s->n_models;
+  if (int rc = doorbell_round_trip(c)) return rc;
+  memcpy(out, mb->picks, (size_t)n * sizeof(lig_mpick));
   return 0;
 }
 

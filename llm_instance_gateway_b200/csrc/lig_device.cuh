@@ -1929,9 +1929,58 @@ __device__ __forceinline__ uint32_t pack_mpick(int pod, uint32_t status, uint32_
   return ((uint32_t)pod & 0xffffu) | (status << 16) | (target << 24);
 }
 
+// L2-only loads (ld.global.cg): for a kernel that outlives uploads (the doorbell kernel), whose
+// L1 is not coherent with the copies that rewrite the tables it reads.
+__device__ __forceinline__ uint4 ld_cg_uint4(const uint4* p) {
+  uint4 r;
+  asm volatile("ld.global.cg.v4.u32 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
+  return r;
+}
+__device__ __forceinline__ uint2 ld_cg_uint2(const uint2* p) {
+  uint2 r;
+  asm volatile("ld.global.cg.v2.u32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
+  return r;
+}
+__device__ __forceinline__ uint32_t ld_cg_u16(const uint16_t* p) {
+  uint16_t r;
+  asm volatile("ld.global.cg.u16 %0, [%1];" : "=h"(r) : "l"(p));
+  return r;
+}
+
+// pick_one with L2-only loads of the class tables (see ld_cg_uint4).
+__device__ __forceinline__ int2 doorbell_pick(const int4 r, const uint4* cls, const uint16_t* lists,
+                                              uint32_t A, uint64_t seed) {
+  const uint32_t critical = (uint32_t)r.y & LIG_REQ_CRITICAL;
+  const uint64_t key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
+  const uint32_t a = min((uint32_t)r.x, A);
+  const uint32_t c = critical * (A + 1u) + a;
+  const uint4 e = ld_cg_uint4(cls + c);
+  const uint32_t k = int31n_entry(seed ^ key, e);
+  const int pod = (int)(short)ld_cg_u16(lists + (e.w + k));
+  return make_int2(pod, (int)(e.x & 0xffff0007u));
+}
+
+// How the model helpers below load the model table and the class tables: from shared memory
+// (the persistent kernel's copies), through the read-only path (__ldg), or L2 only (the doorbell).
+enum class Ld { kSmem, kLdg, kL2 };
+
+template <Ld L>
+__device__ __forceinline__ uint4 ld_model_entry(const uint4* p) {
+  if constexpr (L == Ld::kSmem) return *p;
+  else if constexpr (L == Ld::kLdg) return __ldg(p);
+  else return ld_cg_uint4(p);
+}
+template <Ld L>
+__device__ __forceinline__ uint2 ld_model_target(const uint2* p) {
+  if constexpr (L == Ld::kSmem) return *p;
+  else if constexpr (L == Ld::kLdg) return __ldg(p);
+  else return ld_cg_uint2(p);
+}
+
 // The weighted draw of a model with >= 2 targets (entry e): randomVal = r.Int31n(total), then the
 // first k with randomVal < cum[k]                                                datastore.go:81-97
-template <bool kSmem>
+template <Ld L>
 __device__ __forceinline__ void draw_target(const uint4 e, const ModelTables& mt, uint64_t seed, uint64_t key,
                                             uint32_t* adapter, uint32_t* target) {
   const uint32_t nt = e.x & 0xffu;
@@ -1946,22 +1995,22 @@ __device__ __forceinline__ void draw_target(const uint4 e, const ModelTables& mt
   }
   const uint32_t r = total > 1u ? v - q * total : 0u;
   uint32_t k = 0;
-  uint2 tr = kSmem ? mt.targets[e.w] : __ldg(mt.targets + e.w);
+  uint2 tr = ld_model_target<L>(mt.targets + e.w);
   while (k + 1u < nt && r >= tr.y) {   // first k with randomVal < cum[k]       datastore.go:91-97
     ++k;
-    tr = kSmem ? mt.targets[e.w + k] : __ldg(mt.targets + e.w + k);
+    tr = ld_model_target<L>(mt.targets + e.w + k);
   }
   *adapter = tr.x;
   *target = k;
 }
 
 // resolve: model id -> (adapter, critical, target index); false = LIG_NO_MODEL.
-template <bool kSmem>
+template <Ld L>
 __device__ __forceinline__ bool resolve_model(uint32_t m, const ModelTables& mt, uint64_t seed, uint64_t key,
                                               uint32_t* adapter, uint32_t* critical, uint32_t* target) {
   *adapter = 0xffffffffu; *critical = 0; *target = 255u;
   if (m >= mt.n_models) return false;
-  const uint4 e = kSmem ? mt.entries[m] : __ldg(mt.entries + m);
+  const uint4 e = ld_model_entry<L>(mt.entries + m);
   if (!(e.x & kModelPresent)) return false;
   *critical = (e.x >> 8) & 1u;
   const uint32_t nt = e.x & 0xffu;
@@ -1970,20 +2019,23 @@ __device__ __forceinline__ bool resolve_model(uint32_t m, const ModelTables& mt,
     *target = nt ? 0u : 255u;
     return true;
   }
-  draw_target<kSmem>(e, mt, seed, key, adapter, target);
+  draw_target<L>(e, mt, seed, key, adapter, target);
   return true;
 }
 
-// One model request end to end; the class lookup as in pick_one / pick_one_smem.
-template <bool kSmem>
+// One model request end to end; the class lookup as in pick_one / pick_one_smem / doorbell_pick.
+template <Ld L>
 __device__ __forceinline__ uint32_t pick_model(uint32_t m, uint64_t key, const ModelTables& mt,
                                                const uint4* cls, const uint16_t* lists, uint32_t A,
                                                uint64_t seed) {
   uint32_t adapter, critical, target;
-  if (!resolve_model<kSmem>(m, mt, seed, key, &adapter, &critical, &target))
+  if (!resolve_model<L>(m, mt, seed, key, &adapter, &critical, &target))
     return pack_mpick(-1, (uint32_t)LIG_NO_MODEL, 255u);
   const int4 r = make_int4((int)adapter, (int)critical, (int)(uint32_t)key, (int)(uint32_t)(key >> 32));
-  const int2 p = kSmem ? pick_one_smem(r, cls, lists, A, seed) : pick_one(r, cls, lists, A, seed);
+  int2 p;
+  if constexpr (L == Ld::kSmem) p = pick_one_smem(r, cls, lists, A, seed);
+  else if constexpr (L == Ld::kLdg) p = pick_one(r, cls, lists, A, seed);
+  else p = doorbell_pick(r, cls, lists, A, seed);
   return pack_mpick(p.x, (uint32_t)p.y & 7u, target);
 }
 
@@ -2103,13 +2155,14 @@ lig_pick_models_kernel(const __grid_constant__ MQueueParams qp, const uint4* __r
     // split traffic), so instead of a divergent branch inside each of the 4 requests every lane
     // works off its OWN pending requests — the warp runs the draw max-over-lanes(pending) times
     // (1-2) rather than 4.  (3) the 4 picks.
+    constexpr Ld kMtLd = kTabSmem ? Ld::kSmem : Ld::kLdg;
     const uint32_t m[4] = {ids.x, ids.y, ids.z, ids.w};
     uint32_t adapter[4], tgt[4];
     uint32_t crit = 0, okm = 0, pending = 0;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const bool in_range = m[j] < mt.n_models;
-      const uint4 e = in_range ? (kTabSmem ? mt.entries[m[j]] : __ldg(mt.entries + m[j])) : make_uint4(0, 0, 0, 0);
+      const uint4 e = in_range ? ld_model_entry<kMtLd>(mt.entries + m[j]) : make_uint4(0, 0, 0, 0);
       const uint32_t nt = e.x & 0xffu;
       const bool ok = (e.x & kModelPresent) != 0;
       okm |= (ok ? 1u : 0u) << j;
@@ -2122,9 +2175,9 @@ lig_pick_models_kernel(const __grid_constant__ MQueueParams qp, const uint4* __r
       const int j = __ffs((int)pending) - 1;
       pending &= pending - 1u;
       const uint32_t mj = j == 0 ? m[0] : j == 1 ? m[1] : j == 2 ? m[2] : m[3];
-      const uint4 e = kTabSmem ? mt.entries[mj] : __ldg(mt.entries + mj);
+      const uint4 e = ld_model_entry<kMtLd>(mt.entries + mj);
       uint32_t a, k;
-      draw_target<kTabSmem>(e, mt, it.seed, key0 + (uint64_t)j, &a, &k);
+      draw_target<kMtLd>(e, mt, it.seed, key0 + (uint64_t)j, &a, &k);
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj)
         if (jj == j) { adapter[jj] = a; tgt[jj] = k; }
@@ -2172,11 +2225,11 @@ lig_pick_models_stream_kernel(const uint32_t* __restrict__ ids, uint32_t* __rest
     const uint64_t key = first_index + (uint64_t)i;
     if (reqs_out) {
       uint32_t adapter, critical, target;
-      const bool ok = resolve_model<false>(m, mt, seed, key, &adapter, &critical, &target);
+      const bool ok = resolve_model<Ld::kLdg>(m, mt, seed, key, &adapter, &critical, &target);
       reqs_out[i] = make_int4((int)adapter, (int)critical, (int)(uint32_t)key, (int)(uint32_t)(key >> 32));
       out[i] = pack_mpick(-1, ok ? (uint32_t)LIG_OK : (uint32_t)LIG_NO_MODEL, target);
     } else {
-      out[i] = pick_model<false>(m, key, mt, cls, lists, (uint32_t)A, seed);
+      out[i] = pick_model<Ld::kLdg>(m, key, mt, cls, lists, (uint32_t)A, seed);
     }
   }
 }
@@ -2236,7 +2289,7 @@ lig_pick_count_kernel(const int4* __restrict__ reqs, int2* __restrict__ out, int
 }
 
 // The same for model-id requests (lig_schedule_models_batch_feedback_chain): request i has
-// rand_key = first_index + i and goes through pick_model<false>, so the picks are byte-identical
+// rand_key = first_index + i and goes through pick_model<Ld::kLdg>, so the picks are byte-identical
 // to lig_pick_models_stream_kernel on the same tables.  `ids` / `out` may be mapped host memory;
 // the model table is a resident epoch's, the class tables are the chain's private copy.  The pod
 // is the 16-bit field of the packed pick (0xffff = -1: pods stay below LIG_MAX_PODS = 32768).
@@ -2262,7 +2315,7 @@ lig_pick_models_count_kernel(const uint32_t* __restrict__ ids, uint32_t* __restr
     const int i = first + j * kPickThreads;
     int pod = -1;
     if (i < R) {
-      const uint32_t v = pick_model<false>(m[j], first_index + (uint64_t)i, mt, cls, lists, (uint32_t)A, seed);
+      const uint32_t v = pick_model<Ld::kLdg>(m[j], first_index + (uint64_t)i, mt, cls, lists, (uint32_t)A, seed);
       out[i] = v;
       pod = (int)(int16_t)(v & 0xffffu);
     }
@@ -2281,27 +2334,39 @@ __global__ void lig_feedback_loads_kernel(const int* __restrict__ total, const i
 // One resident CTA polls a mailbox in page-locked host memory.  The host writes the micro-batch
 // (header + descriptors), then the ticket; the CTA schedules it with the same pick_one() and
 // writes the picks and the completion ticket back to host memory.  No kernel launch and no stream
-// synchronisation per micro-batch: the round trip is two PCIe crossings.  Class tables are read
-// with ld.global.cg (L2 only): the kernel outlives snapshot uploads, and L1 is not coherent.
+// synchronisation per micro-batch: the round trip is two PCIe crossings.  Class tables and model
+// tables are read with ld.global.cg (L2 only): the kernel outlives snapshot and model uploads, and
+// L1 is not coherent.
+//
+// Model-id mode (mode == kMailboxModels, lig_stream_submit_models): `reqs` holds `count` 4-byte
+// model ids and `picks` receives `count` 4-byte lig_mpicks; each thread takes 4 consecutive ids,
+// one 16-byte load and one 16-byte store.  The mode's extra header fields (first_index, n_models)
+// sit in the last 16 bytes of the header, which the descriptor mode never reads.
 constexpr int kMailboxCapacity = 4096;   // requests per doorbell
 constexpr uint32_t kMailboxQuit = 0xffffffffu;
+constexpr uint32_t kMailboxDescriptors = 0, kMailboxModels = 1;
 
 struct alignas(64) Mailbox {
   // --- written by the host ---
   uint32_t ticket;            // doorbell: last field written (release); kMailboxQuit = leave the kernel
   uint32_t count;
   uint32_t A;
-  uint32_t reserved0;
+  uint32_t mode;              // kMailboxDescriptors / kMailboxModels
   uint64_t seed;
   const uint4* cls;           // device pointers of the snapshot slot to use
   const uint16_t* lists;
-  uint32_t pad0[6];
+  const unsigned char* mtab;  // model mode: the slot's model blob (ModelHeader first)
+  uint64_t first_index;       // model mode: rand_key of the first id
+  uint32_t n_models;          // model mode
+  uint32_t pad0;
   // --- written by the device ---
   alignas(64) uint32_t done;  // completion ticket (release)
   uint32_t pad1[15];
   alignas(64) lig_req reqs[kMailboxCapacity];
   alignas(64) lig_pick picks[kMailboxCapacity];
 };
+static_assert(offsetof(Mailbox, done) == 64, "the host-written header is one 64-byte line");
+static_assert(offsetof(Mailbox, first_index) == 48, "descriptor mode reads bytes 0-47 of the header only");
 
 __device__ __forceinline__ uint32_t ld_acquire_sys_u32(const uint32_t* p) {
   uint32_t v;
@@ -2317,30 +2382,6 @@ __device__ __forceinline__ int4 ld_sys_int4(const void* p) {
                : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p) : "memory");
   return r;
 }
-__device__ __forceinline__ uint4 ld_cg_uint4(const uint4* p) {
-  uint4 r;
-  asm volatile("ld.global.cg.v4.u32 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
-  return r;
-}
-__device__ __forceinline__ uint32_t ld_cg_u16(const uint16_t* p) {
-  uint16_t r;
-  asm volatile("ld.global.cg.u16 %0, [%1];" : "=h"(r) : "l"(p));
-  return r;
-}
-
-__device__ __forceinline__ int2 doorbell_pick(const int4 r, const uint4* cls, const uint16_t* lists,
-                                              uint32_t A, uint64_t seed) {
-  const uint32_t critical = (uint32_t)r.y & LIG_REQ_CRITICAL;
-  const uint64_t key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
-  const uint32_t a = min((uint32_t)r.x, A);
-  const uint32_t c = critical * (A + 1u) + a;
-  const uint4 e = ld_cg_uint4(cls + c);
-  const uint32_t k = int31n_entry(seed ^ key, e);
-  const int pod = (int)(short)ld_cg_u16(lists + (e.w + k));
-  return make_int2(pod, (int)(e.x & 0xffff0007u));
-}
-
 __global__ void __launch_bounds__(kPickThreads)
 lig_doorbell_kernel(Mailbox* mb) {
   __shared__ uint32_t s_go;
@@ -2359,20 +2400,53 @@ lig_doorbell_kernel(Mailbox* mb) {
     if (!s_go) return;
     // One PCIe round trip for everything a small micro-batch needs: the header (same 64-byte
     // line as the ticket) and this thread's first descriptor are requested together, the
-    // descriptor speculatively (the mailbox always holds kMailboxCapacity slots).
-    const int4 h0 = ld_sys_int4(&mb->ticket);          // ticket, count, A, -
+    // descriptor speculatively (the mailbox always holds kMailboxCapacity slots).  Every word of
+    // h0-h2 is used (mode in h0.w, mtab in h2.zw), so each stays one 16-byte sys load: when only
+    // some words were used, ptxas split them into 4- and 8-byte loads, one more PCIe read per
+    // round trip, ~10 us on H100 (DESIGN.md section 7).  Keep them whole when editing the header.
+    const int4 h0 = ld_sys_int4(&mb->ticket);          // ticket, count, A, mode
     const int4 h1 = ld_sys_int4(&mb->seed);            // seed lo/hi, cls lo/hi
-    const int4 h2 = ld_sys_int4(&mb->lists);           // lists lo/hi, pad
-    int4 r = ld_sys_int4(&mb->reqs[threadIdx.x]);
+    const int4 h2 = ld_sys_int4(&mb->lists);           // lists lo/hi, mtab lo/hi
+    int4 r = ld_sys_int4(&mb->reqs[threadIdx.x]);      // a descriptor, or 4 model ids
     const uint32_t count = (uint32_t)h0.y, A = (uint32_t)h0.z;
     const uint64_t seed = ((uint64_t)(uint32_t)h1.y << 32) | (uint32_t)h1.x;
     const uint4* cls = reinterpret_cast<const uint4*>(((uint64_t)(uint32_t)h1.w << 32) | (uint32_t)h1.z);
     const uint16_t* lists = reinterpret_cast<const uint16_t*>(((uint64_t)(uint32_t)h2.y << 32) | (uint32_t)h2.x);
-    for (uint32_t i = threadIdx.x; i < count; i += kPickThreads) {
-      if (i != threadIdx.x) r = ld_sys_int4(&mb->reqs[i]);
-      const int2 p = doorbell_pick(r, cls, lists, A, seed);
-      asm volatile("st.relaxed.sys.global.v2.s32 [%0], {%1, %2};"
-                   :: "l"(reinterpret_cast<int2*>(&mb->picks[i])), "r"(p.x), "r"(p.y) : "memory");
+    if ((uint32_t)h0.w == kMailboxModels) {
+      const int4 h3 = ld_sys_int4(&mb->first_index);   // first_index lo/hi, n_models, pad
+      const uint64_t first_index = ((uint64_t)(uint32_t)h3.y << 32) | (uint32_t)h3.x;
+      const unsigned char* mtab = reinterpret_cast<const unsigned char*>(((uint64_t)(uint32_t)h2.w << 32) | (uint32_t)h2.z);
+      ModelTables mt;
+      mt.n_models = (uint32_t)h3.z;
+      mt.entries = reinterpret_cast<const uint4*>(mtab + sizeof(ModelHeader));
+      mt.targets = reinterpret_cast<const uint2*>(mt.entries + mt.n_models);
+      uint32_t* out = reinterpret_cast<uint32_t*>(mb->picks);
+      for (uint32_t g = threadIdx.x; 4u * g < count; g += kPickThreads) {   // ids 4g .. 4g+3
+        if (g != threadIdx.x) r = ld_sys_int4(&mb->reqs[g]);
+        const uint32_t m[4] = {(uint32_t)r.x, (uint32_t)r.y, (uint32_t)r.z, (uint32_t)r.w};
+        uint32_t o[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const uint32_t i = 4u * g + (uint32_t)j;
+          o[j] = i < count ? pick_model<Ld::kL2>(m[j], first_index + i, mt, cls, lists, A, seed) : 0u;
+        }
+        if (4u * g + 4u <= count) {
+          asm volatile("st.relaxed.sys.global.v4.u32 [%0], {%1, %2, %3, %4};"
+                       :: "l"(out + 4u * g), "r"(o[0]), "r"(o[1]), "r"(o[2]), "r"(o[3]) : "memory");
+        } else {
+#pragma unroll
+          for (int j = 0; j < 3; ++j)
+            if (4u * g + (uint32_t)j < count)
+              asm volatile("st.relaxed.sys.global.u32 [%0], %1;" :: "l"(out + 4u * g + j), "r"(o[j]) : "memory");
+        }
+      }
+    } else {
+      for (uint32_t i = threadIdx.x; i < count; i += kPickThreads) {
+        if (i != threadIdx.x) r = ld_sys_int4(&mb->reqs[i]);
+        const int2 p = doorbell_pick(r, cls, lists, A, seed);
+        asm volatile("st.relaxed.sys.global.v2.s32 [%0], {%1, %2};"
+                     :: "l"(reinterpret_cast<int2*>(&mb->picks[i])), "r"(p.x), "r"(p.y) : "memory");
+      }
     }
     // the barrier orders every thread's pick stores before thread 0's release store (cumulative)
     __syncthreads();

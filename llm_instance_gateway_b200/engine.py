@@ -292,6 +292,14 @@ class Engine:
         N.check(self._lib.lig_stream_submit(self._ctx, epoch, seed, _ptr(reqs), len(reqs), _ptr(out)))
         return out
 
+    def stream_submit_models(self, epoch: int, seed: int, model_ids: np.ndarray, first_index: int = 0) -> np.ndarray:
+        """One doorbell round trip for model ids: the picks of schedule_models_batch, without a launch."""
+        assert model_ids.dtype == np.uint32 and model_ids.flags.c_contiguous
+        out = np.empty(len(model_ids), dtype=MPICK_DTYPE)
+        N.check(self._lib.lig_stream_submit_models(self._ctx, epoch, seed, first_index, _ptr(model_ids),
+                                                   len(model_ids), _ptr(out)))
+        return out
+
     def read_class(self, epoch: int, critical: bool, adapter_id: int, P: int):
         status, n = C.c_int(), C.c_int()
         lst = np.zeros(max(P, 1), dtype=np.uint16)
