@@ -29,14 +29,16 @@ type packedModels struct {
 	selfIDs    []int32           // the model's own name interned (TargetModels empty, request.go:47)
 	present    []uint8           // 0: requests for it get LIG_NO_MODEL
 	targets    [][]string        // per model: TargetModels names, to map target_idx back to a name
+	names      []string          // per model: the object's Name ("error getting target model name", request.go:49)
 }
 
 func packModels(models []*v1alpha1.InferenceModel, s *packedSnapshot) *packedModels {
 	n := len(models)
 	p := &packedModels{ids: make(map[string]uint32, n), offsets: make([]int32, n+1), critical: make([]uint8, n),
-		selfIDs: make([]int32, n), present: make([]uint8, n), targets: make([][]string, n)}
+		selfIDs: make([]int32, n), present: make([]uint8, n), targets: make([][]string, n), names: make([]string, n)}
 	for m, im := range models {
 		p.ids[im.Spec.ModelName] = uint32(m)
+		p.names[m] = im.Name
 		p.present[m] = 1
 		if im.Spec.Criticality != nil && *im.Spec.Criticality == v1alpha1.Critical { // datastore.go:100-105
 			p.critical[m] = 1
@@ -90,6 +92,13 @@ func (b *pinned) mpicks(n int) []C.lig_mpick   { return unsafe.Slice((*C.lig_mpi
 func (c *ctx) scheduleModels(epoch, seed, firstIndex uint64, in, out *pinned, n int) C.int {
 	return C.lig_schedule_models_batch(c.p, C.uint64_t(epoch), C.uint64_t(seed), C.uint64_t(firstIndex),
 		(*C.uint32_t)(in.ptr), C.int(n), (*C.lig_mpick)(out.ptr))
+}
+
+// scheduleModelsFeedbackChain is scheduleModels inside the load-feedback chain (Options.LoadFeedbackWindow):
+// model-id and descriptor requests share its windows.
+func (c *ctx) scheduleModelsFeedbackChain(epoch, seed, firstIndex uint64, in, out *pinned, n, window int) C.int {
+	return C.lig_schedule_models_batch_feedback_chain(c.p, C.uint64_t(epoch), C.uint64_t(seed), C.uint64_t(firstIndex),
+		(*C.uint32_t)(in.ptr), C.int(n), (*C.lig_mpick)(out.ptr), C.int(window), nil)
 }
 
 // group wraps lig_group: ONE scheduler per ext-proc process owning several GPUs (main.go:137); the

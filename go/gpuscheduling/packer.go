@@ -20,6 +20,7 @@ type packedSnapshot struct {
 	adapterIDs map[string]int32
 	pods       []backend.Pod
 	excluded   int // pods left out of this snapshot: a metric did not fit the device record
+	models     *packedModels // Options.InferenceModels interned against this epoch; nil: none
 }
 
 // packSnapshot interns adapter names (order of first appearance) and narrows the Go-width

@@ -8,6 +8,7 @@ import "C"
 import (
 	"fmt"
 	"math/rand"
+	"sort"
 	"sync"
 	"time"
 
@@ -15,6 +16,7 @@ import (
 	"google.golang.org/grpc/status"
 	klog "k8s.io/klog/v2"
 
+	"inference.networking.x-k8s.io/llm-instance-gateway/api/v1alpha1"
 	"inference.networking.x-k8s.io/llm-instance-gateway/pkg/ext-proc/backend"
 	"inference.networking.x-k8s.io/llm-instance-gateway/pkg/ext-proc/scheduling"
 )
@@ -42,6 +44,11 @@ type Options struct {
 	// uploads a new epoch.  The reference never writes pod metrics while scheduling
 	// (scheduler.go:113-122), so 0 (off) is the reference's behaviour.
 	LoadFeedbackWindow int
+	// InferenceModels is backend.K8sDatastore.InferenceModels (datastore.go:26-31: Spec.ModelName ->
+	// *v1alpha1.InferenceModel).  When set, every Refresh packs it into the new epoch's model table
+	// and ScheduleModel resolves requests on the device.  Deviation from the reference: a change of
+	// an InferenceModel applies from the next refresh tick, not from the next request.
+	InferenceModels *sync.Map
 }
 
 // FilterKind names the filter functions of filter.go / scheduler.go a FilterNode runs.
@@ -76,14 +83,18 @@ func DefaultOptions() Options {
 		KVCacheThreshold: 0.8, QueueThresholdCritical: 5, QueueingThresholdLoRA: 50}
 }
 
+// A waiter carries a descriptor request (req) or a model name (ScheduleModel).
 type waiter struct {
-	req  *scheduling.LLMRequest
-	done chan result
+	req     *scheduling.LLMRequest
+	model   string
+	modelID int64 // flush-time id in the captured epoch's table; -1: answered on the host
+	done    chan result
 }
 
 type result struct {
-	pod backend.Pod
-	err error
+	pod      backend.Pod
+	resolved string
+	err      error
 }
 
 // GPUScheduler implements handlers.Scheduler (pkg/ext-proc/handlers/server.go:37-39).  Swap it
@@ -99,6 +110,10 @@ type GPUScheduler struct {
 	out  *pinned
 	seed uint64
 	rng  *rand.Rand
+	// the model-id lane: ids in, lig_mpicks out, and the first_index of the next device call
+	inIDs      *pinned
+	outM       *pinned
+	firstIndex uint64
 
 	snapMu sync.RWMutex
 	snap   *packedSnapshot
@@ -140,7 +155,22 @@ func NewGPUScheduler(pmp scheduling.PodMetricsProvider, opt Options) (*GPUSchedu
 		c.close()
 		return nil, err
 	}
-	g := &GPUScheduler{pmp: pmp, opt: opt, c: c, in: in, out: out, seed: rand.Uint64(),
+	inIDs, err := allocPinned(opt.MaxBatch * 4)
+	if err != nil {
+		in.free()
+		out.free()
+		c.close()
+		return nil, err
+	}
+	outM, err := allocPinned(opt.MaxBatch * 4)
+	if err != nil {
+		inIDs.free()
+		in.free()
+		out.free()
+		c.close()
+		return nil, err
+	}
+	g := &GPUScheduler{pmp: pmp, opt: opt, c: c, in: in, out: out, inIDs: inIDs, outM: outM, seed: rand.Uint64(),
 		rng: rand.New(rand.NewSource(time.Now().UnixNano())), queue: make(chan *waiter, opt.MaxBatch), stop: make(chan struct{})}
 	if err := g.Refresh(); err != nil {
 		g.Close()
@@ -170,6 +200,8 @@ func (g *GPUScheduler) Close() {
 		}
 		g.in.free()
 		g.out.free()
+		g.inIDs.free()
+		g.outM.free()
 		g.c.close()
 	})
 }
@@ -189,8 +221,54 @@ func (g *GPUScheduler) Refresh() error {
 	if err := g.c.uploadSnapshot(s.epoch, s); err != nil {
 		return err
 	}
+	// The model table goes into the new epoch before the epoch is published: a flush that captures
+	// it maps names against the table the device reads.  Models the device would refuse are left out
+	// (and logged) before packing, so one bad InferenceModel cannot fail every refresh tick.
+	if g.opt.InferenceModels != nil {
+		s.models = packModels(uploadableModels(inferenceModels(g.opt.InferenceModels)), s)
+		if err := g.c.uploadModels(s.epoch, s.models); err != nil {
+			return err
+		}
+	}
 	g.snap = s
 	return nil
+}
+
+// uploadableModels drops, with a log line, the models lig_upload_models refuses with LIG_ERR_RANGE:
+// more than 255 targets, a negative weight, or weights summing above 2^31-1.  A model whose weights
+// sum to <= 0 stays: it is packed as absent.  Requests for a dropped model get "error finding a
+// model object"; valid CRDs (at most 10 targets, weights in [0, 1e6]) never hit this.
+func uploadableModels(models []*v1alpha1.InferenceModel) []*v1alpha1.InferenceModel {
+	out := models[:0:0]
+	for _, im := range models {
+		var sum int64
+		negative := false
+		for _, tm := range im.Spec.TargetModels {
+			sum += int64(tm.Weight)
+			negative = negative || tm.Weight < 0
+		}
+		if len(im.Spec.TargetModels) > 0 && sum > 0 && (len(im.Spec.TargetModels) > 255 || negative || sum > 1<<31-1) {
+			klog.Errorf("gpu scheduler: InferenceModel %s cannot be uploaded (%d targets, weights summing to %d); "+
+				"requests for it are rejected", im.Spec.ModelName, len(im.Spec.TargetModels), sum)
+			continue
+		}
+		out = append(out, im)
+	}
+	return out
+}
+
+// inferenceModels lists the datastore's models in ModelName order (model ids stay stable while the
+// set of names does).
+func inferenceModels(m *sync.Map) []*v1alpha1.InferenceModel {
+	var out []*v1alpha1.InferenceModel
+	m.Range(func(_, v any) bool {
+		if im, ok := v.(*v1alpha1.InferenceModel); ok && im != nil {
+			out = append(out, im)
+		}
+		return true
+	})
+	sort.Slice(out, func(i, j int) bool { return out[i].Spec.ModelName < out[j].Spec.ModelName })
+	return out
 }
 
 func (g *GPUScheduler) refresher() {
@@ -212,23 +290,43 @@ func (g *GPUScheduler) refresher() {
 // Schedule finds the target pod based on metrics and the requested lora adapter
 // (scheduler.go:113-122).  Goroutine-safe and blocking, like the reference's.
 func (g *GPUScheduler) Schedule(req *scheduling.LLMRequest) (backend.Pod, error) {
-	w := &waiter{req: req, done: make(chan result, 1)}
+	r := g.submit(&waiter{req: req, done: make(chan result, 1)})
+	return r.pod, r.err
+}
+
+// ScheduleModel is the resolve step of HandleRequestBody (request.go:42-56) and Schedule in one
+// call, resolved on the device against the model table of Options.InferenceModels.  It returns the
+// resolved target model (the body's "model" rewrite, request.go:60-69) and the pod.  An unknown
+// model, or one whose weights sum to <= 0, gets the reference's error and never reaches the device;
+// errors of the pick are wrapped as request.go:73-75 wraps them.  Without Options.InferenceModels
+// every model is unknown, so a handler calls it only when ResolvesModels reports true (patch 0004).
+// Unverified, like the rest of this package: it has never been compiled.
+func (g *GPUScheduler) ScheduleModel(model string) (string, backend.Pod, error) {
+	r := g.submit(&waiter{model: model, done: make(chan result, 1)})
+	return r.resolved, r.pod, r.err
+}
+
+// ResolvesModels reports whether ScheduleModel has a model table to resolve against
+// (Options.InferenceModels is set).  Without one, the handler keeps the reference's resolve step.
+func (g *GPUScheduler) ResolvesModels() bool { return g.opt.InferenceModels != nil }
+
+func (g *GPUScheduler) submit(w *waiter) result {
 	select {
 	case g.queue <- w:
 	case <-g.stop:
-		return backend.Pod{}, status.Error(codes.Unavailable, "gpu scheduler is shut down")
+		return result{err: status.Error(codes.Unavailable, "gpu scheduler is shut down")}
 	}
 	// A request that slipped into the queue while Close was draining it is answered by the
 	// second arm: stop is closed for good, so no waiter can block forever.
 	select {
 	case r := <-w.done:
-		return r.pod, r.err
+		return r
 	case <-g.stop:
 		select {
 		case r := <-w.done:
-			return r.pod, r.err
+			return r
 		case <-time.After(g.opt.BatchWindow + 10*time.Millisecond):
-			return backend.Pod{}, status.Error(codes.Unavailable, "gpu scheduler is shut down")
+			return result{err: status.Error(codes.Unavailable, "gpu scheduler is shut down")}
 		}
 	}
 }
@@ -259,7 +357,25 @@ func (g *GPUScheduler) batcher() {
 	}
 }
 
-func (g *GPUScheduler) flush(batch []*waiter) {
+// flush makes the descriptor call first, then the model-id call.
+func (g *GPUScheduler) flush(all []*waiter) {
+	var batch, models []*waiter
+	for _, w := range all {
+		if w.req != nil {
+			batch = append(batch, w)
+		} else {
+			models = append(models, w)
+		}
+	}
+	if len(batch) > 0 {
+		g.flushDescriptors(batch)
+	}
+	if len(models) > 0 {
+		g.flushModels(models)
+	}
+}
+
+func (g *GPUScheduler) flushDescriptors(batch []*waiter) {
 	n := len(batch)
 	var snap *packedSnapshot
 	var rc C.int
@@ -311,5 +427,85 @@ func (g *GPUScheduler) flush(batch []*waiter) {
 			var nilErr error
 			w.done <- result{err: fmt.Errorf("failed to apply filter, resulted %v pods, this should never happen: %w", 0, nilErr)}
 		}
+	}
+}
+
+// flushModels maps names to model ids against the captured epoch's table (again after a stale
+// epoch, with the same first index) and sends the ids the host cannot answer to the device.
+func (g *GPUScheduler) flushModels(batch []*waiter) {
+	var snap *packedSnapshot
+	var rc C.int
+	k := 0
+	for attempt := 0; attempt < 4; attempt++ {
+		g.snapMu.RLock()
+		snap = g.snap
+		g.snapMu.RUnlock()
+		ids := g.inIDs.modelIDs(len(batch))
+		k = 0
+		for _, w := range batch {
+			w.modelID = -1
+			if snap.models == nil {
+				continue
+			}
+			if id, ok := snap.models.ids[w.model]; ok && snap.models.present[id] != 0 {
+				w.modelID = int64(id)
+				ids[k] = C.uint32_t(id)
+				k++
+			}
+		}
+		if k == 0 {
+			break
+		}
+		if g.opt.LoadFeedbackWindow > 0 {
+			rc = g.c.scheduleModelsFeedbackChain(snap.epoch, g.seed, g.firstIndex, g.inIDs, g.outM, k, g.opt.LoadFeedbackWindow)
+		} else {
+			rc = g.c.scheduleModels(snap.epoch, g.seed, g.firstIndex, g.inIDs, g.outM, k)
+		}
+		if rc != C.LIG_ERR_STALE_EPOCH {
+			break
+		}
+	}
+	g.firstIndex += uint64(k)
+	picks := g.outM.mpicks(k)
+	j := 0
+	for _, w := range batch {
+		if w.modelID < 0 {
+			if snap.models != nil {
+				if id, ok := snap.models.ids[w.model]; ok { // request.go:48-51
+					w.done <- result{err: fmt.Errorf("error getting target model name for model %v", snap.models.names[id])}
+					continue
+				}
+			}
+			w.done <- result{err: fmt.Errorf("error finding a model object in InferenceModel for input %v", w.model)} // request.go:42-45
+			continue
+		}
+		pk := picks[j]
+		j++
+		if rc != 0 {
+			w.done <- result{err: fmt.Errorf("failed to find target pod: %w",
+				status.Errorf(codes.Internal, "gpu scheduler: %v", ligError("lig_schedule_models_batch", rc)))}
+			continue
+		}
+		resolved := w.model // 255: TargetModels is empty, the name passes through (request.go:47)
+		if pk.target_idx != 255 {
+			resolved = snap.models.targets[w.modelID][int(pk.target_idx)]
+		}
+		var err error
+		switch pk.status {
+		case C.LIG_OK:
+			w.done <- result{pod: snap.pods[int(pk.pod_idx)], resolved: resolved}
+			continue
+		case C.LIG_DROP:
+			inner := status.Errorf(codes.ResourceExhausted, "dropping request due to limited backend resources")
+			err = fmt.Errorf("failed to apply filter, resulted %v pods, this should never happen: %w", 0, inner)
+		case C.LIG_NO_PODS_LEFT:
+			err = fmt.Errorf("failed to apply filter, resulted %v pods, this should never happen: %w", 0, fmt.Errorf("no pods left"))
+		case C.LIG_EMPTY:
+			var nilErr error
+			err = fmt.Errorf("failed to apply filter, resulted %v pods, this should never happen: %w", 0, nilErr)
+		default: // LIG_NO_MODEL: absent models are answered on the host and never sent
+			err = status.Errorf(codes.Internal, "model id %d (%s) has no model entry on the device", w.modelID, w.model)
+		}
+		w.done <- result{resolved: resolved, err: fmt.Errorf("failed to find target pod: %w", err)} // request.go:73-75
 	}
 }

@@ -66,7 +66,9 @@ Status NewScheduler(std::shared_ptr<PodMetricsProvider> pmp, const Options& opt,
   }
   s->h_reqs_ = static_cast<lig_req*>(lig_host_alloc((size_t)opt.max_batch * sizeof(lig_req)));
   s->h_picks_ = static_cast<lig_pick*>(lig_host_alloc((size_t)opt.max_batch * sizeof(lig_pick)));
-  if (!s->h_reqs_ || !s->h_picks_) return LigFailure("lig_host_alloc");
+  s->h_model_ids_ = static_cast<uint32_t*>(lig_host_alloc((size_t)opt.max_batch * sizeof(uint32_t)));
+  s->h_mpicks_ = static_cast<lig_mpick*>(lig_host_alloc((size_t)opt.max_batch * sizeof(lig_mpick)));
+  if (!s->h_reqs_ || !s->h_picks_ || !s->h_model_ids_ || !s->h_mpicks_) return LigFailure("lig_host_alloc");
   uint64_t seed = opt.seed;
   if (seed == 0) {
     std::random_device rd;
@@ -95,6 +97,8 @@ Scheduler::~Scheduler() {
   if (ctx_ && opt_.use_doorbell) lig_stream_close(ctx_);
   if (h_reqs_) lig_host_free(h_reqs_);
   if (h_picks_) lig_host_free(h_picks_);
+  if (h_model_ids_) lig_host_free(h_model_ids_);
+  if (h_mpicks_) lig_host_free(h_mpicks_);
   if (ctx_) lig_destroy(ctx_);
   if (group_) lig_group_destroy(group_);
 }
@@ -103,7 +107,11 @@ Scheduler::~Scheduler() {
 // A failed refresh keeps the previous snapshot — like a failed scrape keeps stale metrics
 // (backend/provider.go:151-156) — but never silently: it is counted and its reason kept.
 Status Scheduler::Refresh() {
-  Status st = RefreshImpl();
+  std::lock_guard<std::mutex> rk(refresh_mu_);
+  return RecordRefresh(RefreshImpl(models_));
+}
+
+Status Scheduler::RecordRefresh(Status st) {
   if (!st.ok()) {
     std::lock_guard<std::mutex> sk(stats_mu_);
     stats_.failed_refreshes++;
@@ -118,8 +126,8 @@ std::string Scheduler::last_refresh_error() const {
   return last_refresh_error_;
 }
 
-Status Scheduler::RefreshImpl() {
-  std::lock_guard<std::mutex> rk(refresh_mu_);
+// Called with refresh_mu_ held.  `models` (null: no list set) is packed against the new epoch.
+Status Scheduler::RefreshImpl(const std::shared_ptr<const ModelList>& models) {
   const auto t_begin = std::chrono::steady_clock::now();
   auto pods = pmp_->AllPodMetrics();
   // A pod whose metrics do not fit the device record (WaitingQueueSize outside int32,
@@ -233,6 +241,44 @@ Status Scheduler::RefreshImpl() {
                                                 ma16.data(), bitmap.data());
     if (rc != 0) return LigFailure(group_ ? "lig_group_upload_snapshot" : "lig_upload_snapshot");
   }
+  // The model table goes into the new epoch before the epoch is published, so a flush that captures
+  // the epoch always finds the table its names were mapped against.
+  if (models) {
+    PackedModelTable& t = packed_models_;
+    if (t.list != models || t.adapter_ids != snap->adapter_ids) {
+      const size_t n = models->models.size();
+      t.target_offsets.assign(n + 1, 0);
+      t.target_adapter_ids.clear();
+      t.target_weights.clear();
+      t.self_adapter_ids.resize(n);
+      t.critical.resize(n);
+      // a name no pod lists, or one interned after this epoch's table (>= A), is id A: no pod matches
+      auto intern = [&](const std::string& name) {
+        auto it = snap->adapter_ids->find(name);
+        return (it == snap->adapter_ids->end() || it->second >= A) ? A : it->second;
+      };
+      for (size_t m = 0; m < n; ++m) {
+        const backend::InferenceModel& im = *models->models[m];
+        t.critical[m] = im.Critical ? 1 : 0;
+        t.self_adapter_ids[m] = intern(im.ModelName);
+        if (models->present[m])
+          for (const backend::TargetModel& tm : im.TargetModels) {
+            t.target_adapter_ids.push_back(intern(tm.Name));
+            t.target_weights.push_back(tm.Weight);
+          }
+        t.target_offsets[m + 1] = (int32_t)t.target_adapter_ids.size();
+      }
+      t.list = models;
+      t.adapter_ids = snap->adapter_ids;
+    }
+    if (lig_upload_models(ctx_, snap->epoch, (int)models->models.size(), t.target_offsets.data(),
+                          t.target_adapter_ids.data(), t.target_weights.data(), t.critical.data(),
+                          t.self_adapter_ids.data(), models->present.data()) != 0) {
+      prev_epoch_ = 0;   // the next refresh uploads in full
+      return LigFailure("lig_upload_models");
+    }
+  }
+  snap->models = models;
   prev_kv_ = kv;
   prev_q_ = q32;
   prev_na_ = na16;
@@ -254,6 +300,48 @@ Status Scheduler::RefreshImpl() {
   return Status{};
 }
 
+Status Scheduler::SetInferenceModels(std::vector<std::shared_ptr<const backend::InferenceModel>> models) {
+  if (group_)
+    return Errorf(InvalidArgument, "SetInferenceModels: model requests need a single device (lig_group has no "
+                                   "model-table calls)");
+  auto list = std::make_shared<ModelList>();
+  for (auto& m : models) {
+    if (!m) return Errorf(InvalidArgument, "SetInferenceModels: nil InferenceModel");
+    auto ins = list->ids.emplace(m->ModelName, (uint32_t)list->models.size());
+    if (ins.second) list->models.push_back(std::move(m));
+    else list->models[ins.first->second] = std::move(m);          // the later one wins
+  }
+  list->present.assign(list->models.size(), 1);
+  for (size_t i = 0; i < list->models.size(); ++i) {
+    const backend::InferenceModel& im = *list->models[i];
+    int64_t total = 0;
+    bool negative = false;
+    for (const backend::TargetModel& tm : im.TargetModels) {
+      total += tm.Weight;
+      negative |= tm.Weight < 0;
+    }
+    if (im.TargetModels.empty()) continue;
+    // no target can be drawn (Go's Int31n panics on 0): "error getting target model name"
+    if (total <= 0) {
+      list->present[i] = 0;
+      continue;
+    }
+    // what lig_upload_models refuses with LIG_ERR_RANGE
+    if (im.TargetModels.size() > 255)
+      return Errorf(InvalidArgument, "SetInferenceModels: model " + im.ModelName + " has " +
+                                         std::to_string(im.TargetModels.size()) + " target models (at most 255)");
+    if (negative) return Errorf(InvalidArgument, "SetInferenceModels: model " + im.ModelName + " has a negative weight");
+    if (total > INT32_MAX)
+      return Errorf(InvalidArgument, "SetInferenceModels: the weights of model " + im.ModelName + " sum to " +
+                                         std::to_string(total) + " (at most 2^31-1)");
+  }
+  std::shared_ptr<const ModelList> next = std::move(list);
+  std::lock_guard<std::mutex> rk(refresh_mu_);
+  Status st = RecordRefresh(RefreshImpl(next));
+  if (st.ok()) models_ = std::move(next);
+  return st;
+}
+
 void Scheduler::RefresherLoop() {
   std::unique_lock<std::mutex> lk(mu_);
   while (!stop_) {
@@ -268,9 +356,28 @@ void Scheduler::RefresherLoop() {
 Status Scheduler::Schedule(const LLMRequest& req, backend::Pod* targetPod) {
   Waiter w;
   w.req = &req;
+  Submit(w);
+  if (w.status.ok() && targetPod) *targetPod = std::move(w.pod);
+  return w.status;
+}
+
+Status Scheduler::ScheduleModel(const std::string& model, std::string* resolvedTargetModel, backend::Pod* targetPod) {
+  Waiter w;
+  w.model = &model;
+  Submit(w);
+  if (w.status.ok() && targetPod) *targetPod = std::move(w.pod);
+  if (resolvedTargetModel) *resolvedTargetModel = std::move(w.resolved);
+  return w.status;
+}
+
+// Queue the waiter for the batcher and block until its result is published.
+void Scheduler::Submit(Waiter& w) {
   {
     std::lock_guard<std::mutex> lk(mu_);
-    if (stop_) return Errorf(Internal, "scheduler is shut down");
+    if (stop_) {
+      w.status = Errorf(Internal, "scheduler is shut down");
+      return;
+    }
     if (pending_.empty()) oldest_ = std::chrono::steady_clock::now();
     pending_.push_back(&w);
     pending_count_.store((int)pending_.size(), std::memory_order_release);
@@ -292,8 +399,6 @@ Status Scheduler::Schedule(const LLMRequest& req, backend::Pod* targetPod) {
     __builtin_ia32_pause();
 #endif
   }
-  if (w.status.ok() && targetPod) *targetPod = std::move(w.pod);
-  return w.status;
 }
 
 void Scheduler::BatcherLoop() {
@@ -336,7 +441,26 @@ void Scheduler::BatcherLoop() {
   }
 }
 
-void Scheduler::Flush(std::vector<Waiter*>& batch) {
+void Scheduler::CountFeedback(uint64_t epoch, int n) {
+  // the chain restarts on every new epoch: "until the next metrics refresh" (Refresh never reuses an
+  // epoch number)
+  const int W = opt_.load_feedback_window;
+  std::lock_guard<std::mutex> sk(stats_mu_);
+  if (epoch != fb_epoch_) {
+    if (fb_epoch_ != 0) stats_.feedback_restarts++;
+    fb_epoch_ = epoch;
+    fb_filled_ = 0;
+  }
+  stats_.feedback_windows += (uint64_t)((fb_filled_ + (int64_t)n) / W);
+  fb_filled_ = (int)((fb_filled_ + (int64_t)n) % W);
+}
+
+// A flush that holds both kinds makes the descriptor calls first, then the model-id calls.
+void Scheduler::Flush(std::vector<Waiter*>& all) {
+  desc_lane_.clear();
+  model_lane_.clear();
+  for (Waiter* w : all) (w->model ? model_lane_ : desc_lane_).push_back(w);
+  std::vector<Waiter*>& batch = desc_lane_;
   size_t done = 0;
   const auto flush_t0 = std::chrono::steady_clock::now();
   double device_us = 0, device_cpu_us = 0;
@@ -372,18 +496,7 @@ void Scheduler::Flush(std::vector<Waiter*>& batch) {
            : (opt_.use_doorbell && n <= lig_stream_capacity())
                ? lig_stream_submit(ctx_, snap->epoch, seed_, h_reqs_, n, h_picks_)
                : lig_schedule_batch(ctx_, snap->epoch, seed_, h_reqs_, n, h_picks_);
-      if (rc == 0 && W > 0) {
-        // the chain restarts on every new epoch: "until the next metrics refresh" (Refresh never
-        // reuses an epoch number)
-        std::lock_guard<std::mutex> sk(stats_mu_);
-        if (snap->epoch != fb_epoch_) {
-          if (fb_epoch_ != 0) stats_.feedback_restarts++;
-          fb_epoch_ = snap->epoch;
-          fb_filled_ = 0;
-        }
-        stats_.feedback_windows += (uint64_t)((fb_filled_ + (int64_t)n) / W);
-        fb_filled_ = (int)((fb_filled_ + (int64_t)n) % W);
-      }
+      if (rc == 0 && W > 0) CountFeedback(snap->epoch, n);
       const double call_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - call_t0).count();
       if (call_us > device_us) {
         device_us = call_us;
@@ -427,6 +540,7 @@ void Scheduler::Flush(std::vector<Waiter*>& batch) {
     }
     done += (size_t)n;
   }
+  FlushModels(model_lane_);
   const double flush_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - flush_t0).count();
   std::lock_guard<std::mutex> sk(stats_mu_);
   if (device_us > stats_.max_device_call_us) {
@@ -435,6 +549,103 @@ void Scheduler::Flush(std::vector<Waiter*>& batch) {
     stats_.slowest_call_batch = stats_.batches ? stats_.batches - 1 : 0;
   }
   stats_.max_flush_us = std::max(stats_.max_flush_us, flush_us);
+}
+
+// The model-id lane: names are mapped to ids against the captured epoch's list; names the host can
+// answer from that list alone never reach the device.  Request k that reaches the device has
+// rand_key = model_index_ + k; a stale-epoch retry maps again and reuses the same first_index.
+void Scheduler::FlushModels(std::vector<Waiter*>& batch) {
+  size_t done = 0;
+  while (done < batch.size()) {
+    const int n = (int)std::min(batch.size() - done, (size_t)opt_.max_batch);
+    std::shared_ptr<const Snapshot> snap;
+    int rc = 0, k = 0;
+    const char* call = "lig_schedule_models_batch";
+    for (int attempt = 0; attempt < 4; ++attempt) {
+      {
+        std::lock_guard<std::mutex> lk(snap_mu_);
+        snap = snap_;
+      }
+      const ModelList* list = snap->models.get();
+      k = 0;
+      for (int i = 0; i < n; ++i) {
+        Waiter* w = batch[done + i];
+        auto it = list ? list->ids.find(*w->model) : decltype(list->ids)::const_iterator{};
+        if (!list || it == list->ids.end()) {                                       // request.go:42-45
+          w->model_id = -1;
+          w->status = Errorf(Unknown, "error finding a model object in InferenceModel for input " + *w->model);
+        } else if (!list->present[it->second]) {                                     // request.go:48-51
+          w->model_id = -1;
+          w->status = Errorf(Unknown, "error getting target model name for model " +
+                                          list->models[it->second]->ModelName);
+        } else {
+          w->model_id = it->second;
+          w->status = Status{};   // a retry may map a name the previous epoch answered on the host
+          h_model_ids_[k++] = it->second;
+        }
+      }
+      if (k == 0) break;
+      const int W = opt_.load_feedback_window;
+      if (W > 0) {
+        call = "lig_schedule_models_batch_feedback_chain";
+        rc = lig_schedule_models_batch_feedback_chain(ctx_, snap->epoch, seed_, model_index_, h_model_ids_, k,
+                                                      h_mpicks_, W, nullptr);
+      } else if (opt_.use_doorbell && k <= lig_stream_capacity()) {
+        call = "lig_stream_submit_models";
+        rc = lig_stream_submit_models(ctx_, snap->epoch, seed_, model_index_, h_model_ids_, k, h_mpicks_);
+      } else {
+        rc = lig_schedule_models_batch(ctx_, snap->epoch, seed_, model_index_, h_model_ids_, k, h_mpicks_);
+      }
+      if (rc == 0 && W > 0) CountFeedback(snap->epoch, k);
+      if (rc != LIG_ERR_STALE_EPOCH) break;
+      std::lock_guard<std::mutex> sk(stats_mu_);
+      stats_.stale_retries++;
+    }
+    if (k > 0) model_index_ += (uint64_t)k;
+    const Status failure = rc != 0 ? LigFailure(call) : Status{};
+    const std::string prefix = "failed to find target pod: ";                        // request.go:73-75
+    for (int i = 0, j = 0; i < n; ++i) {
+      Waiter* w = batch[done + i];
+      if (w->model_id < 0) continue;
+      const lig_mpick& pk = h_mpicks_[j++];
+      if (rc != 0) {
+        w->status = failure;
+        w->status.message = prefix + w->status.message;
+        continue;
+      }
+      const backend::InferenceModel& im = *snap->models->models[(size_t)w->model_id];
+      // 255: TargetModels is empty and the requested name passes through (request.go:47)
+      w->resolved = pk.target_idx == 255 ? *w->model : im.TargetModels[pk.target_idx].Name;
+      if (pk.status == LIG_OK) {
+        w->pod = snap->pods[(size_t)pk.pod_idx];
+      } else if (pk.status == LIG_DROP) {
+        w->status = Errorf(ResourceExhausted, prefix + "failed to apply filter, resulted 0 pods, this should never "
+                                                       "happen: " + kDropInner);
+      } else if (pk.status == LIG_NO_PODS_LEFT) {
+        w->status = Errorf(Unknown, prefix + "failed to apply filter, resulted 0 pods, this should never happen: "
+                                             "no pods left");
+      } else if (pk.status == LIG_EMPTY) {
+        w->status = Errorf(Unknown, prefix + "failed to apply filter, resulted 0 pods, this should never happen: "
+                                             "%!w(<nil>)");
+      } else {   // LIG_NO_MODEL: absent models are answered on the host and never sent
+        w->status = Errorf(Internal, prefix + "rpc error: code = Internal desc = model id " +
+                                         std::to_string(w->model_id) + " (" + im.ModelName +
+                                         ") has no model entry on the device");
+      }
+    }
+    {
+      std::lock_guard<std::mutex> sk(stats_mu_);
+      stats_.model_scheduled += (uint64_t)n;
+      stats_.model_batches += k > 0 ? 1 : 0;
+    }
+    for (int i = 0; i < n; ++i) {
+      Waiter* w = batch[done + i];
+      w->done.store(1, std::memory_order_release);
+      w->done.notify_one();
+      w->done.store(2, std::memory_order_release);   // last access: the caller may now destroy *w
+    }
+    done += (size_t)n;
+  }
 }
 
 Status Scheduler::ScheduleModel(backend::ModelDataStore& datastore, const std::string& model,

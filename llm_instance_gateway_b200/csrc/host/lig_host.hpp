@@ -13,6 +13,16 @@
 // re-packed once per refresh tick (refreshMetricsInterval, pkg/ext-proc/main.go:39) instead of
 // once per request.  No CPU scheduling path exists here: without liblig.so + a CUDA device,
 // NewScheduler fails.
+//
+// Model requests.  ScheduleModel(datastore, ...) resolves a request on the caller's thread
+// (FetchModelData, RandomWeightedDraw, IsCritical) and sends the resolved descriptor through
+// Schedule.  ScheduleModel(model, ...) sends only the model name: SetInferenceModels gives the
+// scheduler the datastore's InferenceModels, every snapshot epoch carries them as a device model
+// table (lig_upload_models, target names interned against that epoch's adapter ids), and the
+// batcher maps names to model ids at flush time and lets the device resolve, draw and pick in one
+// call (lig_schedule_models_batch, lig_stream_submit_models with use_doorbell, or
+// lig_schedule_models_batch_feedback_chain with load_feedback_window).  Pods, adapter ids and the
+// model table always change together, in one published epoch.
 #pragma once
 
 #include <atomic>
@@ -100,7 +110,7 @@ struct LLMRequest {                  // scheduling/types.go:4-11
 };
 
 // google.golang.org/grpc/codes values the path can produce.
-enum Code : int { OK = 0, Unknown = 2, ResourceExhausted = 8, Internal = 13 };
+enum Code : int { OK = 0, Unknown = 2, InvalidArgument = 3, ResourceExhausted = 8, Internal = 13 };
 
 struct Status {                      // a Go `error` carrying a gRPC status code
   int code = OK;
@@ -160,6 +170,8 @@ struct Stats {
   uint64_t excluded_pods = 0;      // pods left out of the last snapshot: a metric did not fit the device record
   uint64_t feedback_windows = 0;   // load-feedback windows closed (Options::load_feedback_window)
   uint64_t feedback_restarts = 0;  // feedback chains restarted on a new epoch after the first one
+  uint64_t model_scheduled = 0;    // ScheduleModel(model, ...) calls completed (host-answered ones included)
+  uint64_t model_batches = 0;      // device calls issued for model-id requests
   double last_pack_us = 0;     // last Refresh: provider slice -> columns + bitmap (host)
   double last_upload_us = 0;   // last Refresh: lig_upload_snapshot (H2D + class tables)
   double max_device_call_us = 0;   // slowest single lig_schedule_batch call (launch + kernel + synchronise)
@@ -190,10 +202,33 @@ class Scheduler {
   Status ScheduleModel(backend::ModelDataStore& datastore, const std::string& model, std::string* resolvedTargetModel,
                        backend::Pod* targetPod);
 
-  // Re-read the provider and upload a new snapshot epoch (call on every metrics refresh).
+  // The same step resolved on the device, against the list last given to SetInferenceModels (none
+  // given: every model is unknown, like an empty datastore).  The batcher maps the name to the
+  // captured epoch's model id at flush time; the device draws the target and picks the pod.
+  // Unknown models and models whose weights sum to <= 0 are answered on the host with the errors
+  // above and take no rand_key and no place in a feedback window.  Other errors are those of
+  // Schedule, prefixed "failed to find target pod: " (request.go:73-75).  Request k that reaches
+  // the device (counted from 0 per scheduler) has rand_key = k: the draw and the pick are those of
+  // lig_schedule_models_batch with first_index = k.  Neither rand_key sequence of the two calls
+  // above is touched.
+  Status ScheduleModel(const std::string& model, std::string* resolvedTargetModel, backend::Pod* targetPod);
+
+  // Replace the InferenceModels that ScheduleModel(model, ...) resolves against; of two models
+  // with one ModelName the later wins (the reference's datastore is a map).  Publishes a new epoch
+  // through Refresh, so the list applies from that epoch on, and like every new epoch it restarts
+  // the load-feedback chain.  A list the device cannot take (a model with more than 255 targets, a
+  // negative weight, weights summing above 2^31-1) or a failed refresh leaves the previous list and
+  // snapshot in force; the error names the model.  Single device only (InvalidArgument otherwise).
+  Status SetInferenceModels(std::vector<std::shared_ptr<const backend::InferenceModel>> models);
+
+  // Re-read the provider and upload a new snapshot epoch (call on every metrics refresh).  With a
+  // model list set, the list is re-interned against the new epoch and uploaded into it before the
+  // epoch is published: a target model that no pod listed matches once a pod loads it.
   Status Refresh();
  private:
-  Status RefreshImpl();
+  struct ModelList;
+  Status RefreshImpl(const std::shared_ptr<const ModelList>& models);
+  Status RecordRefresh(Status st);
  public:
 
   Stats stats() const;
@@ -210,6 +245,21 @@ class Scheduler {
     int A = 0;
     std::shared_ptr<const InternTable> adapter_ids;   // shared between snapshots until a name is added
     std::vector<backend::Pod> pods;
+    std::shared_ptr<const ModelList> models;          // the list this epoch's model table was packed from
+  };
+  // The list SetInferenceModels accepted: dense model id -> InferenceModel, and the name map.
+  struct ModelList {
+    std::vector<std::shared_ptr<const backend::InferenceModel>> models;
+    std::unordered_map<std::string, uint32_t> ids;    // Spec.ModelName -> model id
+    std::vector<uint8_t> present;                     // 0: weights sum to <= 0, no target can be drawn
+  };
+  // The last model table packed for lig_upload_models, reused while neither the list nor the
+  // adapter-id table changed (guarded by refresh_mu_).
+  struct PackedModelTable {
+    std::shared_ptr<const ModelList> list;
+    std::shared_ptr<const InternTable> adapter_ids;
+    std::vector<int32_t> target_offsets, target_adapter_ids, target_weights, self_adapter_ids;
+    std::vector<uint8_t> critical;
   };
   // Packer state kept between refreshes (guarded by refresh_mu_): adapter ids are stable while
   // the table fits max_adapters, and a pod whose ActiveModels keys did not change since the last
@@ -227,10 +277,16 @@ class Scheduler {
   std::atomic<uint64_t> model_draws_{0};
   std::shared_ptr<InternTable> intern_;
   std::vector<PodMemo> memo_;
+  std::shared_ptr<const ModelList> models_;   // SetInferenceModels' list (guarded by refresh_mu_); null: none set
+  PackedModelTable packed_models_;
   // Lives on the caller's stack.  `done` goes 0 -> 1 (result published, the caller may read it)
   // -> 2 (the notifier will not touch the Waiter again, the caller may return and destroy it).
+  // Carries a descriptor request (req) or a model name (model).
   struct Waiter {
     const LLMRequest* req = nullptr;
+    const std::string* model = nullptr;
+    int64_t model_id = -1;       // flush-time id in the captured epoch's table; -1: answered on the host
+    std::string resolved;        // model requests: the resolved target model
     Status status;
     backend::Pod pod;
     std::atomic<uint32_t> done{0};
@@ -238,7 +294,10 @@ class Scheduler {
 
   void BatcherLoop();
   void RefresherLoop();
+  void Submit(Waiter& w);
   void Flush(std::vector<Waiter*>& batch);
+  void FlushModels(std::vector<Waiter*>& batch);
+  void CountFeedback(uint64_t epoch, int n);
 
   std::shared_ptr<PodMetricsProvider> pmp_;
   Options opt_;
@@ -246,6 +305,10 @@ class Scheduler {
   lig_group* group_ = nullptr;     // set instead of ctx_ when Options::devices lists several GPUs
   lig_req* h_reqs_ = nullptr;      // pinned, device-mapped (lig_host_alloc)
   lig_pick* h_picks_ = nullptr;
+  uint32_t* h_model_ids_ = nullptr;   // pinned, max_batch entries each: the model-id lane
+  lig_mpick* h_mpicks_ = nullptr;
+  uint64_t model_index_ = 0;          // first_index of the next model-id device call
+  std::vector<Waiter*> desc_lane_, model_lane_;   // a flush split by kind (batcher thread only)
   uint64_t seed_ = 0;
   uint64_t rng_state_ = 0;
   // the feedback chain as the batcher thread sees it (the library's window count is deterministic)

@@ -24,6 +24,8 @@ struct ligh_provider : public scheduling::PodMetricsProvider {
 struct ligh_scheduler {
   std::shared_ptr<ligh_provider> provider;
   std::unique_ptr<Scheduler> sched;
+  // the list last accepted by ligh_scheduler_set_models, to report which target a call resolved to
+  std::map<std::string, std::shared_ptr<const backend::InferenceModel>> models_by_name;
 };
 
 struct ligh_datastore : public backend::ModelDataStore {     // backend/fake.go: FakeDataStore
@@ -156,6 +158,41 @@ int ligh_schedule_model(ligh_scheduler* s, ligh_datastore* d, const char* model,
   return st.code;
 }
 
+int ligh_scheduler_set_models(ligh_scheduler* s, ligh_datastore* d, char* err, int err_cap) {
+  std::vector<std::shared_ptr<const backend::InferenceModel>> models;
+  {
+    std::lock_guard<std::mutex> lk(d->mu);
+    for (const auto& kv : d->res) models.push_back(kv.second);
+  }
+  std::map<std::string, std::shared_ptr<const backend::InferenceModel>> by_name;
+  for (const auto& m : models) by_name[m->ModelName] = m;
+  scheduling::Status st = s->sched->SetInferenceModels(std::move(models));
+  if (st.ok()) s->models_by_name.swap(by_name);
+  else put(err, err_cap, st.message);
+  return st.code;
+}
+
+int ligh_schedule_model_device(ligh_scheduler* s, const char* model, char* resolved, int resolved_cap, char* name,
+                               int name_cap, char* addr, int addr_cap, char* err, int err_cap) {
+  backend::Pod pod;
+  std::string target;
+  scheduling::Status st = s->sched->ScheduleModel(std::string(model ? model : ""), &target, &pod);
+  put(resolved, resolved_cap, target);
+  if (st.ok()) {
+    put(name, name_cap, pod.Name);
+    put(addr, addr_cap, pod.Address);
+  } else {
+    put(err, err_cap, st.message);
+  }
+  return st.code;
+}
+
+void ligh_model_stats(ligh_scheduler* s, uint64_t out[2]) {
+  scheduling::Stats st = s->sched->stats();
+  out[0] = st.model_scheduled;
+  out[1] = st.model_batches;
+}
+
 ligh_scheduler* ligh_scheduler_new(ligh_provider* p, int device, int max_pods, int max_adapters,
                                    int max_batch, int flush_size, int window_us, int refresh_ms,
                                    uint64_t seed, char* err, int err_cap) {
@@ -280,6 +317,49 @@ int ligh_schedule_concurrent(ligh_scheduler* s, int n_threads, int per_thread,
           out_pod[i] = it == index.end() ? -1 : it->second;
         } else {
           out_pod[i] = -1;
+        }
+      }
+    });
+  }
+  for (auto& x : th) x.join();
+  return 0;
+}
+
+int ligh_schedule_models_concurrent(ligh_scheduler* s, ligh_datastore* d, int n_threads, int per_thread,
+                                    const char* const* models, int n_models, int* out_codes, int* out_pod,
+                                    int* out_target) {
+  if (!s || n_threads < 1 || per_thread < 0 || n_models < 1) return -1;
+  auto pods = s->provider->AllPodMetrics();
+  std::unordered_map<std::string, int> index;
+  for (size_t i = 0; i < pods.size(); ++i) index[pods[i]->pod.Name + "\n" + pods[i]->pod.Address] = (int)i;
+  std::vector<std::thread> th;
+  for (int t = 0; t < n_threads; ++t) {
+    th.emplace_back([&, t] {
+      for (int k = 0; k < per_thread; ++k) {
+        const int i = t * per_thread + k;
+        const std::string model = models[i % n_models];
+        std::string resolved;
+        backend::Pod pod;
+        scheduling::Status st = d ? s->sched->ScheduleModel(*d, model, &resolved, &pod)
+                                  : s->sched->ScheduleModel(model, &resolved, &pod);
+        out_codes[i] = st.code;
+        out_pod[i] = -1;
+        if (st.ok()) {
+          auto it = index.find(pod.Name + "\n" + pod.Address);
+          if (it != index.end()) out_pod[i] = it->second;
+        }
+        // which target the draw chose: its index in the model's TargetModels, 255 = passed through, -1 = none
+        out_target[i] = -1;
+        auto m = d ? d->FetchModelData(model) : nullptr;
+        if (!d) {
+          auto it = s->models_by_name.find(model);
+          if (it != s->models_by_name.end()) m = it->second;
+        }
+        if (!resolved.empty() && m) {
+          const auto& tms = m->TargetModels;
+          for (size_t j = 0; j < tms.size(); ++j)
+            if (tms[j].Name == resolved) { out_target[i] = (int)j; break; }
+          if (out_target[i] < 0 && resolved == model) out_target[i] = 255;
         }
       }
     });

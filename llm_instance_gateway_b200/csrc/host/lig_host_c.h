@@ -62,6 +62,14 @@ int ligh_datastore_set_model(ligh_datastore*, const char* model_name, int critic
                              const char* const* target_names, const int32_t* weights);
 int ligh_schedule_model(ligh_scheduler*, ligh_datastore*, const char* model, char* resolved, int resolved_cap,
                         char* name, int name_cap, char* addr, int addr_cap, char* err, int err_cap);
+/* Scheduler::SetInferenceModels with the datastore's current contents (the list is copied: later
+ * ligh_datastore_set_model calls do not reach the scheduler until the next ligh_scheduler_set_models).
+ * Returns the gRPC code; err receives the refusal. */
+int ligh_scheduler_set_models(ligh_scheduler*, ligh_datastore*, char* err, int err_cap);
+/* Scheduler::ScheduleModel(model, ...): resolved on the device against that list. */
+int ligh_schedule_model_device(ligh_scheduler*, const char* model, char* resolved, int resolved_cap,
+                               char* name, int name_cap, char* addr, int addr_cap, char* err, int err_cap);
+void ligh_model_stats(ligh_scheduler*, uint64_t out[2]); /* model_scheduled, model_batches */
 void ligh_stats(ligh_scheduler*, uint64_t out[9]); /* scheduled, batches, max_batch, refreshes, stale_retries */
 void ligh_feedback_stats(ligh_scheduler*, uint64_t out[2]); /* feedback_windows, feedback_restarts */
 void ligh_refresh_timing(ligh_scheduler*, double out[2]); /* last Refresh: host pack us, lig_upload_snapshot us */
@@ -73,6 +81,13 @@ void ligh_flush_timing(ligh_scheduler*, double out[4]);   /* slowest device call
 int ligh_schedule_concurrent(ligh_scheduler*, int n_threads, int per_thread,
                              const char* const* resolved_models, const int* critical, int n_models,
                              int* out_codes, int* out_pod);
+
+/* The same for model requests: caller i sends models[i % n_models] through ligh_schedule_model_device
+ * (datastore null) or ligh_schedule_model with the datastore.  out_target receives the index of the
+ * resolved name in that model's TargetModels (255: the name passed through, -1: no resolved name). */
+int ligh_schedule_models_concurrent(ligh_scheduler*, ligh_datastore* datastore, int n_threads, int per_thread,
+                                    const char* const* models, int n_models, int* out_codes, int* out_pod,
+                                    int* out_target);
 
 /* Streaming load (BASELINE.json configs[4]): Poisson arrivals at `rate` req/s for `seconds`,
  * spread over n_threads caller threads; latency = completion - scheduled arrival.  Fills

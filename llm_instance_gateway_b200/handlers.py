@@ -99,6 +99,12 @@ class Server:
         if not isinstance(model, str):                                       # request.go:32-35
             raise GoError("model not found in request")
         modelName = model
+        resolves = getattr(self.scheduler, "ResolvesModels", None)
+        if callable(resolves) and resolves():
+            # a scheduler holding the InferenceModels resolves on the device; its errors are already
+            # the ones below (the Go adapter's patch 0004 takes the same branch)
+            modelName, targetPod = self.scheduler.ScheduleModel(model)
+            return self._respond(reqCtx, rb, body, LLMRequest(Model=model, ResolvedTargetModel=modelName), targetPod)
         modelObj = self.datastore.FetchModelData(model)                     # request.go:42-45
         if modelObj is None:
             raise GoError(f"error finding a model object in InferenceModel for input {model}")
@@ -109,14 +115,18 @@ class Server:
             if modelName == "":
                 raise GoError(f"error getting target model name for model {modelObj.Name}")
         llmReq = LLMRequest(Model=model, ResolvedTargetModel=modelName, Critical=IsCritical(modelObj))   # request.go:52-56
-        requestBody = body
-        if llmReq.Model != llmReq.ResolvedTargetModel:                       # request.go:60-69
-            rb["model"] = llmReq.ResolvedTargetModel
-            requestBody = go_json_marshal(rb)
         try:
             targetPod = self.scheduler.Schedule(llmReq)                      # request.go:71-74
         except StatusError as err:
             raise StatusError(err.code, f"failed to find target pod: {err}")   # %w keeps the status code
+        return self._respond(reqCtx, rb, body, llmReq, targetPod)
+
+    def _respond(self, reqCtx: RequestContext, rb: Dict[str, Any], body: bytes, llmReq: LLMRequest,
+                 targetPod) -> Dict[str, Any]:
+        requestBody = body
+        if llmReq.Model != llmReq.ResolvedTargetModel:                       # request.go:60-69
+            rb["model"] = llmReq.ResolvedTargetModel
+            requestBody = go_json_marshal(rb)
         reqCtx.Model = llmReq.Model
         reqCtx.TargetPod = targetPod
         headers = [                                                           # request.go:80-96

@@ -27,6 +27,7 @@ EXPORTED_SYMBOLS = (
     "ligh_schedule_concurrent", "ligh_stream_bench", "ligh_refresh_timing", "ligh_flush_timing",
     "ligh_scheduler_new_devices", "ligh_datastore_new", "ligh_datastore_free", "ligh_datastore_set_model",
     "ligh_schedule_model", "ligh_scheduler_new_tree", "ligh_scheduler_new_feedback", "ligh_feedback_stats",
+    "ligh_scheduler_set_models", "ligh_schedule_model_device", "ligh_model_stats", "ligh_schedule_models_concurrent",
 )
 
 _lib = None
@@ -64,6 +65,12 @@ def load() -> C.CDLL:
     lib.ligh_datastore_free.restype = None
     lib.ligh_datastore_set_model.argtypes = [vp, C.c_char_p, i32, i32, cpp, vp]
     lib.ligh_schedule_model.argtypes = [vp, vp, C.c_char_p, C.c_char_p, i32, C.c_char_p, i32, C.c_char_p, i32, C.c_char_p, i32]
+    lib.ligh_scheduler_set_models.argtypes = [vp, vp, C.c_char_p, i32]
+    lib.ligh_schedule_model_device.argtypes = [vp, C.c_char_p, C.c_char_p, i32, C.c_char_p, i32, C.c_char_p, i32,
+                                               C.c_char_p, i32]
+    lib.ligh_model_stats.argtypes = [vp, vp]
+    lib.ligh_model_stats.restype = None
+    lib.ligh_schedule_models_concurrent.argtypes = [vp, vp, i32, i32, cpp, i32, vp, vp, vp]
     lib.ligh_scheduler_free.argtypes = [vp]
     lib.ligh_scheduler_free.restype = None
     lib.ligh_schedule.argtypes = [vp, C.c_char_p, C.c_char_p, i32, C.c_char_p, i32, C.c_char_p, i32,
@@ -183,9 +190,12 @@ class HostScheduler:
         self._lib.ligh_stats(self._s, out)
         fb = (C.c_uint64 * 2)()
         self._lib.ligh_feedback_stats(self._s, fb)
+        ms = (C.c_uint64 * 2)()
+        self._lib.ligh_model_stats(self._s, ms)
         return dict(zip(("scheduled", "batches", "max_batch", "refreshes", "stale_retries", "failed_refreshes",
                          "excluded_pods", "delta_refreshes", "last_dirty_pods", "feedback_windows",
-                         "feedback_restarts"), map(int, list(out) + list(fb))))
+                         "feedback_restarts", "model_scheduled", "model_batches"),
+                        map(int, list(out) + list(fb) + list(ms))))
 
     def ScheduleModel(self, datastore: "HostDataStore", model: str):  # noqa: N802
         """resolve (FetchModelData + RandomWeightedDraw + IsCritical) + Schedule: (code, resolved, pod, err)."""
@@ -194,6 +204,35 @@ class HostScheduler:
         code = self._lib.ligh_schedule_model(self._s, datastore._d, model.encode(), resolved, 256, name, 256, addr, 256, err, 512)
         pod = Pod(name.value.decode(), addr.value.decode()) if code == GRPC_OK else None
         return code, resolved.value.decode(), pod, err.value.decode("utf-8", "replace")
+
+    def set_inference_models(self, datastore: "HostDataStore") -> None:
+        """Scheduler::SetInferenceModels with the datastore's current models: ScheduleModelOnDevice
+        resolves against them from the epoch this call publishes.  HostSchedulerError on refusal."""
+        err = C.create_string_buffer(512)
+        if self._lib.ligh_scheduler_set_models(self._s, datastore._d, err, 512) != GRPC_OK:
+            raise HostSchedulerError(err.value.decode("utf-8", "replace"))
+
+    def ScheduleModelOnDevice(self, model: str):  # noqa: N802
+        """The resolve step on the device + the pick: (code, resolved, pod, err), as ScheduleModel."""
+        resolved, name, addr = C.create_string_buffer(256), C.create_string_buffer(256), C.create_string_buffer(256)
+        err = C.create_string_buffer(512)
+        code = self._lib.ligh_schedule_model_device(self._s, model.encode(), resolved, 256, name, 256, addr, 256,
+                                                    err, 512)
+        pod = Pod(name.value.decode(), addr.value.decode()) if code == GRPC_OK else None
+        return code, resolved.value.decode(), pod, err.value.decode("utf-8", "replace")
+
+    def schedule_models_concurrent(self, n_threads: int, per_thread: int, models: Sequence[str],
+                                   datastore: Optional["HostDataStore"] = None):
+        """n_threads callers of ScheduleModelOnDevice (or of ScheduleModel with `datastore`), caller i
+        sending models[i % len(models)]: (codes, pod index in the provider's slice or -1, index of the
+        resolved target or 255/-1)."""
+        n = n_threads * per_thread
+        codes, pods, targets = (np.zeros(n, dtype=np.int32) for _ in range(3))
+        rc = self._lib.ligh_schedule_models_concurrent(self._s, datastore._d if datastore else None, n_threads,
+                                                       per_thread, _strs(models), len(models), codes.ctypes.data,
+                                                       pods.ctypes.data, targets.ctypes.data)
+        assert rc == 0
+        return codes, pods, targets
 
     def refresh_timing(self) -> dict:
         out = (C.c_double * 2)()

@@ -12,8 +12,11 @@ server turns into HTTP 429 (handlers/server.go:97-109).  ``NewScheduler(pmp, fil
 caller-built flow chart of the reference's filter nodes (``Filter``, filter.go:17-73) instead of
 ``defaultFilter``; ``DEFAULT_FILTER`` restates defaultFilter node for node.  ``ScheduleBatch`` is the micro-batched
 form the Go adapter uses under load (one C-ABI call per batch); ``NewScheduler(pmp, load_feedback_window=W)``
-carries load feedback across those calls until the next refresh (off by default).  There is no CPU path here:
-without liblig.so or without a CUDA device construction fails.
+carries load feedback across those calls until the next refresh (off by default).  ``SetInferenceModels`` plus
+``ScheduleModel`` / ``ScheduleModelBatch`` take the request's model name instead of a resolved request: the
+resolve step of HandleRequestBody (handlers/request.go:42-56) runs on the device against a model table that
+every snapshot epoch carries.  There is no CPU path here: without liblig.so or without a CUDA device
+construction fails.
 """
 from __future__ import annotations
 
@@ -24,9 +27,9 @@ from typing import Dict, List, Optional, Protocol, Sequence, Tuple
 import numpy as np
 
 from . import _native as N
-from .backend import Pod, PodMetrics
+from .backend import InferenceModel, Pod, PodMetrics
 from .engine import Engine
-from .packer import REQ_DTYPE, PackedSnapshot, pack_pod_metrics
+from .packer import REQ_DTYPE, PackedModels, PackedSnapshot, pack_models, pack_pod_metrics
 
 
 @dataclass
@@ -153,6 +156,31 @@ def _schedule_error(status: int) -> StatusError:
     return StatusError("Unknown", _ERR_PREFIX + "%!w(<nil>)")
 
 
+_POD_PREFIX = "failed to find target pod: "                                  # request.go:73-75
+
+
+def _no_model_entry(model_id: int, name: str) -> str:
+    """LIG_NO_MODEL from the device, which absent models never reach: an Internal status error as
+    the Go adapter wraps it (request.go:73-75)."""
+    return f"{_POD_PREFIX}rpc error: code = Internal desc = model id {model_id} ({name}) has no model entry on the device"
+
+
+def _check_models(models: Sequence[InferenceModel]) -> None:
+    """What lig_upload_models refuses with LIG_ERR_RANGE, named by model.  A model whose weights sum
+    to <= 0 is not refused: pack_models packs it as absent."""
+    for m in models:
+        tms = m.Spec.TargetModels
+        total = sum(int(t.Weight) for t in tms)
+        if not tms or total <= 0:
+            continue
+        if len(tms) > 255:
+            raise ValueError(f"model {m.Spec.ModelName} has {len(tms)} target models (at most 255)")
+        if any(t.Weight < 0 for t in tms):
+            raise ValueError(f"model {m.Spec.ModelName} has a negative weight")
+        if total > (1 << 31) - 1:
+            raise ValueError(f"the weights of model {m.Spec.ModelName} sum to {total} (at most 2^31-1)")
+
+
 class Scheduler:
     def __init__(self, podMetricsProvider: PodMetricsProvider, device: int = 0,
                  max_pods: int = 4096, max_adapters: int = 1024, max_batch: int = 1 << 16,
@@ -165,8 +193,12 @@ class Scheduler:
         self._filter = filter                # None: the built-in defaultFilter
         if filter is not None:
             self._engine.set_filter_tree(filter)
-        self._epoch = 0
+        self._epoch = 0                      # the published epoch
+        self._uploaded = 0                   # the last epoch number used (never reused)
         self._snap: Optional[PackedSnapshot] = None
+        self._models: Optional[List[InferenceModel]] = None          # SetInferenceModels' list
+        self._packed_models: Optional[PackedModels] = None           # that list packed for self._epoch
+        self._model_index = 0                # first_index of the next model-id call
         self._rng = random.Random(seed)      # the Go global source is auto-seeded (scheduler.go:120)
         self._seed = self._rng.getrandbits(64)
 
@@ -178,12 +210,40 @@ class Scheduler:
     # ``Version()`` is re-packed only when the version changes; otherwise every call re-packs,
     # which is exactly the reference's per-call semantics.
     def Refresh(self) -> PackedSnapshot:
+        return self._refresh(self._models)
+
+    def _refresh(self, models: Optional[List[InferenceModel]]) -> PackedSnapshot:
+        # With a model list, the epoch is published only together with its model table, interned
+        # against the epoch's own adapter ids.
         snap = pack_pod_metrics(list(self.podMetricsProvider.AllPodMetrics()))
-        self._epoch += 1
-        self._engine.upload_snapshot(self._epoch, snap)
-        self._snap = snap
+        self._uploaded += 1
+        self._engine.upload_snapshot(self._uploaded, snap)
+        packed = pack_models(models, snap) if models is not None else None
+        if packed is not None:
+            self._engine.upload_models(self._uploaded, packed)
+        self._epoch, self._snap, self._packed_models = self._uploaded, snap, packed
         self._version = self._provider_version()
         return snap
+
+    def SetInferenceModels(self, models: Sequence[InferenceModel]) -> None:
+        """The InferenceModels ScheduleModel resolves against (of two with one ModelName the later
+        wins).  Publishes a new epoch, which restarts the load-feedback chain.  ValueError, naming the
+        model, for a list the device cannot take; the previous list then stays in force."""
+        by_name: Dict[str, int] = {}
+        unique: List[InferenceModel] = []
+        for m in models:                     # the reference's datastore is a map: the later one wins
+            if m.Spec.ModelName in by_name:
+                unique[by_name[m.Spec.ModelName]] = m
+            else:
+                by_name[m.Spec.ModelName] = len(unique)
+                unique.append(m)
+        _check_models(unique)
+        self._refresh(unique)
+        self._models = unique
+
+    def ResolvesModels(self) -> bool:
+        """Whether ScheduleModel has a list to resolve against (SetInferenceModels was called)."""
+        return self._models is not None
 
     def _provider_version(self):
         v = getattr(self.podMetricsProvider, "Version", None)
@@ -214,6 +274,53 @@ class Scheduler:
             else:
                 out.append((None, _schedule_error(int(pk["status"]))))
         return out
+
+    def ScheduleModelBatch(self, names: Sequence[str]) -> List[Tuple[Optional[Pod], str, Optional[StatusError]]]:
+        """The resolve step and the pick on the device, one call per batch: (pod, resolved target
+        model, error) per name.  Names the host answers from the list alone (unknown, or weights
+        summing to <= 0) take no rand_key; request k sent to the device has rand_key = k."""
+        snap = self._current()
+        pm = self._packed_models
+        out: List[Tuple[Optional[Pod], str, Optional[StatusError]]] = [None] * len(names)  # type: ignore
+        ids, slots = [], []
+        for i, name in enumerate(names):
+            m = pm.model_ids.get(name) if pm is not None else None
+            if m is None:                                                       # request.go:42-45
+                out[i] = (None, "", StatusError(
+                    "Unknown", f"error finding a model object in InferenceModel for input {name}"))
+            elif not pm.present[m]:                                             # request.go:48-51
+                out[i] = (None, "", StatusError("Unknown", f"error getting target model name for model {name}"))
+            else:
+                ids.append(m)
+                slots.append(i)
+        if not ids:
+            return out
+        arr = np.array(ids, dtype=np.uint32)
+        if self._window:
+            picks = self._engine.schedule_models_batch_feedback_chain(self._epoch, self._seed, arr, self._window,
+                                                                      first_index=self._model_index)
+        else:
+            picks = self._engine.schedule_models_batch(self._epoch, self._seed, arr, first_index=self._model_index)
+        self._model_index += len(ids)
+        for i, m, pk in zip(slots, ids, picks):
+            t, st = int(pk["target_idx"]), int(pk["status"])
+            resolved = names[i] if t == 255 else pm.target_names[m][t]         # 255: request.go:47
+            if st == N.LIG_OK:
+                out[i] = (snap.pods[int(pk["pod_idx"])], resolved, None)
+            elif st == N.LIG_NO_MODEL:       # absent models never reach the device
+                out[i] = (None, resolved, StatusError("Internal", _no_model_entry(m, names[i])))
+            else:
+                err = _schedule_error(st)
+                out[i] = (None, resolved, StatusError(err.code, _POD_PREFIX + str(err)))
+        return out
+
+    def ScheduleModel(self, name: str) -> Tuple[str, Pod]:
+        """HandleRequestBody's resolve step and Schedule for one request: (resolved target model,
+        pod), or raises StatusError."""
+        pod, resolved, err = self.ScheduleModelBatch([name])[0]
+        if err is not None:
+            raise err
+        return resolved, pod
 
     def Schedule(self, req: LLMRequest) -> Pod:                     # scheduler.go:113-122
         pod, err = self.ScheduleBatch([req])[0]
