@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define LIG_ABI_VERSION 6
+#define LIG_ABI_VERSION 7
 
 /* ---- per-request status (lig_pick.status) ------------------------------------------------------
  * LIG_OK    Schedule returned a pod, nil                      pkg/ext-proc/scheduling/scheduler.go:120-121
@@ -153,7 +153,8 @@ typedef struct lig_filter_node {         /* 32 bytes */
  * nor in (i, n_nodes): edges only point forward, so every table is acyclic, and a node may have
  * several parents (defaultFilter shares queueAndKVCacheFilter).  The direct scan
  * (lig_schedule_scan[_device]) restates the built-in tree only: it returns LIG_ERR_INVALID for an
- * epoch whose tables a caller tree built; lig_read_class reads a caller tree's survivor sets. */
+ * epoch whose tables a caller tree built; lig_filter_batch and lig_read_class return a caller tree's
+ * survivor sets. */
 int  lig_set_filter_tree(lig_ctx* ctx, const lig_filter_node* nodes, int n_nodes);
 
 /* ---- snapshot = the value of PodMetricsProvider.AllPodMetrics() (scheduler.go:108-115,
@@ -389,6 +390,41 @@ int lig_resolve_models(lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64_t fir
  * Submits of both kinds may alternate on one open stream. */
 int lig_stream_submit_models(lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64_t first_index,
                              const uint32_t* model_ids, int n, lig_mpick* out);
+
+/* ---- the survivor sets of a whole batch: Filter.Filter (filter.go:12-15) next to the pick --------
+ * Each call makes the pick of the call it mirrors, byte for byte in `out`, and also returns every
+ * request's survivor list (the slice the filter tree returned, filter.go:44-73) in CSR form:
+ *   - request i's survivors are pods[offsets[i] .. offsets[i+1]): pod indices in ascending order,
+ *     the order of Go's filtered slice.  offsets[0] = 0.  Offsets are int64: the sum can exceed 2^31.
+ *   - LIG_DROP, LIG_EMPTY, LIG_NO_PODS_LEFT and LIG_NO_MODEL requests get an empty list.
+ *   - pod entries at or beyond `capacity` are never written, but `out` and `offsets` are always
+ *     complete, so a first call with capacity = 0 sizes the buffer (pods may then be NULL).  The
+ *     host forms return LIG_ERR_INVALID, after filling `out` and `offsets`, when offsets[R] >
+ *     capacity; the device forms leave that check to the caller.
+ *   - the lists are read from the resident epoch's class tables, whichever build made them (the
+ *     built-in tree, a caller filter tree, compact or strided tables), never from a feedback
+ *     chain's private copy: the survivor sets of the scraped metrics.
+ *   - refused like the call each form mirrors: stale epoch, null buffers, R > max_batch on the host
+ *     forms; the model forms also with LIG_ERR_NO_SNAPSHOT when the epoch has no model table.
+ * Host forms: page-locked buffers are read and written in place, pageable ones are staged; they
+ * block until everything is back.  Device forms: device pointers, enqueued on `stream` (a
+ * cudaStream_t, NULL = legacy default stream), not synchronised. */
+/* descriptors: out is byte for byte lig_schedule_batch(ctx, epoch, seed, reqs, R, out) */
+int lig_filter_batch(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
+                     lig_pick* out, int64_t* offsets /* R + 1 */, uint16_t* pods, int64_t capacity);
+int lig_filter_batch_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* d_reqs, int R,
+                            lig_pick* d_out, int64_t* d_offsets, uint16_t* d_pods, int64_t capacity,
+                            void* stream);
+/* model ids: out is byte for byte lig_schedule_models_batch(ctx, epoch, seed, first_index, ids, R,
+ * out).  Resolved against the epoch's model table as lig_schedule_models_batch does: the call is
+ * ordered behind the table's upload and registers as a reader of the slot, so a later model upload
+ * waits on the device for it. */
+int lig_filter_models_batch(lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                            const uint32_t* model_ids, int R, lig_mpick* out, int64_t* offsets,
+                            uint16_t* pods, int64_t capacity);
+int lig_filter_models_batch_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                                   const uint32_t* d_model_ids, int R, lig_mpick* d_out, int64_t* d_offsets,
+                                   uint16_t* d_pods, int64_t capacity, void* stream);
 
 /* ---- in-batch load feedback (opt-in; the default path never mutates the snapshot) ----------------
  * The reference schedules every request against the scraped metrics as they are

@@ -16,7 +16,7 @@ LIG_DRAW_DOMAIN = 0xA0761D6478BD642F
 LIG_ERR_INVALID, LIG_ERR_CUDA, LIG_ERR_STALE_EPOCH, LIG_ERR_NO_SNAPSHOT, LIG_ERR_RANGE = -1, -2, -3, -4, -5
 LIG_ERR_BUSY, LIG_ERR_NCCL = -6, -7
 LIG_MAX_TICKETS, LIG_COMM_ID_BYTES = 256, 128
-LIG_ABI_VERSION = 6
+LIG_ABI_VERSION = 7
 # filter node kinds of a caller filter tree (lig_set_filter_tree)
 (LIG_F_CRITICAL_REQUEST, LIG_F_LOW_QUEUEING, LIG_F_LORA_AFFINITY, LIG_F_CAN_ACCEPT_NEW_LORA, LIG_F_LOW_LORA_COST,
  LIG_F_NO_QUEUE_AND_LOW_KV, LIG_F_LEAST_QUEUING, LIG_F_LEAST_KV_CACHE, LIG_F_DROP) = range(9)
@@ -43,6 +43,7 @@ EXPORTED_SYMBOLS = (
     "lig_schedule_batch_feedback_chain", "lig_schedule_batch_feedback_chain_device", "lig_feedback_chain_reset",
     "lig_schedule_models_batch_feedback_chain", "lig_schedule_models_batch_feedback_chain_device",
     "lig_stream_submit_models",
+    "lig_filter_batch", "lig_filter_batch_device", "lig_filter_models_batch", "lig_filter_models_batch_device",
 )
 
 
@@ -146,6 +147,11 @@ def load() -> C.CDLL:
     lib.lig_schedule_models_batch_feedback_chain.argtypes = [vp, u64, u64, u64, vp, i32, vp, i32, vp]
     lib.lig_schedule_models_batch_feedback_chain_device.argtypes = [vp, u64, u64, u64, vp, i32, vp, i32, vp, vp]
     lib.lig_feedback_chain_reset.argtypes = [vp]
+    i64 = C.c_int64
+    lib.lig_filter_batch.argtypes = [vp, u64, u64, vp, i32, vp, vp, vp, i64]
+    lib.lig_filter_batch_device.argtypes = [vp, u64, u64, vp, i32, vp, vp, vp, i64, vp]
+    lib.lig_filter_models_batch.argtypes = [vp, u64, u64, u64, vp, i32, vp, vp, vp, i64]
+    lib.lig_filter_models_batch_device.argtypes = [vp, u64, u64, u64, vp, i32, vp, vp, vp, i64, vp]
     lib.lig_update_snapshot.argtypes = [vp, u64, u64, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.lig_pick_kernel_info.argtypes = [vp, u64, C.c_char_p, i32, C.POINTER(i32), C.POINTER(i32),
                                          C.POINTER(i32), C.POINTER(i32)]

@@ -370,6 +370,39 @@ Status Scheduler::ScheduleModel(const std::string& model, std::string* resolvedT
   return w.status;
 }
 
+Status Scheduler::Filter(const LLMRequest& req, std::vector<backend::Pod>* pods) {
+  if (group_)
+    return Errorf(InvalidArgument, "Filter: a scheduler over several devices has no survivor-list call");
+  if (pods) pods->clear();
+  lig_req r{};
+  lig_pick pick{};
+  int64_t offsets[2] = {0, 0};
+  std::vector<uint16_t> list;
+  std::shared_ptr<const Snapshot> snap;
+  int rc = 0;
+  for (int attempt = 0; attempt < 4; ++attempt) {
+    {
+      std::lock_guard<std::mutex> lk(snap_mu_);
+      snap = snap_;
+    }
+    if (!snap) return Errorf(Internal, "Filter: no snapshot uploaded yet");
+    auto it = snap->adapter_ids->find(req.ResolvedTargetModel);   // interned as in Flush
+    r.adapter_id = (it == snap->adapter_ids->end() || it->second >= snap->A) ? snap->A : it->second;
+    r.flags = req.Critical ? LIG_REQ_CRITICAL : 0u;
+    list.resize(std::max<size_t>(snap->pods.size(), 1));   // a survivor list never exceeds P
+    rc = lig_filter_batch(ctx_, snap->epoch, seed_, &r, 1, &pick, offsets, list.data(), (int64_t)list.size());
+    if (rc != LIG_ERR_STALE_EPOCH) break;   // two refreshes raced past this call: re-resolve
+  }
+  if (rc != 0) return LigFailure("lig_filter_batch");
+  if (pick.status == LIG_DROP)                                               // scheduler.go:83-89
+    return Errorf(ResourceExhausted, "dropping request due to limited backend resources");
+  if (pick.status == LIG_NO_PODS_LEFT)                                       // filter.go:88-90
+    return Errorf(Unknown, "no pods left");
+  if (pods)
+    for (int64_t k = offsets[0]; k < offsets[1]; ++k) pods->push_back(snap->pods[list[(size_t)k]]);
+  return Status{};
+}
+
 // Queue the waiter for the batcher and block until its result is published.
 void Scheduler::Submit(Waiter& w) {
   {

@@ -194,6 +194,15 @@ class Scheduler {
   // batch-level (CUDA) failure.                                       scheduler.go:113-122
   Status Schedule(const LLMRequest& req, backend::Pod* targetPod);
 
+  // The reference's Filter interface (filter.go:12-15) run on the current epoch: fills *pods with
+  // the survivors of req's walk of the filter tree (the built-in one or Options::filter), in slice
+  // order.  One blocking lig_filter_batch call on the caller's thread, outside the micro-batcher; no
+  // rand_key is taken.  Errors are the tree's own: ResourceExhausted "dropping request due to
+  // limited backend resources" for the drop leaf, Unknown "no pods left" when a caller tree ends on a
+  // predicate that kept no pod, Internal for a device failure; an empty result is OK with no pods.
+  // A scheduler over several devices refuses it with InvalidArgument.
+  Status Filter(const LLMRequest& req, std::vector<backend::Pod>* pods);
+
   // The resolve step of HandleRequestBody (handlers/request.go:42-56) followed by Schedule:
   // FetchModelData, RandomWeightedDraw when TargetModels is non-empty, IsCritical.  Fills
   // *resolvedTargetModel (the body's "model" is rewritten with it, request.go:60-69).  Errors as the

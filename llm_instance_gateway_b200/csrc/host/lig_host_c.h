@@ -49,6 +49,10 @@ void ligh_scheduler_free(ligh_scheduler*);
 /* Scheduler.Schedule: returns the gRPC code (0 OK, 8 ResourceExhausted, 2 Unknown, 13 Internal). */
 int ligh_schedule(ligh_scheduler*, const char* model, const char* resolved_target_model, int critical,
                   char* name, int name_cap, char* addr, int addr_cap, char* err, int err_cap);
+/* Scheduler::Filter: returns the gRPC code; names receives the survivors' pod names joined by '\n'
+ * (slice order) and *n_pods their count. */
+int ligh_filter(ligh_scheduler*, const char* resolved_target_model, int critical, char* names, int names_cap,
+                int* n_pods, char* err, int err_cap);
 int ligh_refresh(ligh_scheduler*, char* err, int err_cap);
 /* several GPUs behind one scheduler (lig_group_*) */
 ligh_scheduler* ligh_scheduler_new_devices(ligh_provider*, const int* devices, int n_devices, int max_pods,

@@ -1805,6 +1805,176 @@ int lig_resolve_models(lig_ctx* c, uint64_t epoch, uint64_t seed, uint64_t first
   return 0;
 }
 
+// ---- survivor lists of a batch (lig_filter_batch, lig_filter_models_batch) -------------------------
+// One filter call: descriptors (models = false) or model ids, and the four output buffers.
+struct FilterCall {
+  bool models;
+  uint64_t seed, first_index;
+  const void* in;
+  int R;
+  void* out;
+  int64_t* offsets;
+  uint16_t* pods;
+  int64_t capacity;
+  size_t in_bytes() const { return models ? sizeof(uint32_t) : sizeof(lig_req); }
+  size_t out_bytes() const { return models ? sizeof(lig_mpick) : sizeof(lig_pick); }
+};
+
+static int filter_check(const lig_ctx* c, const char* fn, const FilterCall& f) {
+  if (!c || f.R < 0 || f.capacity < 0 || !f.offsets || (f.R > 0 && (!f.in || !f.out)) ||
+      (f.capacity > 0 && !f.pods))
+    return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
+  return 0;
+}
+
+// Enqueue the filter kernel for f (R >= 1, device-visible pointers) against slot s on st, behind the
+// slot's tables, and register st as a reader of the slot.  The look-back state is stream-ordered
+// scratch: allocated, zeroed and freed on st.  Caller holds c->mu.
+static int enqueue_filter(lig_ctx* c, Slot& s, const FilterCall& f, cudaStream_t st) {
+  CUDA_TRY(cudaStreamWaitEvent(st, s.ready, 0));
+  if (f.models) CUDA_TRY(cudaStreamWaitEvent(st, s.models_ready, 0));
+  const int tiles = (f.R + kFilterTile - 1) / kFilterTile;
+  const size_t bytes = (size_t)tiles * sizeof(unsigned long long) + 16;
+  void* scratch = nullptr;
+  CUDA_TRY(cudaMallocAsync(&scratch, bytes, st));
+  cudaError_t e = cudaMemsetAsync(scratch, 0, bytes, st);
+  if (e == cudaSuccess) {
+    FilterOut fo;
+    fo.out = f.out;
+    fo.offsets = reinterpret_cast<long long*>(f.offsets);
+    fo.pods = f.pods;
+    fo.capacity = f.capacity;
+    fo.tiles = static_cast<unsigned long long*>(scratch);
+    fo.tile_counter = reinterpret_cast<uint32_t*>(fo.tiles + tiles);
+    const uint4* cls = reinterpret_cast<const uint4*>(s.d_cls);
+    if (f.models)
+      lig_filter_kernel<true><<<tiles, kFilterThreads, 0, st>>>(f.in, f.R, cls, s.d_lists, s.A, s.d_ctab, s.d_mtab,
+                                                                s.n_models, f.seed, f.first_index, fo);
+    else
+      lig_filter_kernel<false><<<tiles, kFilterThreads, 0, st>>>(f.in, f.R, cls, s.d_lists, s.A, s.d_ctab, nullptr,
+                                                                 0u, f.seed, 0, fo);
+    e = cudaGetLastError();
+  }
+  cudaFreeAsync(scratch, st);
+  if (e != cudaSuccess)
+    return fail(LIG_ERR_CUDA, "survivor-list kernel: %s", cudaGetErrorString(e));
+  c->launches++;
+  return note_reader(s, st);
+}
+
+static int filter_device(lig_ctx* c, const char* fn, uint64_t epoch, const FilterCall& f, void* stream) {
+  if (int rc = filter_check(c, fn, f)) return rc;
+  std::lock_guard<std::mutex> lk(c->mu);
+  Slot* s = nullptr;
+  if (int rc = f.models ? resolve_models_slot(c, epoch, &s) : resolve_slot(c, epoch, &s)) return rc;
+  CUDA_TRY(cudaSetDevice(c->device));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (f.R == 0) {
+    CUDA_TRY(cudaMemsetAsync(f.offsets, 0, sizeof(int64_t), st));
+    return 0;
+  }
+  return enqueue_filter(c, *s, f, st);
+}
+
+// Host buffers: page-locked ones are read and written by the kernel in place; the others are
+// staged in stream-ordered HBM and copied on the call's lane.  Blocks until everything is back.
+static int filter_host(lig_ctx* c, const char* fn, uint64_t epoch, const FilterCall& f) {
+  if (int rc = filter_check(c, fn, f)) return rc;
+  if (f.R > c->max_batch) return fail(LIG_ERR_INVALID, "%s: R=%d exceeds max_batch=%d", fn, f.R, c->max_batch);
+  FilterCall d = f;    // the same call with device-visible pointers
+  const size_t in_b = (size_t)f.R * f.in_bytes(), out_b = (size_t)f.R * f.out_bytes();
+  const size_t off_b = ((size_t)f.R + 1) * sizeof(int64_t);
+  d.in = f.R ? mapped_device_pointer(f.in) : nullptr;
+  d.out = f.R ? mapped_device_pointer(f.out) : nullptr;
+  d.offsets = f.R ? mapped_device_pointer(f.offsets) : nullptr;
+  d.pods = f.R && f.capacity > 0 ? mapped_device_pointer(f.pods) : nullptr;
+  const bool st_in = f.R && !d.in, st_out = f.R && !d.out, st_off = f.R && !d.offsets;
+  const bool st_pods = f.R && f.capacity > 0 && !d.pods;
+  cudaStream_t st = nullptr;
+  unsigned char* stage = nullptr;
+  size_t pods_entries = 0;
+  {
+    std::lock_guard<std::mutex> lk(c->mu);
+    Slot* s = nullptr;
+    if (int rc = f.models ? resolve_models_slot(c, epoch, &s) : resolve_slot(c, epoch, &s)) return rc;
+    if (f.R == 0) {
+      f.offsets[0] = 0;
+      return 0;
+    }
+    CUDA_TRY(cudaSetDevice(c->device));
+    st = c->s_lane[c->next_lane];
+    c->next_lane = (c->next_lane + 1) % kLanes;
+    // a list has at most P entries, so R * P bounds what a staged pod buffer can receive
+    if (st_pods) pods_entries = (size_t)std::min<int64_t>(f.capacity, (int64_t)f.R * (s->P > 0 ? s->P : 1));
+    size_t at = 0, o_in = 0, o_out = 0, o_off = 0, o_pods = 0;
+    auto take = [&](bool on, size_t bytes, size_t* o) { if (on) { *o = at; at = (at + bytes + 255) & ~(size_t)255; } };
+    take(st_in, in_b, &o_in);
+    take(st_out, out_b, &o_out);
+    take(st_off, off_b, &o_off);
+    take(st_pods, pods_entries * sizeof(uint16_t), &o_pods);
+    if (at) {
+      CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&stage), at, st));
+      if (st_in) d.in = stage + o_in;
+      if (st_out) d.out = stage + o_out;
+      if (st_off) d.offsets = reinterpret_cast<int64_t*>(stage + o_off);
+      if (st_pods) d.pods = reinterpret_cast<uint16_t*>(stage + o_pods);
+    }
+    int rc = 0;
+    if (st_in && cudaMemcpyAsync(const_cast<void*>(d.in), f.in, in_b, cudaMemcpyHostToDevice, st) != cudaSuccess)
+      rc = fail(LIG_ERR_CUDA, "%s: staging the requests failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
+    if (!rc) rc = enqueue_filter(c, *s, d, st);
+    if (rc) {
+      if (stage) cudaFreeAsync(stage, st);
+      return rc;
+    }
+  }
+  // the copies back wait for the kernel on the lane; they may block, so not under c->mu
+  cudaError_t e = cudaSuccess;
+  if (st_out && e == cudaSuccess) e = cudaMemcpyAsync(f.out, d.out, out_b, cudaMemcpyDeviceToHost, st);
+  if (st_off && e == cudaSuccess) e = cudaMemcpyAsync(f.offsets, d.offsets, off_b, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  const int64_t total = e == cudaSuccess ? f.offsets[f.R] : 0;
+  if (st_pods && e == cudaSuccess) {
+    const size_t n = (size_t)std::min<int64_t>(total, f.capacity);
+    if (n) e = cudaMemcpyAsync(f.pods, d.pods, n * sizeof(uint16_t), cudaMemcpyDeviceToHost, st);
+  }
+  if (stage) cudaFreeAsync(stage, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(LIG_ERR_CUDA, "%s failed on the device: %s", fn, cudaGetErrorString(e));
+  if (total > f.capacity)
+    return fail(LIG_ERR_INVALID, "%s: the survivor lists need %lld entries, capacity is %lld (out and offsets "
+                                 "are complete)", fn, (long long)total, (long long)f.capacity);
+  return 0;
+}
+
+int lig_filter_batch(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R, lig_pick* out,
+                     int64_t* offsets, uint16_t* pods, int64_t capacity) {
+  return filter_host(c, "lig_filter_batch", epoch,
+                     FilterCall{false, seed, 0, reqs, R, out, offsets, pods, capacity});
+}
+
+int lig_filter_batch_device(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* d_reqs, int R,
+                            lig_pick* d_out, int64_t* d_offsets, uint16_t* d_pods, int64_t capacity,
+                            void* stream) {
+  return filter_device(c, "lig_filter_batch_device", epoch,
+                       FilterCall{false, seed, 0, d_reqs, R, d_out, d_offsets, d_pods, capacity}, stream);
+}
+
+int lig_filter_models_batch(lig_ctx* c, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                            const uint32_t* model_ids, int R, lig_mpick* out, int64_t* offsets,
+                            uint16_t* pods, int64_t capacity) {
+  return filter_host(c, "lig_filter_models_batch", epoch,
+                     FilterCall{true, seed, first_index, model_ids, R, out, offsets, pods, capacity});
+}
+
+int lig_filter_models_batch_device(lig_ctx* c, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                                   const uint32_t* d_model_ids, int R, lig_mpick* d_out, int64_t* d_offsets,
+                                   uint16_t* d_pods, int64_t capacity, void* stream) {
+  return filter_device(c, "lig_filter_models_batch_device", epoch,
+                       FilterCall{true, seed, first_index, d_model_ids, R, d_out, d_offsets, d_pods, capacity},
+                       stream);
+}
+
 int lig_pick_kernel_info(lig_ctx* c, uint64_t epoch, char* name, int name_len, int* grid, int* threads,
                          int* table_bytes, int* tables_in_smem) {
   if (!c) return fail(LIG_ERR_INVALID, "lig_pick_kernel_info: ctx is null");

@@ -1427,14 +1427,17 @@ __global__ void lig_apply_delta_kernel(DeltaView d, double* __restrict__ kv, int
 // contiguous bytes and every store 256.  All loads of a thread are issued before the first use.
 constexpr int kPickThreads = 256;
 
+// `entry` (nullable) receives the class entry the pick used: the survivor-list kernel copies the
+// class's list from it.  Every other caller passes nothing and compiles as without it.
 __device__ __forceinline__ int2 pick_one(const int4 r, const uint4* __restrict__ cls,
                                          const uint16_t* __restrict__ lists, uint32_t A,
-                                         uint64_t seed) {
+                                         uint64_t seed, uint4* entry = nullptr) {
   const uint32_t critical = (uint32_t)r.y & LIG_REQ_CRITICAL;
   const uint64_t key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
   const uint32_t a = min((uint32_t)r.x, A);          // ids outside [0, A) (negative too) -> A
   const uint32_t c = critical * (A + 1u) + a;
   const uint4 e = __ldg(cls + c);                    // {info, magic, q_limit, list_off}
+  if (entry) *entry = e;
   const uint32_t k = int31n_entry(seed ^ key, e);
   // n == 0: list_off is the pool's 0xffff sentinel -> -1
   const int pod = (int)(short)__ldg(lists + (e.w + k));
@@ -2024,17 +2027,18 @@ __device__ __forceinline__ bool resolve_model(uint32_t m, const ModelTables& mt,
 }
 
 // One model request end to end; the class lookup as in pick_one / pick_one_smem / doorbell_pick.
+// `entry` (Ld::kLdg only, nullable): the class entry of the pick, untouched for LIG_NO_MODEL.
 template <Ld L>
 __device__ __forceinline__ uint32_t pick_model(uint32_t m, uint64_t key, const ModelTables& mt,
                                                const uint4* cls, const uint16_t* lists, uint32_t A,
-                                               uint64_t seed) {
+                                               uint64_t seed, uint4* entry = nullptr) {
   uint32_t adapter, critical, target;
   if (!resolve_model<L>(m, mt, seed, key, &adapter, &critical, &target))
     return pack_mpick(-1, (uint32_t)LIG_NO_MODEL, 255u);
   const int4 r = make_int4((int)adapter, (int)critical, (int)(uint32_t)key, (int)(uint32_t)(key >> 32));
   int2 p;
   if constexpr (L == Ld::kSmem) p = pick_one_smem(r, cls, lists, A, seed);
-  else if constexpr (L == Ld::kLdg) p = pick_one(r, cls, lists, A, seed);
+  else if constexpr (L == Ld::kLdg) p = pick_one(r, cls, lists, A, seed, entry);
   else p = doorbell_pick(r, cls, lists, A, seed);
   return pack_mpick(p.x, (uint32_t)p.y & 7u, target);
 }
@@ -2320,6 +2324,203 @@ lig_pick_models_count_kernel(const uint32_t* __restrict__ ids, uint32_t* __restr
       pod = (int)(int16_t)(v & 0xffffu);
     }
     count_window_picks(pod, lane, hist);
+  }
+}
+
+// ---- K2h: every request's survivor list next to its pick (lig_filter_batch, lig_filter_models_batch)
+// One pass over the batch in tiles of kFilterTile requests.  A CTA claims the next tile from a
+// counter (so every lower tile has started: the look-back below cannot wait on a CTA that is not
+// resident), and then
+//   1. picks each request exactly as lig_pick_stream_kernel / lig_pick_models_stream_kernel do
+//      (pick_one / pick_model<Ld::kLdg>: same bytes out) and keeps the class entry the pick used;
+//      n = the entry's survivor count for LIG_OK, else 0;
+//   2. scans the tile's n in shared memory and finds the tile's base offset with a decoupled
+//      look-back over the per-tile state words (Merrill & Garland, "Single-pass Parallel Prefix Scan
+//      with Decoupled Look-back", 2016);
+//   3. writes the tile's int64 offsets, then copies the tile's lists into one contiguous range of
+//      `pods`: output entry j of the tile belongs to the last request whose offset is <= j (binary
+//      search in shared memory), so consecutive threads store consecutive entries.  Entries at or
+//      beyond `capacity` are not written.
+// The lists come from the compact pool when the build sealed one (header bytes != 0), else from
+// the strided rows: the entries of both carry the same survivor sets.
+constexpr int kFilterThreads = 256;
+constexpr int kFilterPerThread = 4;
+constexpr int kFilterTile = kFilterThreads * kFilterPerThread;
+// Tile state: bits 62-63 = flag, bits 0-61 = value (a sum of n stays below 2^31 * 2^15 = 2^46).
+constexpr unsigned long long kScanAggregate = 1ull << 62, kScanPrefix = 2ull << 62;
+constexpr unsigned long long kScanValue = (1ull << 62) - 1;
+
+struct FilterOut {
+  void* out;                      // lig_pick[R] or lig_mpick[R]
+  long long* offsets;             // R + 1 entries
+  uint16_t* pods;                 // capacity entries (null when capacity is 0)
+  long long capacity;
+  unsigned long long* tiles;      // one state word per tile, zero before the launch
+  uint32_t* tile_counter;         // zero before the launch
+};
+
+__device__ __forceinline__ unsigned long long ld_volatile_u64(const unsigned long long* p) {
+  return *reinterpret_cast<const volatile unsigned long long*>(p);
+}
+__device__ __forceinline__ void st_volatile_u64(unsigned long long* p, unsigned long long v) {
+  *reinterpret_cast<volatile unsigned long long*>(p) = v;
+}
+
+// The base of `tile` (the sum of n over all lower tiles), given this tile's own sum.  Warp 0 only.
+__device__ __forceinline__ unsigned long long filter_look_back(unsigned long long* tiles, int tile,
+                                                               unsigned long long total, int lane) {
+  if (tile == 0) {
+    if (lane == 0) st_volatile_u64(tiles, kScanPrefix | total);
+    return 0;
+  }
+  if (lane == 0) st_volatile_u64(tiles + tile, kScanAggregate | total);
+  unsigned long long base = 0;
+  for (int last = tile - 1;; last -= 32) {
+    const int t = last - lane;      // lane 0 looks at the nearest predecessor
+    unsigned long long s = t >= 0 ? ld_volatile_u64(tiles + t) : kScanPrefix;
+    for (;;) {
+      const bool ready = (s >> 62) != 0;
+      if (__all_sync(kFull, ready)) break;
+      if (!ready) s = ld_volatile_u64(tiles + t);
+    }
+    const unsigned prefix = __ballot_sync(kFull, (s >> 62) == (kScanPrefix >> 62));
+    const int stop = prefix ? __ffs(prefix) - 1 : 31;    // nearest tile whose inclusive prefix is known
+    unsigned long long v = lane <= stop ? (s & kScanValue) : 0ull;
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(kFull, v, d);
+    base += v;
+    if (prefix) break;
+  }
+  if (lane == 0) st_volatile_u64(tiles + tile, kScanPrefix | (base + total));
+  return base;
+}
+
+template <bool kModels>
+__global__ void __launch_bounds__(kFilterThreads)
+lig_filter_kernel(const void* __restrict__ in, int R, const uint4* __restrict__ cls,
+                  const uint16_t* __restrict__ lists, int A, const unsigned char* __restrict__ ctab,
+                  const unsigned char* __restrict__ mtab, uint32_t n_models, uint64_t seed,
+                  uint64_t first_index, FilterOut fo) {
+  __shared__ __align__(16) uint32_t s_excl[kFilterTile + 4];   // tile-local exclusive offsets, [kFilterTile] = sum
+  __shared__ uint32_t s_list[kFilterTile];                    // list start of each request
+  __shared__ uint32_t s_warp[kFilterThreads / 32];
+  __shared__ unsigned long long s_base;
+  __shared__ int s_tile;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) s_tile = (int)atomicAdd(fo.tile_counter, 1u);
+  // the compact pool when the build sealed one
+  const CompactHeader hdr = *reinterpret_cast<const CompactHeader*>(ctab);
+  const uint32_t n_classes = 2u * ((uint32_t)A + 1u);
+  const uint4* gcls = cls;
+  const uint16_t* glists = lists;
+  if (hdr.bytes != 0u && hdr.n_classes == n_classes) {
+    gcls = reinterpret_cast<const uint4*>(ctab + sizeof(CompactHeader));
+    glists = reinterpret_cast<const uint16_t*>(ctab + sizeof(CompactHeader) + (size_t)n_classes * sizeof(ClassEntry));
+  }
+  __syncthreads();
+  const int tile = s_tile;
+  const int first = tile * kFilterTile;
+
+  // 1. picks and survivor counts
+  if constexpr (kModels) {
+    ModelTables mt;
+    mt.entries = reinterpret_cast<const uint4*>(mtab + sizeof(ModelHeader));
+    mt.targets = reinterpret_cast<const uint2*>(mt.entries + n_models);
+    mt.n_models = n_models;
+    const uint32_t* ids = static_cast<const uint32_t*>(in);
+    uint32_t* out = static_cast<uint32_t*>(fo.out);
+    uint32_t m[kFilterPerThread];
+#pragma unroll
+    for (int j = 0; j < kFilterPerThread; ++j) {
+      const int i = first + (int)threadIdx.x + j * kFilterThreads;
+      m[j] = i < R ? __ldg(ids + i) : 0u;
+    }
+#pragma unroll
+    for (int j = 0; j < kFilterPerThread; ++j) {
+      const int local = (int)threadIdx.x + j * kFilterThreads;
+      const int i = first + local;
+      uint32_t n = 0, off = 0;
+      if (i < R) {
+        uint4 e = make_uint4(0u, 0u, 0u, 0u);
+        const uint32_t v = pick_model<Ld::kLdg>(m[j], first_index + (uint64_t)i, mt, gcls, glists, (uint32_t)A,
+                                                seed, &e);
+        out[i] = v;
+        if (((v >> 16) & 0xffu) == (uint32_t)LIG_OK) { n = e.x >> 16; off = e.w; }
+      }
+      s_excl[local] = n;
+      s_list[local] = off;
+    }
+  } else {
+    const int4* reqs = static_cast<const int4*>(in);
+    int2* out = static_cast<int2*>(fo.out);
+    int4 r[kFilterPerThread];
+#pragma unroll
+    for (int j = 0; j < kFilterPerThread; ++j) {
+      const int i = first + (int)threadIdx.x + j * kFilterThreads;
+      r[j] = i < R ? ld_stream_int4(reqs + i) : make_int4(0, 0, 0, 0);
+    }
+#pragma unroll
+    for (int j = 0; j < kFilterPerThread; ++j) {
+      const int local = (int)threadIdx.x + j * kFilterThreads;
+      const int i = first + local;
+      uint32_t n = 0, off = 0;
+      if (i < R) {
+        uint4 e;
+        const int2 p = pick_one(r[j], gcls, glists, (uint32_t)A, seed, &e);
+        st_stream_int2(out + i, p);
+        if (((uint32_t)p.y & 7u) == (uint32_t)LIG_OK) { n = e.x >> 16; off = e.w; }
+      }
+      s_excl[local] = n;
+      s_list[local] = off;
+    }
+  }
+  __syncthreads();
+
+  // 2. tile-local exclusive scan (thread t owns requests 4t .. 4t+3), then the look-back
+  uint4 v = reinterpret_cast<const uint4*>(s_excl)[threadIdx.x];
+  const uint32_t own = v.x + v.y + v.z + v.w;
+  uint32_t incl = own;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t y = __shfl_up_sync(kFull, incl, d);
+    if (lane >= d) incl += y;
+  }
+  if (lane == 31) s_warp[warp] = incl;
+  __syncthreads();
+  uint32_t before = 0, total = 0;
+#pragma unroll
+  for (int w = 0; w < kFilterThreads / 32; ++w) {
+    before += w < warp ? s_warp[w] : 0u;
+    total += s_warp[w];
+  }
+  uint32_t run = before + incl - own;
+  const uint4 ex = make_uint4(run, run + v.x, run + v.x + v.y, run + v.x + v.y + v.z);
+  reinterpret_cast<uint4*>(s_excl)[threadIdx.x] = ex;
+  if (threadIdx.x == 0) s_excl[kFilterTile] = total;
+  if (warp == 0) {
+    const unsigned long long base = filter_look_back(fo.tiles, tile, total, lane);
+    if (lane == 0) s_base = base;
+  }
+  __syncthreads();
+  const unsigned long long base = s_base;
+
+  // 3. offsets, then the lists
+#pragma unroll
+  for (int j = 0; j < kFilterPerThread; ++j) {
+    const int local = (int)threadIdx.x + j * kFilterThreads;
+    if (first + local < R) fo.offsets[first + local] = (long long)(base + s_excl[local]);
+  }
+  if (threadIdx.x == 0 && R - first <= kFilterTile) fo.offsets[R] = (long long)(base + total);
+  const long long room = fo.capacity - (long long)base;
+  const uint32_t limit = room <= 0 ? 0u : (room < (long long)total ? (uint32_t)room : total);
+  uint16_t* dst = fo.pods + base;
+  for (uint32_t j = threadIdx.x; j < limit; j += kFilterThreads) {
+    int lo = 0, hi = kFilterTile;   // s_excl[lo] <= j < s_excl[hi]
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (s_excl[mid] <= j) lo = mid; else hi = mid;
+    }
+    dst[j] = __ldg(glists + s_list[lo] + (j - s_excl[lo]));
   }
 }
 

@@ -214,6 +214,64 @@ class Engine:
         """The next feedback-chain call starts a new chain from its epoch's scrape."""
         N.check(self._lib.lig_feedback_chain_reset(self._ctx))
 
+    # ---- survivor lists of a batch: Filter.Filter next to the pick ----
+    def _filter(self, fn, args, R: int, out: np.ndarray, capacity: Optional[int]):
+        """Call a host filter form with a pod buffer of `capacity` entries (default 4 per request);
+        when the lists need more, call once more with exactly what offsets[R] asks for."""
+        offsets = np.full(R + 1, -1, dtype=np.int64)
+        cap = 4 * R if capacity is None else capacity
+        for _ in range(2):
+            pods = np.empty(cap, dtype=np.uint16)
+            rc = fn(self._ctx, *args, _ptr(out), _ptr(offsets), _ptr(pods), cap)
+            if rc == N.LIG_ERR_INVALID and capacity is None and int(offsets[R]) > cap:
+                cap = int(offsets[R])
+                continue
+            break
+        N.check(rc)
+        return out, offsets, pods[: int(offsets[R])]
+
+    def filter_batch(self, epoch: int, seed: int, reqs: np.ndarray, capacity: Optional[int] = None):
+        """lig_filter_batch: (picks, int64 offsets[R + 1], uint16 pods) where request i's survivors are
+        pods[offsets[i]:offsets[i + 1]] and picks equal schedule_batch's.  With `capacity` given, the
+        pod buffer has that many entries and a larger total raises LigError."""
+        assert reqs.dtype == REQ_DTYPE and reqs.flags.c_contiguous
+        R = int(reqs.shape[0])
+        return self._filter(self._lib.lig_filter_batch, (epoch, seed, _ptr(reqs), R), R,
+                            np.empty(R, dtype=PICK_DTYPE), capacity)
+
+    def filter_models_batch(self, epoch: int, seed: int, model_ids: np.ndarray, first_index: int = 0,
+                            capacity: Optional[int] = None):
+        """lig_filter_models_batch: (picks, offsets, pods) as filter_batch, the picks those of
+        schedule_models_batch with the same first_index."""
+        assert model_ids.dtype == np.uint32 and model_ids.flags.c_contiguous
+        R = int(model_ids.shape[0])
+        return self._filter(self._lib.lig_filter_models_batch, (epoch, seed, first_index, _ptr(model_ids), R), R,
+                            np.empty(R, dtype=MPICK_DTYPE), capacity)
+
+    def filter_batch_ptr(self, epoch: int, seed: int, h_reqs: int, R: int, h_out: int, h_offsets: int, h_pods: int,
+                         capacity: int) -> None:
+        N.check(self._lib.lig_filter_batch(self._ctx, epoch, seed, h_reqs or None, R, h_out or None,
+                                           h_offsets or None, h_pods or None, capacity))
+
+    def filter_models_batch_ptr(self, epoch: int, seed: int, first_index: int, h_ids: int, R: int, h_out: int,
+                                h_offsets: int, h_pods: int, capacity: int) -> None:
+        N.check(self._lib.lig_filter_models_batch(self._ctx, epoch, seed, first_index, h_ids or None, R, h_out or None,
+                                                  h_offsets or None, h_pods or None, capacity))
+
+    def filter_batch_device(self, epoch: int, seed: int, d_reqs: int, R: int, d_out: int, d_offsets: int,
+                            d_pods: int, capacity: int, stream: int = 0) -> None:
+        """lig_filter_batch_device: device pointers, enqueued on `stream` (not synchronised); the
+        caller checks offsets[R] against `capacity`."""
+        N.check(self._lib.lig_filter_batch_device(self._ctx, epoch, seed, d_reqs or None, R, d_out or None,
+                                                  d_offsets or None, d_pods or None, capacity, stream or None))
+
+    def filter_models_batch_device(self, epoch: int, seed: int, first_index: int, d_ids: int, R: int, d_out: int,
+                                   d_offsets: int, d_pods: int, capacity: int, stream: int = 0) -> None:
+        """lig_filter_models_batch_device: the model-id form of filter_batch_device."""
+        N.check(self._lib.lig_filter_models_batch_device(self._ctx, epoch, seed, first_index, d_ids or None, R,
+                                                         d_out or None, d_offsets or None, d_pods or None, capacity,
+                                                         stream or None))
+
     def pick_kernel_info(self, epoch: int) -> dict:
         name = C.create_string_buffer(64)
         grid, threads, tb, in_smem = C.c_int(), C.c_int(), C.c_int(), C.c_int()

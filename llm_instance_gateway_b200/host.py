@@ -28,6 +28,7 @@ EXPORTED_SYMBOLS = (
     "ligh_scheduler_new_devices", "ligh_datastore_new", "ligh_datastore_free", "ligh_datastore_set_model",
     "ligh_schedule_model", "ligh_scheduler_new_tree", "ligh_scheduler_new_feedback", "ligh_feedback_stats",
     "ligh_scheduler_set_models", "ligh_schedule_model_device", "ligh_model_stats", "ligh_schedule_models_concurrent",
+    "ligh_filter",
 )
 
 _lib = None
@@ -76,6 +77,7 @@ def load() -> C.CDLL:
     lib.ligh_schedule.argtypes = [vp, C.c_char_p, C.c_char_p, i32, C.c_char_p, i32, C.c_char_p, i32,
                                   C.c_char_p, i32]
     lib.ligh_refresh.argtypes = [vp, C.c_char_p, i32]
+    lib.ligh_filter.argtypes = [vp, C.c_char_p, i32, C.c_char_p, i32, C.POINTER(i32), C.c_char_p, i32]
     lib.ligh_stats.argtypes = [vp, vp]
     lib.ligh_stats.restype = None
     lib.ligh_refresh_timing.argtypes = [vp, vp]
@@ -179,6 +181,14 @@ class HostScheduler:
         if code == GRPC_OK:
             return code, Pod(name.value.decode(), addr.value.decode()), ""
         return code, None, err.value.decode("utf-8", "replace")
+
+    def Filter(self, resolved: str, critical: bool) -> Tuple[int, List[str], str]:  # noqa: N802
+        """Scheduler::Filter: (gRPC code, survivor pod names in slice order, error message)."""
+        cap = 4 << 20
+        names, err, n = C.create_string_buffer(cap), C.create_string_buffer(512), C.c_int(0)
+        code = self._lib.ligh_filter(self._s, resolved.encode(), int(critical), names, cap, C.byref(n), err, 512)
+        pods = names.value.decode().split("\n") if n.value else []
+        return code, pods, err.value.decode("utf-8", "replace") if code != GRPC_OK else ""
 
     def Refresh(self) -> None:  # noqa: N802
         err = C.create_string_buffer(512)

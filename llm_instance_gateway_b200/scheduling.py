@@ -15,7 +15,8 @@ form the Go adapter uses under load (one C-ABI call per batch); ``NewScheduler(p
 carries load feedback across those calls until the next refresh (off by default).  ``SetInferenceModels`` plus
 ``ScheduleModel`` / ``ScheduleModelBatch`` take the request's model name instead of a resolved request: the
 resolve step of HandleRequestBody (handlers/request.go:42-56) runs on the device against a model table that
-every snapshot epoch carries.  There is no CPU path here: without liblig.so or without a CUDA device
+every snapshot epoch carries.  ``FilterBatch`` / ``FilterModelBatch`` return the survivor slices of a whole
+batch (Filter.Filter, filter.go:12-15) in one device call, for any filter tree.  There is no CPU path here: without liblig.so or without a CUDA device
 construction fails.
 """
 from __future__ import annotations
@@ -349,6 +350,55 @@ class Scheduler:
         if st == N.LIG_DROP:
             return [], StatusError("ResourceExhausted", _DROP_DESC)
         return survivors, None
+
+    def _survivors(self, snap: PackedSnapshot, status: int, pods: np.ndarray) -> Tuple[List[Pod], Optional[StatusError]]:
+        if status == N.LIG_DROP:
+            return [], StatusError("ResourceExhausted", _DROP_DESC)
+        if status == N.LIG_NO_PODS_LEFT:
+            return [], StatusError("Unknown", "no pods left")
+        return [snap.pods[int(p)] for p in pods], None
+
+    def FilterBatch(self, reqs: Sequence[LLMRequest]) -> List[Tuple[List[Pod], Optional[StatusError]]]:
+        """Filter for a whole batch in one device call (lig_filter_batch): (survivors, error) per
+        request, as Filter returns them, for the built-in tree and for a caller tree alike.  The
+        scraped epoch, like Filter; the requests take no rand_key."""
+        snap = self._current()
+        arr = np.zeros(len(reqs), dtype=REQ_DTYPE)
+        for i, r in enumerate(reqs):
+            arr[i] = (snap.adapter_id(r.ResolvedTargetModel), N.LIG_REQ_CRITICAL if r.Critical else 0, 0)
+        picks, offsets, pods = self._engine.filter_batch(self._epoch, self._seed, arr)
+        return [self._survivors(snap, int(pk["status"]), pods[offsets[i]:offsets[i + 1]])
+                for i, pk in enumerate(picks)]
+
+    def FilterModelBatch(self, names: Sequence[str]) -> List[Tuple[List[Pod], Optional[StatusError]]]:
+        """The survivors of model requests (lig_filter_models_batch): the resolve step of
+        ScheduleModelBatch, then Filter on the resolved request.  (survivors, error) per name; names
+        the host answers from the list alone get ScheduleModelBatch's errors.  The draws use
+        ScheduleModelBatch's rand_key sequence without advancing it."""
+        snap = self._current()
+        pm = self._packed_models
+        out: List[Tuple[List[Pod], Optional[StatusError]]] = [None] * len(names)  # type: ignore
+        ids, slots = [], []
+        for i, name in enumerate(names):
+            m = pm.model_ids.get(name) if pm is not None else None
+            if m is None:                                                       # request.go:42-45
+                out[i] = ([], StatusError("Unknown", f"error finding a model object in InferenceModel for input {name}"))
+            elif not pm.present[m]:                                             # request.go:48-51
+                out[i] = ([], StatusError("Unknown", f"error getting target model name for model {name}"))
+            else:
+                ids.append(m)
+                slots.append(i)
+        if not ids:
+            return out
+        picks, offsets, pods = self._engine.filter_models_batch(self._epoch, self._seed, np.array(ids, dtype=np.uint32),
+                                                                first_index=self._model_index)
+        for k, (i, m, pk) in enumerate(zip(slots, ids, picks)):
+            st = int(pk["status"])
+            if st == N.LIG_NO_MODEL:         # absent models never reach the device
+                out[i] = ([], StatusError("Internal", _no_model_entry(m, names[i])))
+            else:
+                out[i] = self._survivors(snap, st, pods[offsets[k]:offsets[k + 1]])
+        return out
 
 
 def NewScheduler(pmp: PodMetricsProvider, filter: Optional[Filter] = None, load_feedback_window: int = 0,
