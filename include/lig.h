@@ -107,7 +107,14 @@ int  lig_create(lig_ctx** out, int device, int max_pods, int max_adapters, int m
 void lig_destroy(lig_ctx* ctx);
 
 /* With a caller filter tree set (lig_set_filter_tree) the thresholds are still stored but do not
- * affect the class-table build: every node of a caller tree carries its own thresholds. */
+ * affect the class-table build: every node of a caller tree carries its own thresholds.
+ * Every value of the three fields is legal (Go's thresholds are int and float64): queue thresholds
+ * are compared as int64, the KV threshold as binary64 (a NaN threshold keeps no pod).
+ * Resident epochs whose tables the built-in tree built are rebuilt with the new thresholds before
+ * the call returns; epochs a caller tree built keep their tables.  A rebuild waits for the work
+ * already enqueued against the epoch (on any stream), which sees the old tables, so the call can
+ * block until that work is done; everything enqueued after the return sees the new ones.  A
+ * feedback chain keeps the thresholds it started with (see below). */
 int  lig_set_thresholds(lig_ctx* ctx, const lig_thresholds* t);   /* scheduler.go:15-24 */
 int  lig_get_thresholds(const lig_ctx* ctx, lig_thresholds* t);
 
@@ -166,7 +173,8 @@ int  lig_set_filter_tree(lig_ctx* ctx, const lig_filter_node* nodes, int n_nodes
  *   uint16_t n_active[Ppad]    len(Metrics.ActiveModels)             backend/types.go:19
  *   uint16_t max_active[Ppad]  Metrics.MaxActiveModels (saturated)   backend/types.go:21
  *   uint32_t bitmap[A][W]      bit (a, p) = adapter a in pod p's ActiveModels (adapter-major)
- * Padding pods (index >= P) are ignored by every kernel.
+ * Padding pods (index >= P), their bits in the last word of each bitmap row and the bytes after
+ * the bitmap are ignored by every kernel, whatever they hold.
  */
 size_t lig_snapshot_bytes(int P, int A);
 
@@ -179,7 +187,10 @@ int lig_pack_pods(int P, const int64_t* waiting_queue_size, const int64_t* n_act
                   const int64_t* max_active_models, int32_t* q_out, uint16_t* n_active_out,
                   uint16_t* max_active_out);
 
-/* Pure host helper (no GPU): lay the five arrays out as the packed blob described above. */
+/* Pure host helper (no GPU): lay the five arrays out as the packed blob described above, with
+ * padding pods and tail bits zeroed.  LIG_ERR_INVALID for a null blob, P or A < 0, a null pod
+ * column when P > 0 or a null bitmap when P > 0 and A > 0; LIG_ERR_RANGE when a pod's n_active
+ * exceeds LIG_MAX_ADAPTERS.  Nothing is written when the call is refused. */
 int lig_pack_snapshot(void* blob, int P, int A, const double* kv, const int32_t* q,
                       const uint16_t* n_active, const uint16_t* max_active,
                       const uint32_t* bitmap_adapter_major /* A x ceil(P/32) */);
@@ -187,7 +198,11 @@ int lig_pack_snapshot(void* blob, int P, int A, const double* kv, const int32_t*
 /* Upload a snapshot from host arrays and build the per-class survivor tables on the device.
  * After it returns, `epoch` is resident; the previous epoch stays resident too (two slots), so
  * in-flight batches against it still complete.  Replaces the per-request
- * AllPodMetrics() materialisation of scheduler.go:114-115 by one pack per refresh tick. */
+ * AllPodMetrics() materialisation of scheduler.go:114-115 by one pack per refresh tick.
+ * Refused, before any slot is touched (both resident epochs and their model tables stay as they
+ * were, also when `epoch` is one of them), for the reasons of lig_pack_snapshot and with
+ * LIG_ERR_INVALID for P > max_pods or A > max_adapters.  The _async form and
+ * lig_group_upload_snapshot refuse the same arguments the same way. */
 int lig_upload_snapshot(lig_ctx* ctx, uint64_t epoch, int P, int A, const double* kv,
                         const int32_t* q, const uint16_t* n_active, const uint16_t* max_active,
                         const uint32_t* bitmap_adapter_major);
@@ -214,7 +229,8 @@ int lig_upload_snapshot_async(lig_ctx* ctx, uint64_t epoch, int P, int A, const 
  *   - a pod index is outside [0, P) or appears more than once in pod_idx;
  *   - adapter_offsets[0] != 0, or adapter_offsets decreases anywhere;
  *   - an adapter id is outside [0, A) of the base.
- * The same id twice within one pod's list is allowed (it sets the same bit). */
+ * LIG_ERR_RANGE, likewise before anything is written, when a dirty pod's n_active exceeds
+ * LIG_MAX_ADAPTERS.  The same id twice within one pod's list is allowed (it sets the same bit). */
 int lig_update_snapshot(lig_ctx* ctx, uint64_t new_epoch, uint64_t base_epoch, int n_dirty,
                         const int32_t* pod_idx, const double* kv, const int32_t* q,
                         const uint16_t* n_active, const uint16_t* max_active,
@@ -222,7 +238,10 @@ int lig_update_snapshot(lig_ctx* ctx, uint64_t new_epoch, uint64_t base_epoch, i
 
 /* Same, but the packed blob is already in HBM (e.g. the receive buffer of an NCCL broadcast of
  * the snapshot).  The blob is copied into the ctx on `stream` (a cudaStream_t, may be NULL =
- * legacy default stream); table build is enqueued on the same stream, nothing is synchronised. */
+ * legacy default stream); table build is enqueued on the same stream, nothing is synchronised.
+ * The blob is taken as it is: padding pods may hold anything (they are ignored), and every real
+ * pod's n_active <= LIG_MAX_ADAPTERS is the caller's contract (lig_pack_snapshot checks it on the
+ * host; this form and lig_comm_upload_snapshot_device do not read the blob on the host). */
 int lig_upload_snapshot_device(lig_ctx* ctx, uint64_t epoch, int P, int A, const void* d_blob,
                                void* stream);
 

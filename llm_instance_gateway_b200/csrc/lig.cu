@@ -737,6 +737,56 @@ int submit_mapped(lig_ctx* c, Slot* s, uint64_t seed, const lig_req* dev_in, int
   return 0;
 }
 
+// n_active of a pod record: len(ActiveModels) <= LIG_MAX_ADAPTERS (a uint16 can hold 65535, which
+// beside a saturated MaxActiveModels of 65535 would read as "no room").
+int check_n_active(const uint16_t* na, int n) {
+  for (int i = 0; i < n; ++i)
+    if (na[i] > LIG_MAX_ADAPTERS)
+      return fail(LIG_ERR_RANGE, "pod record %d: n_active %u outside [0, %d]", i, (unsigned)na[i], LIG_MAX_ADAPTERS);
+  return 0;
+}
+
+// The host arrays of a snapshot pack.  Host uploads call this before begin_write, so a refused
+// upload evicts no resident epoch and no model table.
+int check_snapshot_arrays(int P, int A, const double* kv, const int32_t* q, const uint16_t* na,
+                          const uint16_t* ma, const uint32_t* bitmap) {
+  if (P < 0 || A < 0) return fail(LIG_ERR_INVALID, "snapshot shape P=%d A=%d", P, A);
+  if (P > 0 && (!kv || !q || !na || !ma)) return fail(LIG_ERR_INVALID, "null pod column");
+  if (A > 0 && P > 0 && !bitmap) return fail(LIG_ERR_INVALID, "null bitmap");
+  return check_n_active(na, P);
+}
+
+// Lay checked host arrays out as the packed blob (lig.h).
+void pack_blob(void* blob, int P, int A, const double* kv, const int32_t* q, const uint16_t* na,
+               const uint16_t* ma, const uint32_t* bitmap) {
+  const Layout l = layout_for(P, A);
+  unsigned char* b = static_cast<unsigned char*>(blob);
+  if (P == 0) {
+    memset(b, 0, l.total);
+    return;
+  }
+  // copy the P real pods and zero only the padding pods of each column (no full-blob memset)
+  const size_t pad = (size_t)words_for(P) * 32 - (size_t)P;
+  memcpy(b + l.kv, kv, (size_t)P * sizeof(double));
+  memset(b + l.kv + (size_t)P * sizeof(double), 0, pad * sizeof(double));
+  memcpy(b + l.q, q, (size_t)P * sizeof(int32_t));
+  memset(b + l.q + (size_t)P * sizeof(int32_t), 0, pad * sizeof(int32_t));
+  memcpy(b + l.na, na, (size_t)P * sizeof(uint16_t));
+  memset(b + l.na + (size_t)P * sizeof(uint16_t), 0, pad * sizeof(uint16_t));
+  memcpy(b + l.ma, ma, (size_t)P * sizeof(uint16_t));
+  memset(b + l.ma + (size_t)P * sizeof(uint16_t), 0, pad * sizeof(uint16_t));
+  const size_t bm_bytes = (size_t)A * words_for(P) * sizeof(uint32_t);
+  if (A > 0) memcpy(b + l.bitmap, bitmap, bm_bytes);
+  memset(b + l.bitmap + bm_bytes, 0, l.total - l.bitmap - bm_bytes);
+  // bits of padding pods must be clear in the last word of every row
+  const int W = words_for(P), rem = P & 31;
+  if (rem) {
+    uint32_t* bm = reinterpret_cast<uint32_t*>(b + l.bitmap);
+    const uint32_t keep = (1u << rem) - 1u;
+    for (int a = 0; a < A; ++a) bm[(size_t)a * W + (W - 1)] &= keep;
+  }
+}
+
 }  // namespace
 
 // ---- snapshot-writer protocol (lig_internal.hpp) ----------------------------------------------------
@@ -883,34 +933,9 @@ int lig_pack_pods(int P, const int64_t* q, const int64_t* na, const int64_t* ma,
 
 int lig_pack_snapshot(void* blob, int P, int A, const double* kv, const int32_t* q,
                       const uint16_t* na, const uint16_t* ma, const uint32_t* bitmap) {
-  if (!blob || P < 0 || A < 0) return fail(LIG_ERR_INVALID, "lig_pack_snapshot: bad argument");
-  if (P > 0 && (!kv || !q || !na || !ma)) return fail(LIG_ERR_INVALID, "null pod column");
-  if (A > 0 && P > 0 && !bitmap) return fail(LIG_ERR_INVALID, "null bitmap");
-  const Layout l = layout_for(P, A);
-  unsigned char* b = static_cast<unsigned char*>(blob);
-  if (P == 0) memset(b, 0, l.total);
-  if (P > 0) {
-    // copy the P real pods and zero only the padding pods of each column (no full-blob memset)
-    const size_t pad = (size_t)words_for(P) * 32 - (size_t)P;
-    memcpy(b + l.kv, kv, (size_t)P * sizeof(double));
-    memset(b + l.kv + (size_t)P * sizeof(double), 0, pad * sizeof(double));
-    memcpy(b + l.q, q, (size_t)P * sizeof(int32_t));
-    memset(b + l.q + (size_t)P * sizeof(int32_t), 0, pad * sizeof(int32_t));
-    memcpy(b + l.na, na, (size_t)P * sizeof(uint16_t));
-    memset(b + l.na + (size_t)P * sizeof(uint16_t), 0, pad * sizeof(uint16_t));
-    memcpy(b + l.ma, ma, (size_t)P * sizeof(uint16_t));
-    memset(b + l.ma + (size_t)P * sizeof(uint16_t), 0, pad * sizeof(uint16_t));
-    const size_t bm_bytes = (size_t)A * words_for(P) * sizeof(uint32_t);
-    if (A > 0) memcpy(b + l.bitmap, bitmap, bm_bytes);
-    memset(b + l.bitmap + bm_bytes, 0, l.total - l.bitmap - bm_bytes);
-    // bits of padding pods must be clear in the last word of every row
-    const int W = words_for(P), rem = P & 31;
-    if (rem) {
-      uint32_t* bm = reinterpret_cast<uint32_t*>(b + l.bitmap);
-      const uint32_t keep = (1u << rem) - 1u;
-      for (int a = 0; a < A; ++a) bm[(size_t)a * W + (W - 1)] &= keep;
-    }
-  }
+  if (!blob) return fail(LIG_ERR_INVALID, "lig_pack_snapshot: null blob");
+  if (int rc = check_snapshot_arrays(P, A, kv, q, na, ma, bitmap)) return rc;
+  pack_blob(blob, P, A, kv, q, na, ma, bitmap);
   return 0;
 }
 
@@ -1228,13 +1253,16 @@ static int upload_snapshot_impl(lig_ctx* c, uint64_t epoch, int P, int A, const 
                                 const int32_t* q, const uint16_t* na, const uint16_t* ma,
                                 const uint32_t* bitmap, bool synchronise) {
   if (!c) return fail(LIG_ERR_INVALID, "lig_upload_snapshot: ctx is null");
+  // begin_write evicts the slot the epoch replaces: refuse bad arrays before it
+  if (int rc = check_snapshot_arrays(P, A, kv, q, na, ma, bitmap)) return rc;
   ligi::SnapshotWrite w;
   if (int rc = ligi::begin_write(c, epoch, P, A, nullptr, true, &w)) return rc;
   // The ctx lock is NOT held from here to the publish: batches against the other resident epoch
   // keep flowing while this one is packed, copied and its tables are built.  The slot's pinned
   // staging blob is free: begin_write waited for the slot's previous upload.
-  int rc = lig_pack_snapshot(w.h_blob, P, A, kv, q, na, ma, bitmap);
-  if (!rc && cudaMemcpyAsync(w.d_blob, w.h_blob, w.bytes, cudaMemcpyHostToDevice, w.stream) != cudaSuccess)
+  pack_blob(w.h_blob, P, A, kv, q, na, ma, bitmap);
+  int rc = 0;
+  if (cudaMemcpyAsync(w.d_blob, w.h_blob, w.bytes, cudaMemcpyHostToDevice, w.stream) != cudaSuccess)
     rc = fail(LIG_ERR_CUDA, "snapshot H2D copy failed: %s", cudaGetErrorString(cudaGetLastError()));
   if (!rc) rc = ligi::enqueue_build(c, &w);
   if (rc) {
@@ -1290,6 +1318,7 @@ int lig_update_snapshot(lig_ctx* c, uint64_t new_epoch, uint64_t base_epoch, int
         return fail(LIG_ERR_INVALID, "adapter_offsets decrease at entry %d (%d -> %d)", i + 1, a_off[i], a_off[i + 1]);
     for (int k = 0; k < n_ids; ++k)
       if (a_ids[k] < 0 || a_ids[k] >= A) return fail(LIG_ERR_INVALID, "adapter id %d outside [0, %d)", a_ids[k], A);
+    if (int rc = check_n_active(na, n_dirty)) return rc;
   }
   ligi::SnapshotWrite w;
   if (int rc = ligi::begin_write(c, new_epoch, P, A, nullptr, true, &w)) return rc;
