@@ -272,7 +272,8 @@ void  lig_host_free(void* p);
 
 /* Host buffers in, host buffers out.  Nothing is staged through HBM: the pick kernel reads the
  * descriptors from, and writes the picks to, page-locked host memory over PCIe directly.  Blocks
- * until `out` is complete. */
+ * until `out` is complete.  The kernels read a lig_req with one 16-byte load: a request array that
+ * is not 16-byte aligned is staged like pageable memory. */
 int lig_schedule_batch(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
                        lig_pick* out);
 
@@ -282,7 +283,8 @@ int lig_schedule_batch(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_re
  * cudaHostAlloc / cudaHostRegister) and stay untouched until the wait returns.  On success
  * *ticket identifies the in-flight batch; lig_schedule_wait blocks until its picks are complete and
  * releases the ticket.  The ctx lock is held only while the work is enqueued, never while waiting.
- * LIG_ERR_BUSY when all LIG_MAX_TICKETS tickets are in flight. */
+ * LIG_ERR_BUSY when all LIG_MAX_TICKETS tickets are in flight; LIG_ERR_INVALID when `reqs` is not
+ * 16-byte aligned. */
 #define LIG_MAX_TICKETS 256
 int lig_schedule_batch_async(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
                              lig_pick* out, int* ticket);
@@ -295,9 +297,10 @@ int lig_schedule_batch_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const
 
 /* A queue of n_batches HBM-resident batches of R requests each against one epoch, enqueued
  * back to back on `stream` with one pass through the ABI (the micro-batcher's flush of several
- * pending batches).  Batch b uses seed `seed + b`, reads d_reqs[b] and writes d_out[b]; the two
- * pointer arrays are host arrays of device pointers.  Equivalent to n_batches calls of
- * lig_schedule_batch_device. */
+ * pending batches).  Batch b uses seed `seed + b` (mod 2^64: a seed near 2^64 wraps to 0), reads
+ * d_reqs[b] and writes d_out[b]; the two pointer arrays are host arrays of device pointers.
+ * Equivalent to n_batches calls of lig_schedule_batch_device, however long the queue (the library
+ * splits it into several launches where it must). */
 int lig_schedule_batches_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed,
                                 const lig_req* const* d_reqs, int R, lig_pick* const* d_out,
                                 int n_batches, void* stream);
@@ -363,8 +366,9 @@ int lig_read_class(lig_ctx* ctx, uint64_t epoch, int critical, int adapter_id, i
  * randomVal -= Weight[k] (datastore.go:91-97).  A model with exactly one target skips the draw
  * (its result cannot depend on it).  The pick then uses state = seed ^ rand_key as always, so
  * lig_schedule_models_batch(ids) == lig_schedule_batch(descriptors resolved on the host).
- * rand_key of request i of a call is first_index + i (a counter-based key: shards of one batch
- * pass their offset and get the single-device result). */
+ * rand_key of request i of a call is first_index + i, mod 2^64 (a counter-based key: shards of one
+ * batch pass their offset and get the single-device result; a first_index near 2^64 wraps to 0
+ * inside the batch). */
 #define LIG_DRAW_DOMAIN 0xA0761D6478BD642Full
 typedef struct lig_mpick {
   int16_t pod_idx;     /* as lig_pick.pod_idx (-1 unless LIG_OK)                                  */
@@ -383,7 +387,8 @@ int lig_upload_models_async(lig_ctx* ctx, uint64_t epoch, int n_models, const in
 int lig_schedule_models_batch(lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64_t first_index,
                               const uint32_t* model_ids, int R, lig_mpick* out);
 /* HBM-resident queue of n_batches batches of R model ids (4-byte aligned; 16-byte aligned buffers
- * take the TMA path), batch b with seed + b; enqueued on `stream`, not synchronised. */
+ * take the TMA path), batch b with seed + b (mod 2^64) and the same first_index; enqueued on
+ * `stream`, not synchronised. */
 int lig_schedule_models_batches_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64_t first_index,
                                        const uint32_t* const* d_model_ids, int R,
                                        lig_mpick* const* d_out, int n_batches, void* stream);
@@ -425,8 +430,8 @@ int lig_stream_submit_models(lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64
  *     chain's private copy: the survivor sets of the scraped metrics.
  *   - refused like the call each form mirrors: stale epoch, null buffers, R > max_batch on the host
  *     forms; the model forms also with LIG_ERR_NO_SNAPSHOT when the epoch has no model table.
- * Host forms: page-locked buffers are read and written in place, pageable ones are staged; they
- * block until everything is back.  Device forms: device pointers, enqueued on `stream` (a
+ * Host forms: page-locked buffers are read and written in place, pageable ones (and a request
+ * array that is not 16-byte aligned) are staged; they block until everything is back.  Device forms: device pointers, enqueued on `stream` (a
  * cudaStream_t, NULL = legacy default stream), not synchronised. */
 /* descriptors: out is byte for byte lig_schedule_batch(ctx, epoch, seed, reqs, R, out) */
 int lig_filter_batch(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
@@ -588,6 +593,20 @@ int         lig_sm_count(const lig_ctx* ctx);
  * the compact tables (0 = not available / strided tables in use). */
 int         lig_pick_kernel_info(lig_ctx* ctx, uint64_t epoch, char* name, int name_len, int* grid,
                                  int* threads, int* table_bytes, int* tables_in_smem);
+/* The pick kernel of this ctx's most recent pick launch and its template arguments: what the
+ * LIG_* knobs, the buffers' alignment and the table sizes selected for it (0 where a field does
+ * not apply).  Recorded at the launch; kernel is LIG_KERNEL_NONE before the first one. */
+#define LIG_KERNEL_NONE         0
+#define LIG_KERNEL_PERSISTENT   1   /* lig_pick_persistent_kernel<groups, stages, bulk_store, tables_in_smem> */
+#define LIG_KERNEL_LOOP         2   /* lig_pick_loop_kernel<tables_in_smem> */
+#define LIG_KERNEL_PLAIN        3   /* lig_pick_stream_kernel<per_thread> */
+#define LIG_KERNEL_QUEUE        4   /* lig_pick_queue_kernel<per_thread>: the merged queue */
+#define LIG_KERNEL_MODELS       5   /* lig_pick_models_kernel<groups, stages, tables_in_smem> */
+#define LIG_KERNEL_MODELS_PLAIN 6   /* lig_pick_models_stream_kernel */
+typedef struct lig_launch_info {
+  int32_t kernel, groups, stages, bulk_store, tables_in_smem, per_thread;
+} lig_launch_info;
+int         lig_last_pick_launch(lig_ctx* ctx, lig_launch_info* info);
 
 #ifdef __cplusplus
 }

@@ -23,6 +23,8 @@ LIG_ABI_VERSION = 7
 LIG_MAX_FILTER_NODES = 32
 LIG_REQ_CRITICAL = 1
 LIG_MAX_PODS, LIG_MAX_ADAPTERS = 32768, 65534
+(LIG_KERNEL_NONE, LIG_KERNEL_PERSISTENT, LIG_KERNEL_LOOP, LIG_KERNEL_PLAIN, LIG_KERNEL_QUEUE, LIG_KERNEL_MODELS,
+ LIG_KERNEL_MODELS_PLAIN) = range(7)
 
 # Every symbol include/lig.h declares (tests check the library exports all of them).
 EXPORTED_SYMBOLS = (
@@ -44,6 +46,7 @@ EXPORTED_SYMBOLS = (
     "lig_schedule_models_batch_feedback_chain", "lig_schedule_models_batch_feedback_chain_device",
     "lig_stream_submit_models",
     "lig_filter_batch", "lig_filter_batch_device", "lig_filter_models_batch", "lig_filter_models_batch_device",
+    "lig_last_pick_launch",
 )
 
 
@@ -64,6 +67,11 @@ class LigFilterNode(C.Structure):
     _fields_ = [("kind", C.c_int32), ("next_on_success", C.c_int32), ("next_on_failure", C.c_int32),
                 ("next_on_success_or_failure", C.c_int32), ("queue_threshold", C.c_int64),
                 ("kv_threshold", C.c_double)]
+
+
+class LigLaunchInfo(C.Structure):
+    _fields_ = [("kernel", C.c_int32), ("groups", C.c_int32), ("stages", C.c_int32), ("bulk_store", C.c_int32),
+                ("tables_in_smem", C.c_int32), ("per_thread", C.c_int32)]
 
 
 class LigError(RuntimeError):
@@ -155,6 +163,7 @@ def load() -> C.CDLL:
     lib.lig_update_snapshot.argtypes = [vp, u64, u64, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.lig_pick_kernel_info.argtypes = [vp, u64, C.c_char_p, i32, C.POINTER(i32), C.POINTER(i32),
                                          C.POINTER(i32), C.POINTER(i32)]
+    lib.lig_last_pick_launch.argtypes = [vp, C.POINTER(LigLaunchInfo)]
     for name in EXPORTED_SYMBOLS:
         getattr(lib, name)  # AttributeError if the library does not export it
     _lib = lib

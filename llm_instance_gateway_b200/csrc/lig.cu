@@ -131,6 +131,7 @@ struct lig_ctx {
   std::mutex upload_mu;
   std::mutex bounce_mu;
   std::atomic<uint64_t> launches{0};
+  lig_launch_info last_pick{};               // lig_last_pick_launch (under mu)
   void* comm = nullptr;                      // ncclComm_t, owned by lig_multi.cpp
 
   // ---- snapshot deltas (lig_update_snapshot): pinned + device staging of one delta ----
@@ -378,6 +379,7 @@ int launch_pick(lig_ctx* c, const Slot& s, uint64_t seed, const lig_req* d_reqs,
                    (lig_pick_stream_kernel<kPpt><<<grid, kPickThreads, 0, stream>>>(in, out, R, cls, s.d_lists, s.A, seed)));
   CUDA_TRY(cudaGetLastError());
   c->launches++;
+  c->last_pick = lig_launch_info{LIG_KERNEL_PLAIN, 0, 0, 0, 0, c->pick_per_thread};
   return 0;
 }
 
@@ -508,12 +510,14 @@ int launch_persistent(lig_ctx* c, const Slot& s, uint64_t seed, const lig_req* c
       const int cap = c->loop_grid[tab ? 1 : 0];
       const int grid = qp.total_tiles < cap ? qp.total_tiles : cap;
       CUDA_TRY(cudaLaunchKernel(v.fn, dim3((unsigned)grid), dim3((unsigned)v.threads), args, v.smem, st));
+      c->last_pick = lig_launch_info{LIG_KERNEL_LOOP, 0, 0, 0, tab ? 1 : 0, 0};
     } else {
       const bool bulk = c->tma_bulk_store && aligned;
       const PersistVariant v = persist_variant(c->tma_groups, c->tma_stages, bulk, tab);
       const int cap = c->persist_grid[bulk ? 1 : 0][tab ? 1 : 0];
       const int grid = qp.total_tiles < cap ? qp.total_tiles : cap;
       if (int rc = launch_claimed(c, v, grid, qp.total_tiles, args, &tc, st)) return rc;
+      c->last_pick = lig_launch_info{LIG_KERNEL_PERSISTENT, c->tma_groups, c->tma_stages, bulk ? 1 : 0, tab ? 1 : 0, 0};
     }
     c->launches++;
     if (slot >= 0) CUDA_TRY(cudaEventRecord(c->items_free[slot], st));   // after the kernel that reads the table
@@ -558,6 +562,7 @@ int launch_models(lig_ctx* c, const Slot& s, uint64_t seed, uint64_t first_index
           seed + (uint64_t)b, first_index, nullptr);
       CUDA_TRY(cudaGetLastError());
       c->launches++;
+      c->last_pick = lig_launch_info{LIG_KERNEL_MODELS_PLAIN, 0, 0, 0, 0, 0};
     }
     return 0;
   }
@@ -586,6 +591,7 @@ int launch_models(lig_ctx* c, const Slot& s, uint64_t seed, uint64_t first_index
     const int grid = qp.total_tiles < cap ? qp.total_tiles : cap;
     if (int rc = launch_claimed(c, v, grid, qp.total_tiles, args, &tc, st)) return rc;
     c->launches++;
+    c->last_pick = lig_launch_info{LIG_KERNEL_MODELS, c->models_groups, c->models_stages, 0, tab ? 1 : 0, 0};
   }
   return 0;
 }
@@ -713,6 +719,11 @@ T* mapped_device_pointer(T* p) {
   if (at.type != cudaMemoryTypeHost || !at.devicePointer) return nullptr;
   return reinterpret_cast<T*>(at.devicePointer);
 }
+
+// Every pick kernel reads a request with one 16-byte load (the TMA ring in 16-byte aligned tiles),
+// but lig_req itself is only 8-byte aligned: a host request array at an odd 8 bytes is staged
+// through the ctx's aligned bounce buffer (lig_schedule_batch) or refused (the async form).
+bool req_aligned(const lig_req* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 // Enqueue one host-buffer batch (device-visible pointers) on a lane and hand back a ticket.
 // Caller holds c->mu.
@@ -1456,6 +1467,7 @@ int lig_schedule_batches_device(lig_ctx* c, uint64_t epoch, uint64_t seed,
                            c->d_items[slot], R, cls, s->d_lists, s->A)));
       CUDA_TRY(cudaGetLastError());
       c->launches++;
+      c->last_pick = lig_launch_info{LIG_KERNEL_QUEUE, 0, 0, 0, 0, c->pick_per_thread};
       CUDA_TRY(cudaEventRecord(c->items_free[slot], st));    // after the kernel that reads the table
     }
     return note_reader(*s, st);
@@ -1503,6 +1515,8 @@ int lig_schedule_batch_async(lig_ctx* c, uint64_t epoch, uint64_t seed, const li
   lig_pick* dev_out = mapped_device_pointer(out);
   if (!dev_in || !dev_out)
     return fail(LIG_ERR_INVALID, "lig_schedule_batch_async needs page-locked buffers (lig_host_alloc)");
+  if (!req_aligned(dev_in))
+    return fail(LIG_ERR_INVALID, "lig_schedule_batch_async needs a 16-byte aligned request array");
   std::lock_guard<std::mutex> lk(c->mu);
   Slot* s = nullptr;
   if (int rc = resolve_slot(c, epoch, &s)) return rc;
@@ -1536,7 +1550,7 @@ int lig_schedule_batch(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req*
   // bounce through the ctx's pinned buffers.
   const lig_req* dev_in = R ? mapped_device_pointer(reqs) : nullptr;
   lig_pick* dev_out = R ? mapped_device_pointer(out) : nullptr;
-  const bool bounce = R > 0 && !(dev_in && dev_out);
+  const bool bounce = R > 0 && !(dev_in && dev_out && req_aligned(dev_in));
   std::unique_lock<std::mutex> bk(c->bounce_mu, std::defer_lock);
   if (bounce) {
     bk.lock();
@@ -1917,7 +1931,10 @@ static int filter_host(lig_ctx* c, const char* fn, uint64_t epoch, const FilterC
   d.out = f.R ? mapped_device_pointer(f.out) : nullptr;
   d.offsets = f.R ? mapped_device_pointer(f.offsets) : nullptr;
   d.pods = f.R && f.capacity > 0 ? mapped_device_pointer(f.pods) : nullptr;
-  const bool st_in = f.R && !d.in, st_out = f.R && !d.out, st_off = f.R && !d.offsets;
+  // requests that are not aligned to their element (a lig_req array at an odd 8 bytes) are staged
+  // as well: the kernel reads a descriptor with one 16-byte load
+  const bool st_in = f.R && (!d.in || (reinterpret_cast<uintptr_t>(d.in) & (f.in_bytes() - 1)));
+  const bool st_out = f.R && !d.out, st_off = f.R && !d.offsets;
   const bool st_pods = f.R && f.capacity > 0 && !d.pods;
   cudaStream_t st = nullptr;
   unsigned char* stage = nullptr;
@@ -2304,13 +2321,14 @@ static int chain_host(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t seed,
                       int32_t* loads) {
   if (!c || R < 0 || window < 1 || (R > 0 && (!rq.in || !rq.out))) return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
   if (R > c->max_batch) return fail(LIG_ERR_INVALID, "R=%d exceeds max_batch=%d", R, c->max_batch);
-  // as lig_schedule_batch: page-locked buffers are read and written in place, pageable ones bounce
-  // (4-byte model ids and picks fit the 16-byte / 8-byte bounce buffers)
+  // as lig_schedule_batch: page-locked buffers are read and written in place, pageable ones (and
+  // inputs not aligned to their element) bounce (4-byte model ids and picks fit the 16-byte /
+  // 8-byte bounce buffers)
   const void* in = rq.in;
   void* out = rq.out;
   rq.in = R ? mapped_device_pointer(in) : nullptr;
   rq.out = R ? mapped_device_pointer(out) : nullptr;
-  const bool bounce = R > 0 && !(rq.in && rq.out);
+  const bool bounce = R > 0 && !(rq.in && rq.out && !(reinterpret_cast<uintptr_t>(rq.in) & (rq.in_bytes() - 1)));
   std::unique_lock<std::mutex> bk(c->bounce_mu, std::defer_lock);
   if (bounce) {
     bk.lock();
@@ -2539,6 +2557,13 @@ int lig_stream_submit_models(lig_ctx* c, uint64_t epoch, uint64_t seed, uint64_t
 }
 
 uint64_t lig_kernel_launches(const lig_ctx* c) { return c ? c->launches.load() : 0; }
+
+int lig_last_pick_launch(lig_ctx* c, lig_launch_info* info) {
+  if (!c || !info) return fail(LIG_ERR_INVALID, "lig_last_pick_launch: null argument");
+  std::lock_guard<std::mutex> lk(c->mu);
+  *info = c->last_pick;
+  return 0;
+}
 int lig_sm_count(const lig_ctx* c) { return c ? c->sm_count : 0; }
 
 }  // extern "C"

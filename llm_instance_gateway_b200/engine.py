@@ -280,6 +280,12 @@ class Engine:
         return {"kernel": name.value.decode(), "grid": grid.value, "threads": threads.value,
                 "table_bytes": tb.value, "tables_in_smem": bool(in_smem.value)}
 
+    def last_pick_launch(self) -> dict:
+        """The pick kernel of the most recent pick launch and its template arguments (lig.h)."""
+        info = N.LigLaunchInfo()
+        N.check(self._lib.lig_last_pick_launch(self._ctx, C.byref(info)))
+        return {f: getattr(info, f) for f, _ in N.LigLaunchInfo._fields_}
+
     # ---- one process per GPU: NCCL inside the library ----
     def comm_unique_id(self) -> bytes:
         buf = (C.c_char * N.LIG_COMM_ID_BYTES)()

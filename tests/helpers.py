@@ -32,6 +32,15 @@ def pod_key(p: dict):
             p["max_active_models"], tuple(sorted(p["active_models"])))
 
 
+def fold(reqs: np.ndarray, seeds) -> np.ndarray:
+    """The requests whose picks under seed 0 are those of `reqs` under `seeds`: the pick state is
+    seed ^ rand_key, so the seed folds into the key.  `seeds` is a uint64 array that broadcasts
+    against reqs (one seed per batch row)."""
+    f = np.array(reqs, copy=True)
+    f["rand_key"] ^= seeds
+    return f
+
+
 def np_splitmix_int31(state: np.ndarray):
     """Vectorised next()>>33 over uint64 states; returns (new_state, int31)."""
     with np.errstate(over="ignore"):
