@@ -450,6 +450,51 @@ int lig_filter_models_batch_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed, 
                                    const uint32_t* d_model_ids, int R, lig_mpick* d_out, int64_t* d_offsets,
                                    uint16_t* d_pods, int64_t capacity, void* stream);
 
+/* ---- fallback endpoints: the pick and up to LIG_MAX_FALLBACKS more distinct survivors --------------
+ * Schedule returns one pod (scheduler.go:113-122).  When that pod refuses the connection, was evicted
+ * or is overloaded, a proxy can walk the request's fallback row instead of scheduling again: distinct
+ * members of the same survivor set, in an order defined on the request's own random stream.
+ *
+ * The ranking.  Take a LIG_OK request with survivor list L of n pods (ascending pod order, the list
+ * lig_read_class and lig_filter_batch return) and its pick stream state = seed ^ rand_key (rand_key =
+ * first_index + i for model ids).  m = min(n, 1 + n_fallbacks).  perm starts as the identity on
+ * [0, n).
+ *   step 0: r_0 = Int31n(n), the pick's own draws and rejections; ranked entry 0 = L[r_0] = the pick.
+ *   step j = 1 .. m-1: r_j = j + Int31n(n - j) on the stream continued after the last value the
+ *           previous step drew (a power of two masks, otherwise v > 2^31-1-(2^31 % (n-j)) is
+ *           rejected and v % (n-j) taken: Go 1.22, as for the pick).
+ *   every step j swaps perm[j] and perm[r_j]; ranked entry j = L[perm[j]] (a partial Fisher-Yates
+ *   shuffle: over keys every ordered choice of m distinct survivors is equally likely).
+ * Request i's row is fallbacks[i * n_fallbacks .. (i + 1) * n_fallbacks): ranked entries 1 .. m-1 as
+ * pod indices, then -1 to the end of the row.  Requests that are not LIG_OK (DROP, EMPTY,
+ * NO_PODS_LEFT, NO_MODEL) get a row of -1.  The row for n_fallbacks = k is a prefix of the row for any
+ * k' > k.  The lists come from the resident epoch's class tables, whichever build made them, never
+ * from a feedback chain's private copy; the calls neither end nor advance a feedback chain.
+ *
+ * `out` is byte for byte what the call each form mirrors returns.  LIG_ERR_INVALID for n_fallbacks
+ * outside [1, LIG_MAX_FALLBACKS], null buffers, R > max_batch on the host forms, and device buffers
+ * not aligned to their element (requests 16 bytes, picks 8 / 4, rows 2); a stale epoch and a missing
+ * snapshot as the mirrored calls report them; the model forms also LIG_ERR_NO_SNAPSHOT when the
+ * epoch has no model table.  Host forms: page-locked buffers are read and written in place,
+ * pageable or misaligned ones are staged; they block until everything is back.  Device forms: device
+ * pointers, enqueued on `stream` (NULL = legacy default stream), not synchronised.  The model forms
+ * are ordered behind the table's upload and register as readers of the slot, as
+ * lig_filter_models_batch does. */
+#define LIG_MAX_FALLBACKS 8
+/* descriptors: out is byte for byte lig_schedule_batch(ctx, epoch, seed, reqs, R, out) */
+int lig_schedule_batch_fallbacks(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
+                                 lig_pick* out, int n_fallbacks, int16_t* fallbacks);
+int lig_schedule_batch_fallbacks_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* d_reqs,
+                                        int R, lig_pick* d_out, int n_fallbacks, int16_t* d_fallbacks,
+                                        void* stream);
+/* model ids: out is byte for byte lig_schedule_models_batch(ctx, epoch, seed, first_index, ids, R, out) */
+int lig_schedule_models_batch_fallbacks(lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                                        const uint32_t* model_ids, int R, lig_mpick* out, int n_fallbacks,
+                                        int16_t* fallbacks);
+int lig_schedule_models_batch_fallbacks_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                                               const uint32_t* d_model_ids, int R, lig_mpick* d_out,
+                                               int n_fallbacks, int16_t* d_fallbacks, void* stream);
+
 /* ---- in-batch load feedback (opt-in; the default path never mutates the snapshot) ----------------
  * The reference schedules every request against the scraped metrics as they are
  * (scheduler.go:113-122 never writes them), so all requests of one class that arrive inside a

@@ -23,6 +23,7 @@ LIG_ABI_VERSION = 7
 LIG_MAX_FILTER_NODES = 32
 LIG_REQ_CRITICAL = 1
 LIG_MAX_PODS, LIG_MAX_ADAPTERS = 32768, 65534
+LIG_MAX_FALLBACKS = 8
 (LIG_KERNEL_NONE, LIG_KERNEL_PERSISTENT, LIG_KERNEL_LOOP, LIG_KERNEL_PLAIN, LIG_KERNEL_QUEUE, LIG_KERNEL_MODELS,
  LIG_KERNEL_MODELS_PLAIN) = range(7)
 
@@ -47,6 +48,8 @@ EXPORTED_SYMBOLS = (
     "lig_stream_submit_models",
     "lig_filter_batch", "lig_filter_batch_device", "lig_filter_models_batch", "lig_filter_models_batch_device",
     "lig_last_pick_launch",
+    "lig_schedule_batch_fallbacks", "lig_schedule_batch_fallbacks_device", "lig_schedule_models_batch_fallbacks",
+    "lig_schedule_models_batch_fallbacks_device",
 )
 
 
@@ -160,6 +163,10 @@ def load() -> C.CDLL:
     lib.lig_filter_batch_device.argtypes = [vp, u64, u64, vp, i32, vp, vp, vp, i64, vp]
     lib.lig_filter_models_batch.argtypes = [vp, u64, u64, u64, vp, i32, vp, vp, vp, i64]
     lib.lig_filter_models_batch_device.argtypes = [vp, u64, u64, u64, vp, i32, vp, vp, vp, i64, vp]
+    lib.lig_schedule_batch_fallbacks.argtypes = [vp, u64, u64, vp, i32, vp, i32, vp]
+    lib.lig_schedule_batch_fallbacks_device.argtypes = [vp, u64, u64, vp, i32, vp, i32, vp, vp]
+    lib.lig_schedule_models_batch_fallbacks.argtypes = [vp, u64, u64, u64, vp, i32, vp, i32, vp]
+    lib.lig_schedule_models_batch_fallbacks_device.argtypes = [vp, u64, u64, u64, vp, i32, vp, i32, vp, vp]
     lib.lig_update_snapshot.argtypes = [vp, u64, u64, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.lig_pick_kernel_info.argtypes = [vp, u64, C.c_char_p, i32, C.POINTER(i32), C.POINTER(i32),
                                          C.POINTER(i32), C.POINTER(i32)]

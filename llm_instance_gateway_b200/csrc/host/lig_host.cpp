@@ -66,9 +66,11 @@ Status NewScheduler(std::shared_ptr<PodMetricsProvider> pmp, const Options& opt,
   }
   s->h_reqs_ = static_cast<lig_req*>(lig_host_alloc((size_t)opt.max_batch * sizeof(lig_req)));
   s->h_picks_ = static_cast<lig_pick*>(lig_host_alloc((size_t)opt.max_batch * sizeof(lig_pick)));
+  s->h_fallbacks_ = static_cast<int16_t*>(lig_host_alloc((size_t)opt.max_batch * LIG_MAX_FALLBACKS * sizeof(int16_t)));
   s->h_model_ids_ = static_cast<uint32_t*>(lig_host_alloc((size_t)opt.max_batch * sizeof(uint32_t)));
   s->h_mpicks_ = static_cast<lig_mpick*>(lig_host_alloc((size_t)opt.max_batch * sizeof(lig_mpick)));
-  if (!s->h_reqs_ || !s->h_picks_ || !s->h_model_ids_ || !s->h_mpicks_) return LigFailure("lig_host_alloc");
+  if (!s->h_reqs_ || !s->h_picks_ || !s->h_fallbacks_ || !s->h_model_ids_ || !s->h_mpicks_)
+    return LigFailure("lig_host_alloc");
   uint64_t seed = opt.seed;
   if (seed == 0) {
     std::random_device rd;
@@ -97,6 +99,7 @@ Scheduler::~Scheduler() {
   if (ctx_ && opt_.use_doorbell) lig_stream_close(ctx_);
   if (h_reqs_) lig_host_free(h_reqs_);
   if (h_picks_) lig_host_free(h_picks_);
+  if (h_fallbacks_) lig_host_free(h_fallbacks_);
   if (h_model_ids_) lig_host_free(h_model_ids_);
   if (h_mpicks_) lig_host_free(h_mpicks_);
   if (ctx_) lig_destroy(ctx_);
@@ -361,6 +364,26 @@ Status Scheduler::Schedule(const LLMRequest& req, backend::Pod* targetPod) {
   return w.status;
 }
 
+Status Scheduler::ScheduleWithFallbacks(const LLMRequest& req, int n, std::vector<backend::Pod>* pods) {
+  if (pods) pods->clear();
+  if (n < 1 || n > LIG_MAX_FALLBACKS)
+    return Errorf(InvalidArgument, "ScheduleWithFallbacks: n=" + std::to_string(n) + " outside [1, " +
+                                       std::to_string(LIG_MAX_FALLBACKS) + "]");
+  if (opt_.load_feedback_window > 0)
+    return Errorf(InvalidArgument, "ScheduleWithFallbacks: not defined under load_feedback_window (the picks come "
+                                   "from the feedback chain's copy of the snapshot, the fallbacks would not)");
+  if (group_)
+    return Errorf(InvalidArgument, "ScheduleWithFallbacks: a scheduler over several devices has no fallback call");
+  std::vector<backend::Pod> ranked;
+  Waiter w;
+  w.req = &req;
+  w.fallbacks = n;
+  w.pods = &ranked;
+  Submit(w);
+  if (w.status.ok() && pods) *pods = std::move(ranked);
+  return w.status;
+}
+
 Status Scheduler::ScheduleModel(const std::string& model, std::string* resolvedTargetModel, backend::Pod* targetPod) {
   Waiter w;
   w.model = &model;
@@ -504,6 +527,10 @@ void Scheduler::Flush(std::vector<Waiter*>& all) {
   };
   while (done < batch.size()) {
     const int n = (int)std::min(batch.size() - done, (size_t)opt_.max_batch);
+    // any ScheduleWithFallbacks caller in this call: one lig_schedule_batch_fallbacks call with the
+    // largest n asked (rows are prefixes of longer rows, picks are lig_schedule_batch's)
+    int nf = 0;
+    for (int i = 0; i < n; ++i) nf = std::max(nf, batch[done + i]->fallbacks);
     std::shared_ptr<const Snapshot> snap;
     Status failure;
     int rc = 0;
@@ -524,7 +551,8 @@ void Scheduler::Flush(std::vector<Waiter*>& all) {
       const auto call_t0 = std::chrono::steady_clock::now();
       const double cpu_t0 = thread_cpu_us();
       const int W = opt_.load_feedback_window;
-      rc = group_ ? lig_group_schedule_batch(group_, snap->epoch, seed_, h_reqs_, n, h_picks_)
+      rc = nf > 0 ? lig_schedule_batch_fallbacks(ctx_, snap->epoch, seed_, h_reqs_, n, h_picks_, nf, h_fallbacks_)
+           : group_ ? lig_group_schedule_batch(group_, snap->epoch, seed_, h_reqs_, n, h_picks_)
            : W > 0 ? lig_schedule_batch_feedback_chain(ctx_, snap->epoch, seed_, h_reqs_, n, h_picks_, W, nullptr)
            : (opt_.use_doorbell && n <= lig_stream_capacity())
                ? lig_stream_submit(ctx_, snap->epoch, seed_, h_reqs_, n, h_picks_)
@@ -540,13 +568,19 @@ void Scheduler::Flush(std::vector<Waiter*>& all) {
       stats_.stale_retries++;
     }
     if (rc != 0)
-      failure = LigFailure(opt_.load_feedback_window > 0 ? "lig_schedule_batch_feedback_chain" : "lig_schedule_batch");
+      failure = LigFailure(nf > 0 ? "lig_schedule_batch_fallbacks"
+                           : opt_.load_feedback_window > 0 ? "lig_schedule_batch_feedback_chain" : "lig_schedule_batch");
     for (int i = 0; i < n; ++i) {
       Waiter* w = batch[done + i];
       if (rc != 0) {
         w->status = failure;
       } else if (h_picks_[i].status == LIG_OK) {
         w->pod = snap->pods[(size_t)h_picks_[i].pod_idx];          // pods[i].Pod  scheduler.go:121
+        if (w->fallbacks > 0) {
+          w->pods->push_back(w->pod);
+          const int16_t* row = h_fallbacks_ + (size_t)i * (size_t)nf;
+          for (int j = 0; j < w->fallbacks && row[j] >= 0; ++j) w->pods->push_back(snap->pods[(size_t)row[j]]);
+        }
       } else if (h_picks_[i].status == LIG_DROP) {
         w->status = Errorf(ResourceExhausted,                         // scheduler.go:117
                            std::string("failed to apply filter, resulted 0 pods, this should never "
@@ -562,6 +596,7 @@ void Scheduler::Flush(std::vector<Waiter*>& all) {
     {
       std::lock_guard<std::mutex> sk(stats_mu_);
       stats_.scheduled += (uint64_t)n;
+      for (int i = 0; i < n; ++i) stats_.fallback_scheduled += batch[done + i]->fallbacks > 0 ? 1 : 0;
       stats_.batches++;
       stats_.max_batch = std::max<uint64_t>(stats_.max_batch, (uint64_t)n);
     }

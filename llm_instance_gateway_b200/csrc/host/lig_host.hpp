@@ -172,6 +172,7 @@ struct Stats {
   uint64_t feedback_restarts = 0;  // feedback chains restarted on a new epoch after the first one
   uint64_t model_scheduled = 0;    // ScheduleModel(model, ...) calls completed (host-answered ones included)
   uint64_t model_batches = 0;      // device calls issued for model-id requests
+  uint64_t fallback_scheduled = 0; // ScheduleWithFallbacks calls completed
   double last_pack_us = 0;     // last Refresh: provider slice -> columns + bitmap (host)
   double last_upload_us = 0;   // last Refresh: lig_upload_snapshot (H2D + class tables)
   double max_device_call_us = 0;   // slowest single lig_schedule_batch call (launch + kernel + synchronise)
@@ -193,6 +194,17 @@ class Scheduler {
   // handlers/server.go:97-109); Unknown for the "resulted 0 pods" case; Internal for a
   // batch-level (CUDA) failure.                                       scheduler.go:113-122
   Status Schedule(const LLMRequest& req, backend::Pod* targetPod);
+
+  // Schedule plus up to n fallback endpoints (1 <= n <= LIG_MAX_FALLBACKS): fills *pods with the pick
+  // (pods[0], the pod Schedule would have returned for the same rand_key) and then up to n more
+  // distinct survivors in the order a proxy should retry them (include/lig.h, fallback endpoints).
+  // Goes through the micro-batcher and takes the next rand_key like Schedule; errors are Schedule's.
+  // A flush in which any caller asked for fallbacks makes its device call with
+  // lig_schedule_batch_fallbacks (the largest n asked in that flush); plain Schedule callers in it get
+  // the same picks.  InvalidArgument for n outside [1, LIG_MAX_FALLBACKS], with
+  // load_feedback_window > 0 (the picks come from the feedback chain's copy, the fallbacks would not)
+  // and with several devices.
+  Status ScheduleWithFallbacks(const LLMRequest& req, int n, std::vector<backend::Pod>* pods);
 
   // The reference's Filter interface (filter.go:12-15) run on the current epoch: fills *pods with
   // the survivors of req's walk of the filter tree (the built-in one or Options::filter), in slice
@@ -294,6 +306,8 @@ class Scheduler {
   struct Waiter {
     const LLMRequest* req = nullptr;
     const std::string* model = nullptr;
+    int fallbacks = 0;           // ScheduleWithFallbacks: the n asked for (0: Schedule)
+    std::vector<backend::Pod>* pods = nullptr;   // ScheduleWithFallbacks: receives the pick and its row
     int64_t model_id = -1;       // flush-time id in the captured epoch's table; -1: answered on the host
     std::string resolved;        // model requests: the resolved target model
     Status status;
@@ -314,6 +328,7 @@ class Scheduler {
   lig_group* group_ = nullptr;     // set instead of ctx_ when Options::devices lists several GPUs
   lig_req* h_reqs_ = nullptr;      // pinned, device-mapped (lig_host_alloc)
   lig_pick* h_picks_ = nullptr;
+  int16_t* h_fallbacks_ = nullptr;    // pinned, max_batch x LIG_MAX_FALLBACKS rows
   uint32_t* h_model_ids_ = nullptr;   // pinned, max_batch entries each: the model-id lane
   lig_mpick* h_mpicks_ = nullptr;
   uint64_t model_index_ = 0;          // first_index of the next model-id device call

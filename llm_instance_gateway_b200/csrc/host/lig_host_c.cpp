@@ -260,6 +260,23 @@ int ligh_schedule(ligh_scheduler* s, const char* model, const char* resolved, in
   return st.code;
 }
 
+int ligh_schedule_with_fallbacks(ligh_scheduler* s, const char* resolved, int critical, int n, char* names,
+                                 int names_cap, int* n_pods, char* err, int err_cap) {
+  scheduling::LLMRequest req;
+  req.ResolvedTargetModel = resolved ? resolved : "";
+  req.Critical = critical != 0;
+  std::vector<backend::Pod> pods;
+  scheduling::Status st = s->sched->ScheduleWithFallbacks(req, n, &pods);
+  std::string joined;
+  for (size_t i = 0; i < pods.size(); ++i) joined += (i ? "\n" : "") + pods[i].Name;
+  if (n_pods) *n_pods = (int)pods.size();
+  put(names, names_cap, joined);
+  if (!st.ok()) put(err, err_cap, st.message);
+  return st.code;
+}
+
+uint64_t ligh_fallback_scheduled(ligh_scheduler* s) { return s->sched->stats().fallback_scheduled; }
+
 int ligh_filter(ligh_scheduler* s, const char* resolved, int critical, char* names, int names_cap, int* n_pods,
                 char* err, int err_cap) {
   scheduling::LLMRequest req;

@@ -53,6 +53,11 @@ int ligh_schedule(ligh_scheduler*, const char* model, const char* resolved_targe
  * (slice order) and *n_pods their count. */
 int ligh_filter(ligh_scheduler*, const char* resolved_target_model, int critical, char* names, int names_cap,
                 int* n_pods, char* err, int err_cap);
+/* Scheduler::ScheduleWithFallbacks: returns the gRPC code; names receives the pick and then up to n
+ * fallback pods' names joined by '\n' (retry order) and *n_pods their count. */
+int ligh_schedule_with_fallbacks(ligh_scheduler*, const char* resolved_target_model, int critical, int n,
+                                 char* names, int names_cap, int* n_pods, char* err, int err_cap);
+uint64_t ligh_fallback_scheduled(ligh_scheduler*);   /* Stats::fallback_scheduled */
 int ligh_refresh(ligh_scheduler*, char* err, int err_cap);
 /* several GPUs behind one scheduler (lig_group_*) */
 ligh_scheduler* ligh_scheduler_new_devices(ligh_provider*, const int* devices, int n_devices, int max_pods,

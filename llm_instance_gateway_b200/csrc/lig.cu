@@ -2021,6 +2021,144 @@ int lig_filter_models_batch_device(lig_ctx* c, uint64_t epoch, uint64_t seed, ui
                        stream);
 }
 
+// ---- fallback endpoints (lig_schedule_batch_fallbacks, lig_schedule_models_batch_fallbacks) ----------
+struct FallbackCall {
+  bool models;
+  uint64_t seed, first_index;
+  const void* in;
+  int R;
+  void* out;
+  int n_fallbacks;
+  int16_t* fallbacks;
+  size_t in_bytes() const { return models ? sizeof(uint32_t) : sizeof(lig_req); }
+  size_t out_bytes() const { return models ? sizeof(lig_mpick) : sizeof(lig_pick); }
+  size_t row_bytes() const { return (size_t)n_fallbacks * sizeof(int16_t); }
+};
+
+static int fallback_check(const lig_ctx* c, const char* fn, const FallbackCall& f) {
+  if (!c || f.R < 0 || (f.R > 0 && (!f.in || !f.out || !f.fallbacks)))
+    return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
+  if (f.n_fallbacks < 1 || f.n_fallbacks > LIG_MAX_FALLBACKS)
+    return fail(LIG_ERR_INVALID, "%s: n_fallbacks=%d outside [1, %d]", fn, f.n_fallbacks, LIG_MAX_FALLBACKS);
+  return 0;
+}
+
+static bool misaligned(const void* p, size_t align) { return (reinterpret_cast<uintptr_t>(p) & (align - 1)) != 0; }
+
+// Enqueue the fallback kernel for f (R >= 1, device-visible, aligned pointers) against slot s on st,
+// behind the slot's tables, and register st as a reader of the slot.  Caller holds c->mu.
+static int enqueue_fallbacks(lig_ctx* c, Slot& s, const FallbackCall& f, cudaStream_t st) {
+  CUDA_TRY(cudaStreamWaitEvent(st, s.ready, 0));
+  if (f.models) CUDA_TRY(cudaStreamWaitEvent(st, s.models_ready, 0));
+  const int blocks = (f.R + kFallbackThreads - 1) / kFallbackThreads;
+  const uint4* cls = reinterpret_cast<const uint4*>(s.d_cls);
+  if (f.models)
+    lig_pick_fallback_kernel<true><<<blocks, kFallbackThreads, 0, st>>>(
+        f.in, f.out, f.fallbacks, f.R, f.n_fallbacks, cls, s.d_lists, s.A, s.d_ctab, s.d_mtab, s.n_models, f.seed,
+        f.first_index);
+  else
+    lig_pick_fallback_kernel<false><<<blocks, kFallbackThreads, 0, st>>>(
+        f.in, f.out, f.fallbacks, f.R, f.n_fallbacks, cls, s.d_lists, s.A, s.d_ctab, nullptr, 0u, f.seed, 0);
+  CUDA_TRY(cudaGetLastError());
+  c->launches++;
+  return note_reader(s, st);
+}
+
+static int fallback_device(lig_ctx* c, const char* fn, uint64_t epoch, const FallbackCall& f, void* stream) {
+  if (int rc = fallback_check(c, fn, f)) return rc;
+  if (f.R > 0 && (misaligned(f.in, f.in_bytes()) || misaligned(f.out, f.out_bytes()) ||
+                  misaligned(f.fallbacks, sizeof(int16_t))))
+    return fail(LIG_ERR_INVALID, "%s: a device buffer is not aligned to its element", fn);
+  std::lock_guard<std::mutex> lk(c->mu);
+  Slot* s = nullptr;
+  if (int rc = f.models ? resolve_models_slot(c, epoch, &s) : resolve_slot(c, epoch, &s)) return rc;
+  if (f.R == 0) return 0;
+  CUDA_TRY(cudaSetDevice(c->device));
+  return enqueue_fallbacks(c, *s, f, static_cast<cudaStream_t>(stream));
+}
+
+// Host buffers: page-locked, aligned ones are read and written by the kernel in place; the others
+// are staged in stream-ordered HBM and copied on the call's lane.  Blocks until everything is back.
+static int fallback_host(lig_ctx* c, const char* fn, uint64_t epoch, const FallbackCall& f) {
+  if (int rc = fallback_check(c, fn, f)) return rc;
+  if (f.R > c->max_batch) return fail(LIG_ERR_INVALID, "%s: R=%d exceeds max_batch=%d", fn, f.R, c->max_batch);
+  FallbackCall d = f;    // the same call with device-visible pointers
+  const size_t in_b = (size_t)f.R * f.in_bytes(), out_b = (size_t)f.R * f.out_bytes();
+  const size_t rows_b = (size_t)f.R * f.row_bytes();
+  d.in = f.R ? mapped_device_pointer(f.in) : nullptr;
+  d.out = f.R ? mapped_device_pointer(f.out) : nullptr;
+  d.fallbacks = f.R ? mapped_device_pointer(f.fallbacks) : nullptr;
+  // the kernel reads a descriptor with one 16-byte load and stores every element whole
+  const bool st_in = f.R && (!d.in || misaligned(d.in, f.in_bytes()));
+  const bool st_out = f.R && (!d.out || misaligned(d.out, f.out_bytes()));
+  const bool st_rows = f.R && (!d.fallbacks || misaligned(d.fallbacks, sizeof(int16_t)));
+  cudaStream_t st = nullptr;
+  unsigned char* stage = nullptr;
+  {
+    std::lock_guard<std::mutex> lk(c->mu);
+    Slot* s = nullptr;
+    if (int rc = f.models ? resolve_models_slot(c, epoch, &s) : resolve_slot(c, epoch, &s)) return rc;
+    if (f.R == 0) return 0;
+    CUDA_TRY(cudaSetDevice(c->device));
+    st = c->s_lane[c->next_lane];
+    c->next_lane = (c->next_lane + 1) % kLanes;
+    size_t at = 0, o_in = 0, o_out = 0, o_rows = 0;
+    auto take = [&](bool on, size_t bytes, size_t* o) { if (on) { *o = at; at = (at + bytes + 255) & ~(size_t)255; } };
+    take(st_in, in_b, &o_in);
+    take(st_out, out_b, &o_out);
+    take(st_rows, rows_b, &o_rows);
+    if (at) {
+      CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&stage), at, st));
+      if (st_in) d.in = stage + o_in;
+      if (st_out) d.out = stage + o_out;
+      if (st_rows) d.fallbacks = reinterpret_cast<int16_t*>(stage + o_rows);
+    }
+    int rc = 0;
+    if (st_in && cudaMemcpyAsync(const_cast<void*>(d.in), f.in, in_b, cudaMemcpyHostToDevice, st) != cudaSuccess)
+      rc = fail(LIG_ERR_CUDA, "%s: staging the requests failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
+    if (!rc) rc = enqueue_fallbacks(c, *s, d, st);
+    if (rc) {
+      if (stage) cudaFreeAsync(stage, st);
+      return rc;
+    }
+  }
+  // the copies back wait for the kernel on the lane; they may block, so not under c->mu
+  cudaError_t e = cudaSuccess;
+  if (st_out) e = cudaMemcpyAsync(f.out, d.out, out_b, cudaMemcpyDeviceToHost, st);
+  if (st_rows && e == cudaSuccess) e = cudaMemcpyAsync(f.fallbacks, d.fallbacks, rows_b, cudaMemcpyDeviceToHost, st);
+  if (stage) cudaFreeAsync(stage, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(LIG_ERR_CUDA, "%s failed on the device: %s", fn, cudaGetErrorString(e));
+  return 0;
+}
+
+int lig_schedule_batch_fallbacks(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
+                                 lig_pick* out, int n_fallbacks, int16_t* fallbacks) {
+  return fallback_host(c, "lig_schedule_batch_fallbacks", epoch,
+                       FallbackCall{false, seed, 0, reqs, R, out, n_fallbacks, fallbacks});
+}
+
+int lig_schedule_batch_fallbacks_device(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* d_reqs, int R,
+                                        lig_pick* d_out, int n_fallbacks, int16_t* d_fallbacks, void* stream) {
+  return fallback_device(c, "lig_schedule_batch_fallbacks_device", epoch,
+                         FallbackCall{false, seed, 0, d_reqs, R, d_out, n_fallbacks, d_fallbacks}, stream);
+}
+
+int lig_schedule_models_batch_fallbacks(lig_ctx* c, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                                        const uint32_t* model_ids, int R, lig_mpick* out, int n_fallbacks,
+                                        int16_t* fallbacks) {
+  return fallback_host(c, "lig_schedule_models_batch_fallbacks", epoch,
+                       FallbackCall{true, seed, first_index, model_ids, R, out, n_fallbacks, fallbacks});
+}
+
+int lig_schedule_models_batch_fallbacks_device(lig_ctx* c, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                                               const uint32_t* d_model_ids, int R, lig_mpick* d_out,
+                                               int n_fallbacks, int16_t* d_fallbacks, void* stream) {
+  return fallback_device(c, "lig_schedule_models_batch_fallbacks_device", epoch,
+                         FallbackCall{true, seed, first_index, d_model_ids, R, d_out, n_fallbacks, d_fallbacks},
+                         stream);
+}
+
 int lig_pick_kernel_info(lig_ctx* c, uint64_t epoch, char* name, int name_len, int* grid, int* threads,
                          int* table_bytes, int* tables_in_smem) {
   if (!c) return fail(LIG_ERR_INVALID, "lig_pick_kernel_info: ctx is null");

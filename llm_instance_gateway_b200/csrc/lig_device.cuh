@@ -135,7 +135,9 @@ __device__ __forceinline__ uint32_t int31n(uint64_t state, uint32_t n, uint32_t 
 
 // The same draw with the class entry's precomputed magic and rejection limit (no integer division
 // and no branch on n on the hot path).  n <= 1: magic 0 gives q = 0 < q_limit, k = 0.
-__device__ __forceinline__ uint32_t int31n_entry(uint64_t state, const uint4 e) {
+// int31n_entry_next leaves `state` after the last value the draw took (the fallback kernel
+// continues the stream from there); int31n_entry is the same draw on a copy.
+__device__ __forceinline__ uint32_t int31n_entry_next(uint64_t& state, const uint4 e) {
   const uint32_t n = e.x >> 16;
   const uint32_t shift = (e.x >> 4) & 31u;
   uint32_t v = splitmix_int31(state);
@@ -145,6 +147,9 @@ __device__ __forceinline__ uint32_t int31n_entry(uint64_t state, const uint4 e) 
     q = __umulhi(v, e.y) >> shift;
   }
   return n > 1u ? v - q * n : 0u;
+}
+__device__ __forceinline__ uint32_t int31n_entry(uint64_t state, const uint4 e) {
+  return int31n_entry_next(state, e);
 }
 
 // ---- one pass helpers; X is a per-warp mask of W words in shared memory -----------------------
@@ -2521,6 +2526,95 @@ lig_filter_kernel(const void* __restrict__ in, int R, const uint4* __restrict__ 
       if (s_excl[mid] <= j) lo = mid; else hi = mid;
     }
     dst[j] = __ldg(glists + s_list[lo] + (j - s_excl[lo]));
+  }
+}
+
+// ---- K2i: the pick and up to LIG_MAX_FALLBACKS more distinct survivors in retry order
+// (lig_schedule_batch_fallbacks, lig_schedule_models_batch_fallbacks; definition in include/lig.h).
+// One thread per request with plain loads and stores, like lig_pick_stream_kernel /
+// lig_pick_models_stream_kernel, so `in`, `out` and `fallbacks` may be page-locked host memory.
+// The pick is pick_one / pick_model<Ld::kLdg> (same bytes out); the stream then continues from the
+// state after the pick's draws into a partial Fisher-Yates shuffle of the class's list.  The
+// permutation is kept as a record of the (position, value) pairs the swaps wrote: step j reads
+// positions j and r_j >= j only, so a record at a position below j is never looked at again, and
+// the last step's write is never read: at most LIG_MAX_FALLBACKS records, all in registers.
+// Tables: the compact pool when the build sealed one, else the strided rows (as lig_filter_kernel).
+constexpr int kFallbackThreads = 256;
+
+// Go 1.22 Int31n(n) for 0 < n < 2^31, continuing `state` (the division is off the pick itself).
+__device__ __forceinline__ uint32_t int31n_next(uint64_t& state, uint32_t n) {
+  uint32_t v = splitmix_int31(state);
+  if ((n & (n - 1)) == 0) return v & (n - 1);
+  const uint32_t max_accept = 0x7fffffffu - (0x80000000u % n);
+  while (v > max_accept) v = splitmix_int31(state);
+  return v % n;
+}
+
+template <bool kModels>
+__global__ void __launch_bounds__(kFallbackThreads)
+lig_pick_fallback_kernel(const void* __restrict__ in, void* __restrict__ out, int16_t* __restrict__ fallbacks,
+                         int R, int n_fallbacks, const uint4* __restrict__ cls, const uint16_t* __restrict__ lists,
+                         int A, const unsigned char* __restrict__ ctab, const unsigned char* __restrict__ mtab,
+                         uint32_t n_models, uint64_t seed, uint64_t first_index) {
+  const int i = (int)blockIdx.x * kFallbackThreads + (int)threadIdx.x;
+  if (i >= R) return;
+  const CompactHeader hdr = *reinterpret_cast<const CompactHeader*>(ctab);
+  const uint32_t n_classes = 2u * ((uint32_t)A + 1u);
+  const uint4* gcls = cls;
+  const uint16_t* glists = lists;
+  if (hdr.bytes != 0u && hdr.n_classes == n_classes) {
+    gcls = reinterpret_cast<const uint4*>(ctab + sizeof(CompactHeader));
+    glists = reinterpret_cast<const uint16_t*>(ctab + sizeof(CompactHeader) + (size_t)n_classes * sizeof(ClassEntry));
+  }
+  uint4 e = make_uint4(0u, 0u, 0u, 0u);
+  uint64_t key;
+  bool ok;
+  if constexpr (kModels) {
+    ModelTables mt;
+    mt.entries = reinterpret_cast<const uint4*>(mtab + sizeof(ModelHeader));
+    mt.targets = reinterpret_cast<const uint2*>(mt.entries + n_models);
+    mt.n_models = n_models;
+    key = first_index + (uint64_t)i;
+    const uint32_t v = pick_model<Ld::kLdg>(__ldg(static_cast<const uint32_t*>(in) + i), key, mt, gcls, glists,
+                                            (uint32_t)A, seed, &e);
+    static_cast<uint32_t*>(out)[i] = v;
+    ok = ((v >> 16) & 0xffu) == (uint32_t)LIG_OK;
+  } else {
+    const int4 r = ld_stream_int4(static_cast<const int4*>(in) + i);
+    key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
+    const int2 p = pick_one(r, gcls, glists, (uint32_t)A, seed, &e);
+    st_stream_int2(static_cast<int2*>(out) + i, p);
+    ok = ((uint32_t)p.y & 7u) == (uint32_t)LIG_OK;
+  }
+  const uint32_t n = ok ? e.x >> 16 : 0u;
+  const uint32_t m = min(n, (uint32_t)n_fallbacks + 1u);   // ranked entries, the pick included
+  int16_t* row = fallbacks + (size_t)i * (size_t)n_fallbacks;
+  uint64_t state = seed ^ key;
+  uint32_t pos[LIG_MAX_FALLBACKS], val[LIG_MAX_FALLBACKS];
+  if (m >= 2u) {
+    pos[0] = int31n_entry_next(state, e);   // step 0: the pick's own draws, perm[r0] = 0
+    val[0] = 0u;
+  }
+  const uint16_t* list = glists + e.w;
+#pragma unroll
+  for (int j = 1; j <= LIG_MAX_FALLBACKS; ++j) {
+    if (j > n_fallbacks) break;
+    int16_t pod = -1;
+    if ((uint32_t)j < m) {
+      const uint32_t rj = (uint32_t)j + int31n_next(state, n - (uint32_t)j);
+      uint32_t a = (uint32_t)j, b = rj;   // perm[j], perm[r_j]: the latest record wins
+#pragma unroll
+      for (int k = 0; k < j; ++k) {
+        if (pos[k] == (uint32_t)j) a = val[k];
+        if (pos[k] == rj) b = val[k];
+      }
+      pod = (int16_t)__ldg(list + b);
+      if (j < LIG_MAX_FALLBACKS) {
+        pos[j] = rj;
+        val[j] = a;
+      }
+    }
+    row[j - 1] = pod;
   }
 }
 

@@ -272,6 +272,53 @@ class Engine:
                                                          d_out or None, d_offsets or None, d_pods or None, capacity,
                                                          stream or None))
 
+    # ---- fallback endpoints: the pick and up to LIG_MAX_FALLBACKS more distinct survivors ----
+    def schedule_batch_fallbacks(self, epoch: int, seed: int, reqs: np.ndarray, n: int):
+        """lig_schedule_batch_fallbacks: (picks, int16 fallbacks of shape (R, n)); the picks equal
+        schedule_batch's, row i holds request i's next distinct survivors in retry order, -1 padded."""
+        assert reqs.dtype == REQ_DTYPE and reqs.flags.c_contiguous
+        R = int(reqs.shape[0])
+        out = np.empty(R, dtype=PICK_DTYPE)
+        rows = np.empty((R, max(n, 0)), dtype=np.int16)
+        N.check(self._lib.lig_schedule_batch_fallbacks(self._ctx, epoch, seed, _ptr(reqs), R, _ptr(out), n,
+                                                       _ptr(rows)))
+        return out, rows
+
+    def schedule_batch_fallbacks_ptr(self, epoch: int, seed: int, h_reqs: int, R: int, h_out: int, n: int,
+                                     h_fallbacks: int) -> None:
+        N.check(self._lib.lig_schedule_batch_fallbacks(self._ctx, epoch, seed, h_reqs or None, R, h_out or None, n,
+                                                       h_fallbacks or None))
+
+    def schedule_batch_fallbacks_device(self, epoch: int, seed: int, d_reqs: int, R: int, d_out: int, n: int,
+                                        d_fallbacks: int, stream: int = 0) -> None:
+        """Device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_batch_fallbacks_device(self._ctx, epoch, seed, d_reqs or None, R,
+                                                              d_out or None, n, d_fallbacks or None, stream or None))
+
+    def schedule_models_batch_fallbacks(self, epoch: int, seed: int, model_ids: np.ndarray, n: int,
+                                        first_index: int = 0):
+        """lig_schedule_models_batch_fallbacks: (picks, int16 fallbacks (R, n)), the picks those of
+        schedule_models_batch with the same first_index."""
+        assert model_ids.dtype == np.uint32 and model_ids.flags.c_contiguous
+        R = int(model_ids.shape[0])
+        out = np.empty(R, dtype=MPICK_DTYPE)
+        rows = np.empty((R, max(n, 0)), dtype=np.int16)
+        N.check(self._lib.lig_schedule_models_batch_fallbacks(self._ctx, epoch, seed, first_index, _ptr(model_ids), R,
+                                                              _ptr(out), n, _ptr(rows)))
+        return out, rows
+
+    def schedule_models_batch_fallbacks_ptr(self, epoch: int, seed: int, first_index: int, h_ids: int, R: int,
+                                            h_out: int, n: int, h_fallbacks: int) -> None:
+        N.check(self._lib.lig_schedule_models_batch_fallbacks(self._ctx, epoch, seed, first_index, h_ids or None, R,
+                                                              h_out or None, n, h_fallbacks or None))
+
+    def schedule_models_batch_fallbacks_device(self, epoch: int, seed: int, first_index: int, d_ids: int, R: int,
+                                               d_out: int, n: int, d_fallbacks: int, stream: int = 0) -> None:
+        """The model-id form with device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_models_batch_fallbacks_device(self._ctx, epoch, seed, first_index,
+                                                                     d_ids or None, R, d_out or None, n,
+                                                                     d_fallbacks or None, stream or None))
+
     def pick_kernel_info(self, epoch: int) -> dict:
         name = C.create_string_buffer(64)
         grid, threads, tb, in_smem = C.c_int(), C.c_int(), C.c_int(), C.c_int()

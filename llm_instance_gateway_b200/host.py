@@ -28,7 +28,7 @@ EXPORTED_SYMBOLS = (
     "ligh_scheduler_new_devices", "ligh_datastore_new", "ligh_datastore_free", "ligh_datastore_set_model",
     "ligh_schedule_model", "ligh_scheduler_new_tree", "ligh_scheduler_new_feedback", "ligh_feedback_stats",
     "ligh_scheduler_set_models", "ligh_schedule_model_device", "ligh_model_stats", "ligh_schedule_models_concurrent",
-    "ligh_filter",
+    "ligh_filter", "ligh_schedule_with_fallbacks", "ligh_fallback_scheduled",
 )
 
 _lib = None
@@ -78,6 +78,10 @@ def load() -> C.CDLL:
                                   C.c_char_p, i32]
     lib.ligh_refresh.argtypes = [vp, C.c_char_p, i32]
     lib.ligh_filter.argtypes = [vp, C.c_char_p, i32, C.c_char_p, i32, C.POINTER(i32), C.c_char_p, i32]
+    lib.ligh_schedule_with_fallbacks.argtypes = [vp, C.c_char_p, i32, i32, C.c_char_p, i32, C.POINTER(i32),
+                                                 C.c_char_p, i32]
+    lib.ligh_fallback_scheduled.argtypes = [vp]
+    lib.ligh_fallback_scheduled.restype = u64
     lib.ligh_stats.argtypes = [vp, vp]
     lib.ligh_stats.restype = None
     lib.ligh_refresh_timing.argtypes = [vp, vp]
@@ -190,6 +194,15 @@ class HostScheduler:
         pods = names.value.decode().split("\n") if n.value else []
         return code, pods, err.value.decode("utf-8", "replace") if code != GRPC_OK else ""
 
+    def ScheduleWithFallbacks(self, resolved: str, critical: bool, n: int) -> Tuple[int, List[str], str]:  # noqa: N802
+        """Scheduler::ScheduleWithFallbacks: (gRPC code, pod names [pick, fallbacks in retry order], error)."""
+        cap = 64 * 1024
+        names, err, k = C.create_string_buffer(cap), C.create_string_buffer(512), C.c_int(0)
+        code = self._lib.ligh_schedule_with_fallbacks(self._s, resolved.encode(), int(critical), n, names, cap,
+                                                      C.byref(k), err, 512)
+        pods = names.value.decode().split("\n") if k.value else []
+        return code, pods, err.value.decode("utf-8", "replace") if code != GRPC_OK else ""
+
     def Refresh(self) -> None:  # noqa: N802
         err = C.create_string_buffer(512)
         if self._lib.ligh_refresh(self._s, err, 512) != 0:
@@ -204,8 +217,8 @@ class HostScheduler:
         self._lib.ligh_model_stats(self._s, ms)
         return dict(zip(("scheduled", "batches", "max_batch", "refreshes", "stale_retries", "failed_refreshes",
                          "excluded_pods", "delta_refreshes", "last_dirty_pods", "feedback_windows",
-                         "feedback_restarts", "model_scheduled", "model_batches"),
-                        map(int, list(out) + list(fb) + list(ms))))
+                         "feedback_restarts", "model_scheduled", "model_batches", "fallback_scheduled"),
+                        map(int, list(out) + list(fb) + list(ms) + [self._lib.ligh_fallback_scheduled(self._s)])))
 
     def ScheduleModel(self, datastore: "HostDataStore", model: str):  # noqa: N802
         """resolve (FetchModelData + RandomWeightedDraw + IsCritical) + Schedule: (code, resolved, pod, err)."""

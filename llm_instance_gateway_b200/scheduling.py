@@ -16,8 +16,10 @@ carries load feedback across those calls until the next refresh (off by default)
 ``ScheduleModel`` / ``ScheduleModelBatch`` take the request's model name instead of a resolved request: the
 resolve step of HandleRequestBody (handlers/request.go:42-56) runs on the device against a model table that
 every snapshot epoch carries.  ``FilterBatch`` / ``FilterModelBatch`` return the survivor slices of a whole
-batch (Filter.Filter, filter.go:12-15) in one device call, for any filter tree.  There is no CPU path here: without liblig.so or without a CUDA device
-construction fails.
+batch (Filter.Filter, filter.go:12-15) in one device call, for any filter tree.  ``ScheduleBatchWithFallbacks`` /
+``ScheduleWithFallbacks`` / ``ScheduleModelBatchWithFallbacks`` return the pick followed by up to n more distinct
+survivors in retry order (include/lig.h, fallback endpoints).  There is no CPU path here: without liblig.so or
+without a CUDA device construction fails.
 """
 from __future__ import annotations
 
@@ -328,6 +330,82 @@ class Scheduler:
         if err is not None:
             raise err
         return pod
+
+    # ---- fallback endpoints: the pick, then up to n more distinct survivors in retry order ----
+    def _check_fallbacks(self, n: int) -> None:
+        if self._window:
+            raise ValueError("fallback endpoints are not defined under load_feedback_window: the picks come from "
+                             "the feedback chain's copy of the snapshot, the fallbacks would not")
+        if not 1 <= n <= N.LIG_MAX_FALLBACKS:
+            raise ValueError(f"n must be in [1, {N.LIG_MAX_FALLBACKS}], got {n}")
+
+    def ScheduleBatchWithFallbacks(self, reqs: Sequence[LLMRequest], n: int
+                                   ) -> List[Tuple[List[Pod], Optional[StatusError]]]:
+        """ScheduleBatch plus up to n fallback pods per request (lig_schedule_batch_fallbacks):
+        (pods, error) per request, pods[0] the pod ScheduleBatch would have returned, then distinct
+        survivors in the order a proxy should retry them.  One rand_key per request from the same
+        sequence as ScheduleBatch.  ValueError under load_feedback_window."""
+        self._check_fallbacks(n)
+        snap = self._current()
+        arr = np.zeros(len(reqs), dtype=REQ_DTYPE)
+        for i, r in enumerate(reqs):
+            arr[i] = (snap.adapter_id(r.ResolvedTargetModel), N.LIG_REQ_CRITICAL if r.Critical else 0,
+                      self._rng.getrandbits(64))
+        picks, rows = self._engine.schedule_batch_fallbacks(self._epoch, self._seed, arr, n)
+        out: List[Tuple[List[Pod], Optional[StatusError]]] = []
+        for pk, row in zip(picks, rows):
+            if pk["status"] == N.LIG_OK:
+                out.append(([snap.pods[int(pk["pod_idx"])]] + [snap.pods[int(p)] for p in row if p >= 0], None))
+            else:
+                out.append(([], _schedule_error(int(pk["status"]))))
+        return out
+
+    def ScheduleWithFallbacks(self, req: LLMRequest, n: int) -> List[Pod]:
+        """Schedule plus up to n fallback pods: [pick, fallback 1, ...]; raises like Schedule."""
+        pods, err = self.ScheduleBatchWithFallbacks([req], n)[0]
+        if err is not None:
+            raise err
+        return pods
+
+    def ScheduleModelBatchWithFallbacks(self, names: Sequence[str], n: int
+                                        ) -> List[Tuple[List[Pod], str, Optional[StatusError]]]:
+        """ScheduleModelBatch plus up to n fallback pods per request: (pods, resolved target model,
+        error) per name, pods[0] the pod ScheduleModelBatch would have returned.  Host-answered errors
+        and the rand_key sequence (_model_index) as ScheduleModelBatch.  ValueError under
+        load_feedback_window."""
+        self._check_fallbacks(n)
+        snap = self._current()
+        pm = self._packed_models
+        out: List[Tuple[List[Pod], str, Optional[StatusError]]] = [None] * len(names)  # type: ignore
+        ids, slots = [], []
+        for i, name in enumerate(names):
+            m = pm.model_ids.get(name) if pm is not None else None
+            if m is None:                                                       # request.go:42-45
+                out[i] = ([], "", StatusError(
+                    "Unknown", f"error finding a model object in InferenceModel for input {name}"))
+            elif not pm.present[m]:                                             # request.go:48-51
+                out[i] = ([], "", StatusError("Unknown", f"error getting target model name for model {name}"))
+            else:
+                ids.append(m)
+                slots.append(i)
+        if not ids:
+            return out
+        picks, rows = self._engine.schedule_models_batch_fallbacks(self._epoch, self._seed,
+                                                                   np.array(ids, dtype=np.uint32), n,
+                                                                   first_index=self._model_index)
+        self._model_index += len(ids)
+        for i, m, pk, row in zip(slots, ids, picks, rows):
+            t, st = int(pk["target_idx"]), int(pk["status"])
+            resolved = names[i] if t == 255 else pm.target_names[m][t]         # 255: request.go:47
+            if st == N.LIG_OK:
+                pods = [snap.pods[int(pk["pod_idx"])]] + [snap.pods[int(p)] for p in row if p >= 0]
+                out[i] = (pods, resolved, None)
+            elif st == N.LIG_NO_MODEL:       # absent models never reach the device
+                out[i] = ([], resolved, StatusError("Internal", _no_model_entry(m, names[i])))
+            else:
+                err = _schedule_error(st)
+                out[i] = ([], resolved, StatusError(err.code, _POD_PREFIX + str(err)))
+        return out
 
     # Filter-level view (the GPU analogue of Filter.Filter, filter.go:12-15): survivor slice.
     def Filter(self, req: LLMRequest) -> Tuple[List[Pod], Optional[StatusError]]:
