@@ -155,6 +155,13 @@ Status Scheduler::RefreshImpl(const std::shared_ptr<const ModelList>& models) {
   std::vector<double> kv(P);
   std::vector<int64_t> q(P), na(P), ma(P);
   if (!intern_) intern_ = std::make_shared<InternTable>();
+  // From here on the memo (and the intern table) describe this tick.  A return before the epoch is
+  // published leaves the device on an older epoch the memo no longer matches, so that epoch must not
+  // be a delta base: a pod whose names changed would look clean and keep its old bitmap row.
+  struct DeltaBaseReset {
+    uint64_t* base;
+    ~DeltaBaseReset() { if (base) *base = 0; }   // the next refresh uploads in full
+  } reset_base{&prev_epoch_};
   bool table_changed = false;
   std::vector<char> memo_dirty;
   for (int attempt = 0; attempt < 2; ++attempt) {
@@ -276,10 +283,8 @@ Status Scheduler::RefreshImpl(const std::shared_ptr<const ModelList>& models) {
     }
     if (lig_upload_models(ctx_, snap->epoch, (int)models->models.size(), t.target_offsets.data(),
                           t.target_adapter_ids.data(), t.target_weights.data(), t.critical.data(),
-                          t.self_adapter_ids.data(), models->present.data()) != 0) {
-      prev_epoch_ = 0;   // the next refresh uploads in full
+                          t.self_adapter_ids.data(), models->present.data()) != 0)
       return LigFailure("lig_upload_models");
-    }
   }
   snap->models = models;
   prev_kv_ = kv;
@@ -287,6 +292,7 @@ Status Scheduler::RefreshImpl(const std::shared_ptr<const ModelList>& models) {
   prev_na_ = na16;
   prev_ma_ = ma16;
   prev_A_ = A;
+  reset_base.base = nullptr;
   prev_epoch_ = snap->epoch;
   {
     std::lock_guard<std::mutex> lk(snap_mu_);

@@ -245,6 +245,10 @@ class Scheduler {
   // Re-read the provider and upload a new snapshot epoch (call on every metrics refresh).  With a
   // model list set, the list is re-interned against the new epoch and uploaded into it before the
   // epoch is published: a target model that no pod listed matches once a pod loads it.
+  // A refresh uploads only the dirty pods (lig_update_snapshot) when the previous epoch is its base.
+  // A refresh that fails (a refused upload, more than max_pods pods, a refused model table) keeps the
+  // previous epoch for scheduling but not as a delta base: the per-pod memo has already moved to the
+  // refused tick, so the next refresh uploads in full.
   Status Refresh();
  private:
   struct ModelList;
