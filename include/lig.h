@@ -468,8 +468,10 @@ int lig_filter_models_batch_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed, 
  * Request i's row is fallbacks[i * n_fallbacks .. (i + 1) * n_fallbacks): ranked entries 1 .. m-1 as
  * pod indices, then -1 to the end of the row.  Requests that are not LIG_OK (DROP, EMPTY,
  * NO_PODS_LEFT, NO_MODEL) get a row of -1.  The row for n_fallbacks = k is a prefix of the row for any
- * k' > k.  The lists come from the resident epoch's class tables, whichever build made them, never
- * from a feedback chain's private copy; the calls neither end nor advance a feedback chain.
+ * k' > k.  The lists of these four calls come from the resident epoch's class tables, whichever
+ * build made them, never from a feedback chain's private copy; they neither end nor advance a
+ * feedback chain.  Under a chain, lig_schedule_[models_]batch_feedback_chain_fallbacks below rank
+ * the same way on the chain's own tables.
  *
  * `out` is byte for byte what the call each form mirrors returns.  LIG_ERR_INVALID for n_fallbacks
  * outside [1, LIG_MAX_FALLBACKS], null buffers, R > max_batch on the host forms, and device buffers
@@ -577,6 +579,42 @@ int lig_schedule_models_batch_feedback_chain(lig_ctx* ctx, uint64_t epoch, uint6
 int lig_schedule_models_batch_feedback_chain_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed,
                                                     uint64_t first_index, const uint32_t* d_model_ids, int R,
                                                     lig_mpick* d_out, int window, int32_t* d_loads, void* stream);
+/* Fallback rows under the chain.  A chain fallback call is a chain call of its kind in every
+ * respect, plus a row per request:
+ *   1. Picks and loads do not change: the R requests join the chain's sequence and windows exactly
+ *      as a plain chain call's would, each is picked on the private copy's current tables with the
+ *      call's seed and its rand_key, and only the pick is counted (row entries add no load: a
+ *      fallback pod is loaded only if the proxy retries, and the chain's estimate must not depend on
+ *      n_fallbacks).  So `out` and `loads` are byte for byte the plain chain call's on the same
+ *      sequence, and calls with and without rows, of either kind, may alternate in one chain.
+ *   2. Request i's row is the ranking of the fallback calls above, applied to the survivor list of
+ *      its class in the chain's private tables at its position in the sequence: the list its pick
+ *      drew from.  So entry 0 is the pick, the entries are distinct members of the load-adjusted
+ *      survivor set, and the row for k is a prefix of the row for k' > k.  A row depends only on
+ *      (seed, rand_key, the tables at its position): split invariance carries over, and while no
+ *      window of the chain has closed `out` and the rows equal lig_schedule_[models_]batch_fallbacks
+ *      on E byte for byte.
+ *   3. Refused, with nothing written and the chain exactly as it was, for every reason the chain
+ *      call is refused, and for n_fallbacks outside [1, LIG_MAX_FALLBACKS] or a null row buffer when
+ *      R > 0; the device forms also for a row buffer that is not 2-byte aligned.
+ * Host forms: page-locked, aligned rows are written in place; pageable or misaligned ones are staged
+ * in a pinned area of max_batch * LIG_MAX_FALLBACKS int16 that the ctx allocates at first use. */
+int lig_schedule_batch_feedback_chain_fallbacks(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* reqs,
+                                                int R, lig_pick* out, int n_fallbacks, int16_t* fallbacks,
+                                                int window, int32_t* loads);
+int lig_schedule_batch_feedback_chain_fallbacks_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed,
+                                                       const lig_req* d_reqs, int R, lig_pick* d_out,
+                                                       int n_fallbacks, int16_t* d_fallbacks, int window,
+                                                       int32_t* d_loads, void* stream);
+int lig_schedule_models_batch_feedback_chain_fallbacks(lig_ctx* ctx, uint64_t epoch, uint64_t seed,
+                                                       uint64_t first_index, const uint32_t* model_ids, int R,
+                                                       lig_mpick* out, int n_fallbacks, int16_t* fallbacks,
+                                                       int window, int32_t* loads);
+int lig_schedule_models_batch_feedback_chain_fallbacks_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed,
+                                                              uint64_t first_index, const uint32_t* d_model_ids,
+                                                              int R, lig_mpick* d_out, int n_fallbacks,
+                                                              int16_t* d_fallbacks, int window, int32_t* d_loads,
+                                                              void* stream);
 /* The next chain call starts a new chain. */
 int lig_feedback_chain_reset(lig_ctx* ctx);
 

@@ -50,6 +50,8 @@ EXPORTED_SYMBOLS = (
     "lig_last_pick_launch",
     "lig_schedule_batch_fallbacks", "lig_schedule_batch_fallbacks_device", "lig_schedule_models_batch_fallbacks",
     "lig_schedule_models_batch_fallbacks_device",
+    "lig_schedule_batch_feedback_chain_fallbacks", "lig_schedule_batch_feedback_chain_fallbacks_device",
+    "lig_schedule_models_batch_feedback_chain_fallbacks", "lig_schedule_models_batch_feedback_chain_fallbacks_device",
 )
 
 
@@ -167,6 +169,13 @@ def load() -> C.CDLL:
     lib.lig_schedule_batch_fallbacks_device.argtypes = [vp, u64, u64, vp, i32, vp, i32, vp, vp]
     lib.lig_schedule_models_batch_fallbacks.argtypes = [vp, u64, u64, u64, vp, i32, vp, i32, vp]
     lib.lig_schedule_models_batch_fallbacks_device.argtypes = [vp, u64, u64, u64, vp, i32, vp, i32, vp, vp]
+    lib.lig_schedule_batch_feedback_chain_fallbacks.argtypes = [vp, u64, u64, vp, i32, vp, i32, vp, i32, vp]
+    lib.lig_schedule_batch_feedback_chain_fallbacks_device.argtypes = [vp, u64, u64, vp, i32, vp, i32, vp, i32, vp,
+                                                                       vp]
+    lib.lig_schedule_models_batch_feedback_chain_fallbacks.argtypes = [vp, u64, u64, u64, vp, i32, vp, i32, vp, i32,
+                                                                       vp]
+    lib.lig_schedule_models_batch_feedback_chain_fallbacks_device.argtypes = [vp, u64, u64, u64, vp, i32, vp, i32,
+                                                                              vp, i32, vp, vp]
     lib.lig_update_snapshot.argtypes = [vp, u64, u64, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.lig_pick_kernel_info.argtypes = [vp, u64, C.c_char_p, i32, C.POINTER(i32), C.POINTER(i32),
                                          C.POINTER(i32), C.POINTER(i32)]

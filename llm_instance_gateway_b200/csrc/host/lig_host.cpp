@@ -370,16 +370,21 @@ Status Scheduler::Schedule(const LLMRequest& req, backend::Pod* targetPod) {
   return w.status;
 }
 
-Status Scheduler::ScheduleWithFallbacks(const LLMRequest& req, int n, std::vector<backend::Pod>* pods) {
-  if (pods) pods->clear();
+Status Scheduler::CheckFallbacks(const char* fn, int n) const {
   if (n < 1 || n > LIG_MAX_FALLBACKS)
-    return Errorf(InvalidArgument, "ScheduleWithFallbacks: n=" + std::to_string(n) + " outside [1, " +
+    return Errorf(InvalidArgument, std::string(fn) + ": n=" + std::to_string(n) + " outside [1, " +
                                        std::to_string(LIG_MAX_FALLBACKS) + "]");
-  if (opt_.load_feedback_window > 0)
-    return Errorf(InvalidArgument, "ScheduleWithFallbacks: not defined under load_feedback_window (the picks come "
+  if (opt_.load_feedback_window > 0 && !opt_.feedback_fallbacks)
+    return Errorf(InvalidArgument, std::string(fn) + ": not defined under load_feedback_window (the picks come "
                                    "from the feedback chain's copy of the snapshot, the fallbacks would not)");
   if (group_)
-    return Errorf(InvalidArgument, "ScheduleWithFallbacks: a scheduler over several devices has no fallback call");
+    return Errorf(InvalidArgument, std::string(fn) + ": a scheduler over several devices has no fallback call");
+  return Status{};
+}
+
+Status Scheduler::ScheduleWithFallbacks(const LLMRequest& req, int n, std::vector<backend::Pod>* pods) {
+  if (pods) pods->clear();
+  if (Status st = CheckFallbacks("ScheduleWithFallbacks", n); !st.ok()) return st;
   std::vector<backend::Pod> ranked;
   Waiter w;
   w.req = &req;
@@ -395,6 +400,21 @@ Status Scheduler::ScheduleModel(const std::string& model, std::string* resolvedT
   w.model = &model;
   Submit(w);
   if (w.status.ok() && targetPod) *targetPod = std::move(w.pod);
+  if (resolvedTargetModel) *resolvedTargetModel = std::move(w.resolved);
+  return w.status;
+}
+
+Status Scheduler::ScheduleModelWithFallbacks(const std::string& model, int n, std::string* resolvedTargetModel,
+                                             std::vector<backend::Pod>* pods) {
+  if (pods) pods->clear();
+  if (Status st = CheckFallbacks("ScheduleModelWithFallbacks", n); !st.ok()) return st;
+  std::vector<backend::Pod> ranked;
+  Waiter w;
+  w.model = &model;
+  w.fallbacks = n;
+  w.pods = &ranked;
+  Submit(w);
+  if (w.status.ok() && pods) *pods = std::move(ranked);
   if (resolvedTargetModel) *resolvedTargetModel = std::move(w.resolved);
   return w.status;
 }
@@ -557,7 +577,10 @@ void Scheduler::Flush(std::vector<Waiter*>& all) {
       const auto call_t0 = std::chrono::steady_clock::now();
       const double cpu_t0 = thread_cpu_us();
       const int W = opt_.load_feedback_window;
-      rc = nf > 0 ? lig_schedule_batch_fallbacks(ctx_, snap->epoch, seed_, h_reqs_, n, h_picks_, nf, h_fallbacks_)
+      rc = nf > 0 && W > 0
+               ? lig_schedule_batch_feedback_chain_fallbacks(ctx_, snap->epoch, seed_, h_reqs_, n, h_picks_, nf,
+                                                             h_fallbacks_, W, nullptr)
+           : nf > 0 ? lig_schedule_batch_fallbacks(ctx_, snap->epoch, seed_, h_reqs_, n, h_picks_, nf, h_fallbacks_)
            : group_ ? lig_group_schedule_batch(group_, snap->epoch, seed_, h_reqs_, n, h_picks_)
            : W > 0 ? lig_schedule_batch_feedback_chain(ctx_, snap->epoch, seed_, h_reqs_, n, h_picks_, W, nullptr)
            : (opt_.use_doorbell && n <= lig_stream_capacity())
@@ -574,7 +597,8 @@ void Scheduler::Flush(std::vector<Waiter*>& all) {
       stats_.stale_retries++;
     }
     if (rc != 0)
-      failure = LigFailure(nf > 0 ? "lig_schedule_batch_fallbacks"
+      failure = LigFailure(nf > 0 && opt_.load_feedback_window > 0 ? "lig_schedule_batch_feedback_chain_fallbacks"
+                           : nf > 0                         ? "lig_schedule_batch_fallbacks"
                            : opt_.load_feedback_window > 0 ? "lig_schedule_batch_feedback_chain" : "lig_schedule_batch");
     for (int i = 0; i < n; ++i) {
       Waiter* w = batch[done + i];
@@ -633,7 +657,7 @@ void Scheduler::FlushModels(std::vector<Waiter*>& batch) {
   while (done < batch.size()) {
     const int n = (int)std::min(batch.size() - done, (size_t)opt_.max_batch);
     std::shared_ptr<const Snapshot> snap;
-    int rc = 0, k = 0;
+    int rc = 0, k = 0, nf = 0;
     const char* call = "lig_schedule_models_batch";
     for (int attempt = 0; attempt < 4; ++attempt) {
       {
@@ -642,6 +666,7 @@ void Scheduler::FlushModels(std::vector<Waiter*>& batch) {
       }
       const ModelList* list = snap->models.get();
       k = 0;
+      nf = 0;
       for (int i = 0; i < n; ++i) {
         Waiter* w = batch[done + i];
         auto it = list ? list->ids.find(*w->model) : decltype(list->ids)::const_iterator{};
@@ -656,11 +681,22 @@ void Scheduler::FlushModels(std::vector<Waiter*>& batch) {
           w->model_id = it->second;
           w->status = Status{};   // a retry may map a name the previous epoch answered on the host
           h_model_ids_[k++] = it->second;
+          nf = std::max(nf, w->fallbacks);   // rows only for the requests the device sees
         }
       }
       if (k == 0) break;
       const int W = opt_.load_feedback_window;
-      if (W > 0) {
+      // any ScheduleModelWithFallbacks caller among them: one fallback call at the largest n asked
+      // (rows are prefixes of longer rows, picks are the plain call's); never the doorbell
+      if (nf > 0 && W > 0) {
+        call = "lig_schedule_models_batch_feedback_chain_fallbacks";
+        rc = lig_schedule_models_batch_feedback_chain_fallbacks(ctx_, snap->epoch, seed_, model_index_, h_model_ids_,
+                                                                k, h_mpicks_, nf, h_fallbacks_, W, nullptr);
+      } else if (nf > 0) {
+        call = "lig_schedule_models_batch_fallbacks";
+        rc = lig_schedule_models_batch_fallbacks(ctx_, snap->epoch, seed_, model_index_, h_model_ids_, k, h_mpicks_,
+                                                 nf, h_fallbacks_);
+      } else if (W > 0) {
         call = "lig_schedule_models_batch_feedback_chain";
         rc = lig_schedule_models_batch_feedback_chain(ctx_, snap->epoch, seed_, model_index_, h_model_ids_, k,
                                                       h_mpicks_, W, nullptr);
@@ -681,6 +717,7 @@ void Scheduler::FlushModels(std::vector<Waiter*>& batch) {
     for (int i = 0, j = 0; i < n; ++i) {
       Waiter* w = batch[done + i];
       if (w->model_id < 0) continue;
+      const int16_t* row = h_fallbacks_ + (size_t)j * (size_t)nf;
       const lig_mpick& pk = h_mpicks_[j++];
       if (rc != 0) {
         w->status = failure;
@@ -692,6 +729,10 @@ void Scheduler::FlushModels(std::vector<Waiter*>& batch) {
       w->resolved = pk.target_idx == 255 ? *w->model : im.TargetModels[pk.target_idx].Name;
       if (pk.status == LIG_OK) {
         w->pod = snap->pods[(size_t)pk.pod_idx];
+        if (w->fallbacks > 0) {
+          w->pods->push_back(w->pod);
+          for (int f = 0; f < w->fallbacks && row[f] >= 0; ++f) w->pods->push_back(snap->pods[(size_t)row[f]]);
+        }
       } else if (pk.status == LIG_DROP) {
         w->status = Errorf(ResourceExhausted, prefix + "failed to apply filter, resulted 0 pods, this should never "
                                                        "happen: " + kDropInner);
@@ -710,6 +751,7 @@ void Scheduler::FlushModels(std::vector<Waiter*>& batch) {
     {
       std::lock_guard<std::mutex> sk(stats_mu_);
       stats_.model_scheduled += (uint64_t)n;
+      for (int i = 0; i < n; ++i) stats_.fallback_scheduled += batch[done + i]->fallbacks > 0 ? 1 : 0;
       stats_.model_batches += k > 0 ? 1 : 0;
     }
     for (int i = 0; i < n; ++i) {

@@ -156,6 +156,13 @@ struct Options {
   // request is scheduled, until the next refresh replaces the snapshot (each refresh restarts the
   // chain on the new epoch).  0 = off, the reference's behaviour.  Single device, no doorbell.
   int load_feedback_window = 0;
+  // With load_feedback_window > 0: let ScheduleWithFallbacks and ScheduleModelWithFallbacks run as
+  // feedback-chain calls (lig_schedule_[models_]batch_feedback_chain_fallbacks), whose rows rank the
+  // survivors in the chain's load-adjusted tables, the set the pick itself drew from.  Picks and
+  // feedback windows are the same with or without it.  Off by default only because those calls have
+  // always been refused under feedback with InvalidArgument and that refusal is relied upon; without
+  // it they still are.  No effect without load_feedback_window.
+  bool feedback_fallbacks = false;
 };
 
 struct Stats {
@@ -172,7 +179,7 @@ struct Stats {
   uint64_t feedback_restarts = 0;  // feedback chains restarted on a new epoch after the first one
   uint64_t model_scheduled = 0;    // ScheduleModel(model, ...) calls completed (host-answered ones included)
   uint64_t model_batches = 0;      // device calls issued for model-id requests
-  uint64_t fallback_scheduled = 0; // ScheduleWithFallbacks calls completed
+  uint64_t fallback_scheduled = 0; // ScheduleWithFallbacks and ScheduleModelWithFallbacks calls completed
   double last_pack_us = 0;     // last Refresh: provider slice -> columns + bitmap (host)
   double last_upload_us = 0;   // last Refresh: lig_upload_snapshot (H2D + class tables)
   double max_device_call_us = 0;   // slowest single lig_schedule_batch call (launch + kernel + synchronise)
@@ -201,9 +208,11 @@ class Scheduler {
   // Goes through the micro-batcher and takes the next rand_key like Schedule; errors are Schedule's.
   // A flush in which any caller asked for fallbacks makes its device call with
   // lig_schedule_batch_fallbacks (the largest n asked in that flush); plain Schedule callers in it get
-  // the same picks.  InvalidArgument for n outside [1, LIG_MAX_FALLBACKS], with
-  // load_feedback_window > 0 (the picks come from the feedback chain's copy, the fallbacks would not)
-  // and with several devices.
+  // the same picks.  With load_feedback_window > 0 and Options::feedback_fallbacks, that call is
+  // lig_schedule_batch_feedback_chain_fallbacks in place of the chain call: same picks and windows,
+  // rows from the chain's tables.  InvalidArgument for n outside [1, LIG_MAX_FALLBACKS], with
+  // load_feedback_window > 0 and no feedback_fallbacks (the picks come from the feedback chain's
+  // copy), and with several devices.
   Status ScheduleWithFallbacks(const LLMRequest& req, int n, std::vector<backend::Pod>* pods);
 
   // The reference's Filter interface (filter.go:12-15) run on the current epoch: fills *pods with
@@ -233,6 +242,16 @@ class Scheduler {
   // lig_schedule_models_batch with first_index = k.  Neither rand_key sequence of the two calls
   // above is touched.
   Status ScheduleModel(const std::string& model, std::string* resolvedTargetModel, backend::Pod* targetPod);
+
+  // ScheduleModel(model, ...) plus up to n fallback endpoints: *pods gets the pick (the pod
+  // ScheduleModel would have returned for the same rand_key) and then up to n more distinct survivors
+  // in retry order.  Host-answered errors, *resolvedTargetModel and the rand_key sequence are
+  // ScheduleModel's.  A model-id flush with any such caller makes its device call with
+  // lig_schedule_models_batch_fallbacks at the largest n asked among the requests it sends (under
+  // load_feedback_window with Options::feedback_fallbacks, the chain-fallback model call) and skips
+  // the doorbell.  Refused like ScheduleWithFallbacks.
+  Status ScheduleModelWithFallbacks(const std::string& model, int n, std::string* resolvedTargetModel,
+                                    std::vector<backend::Pod>* pods);
 
   // Replace the InferenceModels that ScheduleModel(model, ...) resolves against; of two models
   // with one ModelName the later wins (the reference's datastore is a map).  Publishes a new epoch
@@ -310,8 +329,8 @@ class Scheduler {
   struct Waiter {
     const LLMRequest* req = nullptr;
     const std::string* model = nullptr;
-    int fallbacks = 0;           // ScheduleWithFallbacks: the n asked for (0: Schedule)
-    std::vector<backend::Pod>* pods = nullptr;   // ScheduleWithFallbacks: receives the pick and its row
+    int fallbacks = 0;           // *WithFallbacks: the n asked for (0: Schedule / ScheduleModel)
+    std::vector<backend::Pod>* pods = nullptr;   // *WithFallbacks: receives the pick and its row
     int64_t model_id = -1;       // flush-time id in the captured epoch's table; -1: answered on the host
     std::string resolved;        // model requests: the resolved target model
     Status status;
@@ -325,6 +344,7 @@ class Scheduler {
   void Flush(std::vector<Waiter*>& batch);
   void FlushModels(std::vector<Waiter*>& batch);
   void CountFeedback(uint64_t epoch, int n);
+  Status CheckFallbacks(const char* fn, int n) const;
 
   std::shared_ptr<PodMetricsProvider> pmp_;
   Options opt_;

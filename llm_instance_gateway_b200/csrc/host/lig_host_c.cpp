@@ -187,6 +187,20 @@ int ligh_schedule_model_device(ligh_scheduler* s, const char* model, char* resol
   return st.code;
 }
 
+int ligh_schedule_model_with_fallbacks(ligh_scheduler* s, const char* model, int n, char* resolved, int resolved_cap,
+                                       char* names, int names_cap, int* n_pods, char* err, int err_cap) {
+  std::string target;
+  std::vector<backend::Pod> pods;
+  scheduling::Status st = s->sched->ScheduleModelWithFallbacks(std::string(model ? model : ""), n, &target, &pods);
+  put(resolved, resolved_cap, target);
+  std::string joined;
+  for (size_t i = 0; i < pods.size(); ++i) joined += (i ? "\n" : "") + pods[i].Name;
+  if (n_pods) *n_pods = (int)pods.size();
+  put(names, names_cap, joined);
+  if (!st.ok()) put(err, err_cap, st.message);
+  return st.code;
+}
+
 void ligh_model_stats(ligh_scheduler* s, uint64_t out[2]) {
   scheduling::Stats st = s->sched->stats();
   out[0] = st.model_scheduled;
@@ -207,16 +221,18 @@ ligh_scheduler* ligh_scheduler_new_tree(ligh_provider* p, int device, const int*
                                         int n_nodes, char* err, int err_cap) {
   return ligh_scheduler_new_feedback(p, device, devices, n_devices, max_pods, max_adapters, max_batch, flush_size,
                                      window_us, refresh_ms, seed, busy_poll, caller_spin_us, use_doorbell, nodes,
-                                     n_nodes, 0, err, err_cap);
+                                     n_nodes, 0, 0, err, err_cap);
 }
 
 ligh_scheduler* ligh_scheduler_new_feedback(ligh_provider* p, int device, const int* devices, int n_devices,
                                             int max_pods, int max_adapters, int max_batch, int flush_size,
                                             int window_us, int refresh_ms, uint64_t seed, int busy_poll,
                                             int caller_spin_us, int use_doorbell, const lig_filter_node* nodes,
-                                            int n_nodes, int load_feedback_window, char* err, int err_cap) {
+                                            int n_nodes, int load_feedback_window, int feedback_fallbacks,
+                                            char* err, int err_cap) {
   scheduling::Options o;
   o.load_feedback_window = load_feedback_window;
+  o.feedback_fallbacks = feedback_fallbacks != 0;
   o.device = device;
   if (devices && n_devices > 1) o.devices.assign(devices, devices + n_devices);
   o.busy_poll = busy_poll != 0;

@@ -38,13 +38,14 @@ ligh_scheduler* ligh_scheduler_new_tree(ligh_provider*, int device, const int* d
                                         int busy_poll, int caller_spin_us, int use_doorbell,
                                         const lig_filter_node* nodes, int n_nodes, char* err, int err_cap);
 /* ligh_scheduler_new_tree plus Options::load_feedback_window (0 = off; > 0 flushes through
- * lig_schedule_batch_feedback_chain; refused with several devices or use_doorbell). */
+ * lig_schedule_batch_feedback_chain; refused with several devices or use_doorbell) and
+ * Options::feedback_fallbacks (nonzero: the *WithFallbacks calls run under the chain). */
 ligh_scheduler* ligh_scheduler_new_feedback(ligh_provider*, int device, const int* devices, int n_devices,
                                             int max_pods, int max_adapters, int max_batch, int flush_size,
                                             int batch_window_us, int refresh_interval_ms, uint64_t seed,
                                             int busy_poll, int caller_spin_us, int use_doorbell,
                                             const lig_filter_node* nodes, int n_nodes, int load_feedback_window,
-                                            char* err, int err_cap);
+                                            int feedback_fallbacks, char* err, int err_cap);
 void ligh_scheduler_free(ligh_scheduler*);
 /* Scheduler.Schedule: returns the gRPC code (0 OK, 8 ResourceExhausted, 2 Unknown, 13 Internal). */
 int ligh_schedule(ligh_scheduler*, const char* model, const char* resolved_target_model, int critical,
@@ -78,6 +79,10 @@ int ligh_scheduler_set_models(ligh_scheduler*, ligh_datastore*, char* err, int e
 /* Scheduler::ScheduleModel(model, ...): resolved on the device against that list. */
 int ligh_schedule_model_device(ligh_scheduler*, const char* model, char* resolved, int resolved_cap,
                                char* name, int name_cap, char* addr, int addr_cap, char* err, int err_cap);
+/* Scheduler::ScheduleModelWithFallbacks: returns the gRPC code; resolved receives the resolved target
+ * model, names the pick and then up to n fallback pods' names joined by '\n' and *n_pods their count. */
+int ligh_schedule_model_with_fallbacks(ligh_scheduler*, const char* model, int n, char* resolved, int resolved_cap,
+                                       char* names, int names_cap, int* n_pods, char* err, int err_cap);
 void ligh_model_stats(ligh_scheduler*, uint64_t out[2]); /* model_scheduled, model_batches */
 void ligh_stats(ligh_scheduler*, uint64_t out[9]); /* scheduled, batches, max_batch, refreshes, stale_retries */
 void ligh_feedback_stats(ligh_scheduler*, uint64_t out[2]); /* feedback_windows, feedback_restarts */

@@ -145,6 +145,8 @@ struct lig_ctx {
   int32_t* d_fb_hist = nullptr;               // picks per pod of the current window
   int32_t* d_fb_total = nullptr;              // picks per pod of the chain's closed windows
   int32_t* h_fb_loads = nullptr;              // pinned, mapped: the chain's loads for pageable callers
+  int16_t* h_fb_rows = nullptr;               // pinned, mapped: chain fallback rows for pageable callers
+                                              // (max_batch x LIG_MAX_FALLBACKS, first use, bounce_mu)
   cudaStream_t s_fb = nullptr;                // host-buffer chain calls
   cudaEvent_t fb_free = nullptr;              // the previous feedback call has finished with the scratch
   // The feedback chain (lig_schedule_batch_feedback_chain) the scratch holds between calls; all
@@ -1142,6 +1144,7 @@ static int create_impl(lig_ctx* c, int device, int max_pods, int max_adapters, i
         (const void*)lig_pick_models_stream_kernel, (const void*)lig_apply_delta_kernel,
         (const void*)lig_pick_count_kernel,      (const void*)lig_apply_feedback_kernel,
         (const void*)lig_feedback_loads_kernel,  (const void*)lig_pick_models_count_kernel,
+        (const void*)lig_pick_fallback_count_kernel<false>, (const void*)lig_pick_fallback_count_kernel<true>,
     };
     for (const void* fn : fns) CUDA_TRY(cudaFuncGetAttributes(&fa, fn));
   }
@@ -1190,6 +1193,7 @@ void lig_destroy(lig_ctx* c) {
   cudaFree(c->d_fb_hist);
   cudaFree(c->d_fb_total);
   if (c->h_fb_loads) cudaFreeHost(c->h_fb_loads);
+  if (c->h_fb_rows) cudaFreeHost(c->h_fb_rows);
   if (c->s_fb) cudaStreamDestroy(c->s_fb);
   if (c->fb_free) cudaEventDestroy(c->fb_free);
   if (c->mailbox) cudaFreeHost(c->mailbox);
@@ -2257,13 +2261,17 @@ struct FbReqs {
   uint64_t first_index = 0;              // model ids: rand_key of request 0
   const unsigned char* mtab = nullptr;   // model ids: the model table (set by chain_call)
   uint32_t n_models = 0;
+  bool rows = false;                     // a chain fallback call: request i's row is at
+  int16_t* fallbacks = nullptr;          //   fallbacks + i * n_fallbacks
+  int n_fallbacks = 0;
   size_t in_bytes() const { return models ? sizeof(uint32_t) : sizeof(lig_req); }
   size_t out_bytes() const { return models ? sizeof(lig_mpick) : sizeof(lig_pick); }
 };
 
 // Schedule R requests through the window sequence: each segment is the rest of the open window or
-// of the call, whichever is shorter; one fused pick + count launch per segment; a filled window is
-// closed at once, its tables are rebuilt only when the next segment needs them.
+// of the call, whichever is shorter; one fused pick + count launch per segment (pick + row + count
+// when the call asked for rows); a filled window is closed at once, its tables are rebuilt only
+// when the next segment needs them.
 static int fb_schedule(lig_ctx* c, FbRun& run, uint64_t seed, const FbReqs& rq, int R, cudaStream_t st) {
   Slot& fs = c->fb_scratch;
   for (int pos = 0; pos < R;) {
@@ -2280,7 +2288,18 @@ static int fb_schedule(lig_ctx* c, FbRun& run, uint64_t seed, const FbReqs& rq, 
     const void* in = static_cast<const unsigned char*>(rq.in) + (size_t)pos * rq.in_bytes();
     void* out = static_cast<unsigned char*>(rq.out) + (size_t)pos * rq.out_bytes();
     const int grid = (n + kPickThreads * kCountPerThread - 1) / (kPickThreads * kCountPerThread);
-    if (rq.models)
+    const uint4* fcls = reinterpret_cast<const uint4*>(fs.d_cls);
+    if (rq.rows) {
+      int16_t* rows = rq.fallbacks + (size_t)pos * (size_t)rq.n_fallbacks;
+      const int blocks = (n + kFallbackThreads - 1) / kFallbackThreads;
+      if (rq.models)
+        lig_pick_fallback_count_kernel<true><<<blocks, kFallbackThreads, 0, st>>>(
+            in, out, rows, n, rq.n_fallbacks, fcls, fs.d_lists, fs.A, rq.mtab, rq.n_models, seed,
+            rq.first_index + (uint64_t)pos, c->d_fb_hist);
+      else
+        lig_pick_fallback_count_kernel<false><<<blocks, kFallbackThreads, 0, st>>>(
+            in, out, rows, n, rq.n_fallbacks, fcls, fs.d_lists, fs.A, nullptr, 0u, seed, 0, c->d_fb_hist);
+    } else if (rq.models)
       lig_pick_models_count_kernel<<<grid, kPickThreads, 0, st>>>(
           static_cast<const uint32_t*>(in), static_cast<uint32_t*>(out), n, reinterpret_cast<const uint4*>(fs.d_cls),
           fs.d_lists, fs.A, rq.mtab, rq.n_models, seed, rq.first_index + (uint64_t)pos, c->d_fb_hist);
@@ -2444,10 +2463,22 @@ static int chain_admit(lig_ctx* c, const char* fn) {
   return fb_alloc_scratch(c);
 }
 
+// The row arguments of a chain fallback call; 0 for a plain chain call.
+static int chain_rows_check(const char* fn, const FbReqs& rq, int R) {
+  if (!rq.rows) return 0;
+  if (rq.n_fallbacks < 1 || rq.n_fallbacks > LIG_MAX_FALLBACKS)
+    return fail(LIG_ERR_INVALID, "%s: n_fallbacks=%d outside [1, %d]", fn, rq.n_fallbacks, LIG_MAX_FALLBACKS);
+  if (R > 0 && !rq.fallbacks) return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
+  return 0;
+}
+
 // The device form of both chain calls.
 static int chain_device(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t seed, const FbReqs& rq, int R,
                         int window, int32_t* d_loads, void* stream) {
   if (!c || R < 0 || window < 1 || (R > 0 && (!rq.in || !rq.out))) return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
+  if (int rc = chain_rows_check(fn, rq, R)) return rc;
+  if (R > 0 && rq.rows && misaligned(rq.fallbacks, sizeof(int16_t)))
+    return fail(LIG_ERR_INVALID, "%s: the row buffer is not 2-byte aligned", fn);
   std::lock_guard<std::mutex> fk(c->fb_mu);
   CUDA_TRY(cudaSetDevice(c->device));
   if (int rc = chain_admit(c, fn)) return rc;
@@ -2458,6 +2489,7 @@ static int chain_device(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t see
 static int chain_host(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t seed, FbReqs rq, int R, int window,
                       int32_t* loads) {
   if (!c || R < 0 || window < 1 || (R > 0 && (!rq.in || !rq.out))) return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
+  if (int rc = chain_rows_check(fn, rq, R)) return rc;
   if (R > c->max_batch) return fail(LIG_ERR_INVALID, "R=%d exceeds max_batch=%d", R, c->max_batch);
   // as lig_schedule_batch: page-locked buffers are read and written in place, pageable ones (and
   // inputs not aligned to their element) bounce (4-byte model ids and picks fit the 16-byte /
@@ -2476,6 +2508,23 @@ static int chain_host(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t seed,
       return fail(LIG_ERR_CUDA, "pinned staging buffers are not device-mapped on this platform");
     memcpy(c->h_reqs, in, (size_t)R * rq.in_bytes());
   }
+  // rows: page-locked, 2-byte aligned ones are written in place, the others staged in h_fb_rows
+  int16_t* rows_back = nullptr;                               // the caller's rows, when staged
+  if (R > 0 && rq.rows) {
+    int16_t* rows = rq.fallbacks;
+    rq.fallbacks = mapped_device_pointer(rows);
+    if (!rq.fallbacks || misaligned(rq.fallbacks, sizeof(int16_t))) {
+      if (!bk.owns_lock()) bk.lock();
+      if (!c->h_fb_rows) {
+        CUDA_TRY(cudaSetDevice(c->device));
+        CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&c->h_fb_rows),
+                               (size_t)c->max_batch * LIG_MAX_FALLBACKS * sizeof(int16_t), cudaHostAllocMapped));
+      }
+      if (!(rq.fallbacks = mapped_device_pointer(c->h_fb_rows)))
+        return fail(LIG_ERR_CUDA, "pinned staging buffers are not device-mapped on this platform");
+      rows_back = rows;
+    }
+  }
   std::lock_guard<std::mutex> fk(c->fb_mu);
   CUDA_TRY(cudaSetDevice(c->device));
   if (int rc = chain_admit(c, fn)) return rc;
@@ -2490,6 +2539,7 @@ static int chain_host(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t seed,
     return fail(LIG_ERR_CUDA, "feedback chain call failed on the device: %s", cudaGetErrorString(e));
   }
   if (bounce) memcpy(out, c->h_out, (size_t)R * rq.out_bytes());
+  if (rows_back) memcpy(rows_back, c->h_fb_rows, (size_t)R * (size_t)rq.n_fallbacks * sizeof(int16_t));
   if (loads_bounce && c->fb_scratch.P > 0)
     memcpy(loads, c->h_fb_loads, (size_t)c->fb_scratch.P * sizeof(int32_t));
   return 0;
@@ -2508,6 +2558,13 @@ static FbReqs model_reqs(const uint32_t* ids, lig_mpick* out, uint64_t first_ind
   rq.out = out;
   rq.models = true;
   rq.first_index = first_index;
+  return rq;
+}
+
+static FbReqs with_rows(FbReqs rq, int n_fallbacks, int16_t* fallbacks) {
+  rq.rows = true;
+  rq.n_fallbacks = n_fallbacks;
+  rq.fallbacks = fallbacks;
   return rq;
 }
 
@@ -2535,6 +2592,40 @@ int lig_schedule_models_batch_feedback_chain(lig_ctx* c, uint64_t epoch, uint64_
                                              int32_t* loads) {
   return chain_host(c, "lig_schedule_models_batch_feedback_chain", epoch, seed, model_reqs(ids, out, first_index), R,
                     window, loads);
+}
+
+int lig_schedule_batch_feedback_chain_fallbacks(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* reqs,
+                                                int R, lig_pick* out, int n_fallbacks, int16_t* fallbacks,
+                                                int window, int32_t* loads) {
+  return chain_host(c, "lig_schedule_batch_feedback_chain_fallbacks", epoch, seed,
+                    with_rows(descriptor_reqs(reqs, out), n_fallbacks, fallbacks), R, window, loads);
+}
+
+int lig_schedule_batch_feedback_chain_fallbacks_device(lig_ctx* c, uint64_t epoch, uint64_t seed,
+                                                       const lig_req* d_reqs, int R, lig_pick* d_out,
+                                                       int n_fallbacks, int16_t* d_fallbacks, int window,
+                                                       int32_t* d_loads, void* stream) {
+  return chain_device(c, "lig_schedule_batch_feedback_chain_fallbacks_device", epoch, seed,
+                      with_rows(descriptor_reqs(d_reqs, d_out), n_fallbacks, d_fallbacks), R, window, d_loads,
+                      stream);
+}
+
+int lig_schedule_models_batch_feedback_chain_fallbacks(lig_ctx* c, uint64_t epoch, uint64_t seed,
+                                                       uint64_t first_index, const uint32_t* ids, int R,
+                                                       lig_mpick* out, int n_fallbacks, int16_t* fallbacks,
+                                                       int window, int32_t* loads) {
+  return chain_host(c, "lig_schedule_models_batch_feedback_chain_fallbacks", epoch, seed,
+                    with_rows(model_reqs(ids, out, first_index), n_fallbacks, fallbacks), R, window, loads);
+}
+
+int lig_schedule_models_batch_feedback_chain_fallbacks_device(lig_ctx* c, uint64_t epoch, uint64_t seed,
+                                                              uint64_t first_index, const uint32_t* d_ids, int R,
+                                                              lig_mpick* d_out, int n_fallbacks,
+                                                              int16_t* d_fallbacks, int window, int32_t* d_loads,
+                                                              void* stream) {
+  return chain_device(c, "lig_schedule_models_batch_feedback_chain_fallbacks_device", epoch, seed,
+                      with_rows(model_reqs(d_ids, d_out, first_index), n_fallbacks, d_fallbacks), R, window,
+                      d_loads, stream);
 }
 
 int lig_feedback_chain_reset(lig_ctx* c) {

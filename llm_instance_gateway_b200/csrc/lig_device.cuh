@@ -2550,6 +2550,41 @@ __device__ __forceinline__ uint32_t int31n_next(uint64_t& state, uint32_t n) {
   return v % n;
 }
 
+// Ranked entries 1 .. m-1 of a request's fallback row, then -1 to the end of the row: `state` is
+// the pick's stream (seed ^ rand_key), `e` the class entry the pick used, `ok` whether it is LIG_OK.
+// Shared by the resident-epoch kernel and the feedback chain's.
+__device__ __forceinline__ void write_fallback_row(uint64_t state, const uint4 e, bool ok, int n_fallbacks,
+                                                   const uint16_t* __restrict__ glists, int16_t* __restrict__ row) {
+  const uint32_t n = ok ? e.x >> 16 : 0u;
+  const uint32_t m = min(n, (uint32_t)n_fallbacks + 1u);   // ranked entries, the pick included
+  uint32_t pos[LIG_MAX_FALLBACKS], val[LIG_MAX_FALLBACKS];
+  if (m >= 2u) {
+    pos[0] = int31n_entry_next(state, e);   // step 0: the pick's own draws, perm[r0] = 0
+    val[0] = 0u;
+  }
+  const uint16_t* list = glists + e.w;
+#pragma unroll
+  for (int j = 1; j <= LIG_MAX_FALLBACKS; ++j) {
+    if (j > n_fallbacks) break;
+    int16_t pod = -1;
+    if ((uint32_t)j < m) {
+      const uint32_t rj = (uint32_t)j + int31n_next(state, n - (uint32_t)j);
+      uint32_t a = (uint32_t)j, b = rj;   // perm[j], perm[r_j]: the latest record wins
+#pragma unroll
+      for (int k = 0; k < j; ++k) {
+        if (pos[k] == (uint32_t)j) a = val[k];
+        if (pos[k] == rj) b = val[k];
+      }
+      pod = (int16_t)__ldg(list + b);
+      if (j < LIG_MAX_FALLBACKS) {
+        pos[j] = rj;
+        val[j] = a;
+      }
+    }
+    row[j - 1] = pod;
+  }
+}
+
 template <bool kModels>
 __global__ void __launch_bounds__(kFallbackThreads)
 lig_pick_fallback_kernel(const void* __restrict__ in, void* __restrict__ out, int16_t* __restrict__ fallbacks,
@@ -2586,36 +2621,48 @@ lig_pick_fallback_kernel(const void* __restrict__ in, void* __restrict__ out, in
     st_stream_int2(static_cast<int2*>(out) + i, p);
     ok = ((uint32_t)p.y & 7u) == (uint32_t)LIG_OK;
   }
-  const uint32_t n = ok ? e.x >> 16 : 0u;
-  const uint32_t m = min(n, (uint32_t)n_fallbacks + 1u);   // ranked entries, the pick included
-  int16_t* row = fallbacks + (size_t)i * (size_t)n_fallbacks;
-  uint64_t state = seed ^ key;
-  uint32_t pos[LIG_MAX_FALLBACKS], val[LIG_MAX_FALLBACKS];
-  if (m >= 2u) {
-    pos[0] = int31n_entry_next(state, e);   // step 0: the pick's own draws, perm[r0] = 0
-    val[0] = 0u;
-  }
-  const uint16_t* list = glists + e.w;
-#pragma unroll
-  for (int j = 1; j <= LIG_MAX_FALLBACKS; ++j) {
-    if (j > n_fallbacks) break;
-    int16_t pod = -1;
-    if ((uint32_t)j < m) {
-      const uint32_t rj = (uint32_t)j + int31n_next(state, n - (uint32_t)j);
-      uint32_t a = (uint32_t)j, b = rj;   // perm[j], perm[r_j]: the latest record wins
-#pragma unroll
-      for (int k = 0; k < j; ++k) {
-        if (pos[k] == (uint32_t)j) a = val[k];
-        if (pos[k] == rj) b = val[k];
-      }
-      pod = (int16_t)__ldg(list + b);
-      if (j < LIG_MAX_FALLBACKS) {
-        pos[j] = rj;
-        val[j] = a;
-      }
+  write_fallback_row(seed ^ key, e, ok, n_fallbacks, glists, fallbacks + (size_t)i * (size_t)n_fallbacks);
+}
+
+// The chain segment of lig_schedule_[models_]batch_feedback_chain_fallbacks: the pick and row of
+// lig_pick_fallback_kernel on the chain's private tables (always the strided rows, as the count
+// kernels read them), and the pick counted into the open window like lig_pick_[models_]count_kernel.
+// Row entries are not counted.  One request per thread; a lane past the end still reaches the
+// full-warp match with pod -1.
+template <bool kModels>
+__global__ void __launch_bounds__(kFallbackThreads)
+lig_pick_fallback_count_kernel(const void* __restrict__ in, void* __restrict__ out, int16_t* __restrict__ fallbacks,
+                               int R, int n_fallbacks, const uint4* __restrict__ cls,
+                               const uint16_t* __restrict__ lists, int A, const unsigned char* __restrict__ mtab,
+                               uint32_t n_models, uint64_t seed, uint64_t first_index, int* __restrict__ hist) {
+  const int i = (int)blockIdx.x * kFallbackThreads + (int)threadIdx.x;
+  int pod = -1;
+  if (i < R) {
+    uint4 e = make_uint4(0u, 0u, 0u, 0u);
+    uint64_t key;
+    bool ok;
+    if constexpr (kModels) {
+      ModelTables mt;
+      mt.entries = reinterpret_cast<const uint4*>(mtab + sizeof(ModelHeader));
+      mt.targets = reinterpret_cast<const uint2*>(mt.entries + n_models);
+      mt.n_models = n_models;
+      key = first_index + (uint64_t)i;
+      const uint32_t v = pick_model<Ld::kLdg>(__ldg(static_cast<const uint32_t*>(in) + i), key, mt, cls, lists,
+                                              (uint32_t)A, seed, &e);
+      static_cast<uint32_t*>(out)[i] = v;
+      ok = ((v >> 16) & 0xffu) == (uint32_t)LIG_OK;
+      pod = (int)(int16_t)(v & 0xffffu);
+    } else {
+      const int4 r = ld_stream_int4(static_cast<const int4*>(in) + i);
+      key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
+      const int2 p = pick_one(r, cls, lists, (uint32_t)A, seed, &e);
+      st_stream_int2(static_cast<int2*>(out) + i, p);
+      ok = ((uint32_t)p.y & 7u) == (uint32_t)LIG_OK;
+      pod = p.x;
     }
-    row[j - 1] = pod;
+    write_fallback_row(seed ^ key, e, ok, n_fallbacks, lists, fallbacks + (size_t)i * (size_t)n_fallbacks);
   }
+  count_window_picks(pod, (int)threadIdx.x & 31, hist);
 }
 
 // loads[p] = picks of the closed windows + picks of the open one (the chain's per-pod loads).

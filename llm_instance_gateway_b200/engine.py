@@ -319,6 +319,69 @@ class Engine:
                                                                      d_ids or None, R, d_out or None, n,
                                                                      d_fallbacks or None, stream or None))
 
+    # ---- fallback rows under the feedback chain: a chain call that also returns each request's row ----
+    def schedule_batch_feedback_chain_fallbacks(self, epoch: int, seed: int, reqs: np.ndarray, n: int, window: int,
+                                                loads: Optional[np.ndarray] = None):
+        """lig_schedule_batch_feedback_chain_fallbacks: (picks, int16 fallbacks (R, n)).  The picks and
+        `loads` are schedule_batch_feedback_chain's for the same sequence; row i ranks the survivors of
+        request i's class in the chain's tables at its position, the list its pick drew from."""
+        assert reqs.dtype == REQ_DTYPE and reqs.flags.c_contiguous
+        R = int(reqs.shape[0])
+        out = np.empty(R, dtype=PICK_DTYPE)
+        rows = np.empty((R, max(n, 0)), dtype=np.int16)
+        if loads is not None:
+            assert loads.dtype == np.int32 and loads.flags.c_contiguous
+        N.check(self._lib.lig_schedule_batch_feedback_chain_fallbacks(
+            self._ctx, epoch, seed, _ptr(reqs), R, _ptr(out), n, _ptr(rows), window,
+            _ptr(loads) if loads is not None else None))
+        return out, rows
+
+    def schedule_batch_feedback_chain_fallbacks_ptr(self, epoch: int, seed: int, h_reqs: int, R: int, h_out: int,
+                                                    n: int, h_fallbacks: int, window: int, h_loads: int = 0) -> None:
+        N.check(self._lib.lig_schedule_batch_feedback_chain_fallbacks(self._ctx, epoch, seed, h_reqs or None, R,
+                                                                      h_out or None, n, h_fallbacks or None, window,
+                                                                      h_loads or None))
+
+    def schedule_batch_feedback_chain_fallbacks_device(self, epoch: int, seed: int, d_reqs: int, R: int, d_out: int,
+                                                       n: int, d_fallbacks: int, window: int, d_loads: int = 0,
+                                                       stream: int = 0) -> None:
+        """Device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_batch_feedback_chain_fallbacks_device(
+            self._ctx, epoch, seed, d_reqs or None, R, d_out or None, n, d_fallbacks or None, window,
+            d_loads or None, stream or None))
+
+    def schedule_models_batch_feedback_chain_fallbacks(self, epoch: int, seed: int, model_ids: np.ndarray, n: int,
+                                                       window: int, first_index: int = 0,
+                                                       loads: Optional[np.ndarray] = None):
+        """lig_schedule_models_batch_feedback_chain_fallbacks: (picks, int16 fallbacks (R, n)), the
+        picks and `loads` those of schedule_models_batch_feedback_chain with the same first_index."""
+        assert model_ids.dtype == np.uint32 and model_ids.flags.c_contiguous
+        R = int(model_ids.shape[0])
+        out = np.empty(R, dtype=MPICK_DTYPE)
+        rows = np.empty((R, max(n, 0)), dtype=np.int16)
+        if loads is not None:
+            assert loads.dtype == np.int32 and loads.flags.c_contiguous
+        N.check(self._lib.lig_schedule_models_batch_feedback_chain_fallbacks(
+            self._ctx, epoch, seed, first_index, _ptr(model_ids), R, _ptr(out), n, _ptr(rows), window,
+            _ptr(loads) if loads is not None else None))
+        return out, rows
+
+    def schedule_models_batch_feedback_chain_fallbacks_ptr(self, epoch: int, seed: int, first_index: int, h_ids: int,
+                                                           R: int, h_out: int, n: int, h_fallbacks: int, window: int,
+                                                           h_loads: int = 0) -> None:
+        N.check(self._lib.lig_schedule_models_batch_feedback_chain_fallbacks(
+            self._ctx, epoch, seed, first_index, h_ids or None, R, h_out or None, n, h_fallbacks or None, window,
+            h_loads or None))
+
+    def schedule_models_batch_feedback_chain_fallbacks_device(self, epoch: int, seed: int, first_index: int,
+                                                              d_ids: int, R: int, d_out: int, n: int,
+                                                              d_fallbacks: int, window: int, d_loads: int = 0,
+                                                              stream: int = 0) -> None:
+        """The model-id form with device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_models_batch_feedback_chain_fallbacks_device(
+            self._ctx, epoch, seed, first_index, d_ids or None, R, d_out or None, n, d_fallbacks or None, window,
+            d_loads or None, stream or None))
+
     def pick_kernel_info(self, epoch: int) -> dict:
         name = C.create_string_buffer(64)
         grid, threads, tb, in_smem = C.c_int(), C.c_int(), C.c_int(), C.c_int()

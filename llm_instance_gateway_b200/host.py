@@ -28,7 +28,7 @@ EXPORTED_SYMBOLS = (
     "ligh_scheduler_new_devices", "ligh_datastore_new", "ligh_datastore_free", "ligh_datastore_set_model",
     "ligh_schedule_model", "ligh_scheduler_new_tree", "ligh_scheduler_new_feedback", "ligh_feedback_stats",
     "ligh_scheduler_set_models", "ligh_schedule_model_device", "ligh_model_stats", "ligh_schedule_models_concurrent",
-    "ligh_filter", "ligh_schedule_with_fallbacks", "ligh_fallback_scheduled",
+    "ligh_filter", "ligh_schedule_with_fallbacks", "ligh_fallback_scheduled", "ligh_schedule_model_with_fallbacks",
 )
 
 _lib = None
@@ -57,7 +57,7 @@ def load() -> C.CDLL:
                                             i32, vp, i32, C.c_char_p, i32]
     lib.ligh_scheduler_new_tree.restype = vp
     lib.ligh_scheduler_new_feedback.argtypes = [vp, i32, C.POINTER(i32), i32, i32, i32, i32, i32, i32, i32, u64, i32,
-                                                i32, i32, vp, i32, i32, C.c_char_p, i32]
+                                                i32, i32, vp, i32, i32, i32, C.c_char_p, i32]
     lib.ligh_scheduler_new_feedback.restype = vp
     lib.ligh_feedback_stats.argtypes = [vp, vp]
     lib.ligh_feedback_stats.restype = None
@@ -80,6 +80,8 @@ def load() -> C.CDLL:
     lib.ligh_filter.argtypes = [vp, C.c_char_p, i32, C.c_char_p, i32, C.POINTER(i32), C.c_char_p, i32]
     lib.ligh_schedule_with_fallbacks.argtypes = [vp, C.c_char_p, i32, i32, C.c_char_p, i32, C.POINTER(i32),
                                                  C.c_char_p, i32]
+    lib.ligh_schedule_model_with_fallbacks.argtypes = [vp, C.c_char_p, i32, C.c_char_p, i32, C.c_char_p, i32,
+                                                       C.POINTER(i32), C.c_char_p, i32]
     lib.ligh_fallback_scheduled.argtypes = [vp]
     lib.ligh_fallback_scheduled.restype = u64
     lib.ligh_stats.argtypes = [vp, vp]
@@ -144,13 +146,15 @@ class HostScheduler:
                  max_adapters: int = 1024, max_batch: int = 1 << 16, flush_size: int = 4096,
                  batch_window_us: int = 50, refresh_interval_ms: int = 0, seed: int = 1,
                  busy_poll: bool = False, caller_spin_us: int = 0, use_doorbell: bool = False,
-                 devices: Optional[Sequence[int]] = None, filter=None, load_feedback_window: int = 0):
+                 devices: Optional[Sequence[int]] = None, filter=None, load_feedback_window: int = 0,
+                 feedback_fallbacks: bool = False):
         self._lib = load()
         self.provider = provider
         err = C.create_string_buffer(512)
-        if filter is not None or load_feedback_window:
-            # Options::filter (a scheduling.Filter chart or a node table) and
-            # Options::load_feedback_window (load feedback carried across flushes, 0 = off)
+        if filter is not None or load_feedback_window or feedback_fallbacks:
+            # Options::filter (a scheduling.Filter chart or a node table),
+            # Options::load_feedback_window (load feedback carried across flushes, 0 = off) and
+            # Options::feedback_fallbacks (the *WithFallbacks calls under that feedback)
             from .engine import _node_table
             nodes, n = _node_table(filter)
             devs = list(devices) if devices is not None else []
@@ -159,7 +163,7 @@ class HostScheduler:
                                                             max_adapters, max_batch, flush_size, batch_window_us,
                                                             refresh_interval_ms, seed, int(busy_poll), caller_spin_us,
                                                             int(use_doorbell), C.cast(nodes, C.c_void_p), n,
-                                                            load_feedback_window, err, 512)
+                                                            load_feedback_window, int(feedback_fallbacks), err, 512)
         elif devices is not None and len(devices) > 1:
             arr = (C.c_int * len(devices))(*devices)
             self._s = self._lib.ligh_scheduler_new_devices(provider._p, arr, len(devices), max_pods, max_adapters,
@@ -202,6 +206,17 @@ class HostScheduler:
                                                       C.byref(k), err, 512)
         pods = names.value.decode().split("\n") if k.value else []
         return code, pods, err.value.decode("utf-8", "replace") if code != GRPC_OK else ""
+
+    def ScheduleModelWithFallbacks(self, model: str, n: int) -> Tuple[int, str, List[str], str]:  # noqa: N802
+        """Scheduler::ScheduleModelWithFallbacks: (gRPC code, resolved target model, pod names [pick,
+        fallbacks in retry order], error)."""
+        cap = 64 * 1024
+        resolved, names = C.create_string_buffer(256), C.create_string_buffer(cap)
+        err, k = C.create_string_buffer(512), C.c_int(0)
+        code = self._lib.ligh_schedule_model_with_fallbacks(self._s, model.encode(), n, resolved, 256, names, cap,
+                                                            C.byref(k), err, 512)
+        pods = names.value.decode().split("\n") if k.value else []
+        return code, resolved.value.decode(), pods, err.value.decode("utf-8", "replace") if code != GRPC_OK else ""
 
     def Refresh(self) -> None:  # noqa: N802
         err = C.create_string_buffer(512)

@@ -18,7 +18,8 @@ resolve step of HandleRequestBody (handlers/request.go:42-56) runs on the device
 every snapshot epoch carries.  ``FilterBatch`` / ``FilterModelBatch`` return the survivor slices of a whole
 batch (Filter.Filter, filter.go:12-15) in one device call, for any filter tree.  ``ScheduleBatchWithFallbacks`` /
 ``ScheduleWithFallbacks`` / ``ScheduleModelBatchWithFallbacks`` return the pick followed by up to n more distinct
-survivors in retry order (include/lig.h, fallback endpoints).  There is no CPU path here: without liblig.so or
+survivors in retry order (include/lig.h, fallback endpoints); under load_feedback_window they need
+``feedback_fallbacks=True`` and then rank the feedback chain's own tables.  There is no CPU path here: without liblig.so or
 without a CUDA device construction fails.
 """
 from __future__ import annotations
@@ -187,11 +188,15 @@ def _check_models(models: Sequence[InferenceModel]) -> None:
 class Scheduler:
     def __init__(self, podMetricsProvider: PodMetricsProvider, device: int = 0,
                  max_pods: int = 4096, max_adapters: int = 1024, max_batch: int = 1 << 16,
-                 seed: Optional[int] = None, filter: Optional[Filter] = None, load_feedback_window: int = 0):
+                 seed: Optional[int] = None, filter: Optional[Filter] = None, load_feedback_window: int = 0,
+                 feedback_fallbacks: bool = False):
         if load_feedback_window < 0:
             raise ValueError(f"load_feedback_window must be >= 0, got {load_feedback_window}")
         self.podMetricsProvider = podMetricsProvider
         self._window = load_feedback_window  # 0: the reference's behaviour (no load feedback)
+        # fallback rows under load_feedback_window come from the chain's tables; opt-in because the
+        # *WithFallbacks calls refuse under feedback without it (documented behaviour kept as is)
+        self._feedback_fallbacks = bool(feedback_fallbacks)
         self._engine = Engine(device, max_pods, max_adapters, max_batch)
         self._filter = filter                # None: the built-in defaultFilter
         if filter is not None:
@@ -333,7 +338,7 @@ class Scheduler:
 
     # ---- fallback endpoints: the pick, then up to n more distinct survivors in retry order ----
     def _check_fallbacks(self, n: int) -> None:
-        if self._window:
+        if self._window and not self._feedback_fallbacks:
             raise ValueError("fallback endpoints are not defined under load_feedback_window: the picks come from "
                              "the feedback chain's copy of the snapshot, the fallbacks would not")
         if not 1 <= n <= N.LIG_MAX_FALLBACKS:
@@ -344,14 +349,20 @@ class Scheduler:
         """ScheduleBatch plus up to n fallback pods per request (lig_schedule_batch_fallbacks):
         (pods, error) per request, pods[0] the pod ScheduleBatch would have returned, then distinct
         survivors in the order a proxy should retry them.  One rand_key per request from the same
-        sequence as ScheduleBatch.  ValueError under load_feedback_window."""
+        sequence as ScheduleBatch.  Under load_feedback_window the call is a feedback-chain call
+        (lig_schedule_batch_feedback_chain_fallbacks) when the scheduler was built with
+        feedback_fallbacks=True, and raises ValueError otherwise."""
         self._check_fallbacks(n)
         snap = self._current()
         arr = np.zeros(len(reqs), dtype=REQ_DTYPE)
         for i, r in enumerate(reqs):
             arr[i] = (snap.adapter_id(r.ResolvedTargetModel), N.LIG_REQ_CRITICAL if r.Critical else 0,
                       self._rng.getrandbits(64))
-        picks, rows = self._engine.schedule_batch_fallbacks(self._epoch, self._seed, arr, n)
+        if self._window:
+            picks, rows = self._engine.schedule_batch_feedback_chain_fallbacks(self._epoch, self._seed, arr, n,
+                                                                               self._window)
+        else:
+            picks, rows = self._engine.schedule_batch_fallbacks(self._epoch, self._seed, arr, n)
         out: List[Tuple[List[Pod], Optional[StatusError]]] = []
         for pk, row in zip(picks, rows):
             if pk["status"] == N.LIG_OK:
@@ -371,8 +382,8 @@ class Scheduler:
                                         ) -> List[Tuple[List[Pod], str, Optional[StatusError]]]:
         """ScheduleModelBatch plus up to n fallback pods per request: (pods, resolved target model,
         error) per name, pods[0] the pod ScheduleModelBatch would have returned.  Host-answered errors
-        and the rand_key sequence (_model_index) as ScheduleModelBatch.  ValueError under
-        load_feedback_window."""
+        and the rand_key sequence (_model_index) as ScheduleModelBatch.  Under load_feedback_window
+        as ScheduleBatchWithFallbacks: a chain call with feedback_fallbacks=True, else ValueError."""
         self._check_fallbacks(n)
         snap = self._current()
         pm = self._packed_models
@@ -390,9 +401,13 @@ class Scheduler:
                 slots.append(i)
         if not ids:
             return out
-        picks, rows = self._engine.schedule_models_batch_fallbacks(self._epoch, self._seed,
-                                                                   np.array(ids, dtype=np.uint32), n,
-                                                                   first_index=self._model_index)
+        arr = np.array(ids, dtype=np.uint32)
+        if self._window:
+            picks, rows = self._engine.schedule_models_batch_feedback_chain_fallbacks(
+                self._epoch, self._seed, arr, n, self._window, first_index=self._model_index)
+        else:
+            picks, rows = self._engine.schedule_models_batch_fallbacks(self._epoch, self._seed, arr, n,
+                                                                       first_index=self._model_index)
         self._model_index += len(ids)
         for i, m, pk, row in zip(slots, ids, picks, rows):
             t, st = int(pk["target_idx"]), int(pk["status"])
@@ -480,9 +495,14 @@ class Scheduler:
 
 
 def NewScheduler(pmp: PodMetricsProvider, filter: Optional[Filter] = None, load_feedback_window: int = 0,
-                 **kw) -> Scheduler:  # scheduler.go:93-99
+                 feedback_fallbacks: bool = False, **kw) -> Scheduler:  # scheduler.go:93-99
     """filter: a caller flow chart (None = defaultFilter, the reference's only tree).
     load_feedback_window > 0: ScheduleBatch goes through the load-feedback chain (include/lig.h,
     lig_schedule_batch_feedback_chain): every window of that many requests, counted across calls,
-    adds its picks to the pods' WaitingQueueSize until the next refresh.  0 = off."""
-    return Scheduler(pmp, filter=filter, load_feedback_window=load_feedback_window, **kw)
+    adds its picks to the pods' WaitingQueueSize until the next refresh.  0 = off.
+    feedback_fallbacks: under load_feedback_window, let the *WithFallbacks calls run as chain calls
+    whose rows rank the chain's load-adjusted survivors (lig_schedule_batch_feedback_chain_fallbacks);
+    without it they raise ValueError there, as they always have.  The picks and the chain's loads do
+    not depend on it."""
+    return Scheduler(pmp, filter=filter, load_feedback_window=load_feedback_window,
+                     feedback_fallbacks=feedback_fallbacks, **kw)
