@@ -161,7 +161,7 @@ typedef struct lig_filter_node {         /* 32 bytes */
  * several parents (defaultFilter shares queueAndKVCacheFilter).  The direct scan
  * (lig_schedule_scan[_device]) restates the built-in tree only: it returns LIG_ERR_INVALID for an
  * epoch whose tables a caller tree built; lig_filter_batch and lig_read_class return a caller tree's
- * survivor sets. */
+ * survivor sets, and lig_schedule_batch_excluding walks the tree that built the epoch, per request. */
 int  lig_set_filter_tree(lig_ctx* ctx, const lig_filter_node* nodes, int n_nodes);
 
 /* ---- snapshot = the value of PodMetricsProvider.AllPodMetrics() (scheduler.go:108-115,
@@ -496,6 +496,40 @@ int lig_schedule_models_batch_fallbacks(lig_ctx* ctx, uint64_t epoch, uint64_t s
 int lig_schedule_models_batch_fallbacks_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64_t first_index,
                                                const uint32_t* d_model_ids, int R, lig_mpick* d_out,
                                                int n_fallbacks, int16_t* d_fallbacks, void* stream);
+
+/* ---- retry scheduling: schedule again without the pods a request already tried ------------------------
+ * A fallback row runs out within a class's few survivors.  When every pod a proxy tried refused, the
+ * reference's answer is Scheduler.Schedule over AllPodMetrics() without those pods (what it schedules
+ * once they leave the provider): the range filters are recomputed over the remaining pods, so the
+ * pick can be a pod outside the original survivor set.
+ *
+ * The definition.  Request i comes with row excluded[i * n_excluded .. (i + 1) * n_excluded) of int16
+ * pod indices (the element type of a fallback row, so a proxy can pass back the pick and the row
+ * entries it tried).  Its pool is the epoch's pods in their order minus the distinct entries of the
+ * row that lie in [0, P); entries outside [0, P), -1 padding included, exclude nothing (as an
+ * adapter_id outside [0, A) is a miss, not an error).  The result is Schedule (scheduler.go:113-122)
+ * on that pool: the epoch's tree (the built-in tree with the ctx's thresholds, or the caller tree
+ * that built the epoch, whatever lig_set_filter_tree has set since), n_survivors the size of the
+ * reduced survivor set, the pick Int31n(n) on state seed ^ rand_key taking that survivor in pod
+ * order, pod_idx an index into the epoch's full pod order.  Statuses are those of the schedule
+ * calls; an empty pool runs as Go does with an empty slice (under the built-in tree: LIG_DROP for
+ * critical and sheddable requests alike).  A row that excludes nothing gives lig_schedule_batch's
+ * result byte for byte.  The calls read the resident epoch, never a feedback chain's copy.
+ *
+ * One warp per request walks the tree from its own pool (the direct scan's formulation).
+ * LIG_ERR_INVALID, with nothing written, for n_excluded outside [1, LIG_MAX_EXCLUDED], null buffers
+ * when R > 0, R > max_batch on the host form, and device buffers not aligned to their element
+ * (requests 16 bytes, picks 8, rows 2); a stale epoch and a missing snapshot as lig_schedule_batch
+ * reports them.  Host form: page-locked buffers are read and written in place, pageable or
+ * misaligned ones (a request array at an odd 8 bytes included) are staged; it blocks until the picks
+ * are back.  Device form: device pointers, enqueued on `stream` (NULL = legacy default stream), not
+ * synchronised.  Both register as readers of the epoch's slot. */
+#define LIG_MAX_EXCLUDED 32     /* one lane of the request's warp per entry */
+int lig_schedule_batch_excluding(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
+                                 const int16_t* excluded, int n_excluded, lig_pick* out);
+int lig_schedule_batch_excluding_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* d_reqs,
+                                        int R, const int16_t* d_excluded, int n_excluded, lig_pick* d_out,
+                                        void* stream);
 
 /* ---- in-batch load feedback (opt-in; the default path never mutates the snapshot) ----------------
  * The reference schedules every request against the scraped metrics as they are

@@ -24,6 +24,7 @@ LIG_MAX_FILTER_NODES = 32
 LIG_REQ_CRITICAL = 1
 LIG_MAX_PODS, LIG_MAX_ADAPTERS = 32768, 65534
 LIG_MAX_FALLBACKS = 8
+LIG_MAX_EXCLUDED = 32
 (LIG_KERNEL_NONE, LIG_KERNEL_PERSISTENT, LIG_KERNEL_LOOP, LIG_KERNEL_PLAIN, LIG_KERNEL_QUEUE, LIG_KERNEL_MODELS,
  LIG_KERNEL_MODELS_PLAIN) = range(7)
 
@@ -52,6 +53,7 @@ EXPORTED_SYMBOLS = (
     "lig_schedule_models_batch_fallbacks_device",
     "lig_schedule_batch_feedback_chain_fallbacks", "lig_schedule_batch_feedback_chain_fallbacks_device",
     "lig_schedule_models_batch_feedback_chain_fallbacks", "lig_schedule_models_batch_feedback_chain_fallbacks_device",
+    "lig_schedule_batch_excluding", "lig_schedule_batch_excluding_device",
 )
 
 
@@ -176,6 +178,8 @@ def load() -> C.CDLL:
                                                                        vp]
     lib.lig_schedule_models_batch_feedback_chain_fallbacks_device.argtypes = [vp, u64, u64, u64, vp, i32, vp, i32,
                                                                               vp, i32, vp, vp]
+    lib.lig_schedule_batch_excluding.argtypes = [vp, u64, u64, vp, i32, vp, i32, vp]
+    lib.lig_schedule_batch_excluding_device.argtypes = [vp, u64, u64, vp, i32, vp, i32, vp, vp]
     lib.lig_update_snapshot.argtypes = [vp, u64, u64, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.lig_pick_kernel_info.argtypes = [vp, u64, C.c_char_p, i32, C.POINTER(i32), C.POINTER(i32),
                                          C.POINTER(i32), C.POINTER(i32)]

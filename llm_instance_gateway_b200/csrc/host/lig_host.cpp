@@ -25,6 +25,16 @@ Status LigFailure(const char* what) {
 const char kDropInner[] =
     "rpc error: code = ResourceExhausted desc = dropping request due to limited backend resources";
 
+// Schedule's error for a pick that is not LIG_OK                            scheduler.go:117
+Status PickError(uint16_t status) {
+  if (status == LIG_DROP)
+    return Errorf(ResourceExhausted, std::string("failed to apply filter, resulted 0 pods, this should never "
+                                                 "happen: ") + kDropInner);
+  if (status == LIG_NO_PODS_LEFT)   // a caller tree's predicate leaf kept no pod     filter.go:88-90
+    return Errorf(Unknown, "failed to apply filter, resulted 0 pods, this should never happen: no pods left");
+  return Errorf(Unknown, "failed to apply filter, resulted 0 pods, this should never happen: %!w(<nil>)");
+}
+
 inline uint64_t splitmix_next(uint64_t& s) {
   uint64_t z = (s += 0x9E3779B97F4A7C15ull);
   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
@@ -100,6 +110,7 @@ Scheduler::~Scheduler() {
   if (h_reqs_) lig_host_free(h_reqs_);
   if (h_picks_) lig_host_free(h_picks_);
   if (h_fallbacks_) lig_host_free(h_fallbacks_);
+  if (h_excluded_) lig_host_free(h_excluded_);
   if (h_model_ids_) lig_host_free(h_model_ids_);
   if (h_mpicks_) lig_host_free(h_mpicks_);
   if (ctx_) lig_destroy(ctx_);
@@ -395,6 +406,24 @@ Status Scheduler::ScheduleWithFallbacks(const LLMRequest& req, int n, std::vecto
   return w.status;
 }
 
+Status Scheduler::ScheduleRetry(const LLMRequest& req, const std::vector<backend::Pod>& tried,
+                                backend::Pod* targetPod) {
+  if (tried.size() > (size_t)LIG_MAX_EXCLUDED)
+    return Errorf(InvalidArgument, "ScheduleRetry: " + std::to_string(tried.size()) + " tried pods (at most " +
+                                       std::to_string(LIG_MAX_EXCLUDED) + ")");
+  if (opt_.load_feedback_window > 0)
+    return Errorf(InvalidArgument, "ScheduleRetry: not defined under load_feedback_window (the picks come from the "
+                                   "feedback chain's copy of the snapshot, a retry would not)");
+  if (group_)
+    return Errorf(InvalidArgument, "ScheduleRetry: a scheduler over several devices has no retry call");
+  Waiter w;
+  w.req = &req;
+  w.tried = &tried;
+  Submit(w);
+  if (w.status.ok() && targetPod) *targetPod = std::move(w.pod);
+  return w.status;
+}
+
 Status Scheduler::ScheduleModel(const std::string& model, std::string* resolvedTargetModel, backend::Pod* targetPod) {
   Waiter w;
   w.model = &model;
@@ -541,7 +570,8 @@ void Scheduler::CountFeedback(uint64_t epoch, int n) {
 void Scheduler::Flush(std::vector<Waiter*>& all) {
   desc_lane_.clear();
   model_lane_.clear();
-  for (Waiter* w : all) (w->model ? model_lane_ : desc_lane_).push_back(w);
+  retry_lane_.clear();
+  for (Waiter* w : all) (w->model ? model_lane_ : w->tried ? retry_lane_ : desc_lane_).push_back(w);
   std::vector<Waiter*>& batch = desc_lane_;
   size_t done = 0;
   const auto flush_t0 = std::chrono::steady_clock::now();
@@ -611,16 +641,8 @@ void Scheduler::Flush(std::vector<Waiter*>& all) {
           const int16_t* row = h_fallbacks_ + (size_t)i * (size_t)nf;
           for (int j = 0; j < w->fallbacks && row[j] >= 0; ++j) w->pods->push_back(snap->pods[(size_t)row[j]]);
         }
-      } else if (h_picks_[i].status == LIG_DROP) {
-        w->status = Errorf(ResourceExhausted,                         // scheduler.go:117
-                           std::string("failed to apply filter, resulted 0 pods, this should never "
-                                       "happen: ") + kDropInner);
-      } else if (h_picks_[i].status == LIG_NO_PODS_LEFT) {   // a caller tree's predicate leaf kept no pod
-        w->status = Errorf(Unknown, "failed to apply filter, resulted 0 pods, this should never "
-                                    "happen: no pods left");   // filter.go:88-90
       } else {
-        w->status = Errorf(Unknown, "failed to apply filter, resulted 0 pods, this should never "
-                                    "happen: %!w(<nil>)");
+        w->status = PickError(h_picks_[i].status);
       }
     }
     {
@@ -638,6 +660,7 @@ void Scheduler::Flush(std::vector<Waiter*>& all) {
     }
     done += (size_t)n;
   }
+  FlushRetries(retry_lane_);
   FlushModels(model_lane_);
   const double flush_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - flush_t0).count();
   std::lock_guard<std::mutex> sk(stats_mu_);
@@ -647,6 +670,84 @@ void Scheduler::Flush(std::vector<Waiter*>& all) {
     stats_.slowest_call_batch = stats_.batches ? stats_.batches - 1 : 0;
   }
   stats_.max_flush_us = std::max(stats_.max_flush_us, flush_us);
+}
+
+// The retry lane: one lig_schedule_batch_excluding call per max_batch waiters.  Each waiter's tried
+// pods are matched by value against the captured snapshot; its row holds their indices, -1 padded to
+// the widest row of the call.
+void Scheduler::FlushRetries(std::vector<Waiter*>& batch) {
+  if (batch.empty()) return;
+  Status failure;
+  if (!h_excluded_) {
+    h_excluded_ = static_cast<int16_t*>(lig_host_alloc((size_t)opt_.max_batch * LIG_MAX_EXCLUDED * sizeof(int16_t)));
+    if (!h_excluded_) failure = LigFailure("lig_host_alloc");
+  }
+  std::vector<std::vector<int16_t>> rows;
+  size_t done = 0;
+  while (done < batch.size()) {
+    const int n = (int)std::min(batch.size() - done, (size_t)opt_.max_batch);
+    std::shared_ptr<const Snapshot> snap;
+    int rc = 0, width = 1;
+    for (int attempt = 0; failure.ok() && attempt < 4; ++attempt) {
+      {
+        std::lock_guard<std::mutex> lk(snap_mu_);
+        snap = snap_;
+      }
+      std::unordered_map<std::string, std::vector<int16_t>> where;   // Name + '\0' + Address -> pod indices
+      for (size_t p = 0; p < snap->pods.size(); ++p)
+        where[snap->pods[p].Name + '\0' + snap->pods[p].Address].push_back((int16_t)p);
+      rows.assign((size_t)n, {});
+      width = 1;
+      for (int i = 0; i < n; ++i) {
+        std::vector<int16_t>& row = rows[(size_t)i];
+        for (const backend::Pod& t : *batch[done + i]->tried) {
+          auto it = where.find(t.Name + '\0' + t.Address);
+          if (it != where.end()) row.insert(row.end(), it->second.begin(), it->second.end());
+        }
+        // only pods listed more than once in the slice get past 32: that caller is refused below
+        if ((int)row.size() <= LIG_MAX_EXCLUDED) width = std::max(width, (int)row.size());
+      }
+      for (int i = 0; i < n; ++i) {
+        const LLMRequest& r = *batch[done + i]->req;
+        auto it = snap->adapter_ids->find(r.ResolvedTargetModel);   // interned as in Flush
+        h_reqs_[i].adapter_id = (it == snap->adapter_ids->end() || it->second >= snap->A) ? snap->A : it->second;
+        h_reqs_[i].flags = r.Critical ? LIG_REQ_CRITICAL : 0u;
+        h_reqs_[i].rand_key = splitmix_next(rng_state_);
+        int16_t* row = h_excluded_ + (size_t)i * (size_t)width;
+        const std::vector<int16_t>& ex = rows[(size_t)i];
+        const int k = (int)ex.size() <= width ? (int)ex.size() : 0;
+        for (int j = 0; j < width; ++j) row[j] = j < k ? ex[(size_t)j] : (int16_t)-1;
+      }
+      rc = lig_schedule_batch_excluding(ctx_, snap->epoch, seed_, h_reqs_, n, h_excluded_, width, h_picks_);
+      if (rc != LIG_ERR_STALE_EPOCH) break;   // two refreshes raced past this batch: re-resolve
+      std::lock_guard<std::mutex> sk(stats_mu_);
+      stats_.stale_retries++;
+    }
+    if (failure.ok() && rc != 0) failure = LigFailure("lig_schedule_batch_excluding");
+    for (int i = 0; i < n; ++i) {
+      Waiter* w = batch[done + i];
+      if (!failure.ok()) w->status = failure;
+      else if (rows[(size_t)i].size() > (size_t)LIG_MAX_EXCLUDED)
+        w->status = Errorf(InvalidArgument, "ScheduleRetry: the tried pods match more than " +
+                                                std::to_string(LIG_MAX_EXCLUDED) + " pods of the snapshot");
+      else if (h_picks_[i].status == LIG_OK) w->pod = snap->pods[(size_t)h_picks_[i].pod_idx];
+      else w->status = PickError(h_picks_[i].status);
+    }
+    {
+      std::lock_guard<std::mutex> sk(stats_mu_);
+      stats_.scheduled += (uint64_t)n;
+      stats_.retry_scheduled += (uint64_t)n;
+      stats_.batches++;
+      stats_.max_batch = std::max<uint64_t>(stats_.max_batch, (uint64_t)n);
+    }
+    for (int i = 0; i < n; ++i) {
+      Waiter* w = batch[done + i];
+      w->done.store(1, std::memory_order_release);
+      w->done.notify_one();
+      w->done.store(2, std::memory_order_release);   // last access: the caller may now destroy *w
+    }
+    done += (size_t)n;
+  }
 }
 
 // The model-id lane: names are mapped to ids against the captured epoch's list; names the host can

@@ -180,6 +180,7 @@ struct Stats {
   uint64_t model_scheduled = 0;    // ScheduleModel(model, ...) calls completed (host-answered ones included)
   uint64_t model_batches = 0;      // device calls issued for model-id requests
   uint64_t fallback_scheduled = 0; // ScheduleWithFallbacks and ScheduleModelWithFallbacks calls completed
+  uint64_t retry_scheduled = 0;    // ScheduleRetry calls completed
   double last_pack_us = 0;     // last Refresh: provider slice -> columns + bitmap (host)
   double last_upload_us = 0;   // last Refresh: lig_upload_snapshot (H2D + class tables)
   double max_device_call_us = 0;   // slowest single lig_schedule_batch call (launch + kernel + synchronise)
@@ -214,6 +215,18 @@ class Scheduler {
   // load_feedback_window > 0 and no feedback_fallbacks (the picks come from the feedback chain's
   // copy), and with several devices.
   Status ScheduleWithFallbacks(const LLMRequest& req, int n, std::vector<backend::Pod>* pods);
+
+  // Schedule again without the pods already tried: Schedule over the current epoch's pods minus
+  // `tried` (lig_schedule_batch_excluding), what Schedule returns once those pods have left the
+  // provider.  Tried pods are matched by value (Name and Address) against the snapshot current at
+  // flush time, so a retry after a refresh still excludes the right pods; pods no longer in it are
+  // ignored.  Goes through the micro-batcher and takes the next rand_key from the same sequence as
+  // Schedule, in flush order; a flush's retries make one device call after its plain descriptor
+  // requests, never through the doorbell.  Errors are Schedule's.  InvalidArgument with more than
+  // LIG_MAX_EXCLUDED (32) tried pods, with load_feedback_window > 0 (the picks come from the feedback
+  // chain's copy of the snapshot, a retry would not) and with several devices.  A handler that used
+  // ScheduleModel builds req from the resolved target model it got back and the model's criticality.
+  Status ScheduleRetry(const LLMRequest& req, const std::vector<backend::Pod>& tried, backend::Pod* targetPod);
 
   // The reference's Filter interface (filter.go:12-15) run on the current epoch: fills *pods with
   // the survivors of req's walk of the filter tree (the built-in one or Options::filter), in slice
@@ -331,6 +344,7 @@ class Scheduler {
     const std::string* model = nullptr;
     int fallbacks = 0;           // *WithFallbacks: the n asked for (0: Schedule / ScheduleModel)
     std::vector<backend::Pod>* pods = nullptr;   // *WithFallbacks: receives the pick and its row
+    const std::vector<backend::Pod>* tried = nullptr;   // ScheduleRetry: the pods to leave out
     int64_t model_id = -1;       // flush-time id in the captured epoch's table; -1: answered on the host
     std::string resolved;        // model requests: the resolved target model
     Status status;
@@ -343,6 +357,7 @@ class Scheduler {
   void Submit(Waiter& w);
   void Flush(std::vector<Waiter*>& batch);
   void FlushModels(std::vector<Waiter*>& batch);
+  void FlushRetries(std::vector<Waiter*>& batch);
   void CountFeedback(uint64_t epoch, int n);
   Status CheckFallbacks(const char* fn, int n) const;
 
@@ -356,7 +371,8 @@ class Scheduler {
   uint32_t* h_model_ids_ = nullptr;   // pinned, max_batch entries each: the model-id lane
   lig_mpick* h_mpicks_ = nullptr;
   uint64_t model_index_ = 0;          // first_index of the next model-id device call
-  std::vector<Waiter*> desc_lane_, model_lane_;   // a flush split by kind (batcher thread only)
+  std::vector<Waiter*> desc_lane_, model_lane_, retry_lane_;   // a flush split by kind (batcher thread only)
+  int16_t* h_excluded_ = nullptr;     // pinned, max_batch x LIG_MAX_EXCLUDED rows (first retry flush)
   uint64_t seed_ = 0;
   uint64_t rng_state_ = 0;
   // the feedback chain as the batcher thread sees it (the library's window count is deterministic)

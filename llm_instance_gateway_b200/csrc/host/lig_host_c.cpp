@@ -293,6 +293,28 @@ int ligh_schedule_with_fallbacks(ligh_scheduler* s, const char* resolved, int cr
 
 uint64_t ligh_fallback_scheduled(ligh_scheduler* s) { return s->sched->stats().fallback_scheduled; }
 
+int ligh_schedule_retry(ligh_scheduler* s, const char* resolved, int critical, const char* const* tried_names,
+                        const char* const* tried_addrs, int n_tried, char* name, int name_cap, char* addr, int addr_cap,
+                        char* err, int err_cap) {
+  scheduling::LLMRequest req;
+  req.ResolvedTargetModel = resolved ? resolved : "";
+  req.Critical = critical != 0;
+  std::vector<backend::Pod> tried;
+  for (int i = 0; i < n_tried; ++i)
+    tried.push_back(backend::Pod{tried_names[i] ? tried_names[i] : "", tried_addrs[i] ? tried_addrs[i] : ""});
+  backend::Pod pod;
+  scheduling::Status st = s->sched->ScheduleRetry(req, tried, &pod);
+  if (st.ok()) {
+    put(name, name_cap, pod.Name);
+    put(addr, addr_cap, pod.Address);
+  } else {
+    put(err, err_cap, st.message);
+  }
+  return st.code;
+}
+
+uint64_t ligh_retry_scheduled(ligh_scheduler* s) { return s->sched->stats().retry_scheduled; }
+
 int ligh_filter(ligh_scheduler* s, const char* resolved, int critical, char* names, int names_cap, int* n_pods,
                 char* err, int err_cap) {
   scheduling::LLMRequest req;

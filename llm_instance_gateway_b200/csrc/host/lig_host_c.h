@@ -59,6 +59,12 @@ int ligh_filter(ligh_scheduler*, const char* resolved_target_model, int critical
 int ligh_schedule_with_fallbacks(ligh_scheduler*, const char* resolved_target_model, int critical, int n,
                                  char* names, int names_cap, int* n_pods, char* err, int err_cap);
 uint64_t ligh_fallback_scheduled(ligh_scheduler*);   /* Stats::fallback_scheduled */
+/* Scheduler::ScheduleRetry: returns the gRPC code; the tried pods are given by value as n_tried
+ * (name, address) pairs. */
+int ligh_schedule_retry(ligh_scheduler*, const char* resolved_target_model, int critical, const char* const* tried_names,
+                        const char* const* tried_addrs, int n_tried, char* name, int name_cap, char* addr, int addr_cap,
+                        char* err, int err_cap);
+uint64_t ligh_retry_scheduled(ligh_scheduler*);      /* Stats::retry_scheduled */
 int ligh_refresh(ligh_scheduler*, char* err, int err_cap);
 /* several GPUs behind one scheduler (lig_group_*) */
 ligh_scheduler* ligh_scheduler_new_devices(ligh_provider*, const int* devices, int n_devices, int max_pods,

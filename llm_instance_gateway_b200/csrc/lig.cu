@@ -108,6 +108,7 @@ struct Slot {
   int next_reader = 0;
   uint64_t stamp = 0;               // upload order, to pick the slot to overwrite
   bool caller_tree = false;         // tables built with a caller filter tree (thresholds do not apply)
+  FilterTree tree{};                // that tree (caller_tree only): the retry walk runs the epoch's own tree
 };
 
 constexpr int kLanes = 8;   // streams of the host-buffer path; also the queue streams
@@ -306,6 +307,7 @@ int launch_class_build(lig_ctx* c, Slot& s, cudaStream_t stream, const FilterTre
   const int W = s.W > 0 ? s.W : 1;
   s.caller_tree = tree != nullptr;
   if (tree) {
+    s.tree = *tree;
     // one warp per class; the pod columns go to shared memory when they fit (P up to ~12 K pods)
     const bool staged = s.P > 0 && tree_fixed_bytes(W) + staged_bytes(W) <= c->smem_optin;
     const size_t smem = tree_fixed_bytes(W) + (staged ? staged_bytes(W) : 0);
@@ -1020,6 +1022,10 @@ static int create_impl(lig_ctx* c, int device, int max_pods, int max_adapters, i
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_scan_kernel<false>,
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   const size_t need = scratch_bytes(words_for(max_pods)) > build_fixed_bytes(words_for(max_pods))
                           ? scratch_bytes(words_for(max_pods)) : build_fixed_bytes(words_for(max_pods));
   if (need > c->smem_optin)
@@ -2161,6 +2167,137 @@ int lig_schedule_models_batch_fallbacks_device(lig_ctx* c, uint64_t epoch, uint6
   return fallback_device(c, "lig_schedule_models_batch_fallbacks_device", epoch,
                          FallbackCall{true, seed, first_index, d_model_ids, R, d_out, n_fallbacks, d_fallbacks},
                          stream);
+}
+
+// ---- retry scheduling (lig_schedule_batch_excluding) ---------------------------------------------------
+struct ExcludingCall {
+  uint64_t seed;
+  const lig_req* reqs;
+  int R;
+  lig_pick* out;
+  int n_excluded;
+  const int16_t* excluded;
+  size_t row_bytes() const { return (size_t)n_excluded * sizeof(int16_t); }
+};
+
+static int excluding_check(const lig_ctx* c, const char* fn, const ExcludingCall& x) {
+  if (!c || x.R < 0 || (x.R > 0 && (!x.reqs || !x.out || !x.excluded)))
+    return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
+  if (x.n_excluded < 1 || x.n_excluded > LIG_MAX_EXCLUDED)
+    return fail(LIG_ERR_INVALID, "%s: n_excluded=%d outside [1, %d]", fn, x.n_excluded, LIG_MAX_EXCLUDED);
+  return 0;
+}
+
+// Enqueue the retry kernel for x (R >= 1, device-visible, aligned pointers) against slot s on st,
+// behind the slot's tables, and register st as a reader of the slot.  The scan's launch shape; the
+// walk is the tree that built the slot's tables.  Caller holds c->mu.
+static int enqueue_excluding(lig_ctx* c, Slot& s, const ExcludingCall& x, cudaStream_t st) {
+  static const FilterTree kNoTree{};
+  CUDA_TRY(cudaStreamWaitEvent(st, s.ready, 0));
+  const SnapView v = view_of(s);
+  const bool staged = s.P > 0 && staged_fits(c, s.W);
+  const size_t smem = scratch_bytes(s.W > 0 ? s.W : 1) + (staged ? staged_bytes(s.W) : 0);
+  const int ctas_per_sm = staged ? (smem > 110 * 1024 ? 1 : 2) : 4;
+  const int ctas_needed = (x.R + kWarpsPerCta - 1) / kWarpsPerCta;
+  const int grid = ctas_needed < c->sm_count * ctas_per_sm ? ctas_needed : c->sm_count * ctas_per_sm;
+  const FilterTree& tree = s.caller_tree ? s.tree : kNoTree;
+  const int4* in = reinterpret_cast<const int4*>(x.reqs);
+  int2* out = reinterpret_cast<int2*>(x.out);
+  const Thr thr = thr_of(c);
+  if (s.caller_tree) {
+    if (staged)
+      lig_schedule_excluding_kernel<true, true><<<grid, kCtaThreads, smem, st>>>(
+          v, thr, tree, in, x.excluded, x.n_excluded, out, x.R, x.seed);
+    else
+      lig_schedule_excluding_kernel<false, true><<<grid, kCtaThreads, smem, st>>>(
+          v, thr, tree, in, x.excluded, x.n_excluded, out, x.R, x.seed);
+  } else {
+    if (staged)
+      lig_schedule_excluding_kernel<true, false><<<grid, kCtaThreads, smem, st>>>(
+          v, thr, tree, in, x.excluded, x.n_excluded, out, x.R, x.seed);
+    else
+      lig_schedule_excluding_kernel<false, false><<<grid, kCtaThreads, smem, st>>>(
+          v, thr, tree, in, x.excluded, x.n_excluded, out, x.R, x.seed);
+  }
+  CUDA_TRY(cudaGetLastError());
+  c->launches++;
+  return note_reader(s, st);
+}
+
+int lig_schedule_batch_excluding_device(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* d_reqs, int R,
+                                        const int16_t* d_excluded, int n_excluded, lig_pick* d_out, void* stream) {
+  static const char fn[] = "lig_schedule_batch_excluding_device";
+  const ExcludingCall x{seed, d_reqs, R, d_out, n_excluded, d_excluded};
+  if (int rc = excluding_check(c, fn, x)) return rc;
+  if (R > 0 && (misaligned(d_reqs, sizeof(lig_req)) || misaligned(d_out, sizeof(lig_pick)) ||
+                misaligned(d_excluded, sizeof(int16_t))))
+    return fail(LIG_ERR_INVALID, "%s: a device buffer is not aligned to its element", fn);
+  std::lock_guard<std::mutex> lk(c->mu);
+  Slot* s = nullptr;
+  if (int rc = resolve_slot(c, epoch, &s)) return rc;
+  if (R == 0) return 0;
+  CUDA_TRY(cudaSetDevice(c->device));
+  return enqueue_excluding(c, *s, x, static_cast<cudaStream_t>(stream));
+}
+
+// Host buffers: page-locked, aligned ones are read and written by the kernel in place; the others
+// are staged in stream-ordered HBM and copied on the call's lane.  Blocks until the picks are back.
+int lig_schedule_batch_excluding(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
+                                 const int16_t* excluded, int n_excluded, lig_pick* out) {
+  static const char fn[] = "lig_schedule_batch_excluding";
+  const ExcludingCall x{seed, reqs, R, out, n_excluded, excluded};
+  if (int rc = excluding_check(c, fn, x)) return rc;
+  if (R > c->max_batch) return fail(LIG_ERR_INVALID, "%s: R=%d exceeds max_batch=%d", fn, R, c->max_batch);
+  ExcludingCall d = x;    // the same call with device-visible pointers
+  const size_t in_b = (size_t)R * sizeof(lig_req), out_b = (size_t)R * sizeof(lig_pick);
+  const size_t rows_b = (size_t)R * x.row_bytes();
+  d.reqs = R ? mapped_device_pointer(reqs) : nullptr;
+  d.out = R ? mapped_device_pointer(out) : nullptr;
+  d.excluded = R ? mapped_device_pointer(excluded) : nullptr;
+  // the kernel reads a descriptor with one 16-byte load and stores every pick whole
+  const bool st_in = R && (!d.reqs || misaligned(d.reqs, sizeof(lig_req)));
+  const bool st_out = R && (!d.out || misaligned(d.out, sizeof(lig_pick)));
+  const bool st_rows = R && (!d.excluded || misaligned(d.excluded, sizeof(int16_t)));
+  cudaStream_t st = nullptr;
+  unsigned char* stage = nullptr;
+  {
+    std::lock_guard<std::mutex> lk(c->mu);
+    Slot* s = nullptr;
+    if (int rc = resolve_slot(c, epoch, &s)) return rc;
+    if (R == 0) return 0;
+    CUDA_TRY(cudaSetDevice(c->device));
+    st = c->s_lane[c->next_lane];
+    c->next_lane = (c->next_lane + 1) % kLanes;
+    size_t at = 0, o_in = 0, o_out = 0, o_rows = 0;
+    auto take = [&](bool on, size_t bytes, size_t* o) { if (on) { *o = at; at = (at + bytes + 255) & ~(size_t)255; } };
+    take(st_in, in_b, &o_in);
+    take(st_out, out_b, &o_out);
+    take(st_rows, rows_b, &o_rows);
+    if (at) {
+      CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&stage), at, st));
+      if (st_in) d.reqs = reinterpret_cast<const lig_req*>(stage + o_in);
+      if (st_out) d.out = reinterpret_cast<lig_pick*>(stage + o_out);
+      if (st_rows) d.excluded = reinterpret_cast<const int16_t*>(stage + o_rows);
+    }
+    int rc = 0;
+    if (st_in && cudaMemcpyAsync(const_cast<lig_req*>(d.reqs), reqs, in_b, cudaMemcpyHostToDevice, st) != cudaSuccess)
+      rc = fail(LIG_ERR_CUDA, "%s: staging the requests failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
+    if (!rc && st_rows &&
+        cudaMemcpyAsync(const_cast<int16_t*>(d.excluded), excluded, rows_b, cudaMemcpyHostToDevice, st) != cudaSuccess)
+      rc = fail(LIG_ERR_CUDA, "%s: staging the rows failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
+    if (!rc) rc = enqueue_excluding(c, *s, d, st);
+    if (rc) {
+      if (stage) cudaFreeAsync(stage, st);
+      return rc;
+    }
+  }
+  // the copy back waits for the kernel on the lane; it may block, so not under c->mu
+  cudaError_t e = cudaSuccess;
+  if (st_out) e = cudaMemcpyAsync(out, d.out, out_b, cudaMemcpyDeviceToHost, st);
+  if (stage) cudaFreeAsync(stage, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(LIG_ERR_CUDA, "%s failed on the device: %s", fn, cudaGetErrorString(e));
+  return 0;
 }
 
 int lig_pick_kernel_info(lig_ctx* c, uint64_t epoch, char* name, int name_len, int* grid, int* threads,

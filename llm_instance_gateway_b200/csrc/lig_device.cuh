@@ -248,18 +248,23 @@ struct EvalResult {
 // Walk defaultFilter for one (critical, adapter row) over all P pods, one warp.
 //   X, T : per-warp scratch masks (W words each);  H : the adapter's bitmap row staged in shared
 //   memory (W words), or nullptr when the adapter is in no pod's ActiveModels.
-template <bool kStaged>
+// kRootMask: the root's input is not every pod but the n_root pods of the mask the caller left in T
+// (a request's pool without its excluded pods, lig_schedule_batch_excluding).
+template <bool kStaged, bool kRootMask = false>
 __device__ __forceinline__ EvalResult tree_eval_warp(const Fields& f, const uint32_t* H,
                                                      bool critical, const Thr thr, int P, int W,
-                                                     uint32_t* X, uint32_t* T, int lane) {
+                                                     uint32_t* X, uint32_t* T, int lane,
+                                                     uint32_t n_root = 0) {
   uint32_t n = 0;
-  // criticalRequestPredicate keeps every pod or none; with P == 0 the predicate node yields
+  // criticalRequestPredicate keeps every pod or none; with an empty pool the predicate node yields
   // "no pods left" and the sheddable branch runs.            scheduler.go:26-31, filter.go:179-181
-  if (critical && P > 0) {
+  if (critical && (kRootMask ? n_root > 0 : P > 0)) {
     // "low queueing filter": q < queueingThresholdLoRA        scheduler.go:58-60, filter.go:124-126
     for (int w = 0; w < W; ++w) {
       int p = w * 32 + lane;
-      bool keep = p < P && (long long)ld_q<kStaged>(f, p) < thr.q_lora;
+      bool in_pool;
+      if constexpr (kRootMask) in_pool = (T[w] >> lane) & 1u; else in_pool = p < P;
+      bool keep = in_pool && (long long)ld_q<kStaged>(f, p) < thr.q_lora;
       uint32_t nw = __ballot_sync(kFull, keep);
       if (lane == 0) X[w] = nw;
       n += __popc(nw);
@@ -300,18 +305,25 @@ __device__ __forceinline__ EvalResult tree_eval_warp(const Fields& f, const uint
       return {X, n, n ? (uint32_t)LIG_OK : (uint32_t)LIG_EMPTY};
     }
     // low-queueing failed: its input (all pods) goes to queueLoRAAndKVCacheFilter   scheduler.go:71
-    for (int w = lane; w < W; w += 32) {
-      int rem = P - w * 32;
-      X[w] = rem >= 32 ? 0xffffffffu : ((1u << rem) - 1u);
+    if constexpr (kRootMask) {
+      uint32_t* s = X; X = T; T = s;
+      n = n_root;
+    } else {
+      for (int w = lane; w < W; w += 32) {
+        int rem = P - w * 32;
+        X[w] = rem >= 32 ? 0xffffffffu : ((1u << rem) - 1u);
+      }
+      __syncwarp();
+      n = (uint32_t)P;
     }
-    __syncwarp();
-    n = (uint32_t)P;
   } else {
     // "has capacity for sheddable requests"                     scheduler.go:74-79, filter.go:183-187
     for (int w = 0; w < W; ++w) {
       int p = w * 32 + lane;
       bool keep = false;
-      if (p < P) {
+      bool in_pool;
+      if constexpr (kRootMask) in_pool = (T[w] >> lane) & 1u; else in_pool = p < P;
+      if (in_pool) {
         keep = (long long)ld_q<kStaged>(f, p) <= thr.q_crit && ld_kv<kStaged>(f, p) <= thr.kv_thr;
       }
       uint32_t nw = __ballot_sync(kFull, keep);
@@ -1286,16 +1298,20 @@ __device__ __forceinline__ bool node_keeps(const lig_filter_node& nd, const Fiel
 
 // Walk the caller's tree for one (critical, adapter row), one warp.  H: the adapter's bitmap row in
 // shared memory, or nullptr for an adapter in no pod's ActiveModels (a Go map miss on every pod).
-template <bool kStaged>
+// kRootMask: the root's input is the n_root pods of the mask the caller left in `in`, not every pod.
+template <bool kStaged, bool kRootMask = false>
 __device__ __forceinline__ EvalResult tree_walk_warp(const Fields& f, const lig_filter_node* nodes,
                                                      const uint32_t* H, bool critical, int P, int W,
-                                                     uint32_t* in, uint32_t* res, int lane) {
-  for (int w = lane; w < W; w += 32) {   // the root's input: AllPodMetrics()    scheduler.go:115
-    const int rem = P - w * 32;
-    in[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
+                                                     uint32_t* in, uint32_t* res, int lane,
+                                                     uint32_t n_root = 0) {
+  if constexpr (!kRootMask) {
+    for (int w = lane; w < W; w += 32) {   // the root's input: AllPodMetrics()    scheduler.go:115
+      const int rem = P - w * 32;
+      in[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
+    }
+    __syncwarp();
   }
-  __syncwarp();
-  uint32_t n = (uint32_t)P;
+  uint32_t n = kRootMask ? n_root : (uint32_t)P;
   int i = 0;
   for (;;) {
     const lig_filter_node nd = nodes[i];
@@ -2831,6 +2847,62 @@ lig_scan_kernel(SnapView s, Thr thr, const int4* __restrict__ reqs, int2* __rest
     if (masks) {
       uint32_t* dst = masks + (size_t)i * s.W;
       for (int w = lane; w < s.W; w += 32) dst[w] = e.n ? e.mask[w] : 0u;
+    }
+    if (lane == 0) out[i] = make_int2(pod, (int)(e.status | (e.n << 16)));
+    __syncwarp();
+  }
+}
+
+// ---- retry scheduling: the tree over each request's pool without the pods it excludes --------------
+// The scan's launch shape (one warp per request, columns staged when they fit).  Lanes 0 .. n_excluded-1
+// each take one entry of the request's row and clear that pod's bit in the warp's root mask: a
+// shared-memory atomicAnd, so a duplicate clears nothing twice, and entries outside [0, P) clear
+// nothing.  The walk starts from that mask: the built-in tree, or (kTree) the caller tree that built
+// the epoch.  Requests and rows are read with plain loads: they may be page-locked host memory.
+template <bool kStaged, bool kTree>
+__global__ void __launch_bounds__(kCtaThreads)
+lig_schedule_excluding_kernel(SnapView s, Thr thr, const __grid_constant__ FilterTree tree, const int4* reqs,
+                              const int16_t* excluded, int n_excluded, int2* out, int R, uint64_t seed) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint32_t* X = reinterpret_cast<uint32_t*>(smem) + (size_t)warp * 3 * s.W;
+  uint32_t* T = X + s.W;       // the root mask: the built-in walk's second scratch mask, a tree walk's `in`
+  uint32_t* H = T + s.W;
+  Fields f{s.kv, s.q, s.n_active, s.max_active};
+  if constexpr (kStaged) {
+    f = stage_fields(s, smem + scratch_bytes(s.W));
+    __syncthreads();
+  }
+  for (int i = blockIdx.x * kWarpsPerCta + warp; i < R; i += gridDim.x * kWarpsPerCta) {
+    const int4 r = reqs[i];    // whole warp reads the same 16 bytes (broadcast)
+    const int ex = lane < n_excluded ? excluded[(size_t)i * n_excluded + lane] : -1;
+    const bool critical = ((uint32_t)r.y & LIG_REQ_CRITICAL) != 0;
+    const uint64_t key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
+    const uint32_t* Hrow = stage_adapter_row(s, r.x, H, lane);
+    for (int w = lane; w < s.W; w += 32) {   // the request's pool: every pod ...
+      const int rem = s.P - w * 32;
+      T[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
+    }
+    __syncwarp();
+    if (ex >= 0 && ex < s.P) atomicAnd(T + (ex >> 5), ~(1u << (ex & 31)));   // ... but the excluded
+    __syncwarp();
+    uint32_t n = 0;
+    for (int w = lane; w < s.W; w += 32) n += __popc(T[w]);
+    n = __reduce_add_sync(kFull, n);
+    EvalResult e;
+    if constexpr (kTree)
+      e = tree_walk_warp<kStaged, true>(f, tree.nodes, Hrow, critical, s.P, s.W, T, X, lane, n);
+    else
+      e = tree_eval_warp<kStaged, true>(f, Hrow, critical, thr, s.P, s.W, X, T, lane, n);
+    int pod = -1;
+    if (e.n > 0) {
+      uint32_t k = int31n(seed ^ key, e.n, max_accept_for(e.n));
+      for (int w = 0; w < s.W; ++w) {  // k-th survivor in pod order = pods[k]   scheduler.go:121
+        uint32_t word = e.mask[w];
+        uint32_t c = __popc(word);
+        if (k < c) { pod = w * 32 + (int)__fns(word, 0, (int)k + 1); break; }
+        k -= c;
+      }
     }
     if (lane == 0) out[i] = make_int2(pod, (int)(e.status | (e.n << 16)));
     __syncwarp();

@@ -295,6 +295,32 @@ class Engine:
         N.check(self._lib.lig_schedule_batch_fallbacks_device(self._ctx, epoch, seed, d_reqs or None, R,
                                                               d_out or None, n, d_fallbacks or None, stream or None))
 
+    # ---- retry scheduling: the tree again over each request's pool without the pods it excludes ----
+    def schedule_batch_excluding(self, epoch: int, seed: int, reqs: np.ndarray, excluded: np.ndarray) -> np.ndarray:
+        """lig_schedule_batch_excluding: excluded is an int16 array of shape (R, n_excluded) of pod indices
+        (entries outside [0, P) exclude nothing); request i is scheduled over the epoch's pods without
+        the pods of row i."""
+        assert reqs.dtype == REQ_DTYPE and reqs.flags.c_contiguous
+        assert excluded.dtype == np.int16 and excluded.flags.c_contiguous and excluded.ndim == 2
+        R = int(reqs.shape[0])
+        assert excluded.shape[0] == R
+        out = np.empty(R, dtype=PICK_DTYPE)
+        N.check(self._lib.lig_schedule_batch_excluding(self._ctx, epoch, seed, _ptr(reqs), R, _ptr(excluded),
+                                                       int(excluded.shape[1]), _ptr(out)))
+        return out
+
+    def schedule_batch_excluding_ptr(self, epoch: int, seed: int, h_reqs: int, R: int, h_excluded: int,
+                                     n_excluded: int, h_out: int) -> None:
+        N.check(self._lib.lig_schedule_batch_excluding(self._ctx, epoch, seed, h_reqs or None, R, h_excluded or None,
+                                                       n_excluded, h_out or None))
+
+    def schedule_batch_excluding_device(self, epoch: int, seed: int, d_reqs: int, R: int, d_excluded: int,
+                                        n_excluded: int, d_out: int, stream: int = 0) -> None:
+        """Device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_batch_excluding_device(self._ctx, epoch, seed, d_reqs or None, R,
+                                                              d_excluded or None, n_excluded, d_out or None,
+                                                              stream or None))
+
     def schedule_models_batch_fallbacks(self, epoch: int, seed: int, model_ids: np.ndarray, n: int,
                                         first_index: int = 0):
         """lig_schedule_models_batch_fallbacks: (picks, int16 fallbacks (R, n)), the picks those of

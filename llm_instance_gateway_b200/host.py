@@ -29,6 +29,7 @@ EXPORTED_SYMBOLS = (
     "ligh_schedule_model", "ligh_scheduler_new_tree", "ligh_scheduler_new_feedback", "ligh_feedback_stats",
     "ligh_scheduler_set_models", "ligh_schedule_model_device", "ligh_model_stats", "ligh_schedule_models_concurrent",
     "ligh_filter", "ligh_schedule_with_fallbacks", "ligh_fallback_scheduled", "ligh_schedule_model_with_fallbacks",
+    "ligh_schedule_retry", "ligh_retry_scheduled",
 )
 
 _lib = None
@@ -83,6 +84,10 @@ def load() -> C.CDLL:
     lib.ligh_schedule_model_with_fallbacks.argtypes = [vp, C.c_char_p, i32, C.c_char_p, i32, C.c_char_p, i32,
                                                        C.POINTER(i32), C.c_char_p, i32]
     lib.ligh_fallback_scheduled.argtypes = [vp]
+    lib.ligh_schedule_retry.argtypes = [vp, C.c_char_p, i32, cpp, cpp, i32, C.c_char_p, i32, C.c_char_p, i32,
+                                        C.c_char_p, i32]
+    lib.ligh_retry_scheduled.argtypes = [vp]
+    lib.ligh_retry_scheduled.restype = u64
     lib.ligh_fallback_scheduled.restype = u64
     lib.ligh_stats.argtypes = [vp, vp]
     lib.ligh_stats.restype = None
@@ -207,6 +212,19 @@ class HostScheduler:
         pods = names.value.decode().split("\n") if k.value else []
         return code, pods, err.value.decode("utf-8", "replace") if code != GRPC_OK else ""
 
+    def ScheduleRetry(self, resolved: str, critical: bool, tried: Sequence[Pod]
+                      ) -> Tuple[int, Optional[Pod], str]:  # noqa: N802
+        """Scheduler::ScheduleRetry: Schedule without the pods in `tried` (matched by value):
+        (gRPC code, pod, error)."""
+        name, addr = C.create_string_buffer(256), C.create_string_buffer(256)
+        err = C.create_string_buffer(512)
+        code = self._lib.ligh_schedule_retry(self._s, resolved.encode(), int(critical), _strs([p.Name for p in tried]),
+                                             _strs([p.Address for p in tried]), len(tried), name, 256, addr, 256,
+                                             err, 512)
+        if code == GRPC_OK:
+            return code, Pod(name.value.decode(), addr.value.decode()), ""
+        return code, None, err.value.decode("utf-8", "replace")
+
     def ScheduleModelWithFallbacks(self, model: str, n: int) -> Tuple[int, str, List[str], str]:  # noqa: N802
         """Scheduler::ScheduleModelWithFallbacks: (gRPC code, resolved target model, pod names [pick,
         fallbacks in retry order], error)."""
@@ -232,8 +250,10 @@ class HostScheduler:
         self._lib.ligh_model_stats(self._s, ms)
         return dict(zip(("scheduled", "batches", "max_batch", "refreshes", "stale_retries", "failed_refreshes",
                          "excluded_pods", "delta_refreshes", "last_dirty_pods", "feedback_windows",
-                         "feedback_restarts", "model_scheduled", "model_batches", "fallback_scheduled"),
-                        map(int, list(out) + list(fb) + list(ms) + [self._lib.ligh_fallback_scheduled(self._s)])))
+                         "feedback_restarts", "model_scheduled", "model_batches", "fallback_scheduled",
+                         "retry_scheduled"),
+                        map(int, list(out) + list(fb) + list(ms) + [self._lib.ligh_fallback_scheduled(self._s),
+                                                                    self._lib.ligh_retry_scheduled(self._s)])))
 
     def ScheduleModel(self, datastore: "HostDataStore", model: str):  # noqa: N802
         """resolve (FetchModelData + RandomWeightedDraw + IsCritical) + Schedule: (code, resolved, pod, err)."""

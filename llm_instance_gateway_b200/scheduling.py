@@ -19,8 +19,10 @@ every snapshot epoch carries.  ``FilterBatch`` / ``FilterModelBatch`` return the
 batch (Filter.Filter, filter.go:12-15) in one device call, for any filter tree.  ``ScheduleBatchWithFallbacks`` /
 ``ScheduleWithFallbacks`` / ``ScheduleModelBatchWithFallbacks`` return the pick followed by up to n more distinct
 survivors in retry order (include/lig.h, fallback endpoints); under load_feedback_window they need
-``feedback_fallbacks=True`` and then rank the feedback chain's own tables.  There is no CPU path here: without liblig.so or
-without a CUDA device construction fails.
+``feedback_fallbacks=True`` and then rank the feedback chain's own tables.  ``ScheduleRetry`` / ``ScheduleBatchRetry``
+schedule a request again without the pods it already tried, as Schedule would once those pods left the provider
+(lig_schedule_batch_excluding).  There is no CPU path here: without liblig.so or without a CUDA device construction
+fails.
 """
 from __future__ import annotations
 
@@ -421,6 +423,50 @@ class Scheduler:
                 err = _schedule_error(st)
                 out[i] = ([], resolved, StatusError(err.code, _POD_PREFIX + str(err)))
         return out
+
+    # ---- retry scheduling: Schedule again over the pool without the pods already tried ----
+    def ScheduleBatchRetry(self, reqs: Sequence[LLMRequest], tried_lists: Sequence[Sequence[Pod]]
+                           ) -> List[Tuple[Optional[Pod], Optional[StatusError]]]:
+        """ScheduleBatch with request i scheduled over the current snapshot's pods without the pods of
+        tried_lists[i] (lig_schedule_batch_excluding): what Schedule returns once those pods have left
+        the provider.  Tried pods are matched by value against the snapshot current when the call
+        runs; those no longer in it are ignored.  One rand_key per request from ScheduleBatch's
+        sequence; errors as ScheduleBatch.  ValueError for more than LIG_MAX_EXCLUDED tried pods and
+        under load_feedback_window (the picks come from the chain's load-adjusted copy of the
+        snapshot; a retry would not)."""
+        if self._window:
+            raise ValueError("retries are not defined under load_feedback_window: the picks come from the feedback "
+                             "chain's load-adjusted copy of the snapshot, a retry would not")
+        if len(tried_lists) != len(reqs):
+            raise ValueError(f"{len(reqs)} requests but {len(tried_lists)} tried lists")
+        for tried in tried_lists:
+            if len(tried) > N.LIG_MAX_EXCLUDED:
+                raise ValueError(f"{len(tried)} tried pods (at most {N.LIG_MAX_EXCLUDED})")
+        snap = self._current()
+        where: Dict[Pod, List[int]] = {}
+        for p, pod in enumerate(snap.pods):
+            where.setdefault(pod, []).append(p)
+        rows = [[p for pod in tried for p in where.get(pod, ())] for tried in tried_lists]
+        width = max([1] + [len(r) for r in rows])
+        if width > N.LIG_MAX_EXCLUDED:
+            raise ValueError(f"the tried pods match {width} pods of the snapshot (at most {N.LIG_MAX_EXCLUDED})")
+        excluded = np.full((len(reqs), width), -1, dtype=np.int16)
+        for i, r in enumerate(rows):
+            excluded[i, :len(r)] = r
+        arr = np.zeros(len(reqs), dtype=REQ_DTYPE)
+        for i, r in enumerate(reqs):
+            arr[i] = (snap.adapter_id(r.ResolvedTargetModel), N.LIG_REQ_CRITICAL if r.Critical else 0,
+                      self._rng.getrandbits(64))
+        picks = self._engine.schedule_batch_excluding(self._epoch, self._seed, arr, excluded)
+        return [(snap.pods[int(pk["pod_idx"])], None) if pk["status"] == N.LIG_OK
+                else (None, _schedule_error(int(pk["status"]))) for pk in picks]
+
+    def ScheduleRetry(self, req: LLMRequest, tried: Sequence[Pod]) -> Pod:
+        """Schedule over the pool without the pods in `tried`; raises like Schedule."""
+        pod, err = self.ScheduleBatchRetry([req], [tried])[0]
+        if err is not None:
+            raise err
+        return pod
 
     # Filter-level view (the GPU analogue of Filter.Filter, filter.go:12-15): survivor slice.
     def Filter(self, req: LLMRequest) -> Tuple[List[Pod], Optional[StatusError]]:
