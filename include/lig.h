@@ -514,7 +514,8 @@ int lig_schedule_models_batch_fallbacks_device(lig_ctx* ctx, uint64_t epoch, uin
  * order, pod_idx an index into the epoch's full pod order.  Statuses are those of the schedule
  * calls; an empty pool runs as Go does with an empty slice (under the built-in tree: LIG_DROP for
  * critical and sheddable requests alike).  A row that excludes nothing gives lig_schedule_batch's
- * result byte for byte.  The calls read the resident epoch, never a feedback chain's copy.
+ * result byte for byte.  The calls read the resident epoch, never a feedback chain's copy; under a
+ * chain, lig_schedule_batch_feedback_chain_excluding below walks the chain's copy.
  *
  * One warp per request walks the tree from its own pool (the direct scan's formulation).
  * LIG_ERR_INVALID, with nothing written, for n_excluded outside [1, LIG_MAX_EXCLUDED], null buffers
@@ -649,6 +650,38 @@ int lig_schedule_models_batch_feedback_chain_fallbacks_device(lig_ctx* ctx, uint
                                                               int R, lig_mpick* d_out, int n_fallbacks,
                                                               int16_t* d_fallbacks, int window, int32_t* d_loads,
                                                               void* stream);
+/* Retries under the chain.  A chain retry call is a descriptor chain call in every respect, plus a
+ * row of excluded pods per request in the format of lig_schedule_batch_excluding (int16, n_excluded
+ * in [1, LIG_MAX_EXCLUDED], entries outside [0, P), -1 included, exclude nothing):
+ *   1. Sequence and windows: the R requests join the chain's sequence and windows exactly as a plain
+ *      chain call's would; window boundaries ignore call boundaries, retry calls may alternate with
+ *      plain, model-id and fallback chain calls, and the restart rules are unchanged.
+ *   2. Request i gets what lig_schedule_batch_excluding would return for it on the chain's private
+ *      copy at its position in the sequence, with the call's seed and its rand_key, except that the
+ *      pool is the chain's (its WaitingQueueSize has grown by every window closed so far) and the
+ *      tree is the one the chain's windows are rebuilt with (the caller tree and thresholds in force
+ *      when the chain started, not the epoch's own tree and not the ctx's current thresholds).
+ *      pod_idx is in E's pod order; empty pools and statuses are the resident retry's.
+ *   3. Only a LIG_OK pick adds one to its pod in the open window; DROP, EMPTY and NO_PODS_LEFT count
+ *      toward the window's length.  `loads` as for the other chain calls.
+ *   So rows that exclude nothing give the plain chain call's `out` and `loads` byte for byte; while
+ *   no window has closed, and the chain's tree and thresholds are those E was built with, `out` is
+ *   lig_schedule_batch_excluding's on E byte for byte; and results do not depend on how the requests
+ *   are split into calls.  A retry segment reads no class table, so it never rebuilds the tables of
+ *   a closed window: the next table-reading segment does, once.
+ *   4. Refused, with nothing written and the chain exactly as it was, for every reason a chain call
+ *      is refused and every reason lig_schedule_batch_excluding is refused (n_excluded, null buffers
+ *      when R > 0, R > max_batch on the host form, device buffers not aligned to their element).
+ * Host form: page-locked, aligned buffers are used in place; pageable or misaligned requests and
+ * picks bounce as for the plain chain call, and such rows are staged in stream-ordered device memory;
+ * it blocks.  Device form: device pointers, enqueued on `stream`, not synchronised. */
+int lig_schedule_batch_feedback_chain_excluding(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* reqs,
+                                                int R, const int16_t* excluded, int n_excluded, lig_pick* out,
+                                                int window, int32_t* loads);
+int lig_schedule_batch_feedback_chain_excluding_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed,
+                                                       const lig_req* d_reqs, int R, const int16_t* d_excluded,
+                                                       int n_excluded, lig_pick* d_out, int window,
+                                                       int32_t* d_loads, void* stream);
 /* The next chain call starts a new chain. */
 int lig_feedback_chain_reset(lig_ctx* ctx);
 

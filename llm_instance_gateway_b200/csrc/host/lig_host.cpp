@@ -411,7 +411,7 @@ Status Scheduler::ScheduleRetry(const LLMRequest& req, const std::vector<backend
   if (tried.size() > (size_t)LIG_MAX_EXCLUDED)
     return Errorf(InvalidArgument, "ScheduleRetry: " + std::to_string(tried.size()) + " tried pods (at most " +
                                        std::to_string(LIG_MAX_EXCLUDED) + ")");
-  if (opt_.load_feedback_window > 0)
+  if (opt_.load_feedback_window > 0 && !opt_.feedback_retries)
     return Errorf(InvalidArgument, "ScheduleRetry: not defined under load_feedback_window (the picks come from the "
                                    "feedback chain's copy of the snapshot, a retry would not)");
   if (group_)
@@ -672,9 +672,11 @@ void Scheduler::Flush(std::vector<Waiter*>& all) {
   stats_.max_flush_us = std::max(stats_.max_flush_us, flush_us);
 }
 
-// The retry lane: one lig_schedule_batch_excluding call per max_batch waiters.  Each waiter's tried
-// pods are matched by value against the captured snapshot; its row holds their indices, -1 padded to
-// the widest row of the call.
+// The retry lane: one lig_schedule_batch_excluding call per max_batch waiters (under
+// load_feedback_window, lig_schedule_batch_feedback_chain_excluding).  Each waiter's tried pods are
+// matched by value against the captured snapshot; its row holds their indices, -1 padded to the
+// widest row of the call.  Every waiter takes a rand_key; under the chain a waiter refused on the
+// host is left out of the call, since its pick would load a pod and shift every later window.
 void Scheduler::FlushRetries(std::vector<Waiter*>& batch) {
   if (batch.empty()) return;
   Status failure;
@@ -683,11 +685,13 @@ void Scheduler::FlushRetries(std::vector<Waiter*>& batch) {
     if (!h_excluded_) failure = LigFailure("lig_host_alloc");
   }
   std::vector<std::vector<int16_t>> rows;
+  std::vector<int> slot;   // waiter i's request in the call, -1 when left out
+  const int W = opt_.load_feedback_window;
   size_t done = 0;
   while (done < batch.size()) {
     const int n = (int)std::min(batch.size() - done, (size_t)opt_.max_batch);
     std::shared_ptr<const Snapshot> snap;
-    int rc = 0, width = 1;
+    int rc = 0, width = 1, k = 0;
     for (int attempt = 0; failure.ok() && attempt < 4; ++attempt) {
       {
         std::lock_guard<std::mutex> lk(snap_mu_);
@@ -707,31 +711,46 @@ void Scheduler::FlushRetries(std::vector<Waiter*>& batch) {
         // only pods listed more than once in the slice get past 32: that caller is refused below
         if ((int)row.size() <= LIG_MAX_EXCLUDED) width = std::max(width, (int)row.size());
       }
+      slot.assign((size_t)n, -1);
+      k = 0;
       for (int i = 0; i < n; ++i) {
         const LLMRequest& r = *batch[done + i]->req;
-        auto it = snap->adapter_ids->find(r.ResolvedTargetModel);   // interned as in Flush
-        h_reqs_[i].adapter_id = (it == snap->adapter_ids->end() || it->second >= snap->A) ? snap->A : it->second;
-        h_reqs_[i].flags = r.Critical ? LIG_REQ_CRITICAL : 0u;
-        h_reqs_[i].rand_key = splitmix_next(rng_state_);
-        int16_t* row = h_excluded_ + (size_t)i * (size_t)width;
+        const uint64_t key = splitmix_next(rng_state_);
         const std::vector<int16_t>& ex = rows[(size_t)i];
-        const int k = (int)ex.size() <= width ? (int)ex.size() : 0;
-        for (int j = 0; j < width; ++j) row[j] = j < k ? ex[(size_t)j] : (int16_t)-1;
+        if (W > 0 && ex.size() > (size_t)LIG_MAX_EXCLUDED) continue;
+        slot[(size_t)i] = k;
+        auto it = snap->adapter_ids->find(r.ResolvedTargetModel);   // interned as in Flush
+        h_reqs_[k].adapter_id = (it == snap->adapter_ids->end() || it->second >= snap->A) ? snap->A : it->second;
+        h_reqs_[k].flags = r.Critical ? LIG_REQ_CRITICAL : 0u;
+        h_reqs_[k].rand_key = key;
+        int16_t* row = h_excluded_ + (size_t)k * (size_t)width;
+        const int m = (int)ex.size() <= width ? (int)ex.size() : 0;
+        for (int j = 0; j < width; ++j) row[j] = j < m ? ex[(size_t)j] : (int16_t)-1;
+        ++k;
       }
-      rc = lig_schedule_batch_excluding(ctx_, snap->epoch, seed_, h_reqs_, n, h_excluded_, width, h_picks_);
+      if (W > 0) {
+        rc = k > 0 ? lig_schedule_batch_feedback_chain_excluding(ctx_, snap->epoch, seed_, h_reqs_, k, h_excluded_,
+                                                                 width, h_picks_, W, nullptr)
+                   : 0;
+        if (rc == 0) CountFeedback(snap->epoch, k);
+      } else {
+        rc = lig_schedule_batch_excluding(ctx_, snap->epoch, seed_, h_reqs_, n, h_excluded_, width, h_picks_);
+      }
       if (rc != LIG_ERR_STALE_EPOCH) break;   // two refreshes raced past this batch: re-resolve
       std::lock_guard<std::mutex> sk(stats_mu_);
       stats_.stale_retries++;
     }
-    if (failure.ok() && rc != 0) failure = LigFailure("lig_schedule_batch_excluding");
+    if (failure.ok() && rc != 0)
+      failure = LigFailure(W > 0 ? "lig_schedule_batch_feedback_chain_excluding" : "lig_schedule_batch_excluding");
     for (int i = 0; i < n; ++i) {
       Waiter* w = batch[done + i];
+      const lig_pick* pk = failure.ok() && slot[(size_t)i] >= 0 ? &h_picks_[slot[(size_t)i]] : nullptr;
       if (!failure.ok()) w->status = failure;
       else if (rows[(size_t)i].size() > (size_t)LIG_MAX_EXCLUDED)
         w->status = Errorf(InvalidArgument, "ScheduleRetry: the tried pods match more than " +
                                                 std::to_string(LIG_MAX_EXCLUDED) + " pods of the snapshot");
-      else if (h_picks_[i].status == LIG_OK) w->pod = snap->pods[(size_t)h_picks_[i].pod_idx];
-      else w->status = PickError(h_picks_[i].status);
+      else if (pk->status == LIG_OK) w->pod = snap->pods[(size_t)pk->pod_idx];
+      else w->status = PickError(pk->status);
     }
     {
       std::lock_guard<std::mutex> sk(stats_mu_);

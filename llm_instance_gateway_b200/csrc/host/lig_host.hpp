@@ -163,6 +163,12 @@ struct Options {
   // always been refused under feedback with InvalidArgument and that refusal is relied upon; without
   // it they still are.  No effect without load_feedback_window.
   bool feedback_fallbacks = false;
+  // With load_feedback_window > 0: let ScheduleRetry run as feedback-chain calls
+  // (lig_schedule_batch_feedback_chain_excluding): a retry is scheduled on the chain's load-adjusted
+  // copy without the pods it tried, and its pick counts toward the chain's windows like any other.
+  // Off by default because ScheduleRetry has always been refused under feedback with InvalidArgument;
+  // without it, it still is.  No effect without load_feedback_window.
+  bool feedback_retries = false;
 };
 
 struct Stats {
@@ -223,8 +229,9 @@ class Scheduler {
   // ignored.  Goes through the micro-batcher and takes the next rand_key from the same sequence as
   // Schedule, in flush order; a flush's retries make one device call after its plain descriptor
   // requests, never through the doorbell.  Errors are Schedule's.  InvalidArgument with more than
-  // LIG_MAX_EXCLUDED (32) tried pods, with load_feedback_window > 0 (the picks come from the feedback
-  // chain's copy of the snapshot, a retry would not) and with several devices.  A handler that used
+  // LIG_MAX_EXCLUDED (32) tried pods, with load_feedback_window > 0 unless Options::feedback_retries
+  // (then the flush's retries make one lig_schedule_batch_feedback_chain_excluding call instead, and a
+  // waiter refused on the host is left out of it, so it loads no pod) and with several devices.  A handler that used
   // ScheduleModel builds req from the resolved target model it got back and the model's criticality.
   Status ScheduleRetry(const LLMRequest& req, const std::vector<backend::Pod>& tried, backend::Pod* targetPod);
 

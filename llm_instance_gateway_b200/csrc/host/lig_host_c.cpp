@@ -221,7 +221,7 @@ ligh_scheduler* ligh_scheduler_new_tree(ligh_provider* p, int device, const int*
                                         int n_nodes, char* err, int err_cap) {
   return ligh_scheduler_new_feedback(p, device, devices, n_devices, max_pods, max_adapters, max_batch, flush_size,
                                      window_us, refresh_ms, seed, busy_poll, caller_spin_us, use_doorbell, nodes,
-                                     n_nodes, 0, 0, err, err_cap);
+                                     n_nodes, 0, 0, 0, err, err_cap);
 }
 
 ligh_scheduler* ligh_scheduler_new_feedback(ligh_provider* p, int device, const int* devices, int n_devices,
@@ -229,10 +229,11 @@ ligh_scheduler* ligh_scheduler_new_feedback(ligh_provider* p, int device, const 
                                             int window_us, int refresh_ms, uint64_t seed, int busy_poll,
                                             int caller_spin_us, int use_doorbell, const lig_filter_node* nodes,
                                             int n_nodes, int load_feedback_window, int feedback_fallbacks,
-                                            char* err, int err_cap) {
+                                            int feedback_retries, char* err, int err_cap) {
   scheduling::Options o;
   o.load_feedback_window = load_feedback_window;
   o.feedback_fallbacks = feedback_fallbacks != 0;
+  o.feedback_retries = feedback_retries != 0;
   o.device = device;
   if (devices && n_devices > 1) o.devices.assign(devices, devices + n_devices);
   o.busy_poll = busy_poll != 0;

@@ -39,13 +39,14 @@ ligh_scheduler* ligh_scheduler_new_tree(ligh_provider*, int device, const int* d
                                         const lig_filter_node* nodes, int n_nodes, char* err, int err_cap);
 /* ligh_scheduler_new_tree plus Options::load_feedback_window (0 = off; > 0 flushes through
  * lig_schedule_batch_feedback_chain; refused with several devices or use_doorbell) and
- * Options::feedback_fallbacks (nonzero: the *WithFallbacks calls run under the chain). */
+ * Options::feedback_fallbacks (nonzero: the *WithFallbacks calls run under the chain) and
+ * Options::feedback_retries (nonzero: ScheduleRetry runs under the chain). */
 ligh_scheduler* ligh_scheduler_new_feedback(ligh_provider*, int device, const int* devices, int n_devices,
                                             int max_pods, int max_adapters, int max_batch, int flush_size,
                                             int batch_window_us, int refresh_interval_ms, uint64_t seed,
                                             int busy_poll, int caller_spin_us, int use_doorbell,
                                             const lig_filter_node* nodes, int n_nodes, int load_feedback_window,
-                                            int feedback_fallbacks, char* err, int err_cap);
+                                            int feedback_fallbacks, int feedback_retries, char* err, int err_cap);
 void ligh_scheduler_free(ligh_scheduler*);
 /* Scheduler.Schedule: returns the gRPC code (0 OK, 8 ResourceExhausted, 2 Unknown, 13 Internal). */
 int ligh_schedule(ligh_scheduler*, const char* model, const char* resolved_target_model, int critical,

@@ -600,21 +600,35 @@ int launch_models(lig_ctx* c, const Slot& s, uint64_t seed, uint64_t first_index
   return 0;
 }
 
+// The launch shape of the per-request walks (the direct scan and the retry walk) over R >= 1
+// requests of slot s: one warp per request, the pod columns staged in shared memory when they fit.
+struct ScanShape {
+  bool staged;
+  size_t smem;
+  int grid;
+};
+
+static ScanShape scan_shape(const lig_ctx* c, const Slot& s, int R) {
+  ScanShape sh;
+  sh.staged = s.P > 0 && staged_fits(c, s.W);
+  sh.smem = scratch_bytes(s.W > 0 ? s.W : 1) + (sh.staged ? staged_bytes(s.W) : 0);
+  const int ctas_per_sm = sh.staged ? (sh.smem > 110 * 1024 ? 1 : 2) : 4;
+  const int ctas_needed = (R + kWarpsPerCta - 1) / kWarpsPerCta;
+  sh.grid = ctas_needed < c->sm_count * ctas_per_sm ? ctas_needed : c->sm_count * ctas_per_sm;
+  return sh;
+}
+
 int launch_scan(lig_ctx* c, const Slot& s, uint64_t seed, const lig_req* d_reqs, int R,
                 lig_pick* d_out, uint32_t* d_masks, cudaStream_t stream) {
   if (R == 0) return 0;
   const SnapView v = view_of(s);
-  const bool staged = s.P > 0 && staged_fits(c, s.W);
-  const size_t smem = scratch_bytes(s.W > 0 ? s.W : 1) + (staged ? staged_bytes(s.W) : 0);
-  const int ctas_per_sm = staged ? (smem > 110 * 1024 ? 1 : 2) : 4;
-  const int ctas_needed = (R + kWarpsPerCta - 1) / kWarpsPerCta;
-  int grid = ctas_needed < c->sm_count * ctas_per_sm ? ctas_needed : c->sm_count * ctas_per_sm;
-  if (staged) {
-    lig_scan_kernel<true><<<grid, kCtaThreads, smem, stream>>>(
+  const ScanShape sh = scan_shape(c, s, R);
+  if (sh.staged) {
+    lig_scan_kernel<true><<<sh.grid, kCtaThreads, sh.smem, stream>>>(
         v, thr_of(c), reinterpret_cast<const int4*>(d_reqs), reinterpret_cast<int2*>(d_out), R,
         d_masks, seed);
   } else {
-    lig_scan_kernel<false><<<grid, kCtaThreads, smem, stream>>>(
+    lig_scan_kernel<false><<<sh.grid, kCtaThreads, sh.smem, stream>>>(
         v, thr_of(c), reinterpret_cast<const int4*>(d_reqs), reinterpret_cast<int2*>(d_out), R,
         d_masks, seed);
   }
@@ -1026,6 +1040,10 @@ static int create_impl(lig_ctx* c, int device, int max_pods, int max_adapters, i
   CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_count_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_count_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_count_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_count_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   const size_t need = scratch_bytes(words_for(max_pods)) > build_fixed_bytes(words_for(max_pods))
                           ? scratch_bytes(words_for(max_pods)) : build_fixed_bytes(words_for(max_pods));
   if (need > c->smem_optin)
@@ -2188,37 +2206,43 @@ static int excluding_check(const lig_ctx* c, const char* fn, const ExcludingCall
   return 0;
 }
 
-// Enqueue the retry kernel for x (R >= 1, device-visible, aligned pointers) against slot s on st,
-// behind the slot's tables, and register st as a reader of the slot.  The scan's launch shape; the
-// walk is the tree that built the slot's tables.  Caller holds c->mu.
-static int enqueue_excluding(lig_ctx* c, Slot& s, const ExcludingCall& x, cudaStream_t st) {
+// Launch the retry walk for x (R >= 1, device-visible, aligned pointers) over slot s on st, with the
+// scan's launch shape: `tree` (null = the built-in tree with `thr`); `hist` non-null counts each
+// LIG_OK pick into it (the feedback chain's segment).  The caller checks the launch.
+static void launch_excluding(const lig_ctx* c, const Slot& s, const Thr& thr, const FilterTree* tree,
+                             const ExcludingCall& x, int* hist, cudaStream_t st) {
   static const FilterTree kNoTree{};
-  CUDA_TRY(cudaStreamWaitEvent(st, s.ready, 0));
+  const ScanShape sh = scan_shape(c, s, x.R);
   const SnapView v = view_of(s);
-  const bool staged = s.P > 0 && staged_fits(c, s.W);
-  const size_t smem = scratch_bytes(s.W > 0 ? s.W : 1) + (staged ? staged_bytes(s.W) : 0);
-  const int ctas_per_sm = staged ? (smem > 110 * 1024 ? 1 : 2) : 4;
-  const int ctas_needed = (x.R + kWarpsPerCta - 1) / kWarpsPerCta;
-  const int grid = ctas_needed < c->sm_count * ctas_per_sm ? ctas_needed : c->sm_count * ctas_per_sm;
-  const FilterTree& tree = s.caller_tree ? s.tree : kNoTree;
+  const FilterTree& t = tree ? *tree : kNoTree;
   const int4* in = reinterpret_cast<const int4*>(x.reqs);
   int2* out = reinterpret_cast<int2*>(x.out);
-  const Thr thr = thr_of(c);
-  if (s.caller_tree) {
-    if (staged)
-      lig_schedule_excluding_kernel<true, true><<<grid, kCtaThreads, smem, st>>>(
-          v, thr, tree, in, x.excluded, x.n_excluded, out, x.R, x.seed);
+  auto launch = [&](auto staged, auto caller_tree) {
+    constexpr bool kS = decltype(staged)::value, kT = decltype(caller_tree)::value;
+    if (hist)
+      lig_schedule_excluding_count_kernel<kS, kT><<<sh.grid, kCtaThreads, sh.smem, st>>>(
+          v, thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, hist);
     else
-      lig_schedule_excluding_kernel<false, true><<<grid, kCtaThreads, smem, st>>>(
-          v, thr, tree, in, x.excluded, x.n_excluded, out, x.R, x.seed);
+      lig_schedule_excluding_kernel<kS, kT><<<sh.grid, kCtaThreads, sh.smem, st>>>(
+          v, thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed);
+  };
+  using Y = std::true_type;
+  using N = std::false_type;
+  if (tree) {
+    if (sh.staged) launch(Y{}, Y{});
+    else launch(N{}, Y{});
   } else {
-    if (staged)
-      lig_schedule_excluding_kernel<true, false><<<grid, kCtaThreads, smem, st>>>(
-          v, thr, tree, in, x.excluded, x.n_excluded, out, x.R, x.seed);
-    else
-      lig_schedule_excluding_kernel<false, false><<<grid, kCtaThreads, smem, st>>>(
-          v, thr, tree, in, x.excluded, x.n_excluded, out, x.R, x.seed);
+    if (sh.staged) launch(Y{}, N{});
+    else launch(N{}, N{});
   }
+}
+
+// Enqueue the retry kernel for x (R >= 1, device-visible, aligned pointers) against slot s on st,
+// behind the slot's tables, and register st as a reader of the slot.  The walk is the tree that
+// built the slot's tables.  Caller holds c->mu.
+static int enqueue_excluding(lig_ctx* c, Slot& s, const ExcludingCall& x, cudaStream_t st) {
+  CUDA_TRY(cudaStreamWaitEvent(st, s.ready, 0));
+  launch_excluding(c, s, thr_of(c), s.caller_tree ? &s.tree : nullptr, x, nullptr, st);
   CUDA_TRY(cudaGetLastError());
   c->launches++;
   return note_reader(s, st);
@@ -2401,6 +2425,9 @@ struct FbReqs {
   bool rows = false;                     // a chain fallback call: request i's row is at
   int16_t* fallbacks = nullptr;          //   fallbacks + i * n_fallbacks
   int n_fallbacks = 0;
+  bool retry = false;                    // a chain retry call: request i excludes the pods of
+  const int16_t* excluded = nullptr;     //   excluded + i * n_excluded
+  int n_excluded = 0;
   size_t in_bytes() const { return models ? sizeof(uint32_t) : sizeof(lig_req); }
   size_t out_bytes() const { return models ? sizeof(lig_mpick) : sizeof(lig_pick); }
 };
@@ -2408,12 +2435,13 @@ struct FbReqs {
 // Schedule R requests through the window sequence: each segment is the rest of the open window or
 // of the call, whichever is shorter; one fused pick + count launch per segment (pick + row + count
 // when the call asked for rows); a filled window is closed at once, its tables are rebuilt only
-// when the next segment needs them.
+// when the next segment needs them.  A retry segment walks the tree over the scratch's pod columns
+// and reads no class table: it leaves them stale, so a later table-reading segment rebuilds once.
 static int fb_schedule(lig_ctx* c, FbRun& run, uint64_t seed, const FbReqs& rq, int R, cudaStream_t st) {
   Slot& fs = c->fb_scratch;
   for (int pos = 0; pos < R;) {
     const int n = (R - pos) < (run.window - run.filled) ? (R - pos) : (run.window - run.filled);
-    {
+    if (!rq.retry) {
       std::lock_guard<std::mutex> lk(c->mu);                 // launch counters, build debug stamps
       if (run.stale) {
         if (int rc = launch_class_build(c, fs, st, run.tree, &run.thr)) return rc;
@@ -2426,7 +2454,11 @@ static int fb_schedule(lig_ctx* c, FbRun& run, uint64_t seed, const FbReqs& rq, 
     void* out = static_cast<unsigned char*>(rq.out) + (size_t)pos * rq.out_bytes();
     const int grid = (n + kPickThreads * kCountPerThread - 1) / (kPickThreads * kCountPerThread);
     const uint4* fcls = reinterpret_cast<const uint4*>(fs.d_cls);
-    if (rq.rows) {
+    if (rq.retry) {
+      const ExcludingCall x{seed, static_cast<const lig_req*>(in), n, static_cast<lig_pick*>(out), rq.n_excluded,
+                            rq.excluded + (size_t)pos * (size_t)rq.n_excluded};
+      launch_excluding(c, fs, run.thr, run.tree, x, c->d_fb_hist, st);
+    } else if (rq.rows) {
       int16_t* rows = rq.fallbacks + (size_t)pos * (size_t)rq.n_fallbacks;
       const int blocks = (n + kFallbackThreads - 1) / kFallbackThreads;
       if (rq.models)
@@ -2600,8 +2632,13 @@ static int chain_admit(lig_ctx* c, const char* fn) {
   return fb_alloc_scratch(c);
 }
 
-// The row arguments of a chain fallback call; 0 for a plain chain call.
+// The row arguments of a chain fallback or retry call; 0 for a plain chain call.
 static int chain_rows_check(const char* fn, const FbReqs& rq, int R) {
+  if (rq.retry) {
+    if (rq.n_excluded < 1 || rq.n_excluded > LIG_MAX_EXCLUDED)
+      return fail(LIG_ERR_INVALID, "%s: n_excluded=%d outside [1, %d]", fn, rq.n_excluded, LIG_MAX_EXCLUDED);
+    if (R > 0 && !rq.excluded) return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
+  }
   if (!rq.rows) return 0;
   if (rq.n_fallbacks < 1 || rq.n_fallbacks > LIG_MAX_FALLBACKS)
     return fail(LIG_ERR_INVALID, "%s: n_fallbacks=%d outside [1, %d]", fn, rq.n_fallbacks, LIG_MAX_FALLBACKS);
@@ -2609,13 +2646,16 @@ static int chain_rows_check(const char* fn, const FbReqs& rq, int R) {
   return 0;
 }
 
-// The device form of both chain calls.
+// The device form of every chain call.
 static int chain_device(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t seed, const FbReqs& rq, int R,
                         int window, int32_t* d_loads, void* stream) {
   if (!c || R < 0 || window < 1 || (R > 0 && (!rq.in || !rq.out))) return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
   if (int rc = chain_rows_check(fn, rq, R)) return rc;
   if (R > 0 && rq.rows && misaligned(rq.fallbacks, sizeof(int16_t)))
     return fail(LIG_ERR_INVALID, "%s: the row buffer is not 2-byte aligned", fn);
+  if (R > 0 && rq.retry && (misaligned(rq.in, sizeof(lig_req)) || misaligned(rq.out, sizeof(lig_pick)) ||
+                            misaligned(rq.excluded, sizeof(int16_t))))
+    return fail(LIG_ERR_INVALID, "%s: a device buffer is not aligned to its element", fn);
   std::lock_guard<std::mutex> fk(c->fb_mu);
   CUDA_TRY(cudaSetDevice(c->device));
   if (int rc = chain_admit(c, fn)) return rc;
@@ -2635,7 +2675,8 @@ static int chain_host(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t seed,
   void* out = rq.out;
   rq.in = R ? mapped_device_pointer(in) : nullptr;
   rq.out = R ? mapped_device_pointer(out) : nullptr;
-  const bool bounce = R > 0 && !(rq.in && rq.out && !(reinterpret_cast<uintptr_t>(rq.in) & (rq.in_bytes() - 1)));
+  const bool bounce = R > 0 && !(rq.in && rq.out && !(reinterpret_cast<uintptr_t>(rq.in) & (rq.in_bytes() - 1)) &&
+                                 !(rq.retry && misaligned(rq.out, sizeof(lig_pick))));
   std::unique_lock<std::mutex> bk(c->bounce_mu, std::defer_lock);
   if (bounce) {
     bk.lock();
@@ -2669,7 +2710,25 @@ static int chain_host(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t seed,
   const bool loads_bounce = loads && !dev_loads;
   if (loads_bounce && !(dev_loads = mapped_device_pointer(c->h_fb_loads)))
     return fail(LIG_ERR_CUDA, "pinned staging buffers are not device-mapped on this platform");
-  if (int rc = chain_call(c, epoch, seed, rq, R, window, dev_loads, c->s_fb)) return rc;
+  // retry rows: page-locked, 2-byte aligned ones are read in place, the others staged in
+  // stream-ordered HBM (as lig_schedule_batch_excluding does)
+  int16_t* stage = nullptr;
+  if (R > 0 && rq.retry) {
+    const int16_t* rows = rq.excluded;
+    rq.excluded = mapped_device_pointer(rows);
+    if (!rq.excluded || misaligned(rq.excluded, sizeof(int16_t))) {
+      const size_t rows_b = (size_t)R * (size_t)rq.n_excluded * sizeof(int16_t);
+      CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&stage), rows_b, c->s_fb));
+      if (cudaMemcpyAsync(stage, rows, rows_b, cudaMemcpyHostToDevice, c->s_fb) != cudaSuccess) {
+        cudaFreeAsync(stage, c->s_fb);
+        return fail(LIG_ERR_CUDA, "%s: staging the rows failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
+      }
+      rq.excluded = stage;
+    }
+  }
+  const int rc = chain_call(c, epoch, seed, rq, R, window, dev_loads, c->s_fb);
+  if (stage) cudaFreeAsync(stage, c->s_fb);
+  if (rc) return rc;
   const cudaError_t e = cudaStreamSynchronize(c->s_fb);
   if (e != cudaSuccess) {
     c->chain_live = false;
@@ -2763,6 +2822,29 @@ int lig_schedule_models_batch_feedback_chain_fallbacks_device(lig_ctx* c, uint64
   return chain_device(c, "lig_schedule_models_batch_feedback_chain_fallbacks_device", epoch, seed,
                       with_rows(model_reqs(d_ids, d_out, first_index), n_fallbacks, d_fallbacks), R, window,
                       d_loads, stream);
+}
+
+static FbReqs with_excluded(FbReqs rq, const int16_t* excluded, int n_excluded) {
+  rq.retry = true;
+  rq.excluded = excluded;
+  rq.n_excluded = n_excluded;
+  return rq;
+}
+
+int lig_schedule_batch_feedback_chain_excluding(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* reqs,
+                                                int R, const int16_t* excluded, int n_excluded, lig_pick* out,
+                                                int window, int32_t* loads) {
+  return chain_host(c, "lig_schedule_batch_feedback_chain_excluding", epoch, seed,
+                    with_excluded(descriptor_reqs(reqs, out), excluded, n_excluded), R, window, loads);
+}
+
+int lig_schedule_batch_feedback_chain_excluding_device(lig_ctx* c, uint64_t epoch, uint64_t seed,
+                                                       const lig_req* d_reqs, int R, const int16_t* d_excluded,
+                                                       int n_excluded, lig_pick* d_out, int window,
+                                                       int32_t* d_loads, void* stream) {
+  return chain_device(c, "lig_schedule_batch_feedback_chain_excluding_device", epoch, seed,
+                      with_excluded(descriptor_reqs(d_reqs, d_out), d_excluded, n_excluded), R, window, d_loads,
+                      stream);
 }
 
 int lig_feedback_chain_reset(lig_ctx* c) {

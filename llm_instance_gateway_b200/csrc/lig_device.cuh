@@ -2909,4 +2909,65 @@ lig_schedule_excluding_kernel(SnapView s, Thr thr, const __grid_constant__ Filte
   }
 }
 
+// The chain segment of lig_schedule_batch_feedback_chain_excluding: lig_schedule_excluding_kernel's
+// walk, step for step, on the chain's private copy (its q column has grown by every closed window)
+// with the tree and thresholds the chain started with, plus the count: lane 0 adds each LIG_OK pick
+// to the open window's histogram, one atomic per request (one warp per request: no cross-lane match
+// as in count_window_picks).  A separate body, not a shared __forceinline__ one or a template flag
+// on the resident kernel: both of those change ptxas's register allocation of the resident
+// caller-tree forms (a 16-byte stack frame appears in the staged one).
+template <bool kStaged, bool kTree>
+__global__ void __launch_bounds__(kCtaThreads)
+lig_schedule_excluding_count_kernel(SnapView s, Thr thr, const __grid_constant__ FilterTree tree, const int4* reqs,
+                                    const int16_t* excluded, int n_excluded, int2* out, int R, uint64_t seed,
+                                    int* __restrict__ hist) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint32_t* X = reinterpret_cast<uint32_t*>(smem) + (size_t)warp * 3 * s.W;
+  uint32_t* T = X + s.W;
+  uint32_t* H = T + s.W;
+  Fields f{s.kv, s.q, s.n_active, s.max_active};
+  if constexpr (kStaged) {
+    f = stage_fields(s, smem + scratch_bytes(s.W));
+    __syncthreads();
+  }
+  for (int i = blockIdx.x * kWarpsPerCta + warp; i < R; i += gridDim.x * kWarpsPerCta) {
+    const int4 r = reqs[i];
+    const int ex = lane < n_excluded ? excluded[(size_t)i * n_excluded + lane] : -1;
+    const bool critical = ((uint32_t)r.y & LIG_REQ_CRITICAL) != 0;
+    const uint64_t key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
+    const uint32_t* Hrow = stage_adapter_row(s, r.x, H, lane);
+    for (int w = lane; w < s.W; w += 32) {
+      const int rem = s.P - w * 32;
+      T[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
+    }
+    __syncwarp();
+    if (ex >= 0 && ex < s.P) atomicAnd(T + (ex >> 5), ~(1u << (ex & 31)));
+    __syncwarp();
+    uint32_t n = 0;
+    for (int w = lane; w < s.W; w += 32) n += __popc(T[w]);
+    n = __reduce_add_sync(kFull, n);
+    EvalResult e;
+    if constexpr (kTree)
+      e = tree_walk_warp<kStaged, true>(f, tree.nodes, Hrow, critical, s.P, s.W, T, X, lane, n);
+    else
+      e = tree_eval_warp<kStaged, true>(f, Hrow, critical, thr, s.P, s.W, X, T, lane, n);
+    int pod = -1;
+    if (e.n > 0) {
+      uint32_t k = int31n(seed ^ key, e.n, max_accept_for(e.n));
+      for (int w = 0; w < s.W; ++w) {
+        uint32_t word = e.mask[w];
+        uint32_t c = __popc(word);
+        if (k < c) { pod = w * 32 + (int)__fns(word, 0, (int)k + 1); break; }
+        k -= c;
+      }
+    }
+    if (lane == 0) {
+      out[i] = make_int2(pod, (int)(e.status | (e.n << 16)));
+      if (pod >= 0) atomicAdd(hist + pod, 1);   // pod >= 0 only for LIG_OK
+    }
+    __syncwarp();
+  }
+}
+
 }  // namespace lig

@@ -321,6 +321,39 @@ class Engine:
                                                               d_excluded or None, n_excluded, d_out or None,
                                                               stream or None))
 
+    # ---- retries under the feedback chain: a chain call whose requests exclude the pods they tried ----
+    def schedule_batch_feedback_chain_excluding(self, epoch: int, seed: int, reqs: np.ndarray, excluded: np.ndarray,
+                                                window: int, loads: Optional[np.ndarray] = None) -> np.ndarray:
+        """lig_schedule_batch_feedback_chain_excluding: request i is scheduled as schedule_batch_excluding
+        would on the chain's load-adjusted copy at its position in the chain's sequence, and its pick
+        counts toward the open window.  `loads` as schedule_batch_feedback_chain's."""
+        assert reqs.dtype == REQ_DTYPE and reqs.flags.c_contiguous
+        assert excluded.dtype == np.int16 and excluded.flags.c_contiguous and excluded.ndim == 2
+        R = int(reqs.shape[0])
+        assert excluded.shape[0] == R
+        out = np.empty(R, dtype=PICK_DTYPE)
+        if loads is not None:
+            assert loads.dtype == np.int32 and loads.flags.c_contiguous
+        N.check(self._lib.lig_schedule_batch_feedback_chain_excluding(
+            self._ctx, epoch, seed, _ptr(reqs), R, _ptr(excluded), int(excluded.shape[1]), _ptr(out), window,
+            _ptr(loads) if loads is not None else None))
+        return out
+
+    def schedule_batch_feedback_chain_excluding_ptr(self, epoch: int, seed: int, h_reqs: int, R: int, h_excluded: int,
+                                                    n_excluded: int, h_out: int, window: int,
+                                                    h_loads: int = 0) -> None:
+        N.check(self._lib.lig_schedule_batch_feedback_chain_excluding(self._ctx, epoch, seed, h_reqs or None, R,
+                                                                      h_excluded or None, n_excluded, h_out or None,
+                                                                      window, h_loads or None))
+
+    def schedule_batch_feedback_chain_excluding_device(self, epoch: int, seed: int, d_reqs: int, R: int,
+                                                       d_excluded: int, n_excluded: int, d_out: int, window: int,
+                                                       d_loads: int = 0, stream: int = 0) -> None:
+        """Device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_batch_feedback_chain_excluding_device(
+            self._ctx, epoch, seed, d_reqs or None, R, d_excluded or None, n_excluded, d_out or None, window,
+            d_loads or None, stream or None))
+
     def schedule_models_batch_fallbacks(self, epoch: int, seed: int, model_ids: np.ndarray, n: int,
                                         first_index: int = 0):
         """lig_schedule_models_batch_fallbacks: (picks, int16 fallbacks (R, n)), the picks those of

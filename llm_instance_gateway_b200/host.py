@@ -58,7 +58,7 @@ def load() -> C.CDLL:
                                             i32, vp, i32, C.c_char_p, i32]
     lib.ligh_scheduler_new_tree.restype = vp
     lib.ligh_scheduler_new_feedback.argtypes = [vp, i32, C.POINTER(i32), i32, i32, i32, i32, i32, i32, i32, u64, i32,
-                                                i32, i32, vp, i32, i32, i32, C.c_char_p, i32]
+                                                i32, i32, vp, i32, i32, i32, i32, C.c_char_p, i32]
     lib.ligh_scheduler_new_feedback.restype = vp
     lib.ligh_feedback_stats.argtypes = [vp, vp]
     lib.ligh_feedback_stats.restype = None
@@ -152,14 +152,15 @@ class HostScheduler:
                  batch_window_us: int = 50, refresh_interval_ms: int = 0, seed: int = 1,
                  busy_poll: bool = False, caller_spin_us: int = 0, use_doorbell: bool = False,
                  devices: Optional[Sequence[int]] = None, filter=None, load_feedback_window: int = 0,
-                 feedback_fallbacks: bool = False):
+                 feedback_fallbacks: bool = False, feedback_retries: bool = False):
         self._lib = load()
         self.provider = provider
         err = C.create_string_buffer(512)
-        if filter is not None or load_feedback_window or feedback_fallbacks:
+        if filter is not None or load_feedback_window or feedback_fallbacks or feedback_retries:
             # Options::filter (a scheduling.Filter chart or a node table),
             # Options::load_feedback_window (load feedback carried across flushes, 0 = off) and
-            # Options::feedback_fallbacks (the *WithFallbacks calls under that feedback)
+            # Options::feedback_fallbacks / feedback_retries (the *WithFallbacks calls and ScheduleRetry
+            # under that feedback)
             from .engine import _node_table
             nodes, n = _node_table(filter)
             devs = list(devices) if devices is not None else []
@@ -168,7 +169,8 @@ class HostScheduler:
                                                             max_adapters, max_batch, flush_size, batch_window_us,
                                                             refresh_interval_ms, seed, int(busy_poll), caller_spin_us,
                                                             int(use_doorbell), C.cast(nodes, C.c_void_p), n,
-                                                            load_feedback_window, int(feedback_fallbacks), err, 512)
+                                                            load_feedback_window, int(feedback_fallbacks),
+                                                            int(feedback_retries), err, 512)
         elif devices is not None and len(devices) > 1:
             arr = (C.c_int * len(devices))(*devices)
             self._s = self._lib.ligh_scheduler_new_devices(provider._p, arr, len(devices), max_pods, max_adapters,

@@ -21,7 +21,8 @@ batch (Filter.Filter, filter.go:12-15) in one device call, for any filter tree. 
 survivors in retry order (include/lig.h, fallback endpoints); under load_feedback_window they need
 ``feedback_fallbacks=True`` and then rank the feedback chain's own tables.  ``ScheduleRetry`` / ``ScheduleBatchRetry``
 schedule a request again without the pods it already tried, as Schedule would once those pods left the provider
-(lig_schedule_batch_excluding).  There is no CPU path here: without liblig.so or without a CUDA device construction
+(lig_schedule_batch_excluding); under load_feedback_window they need ``feedback_retries=True`` and then run as
+feedback-chain calls.  There is no CPU path here: without liblig.so or without a CUDA device construction
 fails.
 """
 from __future__ import annotations
@@ -191,7 +192,7 @@ class Scheduler:
     def __init__(self, podMetricsProvider: PodMetricsProvider, device: int = 0,
                  max_pods: int = 4096, max_adapters: int = 1024, max_batch: int = 1 << 16,
                  seed: Optional[int] = None, filter: Optional[Filter] = None, load_feedback_window: int = 0,
-                 feedback_fallbacks: bool = False):
+                 feedback_fallbacks: bool = False, feedback_retries: bool = False):
         if load_feedback_window < 0:
             raise ValueError(f"load_feedback_window must be >= 0, got {load_feedback_window}")
         self.podMetricsProvider = podMetricsProvider
@@ -199,6 +200,8 @@ class Scheduler:
         # fallback rows under load_feedback_window come from the chain's tables; opt-in because the
         # *WithFallbacks calls refuse under feedback without it (documented behaviour kept as is)
         self._feedback_fallbacks = bool(feedback_fallbacks)
+        # retries under load_feedback_window run on the chain's copy and load it; opt-in for the same reason
+        self._feedback_retries = bool(feedback_retries)
         self._engine = Engine(device, max_pods, max_adapters, max_batch)
         self._filter = filter                # None: the built-in defaultFilter
         if filter is not None:
@@ -431,10 +434,11 @@ class Scheduler:
         tried_lists[i] (lig_schedule_batch_excluding): what Schedule returns once those pods have left
         the provider.  Tried pods are matched by value against the snapshot current when the call
         runs; those no longer in it are ignored.  One rand_key per request from ScheduleBatch's
-        sequence; errors as ScheduleBatch.  ValueError for more than LIG_MAX_EXCLUDED tried pods and
-        under load_feedback_window (the picks come from the chain's load-adjusted copy of the
-        snapshot; a retry would not)."""
-        if self._window:
+        sequence; errors as ScheduleBatch.  ValueError for more than LIG_MAX_EXCLUDED tried pods.  Under
+        load_feedback_window the call is a feedback-chain call (lig_schedule_batch_feedback_chain_excluding:
+        the pool is the chain's load-adjusted copy, and each pick counts toward the chain's windows)
+        when the scheduler was built with feedback_retries=True, and raises ValueError otherwise."""
+        if self._window and not self._feedback_retries:
             raise ValueError("retries are not defined under load_feedback_window: the picks come from the feedback "
                              "chain's load-adjusted copy of the snapshot, a retry would not")
         if len(tried_lists) != len(reqs):
@@ -457,7 +461,11 @@ class Scheduler:
         for i, r in enumerate(reqs):
             arr[i] = (snap.adapter_id(r.ResolvedTargetModel), N.LIG_REQ_CRITICAL if r.Critical else 0,
                       self._rng.getrandbits(64))
-        picks = self._engine.schedule_batch_excluding(self._epoch, self._seed, arr, excluded)
+        if self._window:
+            picks = self._engine.schedule_batch_feedback_chain_excluding(self._epoch, self._seed, arr, excluded,
+                                                                         self._window)
+        else:
+            picks = self._engine.schedule_batch_excluding(self._epoch, self._seed, arr, excluded)
         return [(snap.pods[int(pk["pod_idx"])], None) if pk["status"] == N.LIG_OK
                 else (None, _schedule_error(int(pk["status"]))) for pk in picks]
 
@@ -541,7 +549,8 @@ class Scheduler:
 
 
 def NewScheduler(pmp: PodMetricsProvider, filter: Optional[Filter] = None, load_feedback_window: int = 0,
-                 feedback_fallbacks: bool = False, **kw) -> Scheduler:  # scheduler.go:93-99
+                 feedback_fallbacks: bool = False, feedback_retries: bool = False,
+                 **kw) -> Scheduler:  # scheduler.go:93-99
     """filter: a caller flow chart (None = defaultFilter, the reference's only tree).
     load_feedback_window > 0: ScheduleBatch goes through the load-feedback chain (include/lig.h,
     lig_schedule_batch_feedback_chain): every window of that many requests, counted across calls,
@@ -549,6 +558,10 @@ def NewScheduler(pmp: PodMetricsProvider, filter: Optional[Filter] = None, load_
     feedback_fallbacks: under load_feedback_window, let the *WithFallbacks calls run as chain calls
     whose rows rank the chain's load-adjusted survivors (lig_schedule_batch_feedback_chain_fallbacks);
     without it they raise ValueError there, as they always have.  The picks and the chain's loads do
-    not depend on it."""
+    not depend on it.
+    feedback_retries: under load_feedback_window, let ScheduleRetry / ScheduleBatchRetry run as chain calls
+    (lig_schedule_batch_feedback_chain_excluding): each retry is scheduled on the chain's load-adjusted copy
+    without the pods it tried, and its pick loads the chain like any other; without it they raise
+    ValueError there, as they always have."""
     return Scheduler(pmp, filter=filter, load_feedback_window=load_feedback_window,
-                     feedback_fallbacks=feedback_fallbacks, **kw)
+                     feedback_fallbacks=feedback_fallbacks, feedback_retries=feedback_retries, **kw)
