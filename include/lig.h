@@ -532,6 +532,43 @@ int lig_schedule_batch_excluding_device(lig_ctx* ctx, uint64_t epoch, uint64_t s
                                         int R, const int16_t* d_excluded, int n_excluded, lig_pick* d_out,
                                         void* stream);
 
+/* ---- retry scheduling with fallback rows: the retry's pick and up to LIG_MAX_FALLBACKS more survivors ----
+ * A retry returns one pod, so once a proxy has used up the first fallback row every further attempt
+ * costs a whole retry call.  These calls return, with the retry's pick, a fallback row of the reduced
+ * survivor set, so one round trip serves up to 1 + n_fallbacks attempts.
+ *
+ * The definition.  Request i, with its descriptor, its excluded row (format and rules of
+ * lig_schedule_batch_excluding), seed and n_fallbacks = k:
+ *   out[i] is what lig_schedule_batch_excluding returns for it, byte for byte: the same pool, the
+ *   same tree (the epoch's built-in tree with the ctx's thresholds, or the caller tree that built
+ *   the epoch), the same status and n_survivors.
+ *   Its row, fallbacks[i * k .. (i + 1) * k), is the fallback ranking of the section above applied to
+ *   L' = the reduced survivor set in ascending pod order (the set the retry's pick drew from), with
+ *   n' = n_survivors: step 0 is the pick's own Int31n(n') draws on state seed ^ rand_key, rejections
+ *   included; steps j = 1 .. m-1 (m = min(n', 1 + k)) draw j + Int31n(n' - j) on the continued
+ *   stream, each swapping in a partial Fisher-Yates shuffle.  The row holds L'[perm[1]] ..
+ *   L'[perm[m-1]] as pod indices in the epoch's pod order, then -1 up to k entries.  A request that is
+ *   not LIG_OK gets a row of -1.
+ * So no row entry is an excluded pod, entries are distinct, the row for k is a prefix of the row for
+ * any k' > k, and a row that excludes nothing gives lig_schedule_batch_fallbacks's out and row byte
+ * for byte (the reduced set is then the class's list).  The calls read the resident epoch only and
+ * neither end nor advance a feedback chain.
+ *
+ * LIG_ERR_INVALID, with nothing written, for every reason either parent call refuses: n_excluded
+ * outside [1, LIG_MAX_EXCLUDED], n_fallbacks outside [1, LIG_MAX_FALLBACKS], null buffers when R > 0,
+ * R > max_batch on the host form, and device buffers not aligned to their element (requests 16
+ * bytes, picks 8, both kinds of row 2); a stale epoch and a missing snapshot as lig_schedule_batch
+ * reports them.  Host form: page-locked, aligned buffers are used in place, pageable or misaligned
+ * ones (a request array at an odd 8 bytes included) are staged; it blocks until picks and rows are
+ * back.  Device form: device pointers, enqueued on `stream` (NULL = legacy default stream), not
+ * synchronised.  Both register as readers of the epoch's slot. */
+int lig_schedule_batch_excluding_fallbacks(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
+                                           const int16_t* excluded, int n_excluded, lig_pick* out,
+                                           int n_fallbacks, int16_t* fallbacks);
+int lig_schedule_batch_excluding_fallbacks_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed, const lig_req* d_reqs,
+                                                  int R, const int16_t* d_excluded, int n_excluded, lig_pick* d_out,
+                                                  int n_fallbacks, int16_t* d_fallbacks, void* stream);
+
 /* ---- in-batch load feedback (opt-in; the default path never mutates the snapshot) ----------------
  * The reference schedules every request against the scraped metrics as they are
  * (scheduler.go:113-122 never writes them), so all requests of one class that arrive inside a

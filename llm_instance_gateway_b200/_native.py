@@ -55,6 +55,7 @@ EXPORTED_SYMBOLS = (
     "lig_schedule_models_batch_feedback_chain_fallbacks", "lig_schedule_models_batch_feedback_chain_fallbacks_device",
     "lig_schedule_batch_excluding", "lig_schedule_batch_excluding_device",
     "lig_schedule_batch_feedback_chain_excluding", "lig_schedule_batch_feedback_chain_excluding_device",
+    "lig_schedule_batch_excluding_fallbacks", "lig_schedule_batch_excluding_fallbacks_device",
 )
 
 
@@ -181,6 +182,8 @@ def load() -> C.CDLL:
                                                                               vp, i32, vp, vp]
     lib.lig_schedule_batch_excluding.argtypes = [vp, u64, u64, vp, i32, vp, i32, vp]
     lib.lig_schedule_batch_excluding_device.argtypes = [vp, u64, u64, vp, i32, vp, i32, vp, vp]
+    lib.lig_schedule_batch_excluding_fallbacks.argtypes = [vp, u64, u64, vp, i32, vp, i32, vp, i32, vp]
+    lib.lig_schedule_batch_excluding_fallbacks_device.argtypes = [vp, u64, u64, vp, i32, vp, i32, vp, i32, vp, vp]
     lib.lig_schedule_batch_feedback_chain_excluding.argtypes = [vp, u64, u64, vp, i32, vp, i32, vp, i32, vp]
     lib.lig_schedule_batch_feedback_chain_excluding_device.argtypes = [vp, u64, u64, vp, i32, vp, i32, vp, i32, vp,
                                                                        vp]

@@ -424,6 +424,31 @@ Status Scheduler::ScheduleRetry(const LLMRequest& req, const std::vector<backend
   return w.status;
 }
 
+Status Scheduler::ScheduleRetryWithFallbacks(const LLMRequest& req, const std::vector<backend::Pod>& tried, int n,
+                                             std::vector<backend::Pod>* pods) {
+  if (pods) pods->clear();
+  if (n < 1 || n > LIG_MAX_FALLBACKS)
+    return Errorf(InvalidArgument, "ScheduleRetryWithFallbacks: n=" + std::to_string(n) + " outside [1, " +
+                                       std::to_string(LIG_MAX_FALLBACKS) + "]");
+  if (tried.size() > (size_t)LIG_MAX_EXCLUDED)
+    return Errorf(InvalidArgument, "ScheduleRetryWithFallbacks: " + std::to_string(tried.size()) +
+                                       " tried pods (at most " + std::to_string(LIG_MAX_EXCLUDED) + ")");
+  if (opt_.load_feedback_window > 0)
+    return Errorf(InvalidArgument, "ScheduleRetryWithFallbacks: not defined under load_feedback_window (the picks "
+                                   "come from the feedback chain's copy of the snapshot, these would not)");
+  if (group_)
+    return Errorf(InvalidArgument, "ScheduleRetryWithFallbacks: a scheduler over several devices has no retry call");
+  std::vector<backend::Pod> ranked;
+  Waiter w;
+  w.req = &req;
+  w.tried = &tried;
+  w.fallbacks = n;
+  w.pods = &ranked;
+  Submit(w);
+  if (w.status.ok() && pods) *pods = std::move(ranked);
+  return w.status;
+}
+
 Status Scheduler::ScheduleModel(const std::string& model, std::string* resolvedTargetModel, backend::Pod* targetPod) {
   Waiter w;
   w.model = &model;
@@ -673,7 +698,9 @@ void Scheduler::Flush(std::vector<Waiter*>& all) {
 }
 
 // The retry lane: one lig_schedule_batch_excluding call per max_batch waiters (under
-// load_feedback_window, lig_schedule_batch_feedback_chain_excluding).  Each waiter's tried pods are
+// load_feedback_window, lig_schedule_batch_feedback_chain_excluding; with a ScheduleRetryWithFallbacks
+// caller among them, lig_schedule_batch_excluding_fallbacks at the largest n asked, whose picks are the
+// same).  Each waiter's tried pods are
 // matched by value against the captured snapshot; its row holds their indices, -1 padded to the
 // widest row of the call.  Every waiter takes a rand_key; under the chain a waiter refused on the
 // host is left out of the call, since its pick would load a pod and shift every later window.
@@ -690,6 +717,8 @@ void Scheduler::FlushRetries(std::vector<Waiter*>& batch) {
   size_t done = 0;
   while (done < batch.size()) {
     const int n = (int)std::min(batch.size() - done, (size_t)opt_.max_batch);
+    int nf = 0;   // ScheduleRetryWithFallbacks callers (never under the chain): the largest n asked
+    for (int i = 0; i < n; ++i) nf = std::max(nf, batch[done + i]->fallbacks);
     std::shared_ptr<const Snapshot> snap;
     int rc = 0, width = 1, k = 0;
     for (int attempt = 0; failure.ok() && attempt < 4; ++attempt) {
@@ -733,6 +762,9 @@ void Scheduler::FlushRetries(std::vector<Waiter*>& batch) {
                                                                  width, h_picks_, W, nullptr)
                    : 0;
         if (rc == 0) CountFeedback(snap->epoch, k);
+      } else if (nf > 0) {
+        rc = lig_schedule_batch_excluding_fallbacks(ctx_, snap->epoch, seed_, h_reqs_, n, h_excluded_, width, h_picks_,
+                                                    nf, h_fallbacks_);
       } else {
         rc = lig_schedule_batch_excluding(ctx_, snap->epoch, seed_, h_reqs_, n, h_excluded_, width, h_picks_);
       }
@@ -741,7 +773,9 @@ void Scheduler::FlushRetries(std::vector<Waiter*>& batch) {
       stats_.stale_retries++;
     }
     if (failure.ok() && rc != 0)
-      failure = LigFailure(W > 0 ? "lig_schedule_batch_feedback_chain_excluding" : "lig_schedule_batch_excluding");
+      failure = LigFailure(W > 0    ? "lig_schedule_batch_feedback_chain_excluding"
+                           : nf > 0 ? "lig_schedule_batch_excluding_fallbacks"
+                                    : "lig_schedule_batch_excluding");
     for (int i = 0; i < n; ++i) {
       Waiter* w = batch[done + i];
       const lig_pick* pk = failure.ok() && slot[(size_t)i] >= 0 ? &h_picks_[slot[(size_t)i]] : nullptr;
@@ -749,8 +783,16 @@ void Scheduler::FlushRetries(std::vector<Waiter*>& batch) {
       else if (rows[(size_t)i].size() > (size_t)LIG_MAX_EXCLUDED)
         w->status = Errorf(InvalidArgument, "ScheduleRetry: the tried pods match more than " +
                                                 std::to_string(LIG_MAX_EXCLUDED) + " pods of the snapshot");
-      else if (pk->status == LIG_OK) w->pod = snap->pods[(size_t)pk->pod_idx];
-      else w->status = PickError(pk->status);
+      else if (pk->status == LIG_OK) {
+        w->pod = snap->pods[(size_t)pk->pod_idx];
+        if (w->fallbacks > 0) {
+          w->pods->push_back(w->pod);
+          const int16_t* row = h_fallbacks_ + (size_t)slot[(size_t)i] * (size_t)nf;
+          for (int j = 0; j < w->fallbacks && row[j] >= 0; ++j) w->pods->push_back(snap->pods[(size_t)row[j]]);
+        }
+      } else {
+        w->status = PickError(pk->status);
+      }
     }
     {
       std::lock_guard<std::mutex> sk(stats_mu_);

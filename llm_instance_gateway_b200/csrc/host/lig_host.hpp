@@ -186,7 +186,7 @@ struct Stats {
   uint64_t model_scheduled = 0;    // ScheduleModel(model, ...) calls completed (host-answered ones included)
   uint64_t model_batches = 0;      // device calls issued for model-id requests
   uint64_t fallback_scheduled = 0; // ScheduleWithFallbacks and ScheduleModelWithFallbacks calls completed
-  uint64_t retry_scheduled = 0;    // ScheduleRetry calls completed
+  uint64_t retry_scheduled = 0;    // ScheduleRetry and ScheduleRetryWithFallbacks calls completed
   double last_pack_us = 0;     // last Refresh: provider slice -> columns + bitmap (host)
   double last_upload_us = 0;   // last Refresh: lig_upload_snapshot (H2D + class tables)
   double max_device_call_us = 0;   // slowest single lig_schedule_batch call (launch + kernel + synchronise)
@@ -234,6 +234,19 @@ class Scheduler {
   // waiter refused on the host is left out of it, so it loads no pod) and with several devices.  A handler that used
   // ScheduleModel builds req from the resolved target model it got back and the model's criticality.
   Status ScheduleRetry(const LLMRequest& req, const std::vector<backend::Pod>& tried, backend::Pod* targetPod);
+
+  // ScheduleRetry plus up to n fallback endpoints (1 <= n <= LIG_MAX_FALLBACKS): fills *pods with the
+  // retry's pick (pods[0], the pod ScheduleRetry would have returned for the same rand_key and tried
+  // pods) and then up to n more distinct survivors of the same reduced pool, none of them tried, in the
+  // order a proxy should try them (lig_schedule_batch_excluding_fallbacks), so one call serves several
+  // attempts.  Goes through the retry lane like ScheduleRetry: a flush whose retry lane holds any such
+  // caller makes one lig_schedule_batch_excluding_fallbacks call at the largest n asked in it, and plain
+  // ScheduleRetry callers in it get the same picks.  Never through the doorbell; counted in
+  // Stats::retry_scheduled.  Errors are Schedule's.  InvalidArgument for n outside
+  // [1, LIG_MAX_FALLBACKS], more than LIG_MAX_EXCLUDED tried pods, load_feedback_window > 0 (there is
+  // no feedback-chain form of the call, whatever Options::feedback_retries says) and several devices.
+  Status ScheduleRetryWithFallbacks(const LLMRequest& req, const std::vector<backend::Pod>& tried, int n,
+                                    std::vector<backend::Pod>* pods);
 
   // The reference's Filter interface (filter.go:12-15) run on the current epoch: fills *pods with
   // the survivors of req's walk of the filter tree (the built-in one or Options::filter), in slice

@@ -314,6 +314,25 @@ int ligh_schedule_retry(ligh_scheduler* s, const char* resolved, int critical, c
   return st.code;
 }
 
+int ligh_schedule_retry_with_fallbacks(ligh_scheduler* s, const char* resolved, int critical,
+                                       const char* const* tried_names, const char* const* tried_addrs, int n_tried,
+                                       int n, char* names, int names_cap, int* n_pods, char* err, int err_cap) {
+  scheduling::LLMRequest req;
+  req.ResolvedTargetModel = resolved ? resolved : "";
+  req.Critical = critical != 0;
+  std::vector<backend::Pod> tried;
+  for (int i = 0; i < n_tried; ++i)
+    tried.push_back(backend::Pod{tried_names[i] ? tried_names[i] : "", tried_addrs[i] ? tried_addrs[i] : ""});
+  std::vector<backend::Pod> pods;
+  scheduling::Status st = s->sched->ScheduleRetryWithFallbacks(req, tried, n, &pods);
+  std::string joined;
+  for (size_t i = 0; i < pods.size(); ++i) joined += (i ? "\n" : "") + pods[i].Name;
+  if (n_pods) *n_pods = (int)pods.size();
+  put(names, names_cap, joined);
+  if (!st.ok()) put(err, err_cap, st.message);
+  return st.code;
+}
+
 uint64_t ligh_retry_scheduled(ligh_scheduler* s) { return s->sched->stats().retry_scheduled; }
 
 int ligh_filter(ligh_scheduler* s, const char* resolved, int critical, char* names, int names_cap, int* n_pods,

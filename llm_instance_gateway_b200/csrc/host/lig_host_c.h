@@ -65,6 +65,12 @@ uint64_t ligh_fallback_scheduled(ligh_scheduler*);   /* Stats::fallback_schedule
 int ligh_schedule_retry(ligh_scheduler*, const char* resolved_target_model, int critical, const char* const* tried_names,
                         const char* const* tried_addrs, int n_tried, char* name, int name_cap, char* addr, int addr_cap,
                         char* err, int err_cap);
+/* Scheduler::ScheduleRetryWithFallbacks: returns the gRPC code; the tried pods as ligh_schedule_retry's;
+ * names receives the retry's pick and then up to n fallback pods' names joined by '\n' (retry order)
+ * and *n_pods their count. */
+int ligh_schedule_retry_with_fallbacks(ligh_scheduler*, const char* resolved_target_model, int critical,
+                                       const char* const* tried_names, const char* const* tried_addrs, int n_tried,
+                                       int n, char* names, int names_cap, int* n_pods, char* err, int err_cap);
 uint64_t ligh_retry_scheduled(ligh_scheduler*);      /* Stats::retry_scheduled */
 int ligh_refresh(ligh_scheduler*, char* err, int err_cap);
 /* several GPUs behind one scheduler (lig_group_*) */

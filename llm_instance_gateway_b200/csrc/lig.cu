@@ -1044,6 +1044,10 @@ static int create_impl(lig_ctx* c, int device, int max_pods, int max_adapters, i
   CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_count_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_count_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_count_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   const size_t need = scratch_bytes(words_for(max_pods)) > build_fixed_bytes(words_for(max_pods))
                           ? scratch_bytes(words_for(max_pods)) : build_fixed_bytes(words_for(max_pods));
   if (need > c->smem_optin)
@@ -2318,6 +2322,133 @@ int lig_schedule_batch_excluding(lig_ctx* c, uint64_t epoch, uint64_t seed, cons
   // the copy back waits for the kernel on the lane; it may block, so not under c->mu
   cudaError_t e = cudaSuccess;
   if (st_out) e = cudaMemcpyAsync(out, d.out, out_b, cudaMemcpyDeviceToHost, st);
+  if (stage) cudaFreeAsync(stage, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(LIG_ERR_CUDA, "%s failed on the device: %s", fn, cudaGetErrorString(e));
+  return 0;
+}
+
+// ---- retry scheduling with fallback rows (lig_schedule_batch_excluding_fallbacks) ----------------------
+// The retry call's arguments plus a row of n_fallbacks int16 per request; every retry rule applies.
+static int excluding_fallbacks_check(const lig_ctx* c, const char* fn, const ExcludingCall& x, int n_fallbacks,
+                                     const int16_t* fallbacks) {
+  if (int rc = excluding_check(c, fn, x)) return rc;
+  if (x.R > 0 && !fallbacks) return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
+  if (n_fallbacks < 1 || n_fallbacks > LIG_MAX_FALLBACKS)
+    return fail(LIG_ERR_INVALID, "%s: n_fallbacks=%d outside [1, %d]", fn, n_fallbacks, LIG_MAX_FALLBACKS);
+  return 0;
+}
+
+// Enqueue the retry-with-rows kernel for x (R >= 1, device-visible, aligned pointers) against slot s on
+// st, behind the slot's tables, with the scan's launch shape and the tree that built the slot's
+// tables, and register st as a reader of the slot.  Caller holds c->mu.
+static int enqueue_excluding_fallbacks(lig_ctx* c, Slot& s, const ExcludingCall& x, int n_fallbacks,
+                                       int16_t* fallbacks, cudaStream_t st) {
+  static const FilterTree kNoTree{};
+  CUDA_TRY(cudaStreamWaitEvent(st, s.ready, 0));
+  const ScanShape sh = scan_shape(c, s, x.R);
+  const SnapView v = view_of(s);
+  const FilterTree& t = s.caller_tree ? s.tree : kNoTree;
+  const Thr thr = thr_of(c);
+  const int4* in = reinterpret_cast<const int4*>(x.reqs);
+  int2* out = reinterpret_cast<int2*>(x.out);
+  auto launch = [&](auto staged, auto caller_tree) {
+    constexpr bool kS = decltype(staged)::value, kT = decltype(caller_tree)::value;
+    lig_schedule_excluding_fallback_kernel<kS, kT><<<sh.grid, kCtaThreads, sh.smem, st>>>(
+        v, thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, n_fallbacks, fallbacks);
+  };
+  using Y = std::true_type;
+  using N = std::false_type;
+  if (s.caller_tree) {
+    if (sh.staged) launch(Y{}, Y{});
+    else launch(N{}, Y{});
+  } else {
+    if (sh.staged) launch(Y{}, N{});
+    else launch(N{}, N{});
+  }
+  CUDA_TRY(cudaGetLastError());
+  c->launches++;
+  return note_reader(s, st);
+}
+
+int lig_schedule_batch_excluding_fallbacks_device(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* d_reqs,
+                                                  int R, const int16_t* d_excluded, int n_excluded, lig_pick* d_out,
+                                                  int n_fallbacks, int16_t* d_fallbacks, void* stream) {
+  static const char fn[] = "lig_schedule_batch_excluding_fallbacks_device";
+  const ExcludingCall x{seed, d_reqs, R, d_out, n_excluded, d_excluded};
+  if (int rc = excluding_fallbacks_check(c, fn, x, n_fallbacks, d_fallbacks)) return rc;
+  if (R > 0 && (misaligned(d_reqs, sizeof(lig_req)) || misaligned(d_out, sizeof(lig_pick)) ||
+                misaligned(d_excluded, sizeof(int16_t)) || misaligned(d_fallbacks, sizeof(int16_t))))
+    return fail(LIG_ERR_INVALID, "%s: a device buffer is not aligned to its element", fn);
+  std::lock_guard<std::mutex> lk(c->mu);
+  Slot* s = nullptr;
+  if (int rc = resolve_slot(c, epoch, &s)) return rc;
+  if (R == 0) return 0;
+  CUDA_TRY(cudaSetDevice(c->device));
+  return enqueue_excluding_fallbacks(c, *s, x, n_fallbacks, d_fallbacks, static_cast<cudaStream_t>(stream));
+}
+
+// Host buffers, as lig_schedule_batch_excluding handles them: page-locked, aligned ones are read and
+// written by the kernel in place; the others are staged in stream-ordered HBM and copied on the
+// call's lane.  Blocks until the picks and rows are back.
+int lig_schedule_batch_excluding_fallbacks(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
+                                           const int16_t* excluded, int n_excluded, lig_pick* out,
+                                           int n_fallbacks, int16_t* fallbacks) {
+  static const char fn[] = "lig_schedule_batch_excluding_fallbacks";
+  const ExcludingCall x{seed, reqs, R, out, n_excluded, excluded};
+  if (int rc = excluding_fallbacks_check(c, fn, x, n_fallbacks, fallbacks)) return rc;
+  if (R > c->max_batch) return fail(LIG_ERR_INVALID, "%s: R=%d exceeds max_batch=%d", fn, R, c->max_batch);
+  ExcludingCall d = x;    // the same call with device-visible pointers
+  const size_t in_b = (size_t)R * sizeof(lig_req), out_b = (size_t)R * sizeof(lig_pick);
+  const size_t rows_b = (size_t)R * x.row_bytes(), fb_b = (size_t)R * (size_t)n_fallbacks * sizeof(int16_t);
+  d.reqs = R ? mapped_device_pointer(reqs) : nullptr;
+  d.out = R ? mapped_device_pointer(out) : nullptr;
+  d.excluded = R ? mapped_device_pointer(excluded) : nullptr;
+  int16_t* d_fb = R ? mapped_device_pointer(fallbacks) : nullptr;
+  // the kernel reads a descriptor with one 16-byte load and stores every pick whole
+  const bool st_in = R && (!d.reqs || misaligned(d.reqs, sizeof(lig_req)));
+  const bool st_out = R && (!d.out || misaligned(d.out, sizeof(lig_pick)));
+  const bool st_rows = R && (!d.excluded || misaligned(d.excluded, sizeof(int16_t)));
+  const bool st_fb = R && (!d_fb || misaligned(d_fb, sizeof(int16_t)));
+  cudaStream_t st = nullptr;
+  unsigned char* stage = nullptr;
+  {
+    std::lock_guard<std::mutex> lk(c->mu);
+    Slot* s = nullptr;
+    if (int rc = resolve_slot(c, epoch, &s)) return rc;
+    if (R == 0) return 0;
+    CUDA_TRY(cudaSetDevice(c->device));
+    st = c->s_lane[c->next_lane];
+    c->next_lane = (c->next_lane + 1) % kLanes;
+    size_t at = 0, o_in = 0, o_out = 0, o_rows = 0, o_fb = 0;
+    auto take = [&](bool on, size_t bytes, size_t* o) { if (on) { *o = at; at = (at + bytes + 255) & ~(size_t)255; } };
+    take(st_in, in_b, &o_in);
+    take(st_out, out_b, &o_out);
+    take(st_rows, rows_b, &o_rows);
+    take(st_fb, fb_b, &o_fb);
+    if (at) {
+      CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&stage), at, st));
+      if (st_in) d.reqs = reinterpret_cast<const lig_req*>(stage + o_in);
+      if (st_out) d.out = reinterpret_cast<lig_pick*>(stage + o_out);
+      if (st_rows) d.excluded = reinterpret_cast<const int16_t*>(stage + o_rows);
+      if (st_fb) d_fb = reinterpret_cast<int16_t*>(stage + o_fb);
+    }
+    int rc = 0;
+    if (st_in && cudaMemcpyAsync(const_cast<lig_req*>(d.reqs), reqs, in_b, cudaMemcpyHostToDevice, st) != cudaSuccess)
+      rc = fail(LIG_ERR_CUDA, "%s: staging the requests failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
+    if (!rc && st_rows &&
+        cudaMemcpyAsync(const_cast<int16_t*>(d.excluded), excluded, rows_b, cudaMemcpyHostToDevice, st) != cudaSuccess)
+      rc = fail(LIG_ERR_CUDA, "%s: staging the rows failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
+    if (!rc) rc = enqueue_excluding_fallbacks(c, *s, d, n_fallbacks, d_fb, st);
+    if (rc) {
+      if (stage) cudaFreeAsync(stage, st);
+      return rc;
+    }
+  }
+  // the copies back wait for the kernel on the lane; they may block, so not under c->mu
+  cudaError_t e = cudaSuccess;
+  if (st_out) e = cudaMemcpyAsync(out, d.out, out_b, cudaMemcpyDeviceToHost, st);
+  if (st_fb && e == cudaSuccess) e = cudaMemcpyAsync(fallbacks, d_fb, fb_b, cudaMemcpyDeviceToHost, st);
   if (stage) cudaFreeAsync(stage, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   if (e != cudaSuccess) return fail(LIG_ERR_CUDA, "%s failed on the device: %s", fn, cudaGetErrorString(e));

@@ -321,6 +321,38 @@ class Engine:
                                                               d_excluded or None, n_excluded, d_out or None,
                                                               stream or None))
 
+    # ---- retry scheduling with fallback rows: the retry's pick and more survivors of the reduced pool ----
+    def schedule_batch_excluding_fallbacks(self, epoch: int, seed: int, reqs: np.ndarray, excluded: np.ndarray,
+                                           n: int):
+        """lig_schedule_batch_excluding_fallbacks: (picks, int16 fallbacks of shape (R, n)); the picks equal
+        schedule_batch_excluding's, row i holds request i's next distinct survivors of its reduced pool in
+        retry order, -1 padded."""
+        assert reqs.dtype == REQ_DTYPE and reqs.flags.c_contiguous
+        assert excluded.dtype == np.int16 and excluded.flags.c_contiguous and excluded.ndim == 2
+        R = int(reqs.shape[0])
+        assert excluded.shape[0] == R
+        out = np.empty(R, dtype=PICK_DTYPE)
+        rows = np.empty((R, max(n, 0)), dtype=np.int16)
+        N.check(self._lib.lig_schedule_batch_excluding_fallbacks(self._ctx, epoch, seed, _ptr(reqs), R,
+                                                                 _ptr(excluded), int(excluded.shape[1]), _ptr(out),
+                                                                 n, _ptr(rows)))
+        return out, rows
+
+    def schedule_batch_excluding_fallbacks_ptr(self, epoch: int, seed: int, h_reqs: int, R: int, h_excluded: int,
+                                               n_excluded: int, h_out: int, n: int, h_fallbacks: int) -> None:
+        N.check(self._lib.lig_schedule_batch_excluding_fallbacks(self._ctx, epoch, seed, h_reqs or None, R,
+                                                                 h_excluded or None, n_excluded, h_out or None, n,
+                                                                 h_fallbacks or None))
+
+    def schedule_batch_excluding_fallbacks_device(self, epoch: int, seed: int, d_reqs: int, R: int, d_excluded: int,
+                                                  n_excluded: int, d_out: int, n: int, d_fallbacks: int,
+                                                  stream: int = 0) -> None:
+        """Device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_batch_excluding_fallbacks_device(self._ctx, epoch, seed, d_reqs or None, R,
+                                                                        d_excluded or None, n_excluded,
+                                                                        d_out or None, n, d_fallbacks or None,
+                                                                        stream or None))
+
     # ---- retries under the feedback chain: a chain call whose requests exclude the pods they tried ----
     def schedule_batch_feedback_chain_excluding(self, epoch: int, seed: int, reqs: np.ndarray, excluded: np.ndarray,
                                                 window: int, loads: Optional[np.ndarray] = None) -> np.ndarray:

@@ -29,7 +29,7 @@ EXPORTED_SYMBOLS = (
     "ligh_schedule_model", "ligh_scheduler_new_tree", "ligh_scheduler_new_feedback", "ligh_feedback_stats",
     "ligh_scheduler_set_models", "ligh_schedule_model_device", "ligh_model_stats", "ligh_schedule_models_concurrent",
     "ligh_filter", "ligh_schedule_with_fallbacks", "ligh_fallback_scheduled", "ligh_schedule_model_with_fallbacks",
-    "ligh_schedule_retry", "ligh_retry_scheduled",
+    "ligh_schedule_retry", "ligh_retry_scheduled", "ligh_schedule_retry_with_fallbacks",
 )
 
 _lib = None
@@ -86,6 +86,8 @@ def load() -> C.CDLL:
     lib.ligh_fallback_scheduled.argtypes = [vp]
     lib.ligh_schedule_retry.argtypes = [vp, C.c_char_p, i32, cpp, cpp, i32, C.c_char_p, i32, C.c_char_p, i32,
                                         C.c_char_p, i32]
+    lib.ligh_schedule_retry_with_fallbacks.argtypes = [vp, C.c_char_p, i32, cpp, cpp, i32, i32, C.c_char_p, i32,
+                                                       C.POINTER(i32), C.c_char_p, i32]
     lib.ligh_retry_scheduled.argtypes = [vp]
     lib.ligh_retry_scheduled.restype = u64
     lib.ligh_fallback_scheduled.restype = u64
@@ -226,6 +228,19 @@ class HostScheduler:
         if code == GRPC_OK:
             return code, Pod(name.value.decode(), addr.value.decode()), ""
         return code, None, err.value.decode("utf-8", "replace")
+
+    def ScheduleRetryWithFallbacks(self, resolved: str, critical: bool, tried: Sequence[Pod], n: int
+                                   ) -> Tuple[int, List[str], str]:  # noqa: N802
+        """Scheduler::ScheduleRetryWithFallbacks: ScheduleRetry plus up to n fallback pods of the same reduced
+        pool: (gRPC code, pod names [pick, fallbacks in retry order], error)."""
+        cap = 64 * 1024
+        names, err, k = C.create_string_buffer(cap), C.create_string_buffer(512), C.c_int(0)
+        code = self._lib.ligh_schedule_retry_with_fallbacks(self._s, resolved.encode(), int(critical),
+                                                            _strs([p.Name for p in tried]),
+                                                            _strs([p.Address for p in tried]), len(tried), n, names,
+                                                            cap, C.byref(k), err, 512)
+        pods = names.value.decode().split("\n") if k.value else []
+        return code, pods, err.value.decode("utf-8", "replace") if code != GRPC_OK else ""
 
     def ScheduleModelWithFallbacks(self, model: str, n: int) -> Tuple[int, str, List[str], str]:  # noqa: N802
         """Scheduler::ScheduleModelWithFallbacks: (gRPC code, resolved target model, pod names [pick,

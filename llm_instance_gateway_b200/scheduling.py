@@ -22,7 +22,9 @@ survivors in retry order (include/lig.h, fallback endpoints); under load_feedbac
 ``feedback_fallbacks=True`` and then rank the feedback chain's own tables.  ``ScheduleRetry`` / ``ScheduleBatchRetry``
 schedule a request again without the pods it already tried, as Schedule would once those pods left the provider
 (lig_schedule_batch_excluding); under load_feedback_window they need ``feedback_retries=True`` and then run as
-feedback-chain calls.  There is no CPU path here: without liblig.so or without a CUDA device construction
+feedback-chain calls.  ``ScheduleRetryWithFallbacks`` / ``ScheduleBatchRetryWithFallbacks`` return the retry's
+pick followed by up to n more distinct survivors of the reduced pool (lig_schedule_batch_excluding_fallbacks), so
+one call serves several attempts; they have no feedback-chain form.  There is no CPU path here: without liblig.so or without a CUDA device construction
 fails.
 """
 from __future__ import annotations
@@ -428,19 +430,9 @@ class Scheduler:
         return out
 
     # ---- retry scheduling: Schedule again over the pool without the pods already tried ----
-    def ScheduleBatchRetry(self, reqs: Sequence[LLMRequest], tried_lists: Sequence[Sequence[Pod]]
-                           ) -> List[Tuple[Optional[Pod], Optional[StatusError]]]:
-        """ScheduleBatch with request i scheduled over the current snapshot's pods without the pods of
-        tried_lists[i] (lig_schedule_batch_excluding): what Schedule returns once those pods have left
-        the provider.  Tried pods are matched by value against the snapshot current when the call
-        runs; those no longer in it are ignored.  One rand_key per request from ScheduleBatch's
-        sequence; errors as ScheduleBatch.  ValueError for more than LIG_MAX_EXCLUDED tried pods.  Under
-        load_feedback_window the call is a feedback-chain call (lig_schedule_batch_feedback_chain_excluding:
-        the pool is the chain's load-adjusted copy, and each pick counts toward the chain's windows)
-        when the scheduler was built with feedback_retries=True, and raises ValueError otherwise."""
-        if self._window and not self._feedback_retries:
-            raise ValueError("retries are not defined under load_feedback_window: the picks come from the feedback "
-                             "chain's load-adjusted copy of the snapshot, a retry would not")
+    def _retry_batch(self, reqs: Sequence[LLMRequest], tried_lists: Sequence[Sequence[Pod]]):
+        """(snapshot, descriptors, excluded rows) of a retry batch: tried pods matched by value against the
+        current snapshot, one rand_key per request from ScheduleBatch's sequence."""
         if len(tried_lists) != len(reqs):
             raise ValueError(f"{len(reqs)} requests but {len(tried_lists)} tried lists")
         for tried in tried_lists:
@@ -461,6 +453,22 @@ class Scheduler:
         for i, r in enumerate(reqs):
             arr[i] = (snap.adapter_id(r.ResolvedTargetModel), N.LIG_REQ_CRITICAL if r.Critical else 0,
                       self._rng.getrandbits(64))
+        return snap, arr, excluded
+
+    def ScheduleBatchRetry(self, reqs: Sequence[LLMRequest], tried_lists: Sequence[Sequence[Pod]]
+                           ) -> List[Tuple[Optional[Pod], Optional[StatusError]]]:
+        """ScheduleBatch with request i scheduled over the current snapshot's pods without the pods of
+        tried_lists[i] (lig_schedule_batch_excluding): what Schedule returns once those pods have left
+        the provider.  Tried pods are matched by value against the snapshot current when the call
+        runs; those no longer in it are ignored.  One rand_key per request from ScheduleBatch's
+        sequence; errors as ScheduleBatch.  ValueError for more than LIG_MAX_EXCLUDED tried pods.  Under
+        load_feedback_window the call is a feedback-chain call (lig_schedule_batch_feedback_chain_excluding:
+        the pool is the chain's load-adjusted copy, and each pick counts toward the chain's windows)
+        when the scheduler was built with feedback_retries=True, and raises ValueError otherwise."""
+        if self._window and not self._feedback_retries:
+            raise ValueError("retries are not defined under load_feedback_window: the picks come from the feedback "
+                             "chain's load-adjusted copy of the snapshot, a retry would not")
+        snap, arr, excluded = self._retry_batch(reqs, tried_lists)
         if self._window:
             picks = self._engine.schedule_batch_feedback_chain_excluding(self._epoch, self._seed, arr, excluded,
                                                                          self._window)
@@ -475,6 +483,32 @@ class Scheduler:
         if err is not None:
             raise err
         return pod
+
+    def ScheduleBatchRetryWithFallbacks(self, reqs: Sequence[LLMRequest], tried_lists: Sequence[Sequence[Pod]],
+                                        n: int) -> List[Tuple[List[Pod], Optional[StatusError]]]:
+        """ScheduleBatchRetry plus up to n fallback pods per request (lig_schedule_batch_excluding_fallbacks):
+        (pods, error) per request, pods[0] the pod ScheduleBatchRetry would have returned, then distinct
+        survivors of the same reduced pool in the order a proxy should try them, none of them tried.
+        Tried pods, the rand_key sequence and errors as ScheduleBatchRetry.  ValueError for n outside
+        [1, LIG_MAX_FALLBACKS], more than LIG_MAX_EXCLUDED tried pods, and under load_feedback_window
+        (there is no feedback-chain form of this call)."""
+        if self._window:
+            raise ValueError("retries with fallbacks are not defined under load_feedback_window: the picks come "
+                             "from the feedback chain's load-adjusted copy of the snapshot, these would not")
+        if not 1 <= n <= N.LIG_MAX_FALLBACKS:
+            raise ValueError(f"n must be in [1, {N.LIG_MAX_FALLBACKS}], got {n}")
+        snap, arr, excluded = self._retry_batch(reqs, tried_lists)
+        picks, rows = self._engine.schedule_batch_excluding_fallbacks(self._epoch, self._seed, arr, excluded, n)
+        return [([snap.pods[int(pk["pod_idx"])]] + [snap.pods[int(p)] for p in row if p >= 0], None)
+                if pk["status"] == N.LIG_OK else ([], _schedule_error(int(pk["status"])))
+                for pk, row in zip(picks, rows)]
+
+    def ScheduleRetryWithFallbacks(self, req: LLMRequest, tried: Sequence[Pod], n: int) -> List[Pod]:
+        """ScheduleRetry plus up to n fallback pods: [pick, fallback 1, ...]; raises like Schedule."""
+        pods, err = self.ScheduleBatchRetryWithFallbacks([req], [tried], n)[0]
+        if err is not None:
+            raise err
+        return pods
 
     # Filter-level view (the GPU analogue of Filter.Filter, filter.go:12-15): survivor slice.
     def Filter(self, req: LLMRequest) -> Tuple[List[Pod], Optional[StatusError]]:
