@@ -719,6 +719,42 @@ int lig_schedule_batch_feedback_chain_excluding_device(lig_ctx* ctx, uint64_t ep
                                                        const lig_req* d_reqs, int R, const int16_t* d_excluded,
                                                        int n_excluded, lig_pick* d_out, int window,
                                                        int32_t* d_loads, void* stream);
+/* Retries with fallback rows under the chain.  A chain retry call with rows is
+ * lig_schedule_batch_feedback_chain_excluding in every respect, plus a fallback row per request, as
+ * lig_schedule_batch_feedback_chain_fallbacks adds rows to the plain chain call:
+ *   1. Sequence, windows, picks and loads do not change: request i's `out` is what
+ *      lig_schedule_batch_feedback_chain_excluding returns for it at the same position, byte for byte
+ *      (the chain's private copy, the tree and thresholds the chain started with, the call's seed and
+ *      its rand_key).  Only a LIG_OK pick adds load; row entries add none, so `loads` does not depend
+ *      on n_fallbacks.  Calls with and without rows, of every kind (plain, model-id, fallback,
+ *      retry), may alternate in one chain, and the restart rules are unchanged.
+ *   2. Request i's row is the ranking of lig_schedule_batch_excluding_fallbacks applied to the
+ *      chain's pool instead of the epoch's: L' = the reduced survivor set of that walk in ascending
+ *      pod order, n' = n_survivors; step 0 is the pick's own Int31n(n') draws on seed ^ rand_key,
+ *      steps j = 1 .. m-1 draw j + Int31n(n' - j) on the continued stream; entries are pod indices in
+ *      E's pod order, padded with -1 up to k; a request that is not LIG_OK gets a row of -1.
+ *   So no row entry is an excluded pod, the entries are distinct, the row for k is a prefix of the
+ *   row for k' > k, and results do not depend on how the requests are split into calls.  Rows that
+ *   exclude nothing give lig_schedule_batch_feedback_chain_fallbacks's `out`, rows and `loads` byte
+ *   for byte; while no window has closed, and the chain's tree and thresholds are those E was built
+ *   with, `out` and the rows are lig_schedule_batch_excluding_fallbacks's on E byte for byte.  Like a
+ *   chain retry segment, a segment of this call reads no class table.
+ *   3. Refused, with nothing written and the chain exactly as it was, for every reason the chain
+ *      retry call is refused and every reason the chain fallback calls are refused (n_fallbacks
+ *      outside [1, LIG_MAX_FALLBACKS], a null row buffer when R > 0, a device row buffer that is not
+ *      2-byte aligned).
+ * Host form: excluded rows are staged as for the chain retry call, fallback rows as for the chain
+ * fallback calls; it blocks.  Device form: device pointers, enqueued on `stream`, not synchronised. */
+int lig_schedule_batch_feedback_chain_excluding_fallbacks(lig_ctx* ctx, uint64_t epoch, uint64_t seed,
+                                                          const lig_req* reqs, int R, const int16_t* excluded,
+                                                          int n_excluded, lig_pick* out, int n_fallbacks,
+                                                          int16_t* fallbacks, int window, int32_t* loads);
+int lig_schedule_batch_feedback_chain_excluding_fallbacks_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed,
+                                                                 const lig_req* d_reqs, int R,
+                                                                 const int16_t* d_excluded, int n_excluded,
+                                                                 lig_pick* d_out, int n_fallbacks,
+                                                                 int16_t* d_fallbacks, int window,
+                                                                 int32_t* d_loads, void* stream);
 /* The next chain call starts a new chain. */
 int lig_feedback_chain_reset(lig_ctx* ctx);
 

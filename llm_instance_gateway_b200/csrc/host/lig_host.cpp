@@ -433,9 +433,10 @@ Status Scheduler::ScheduleRetryWithFallbacks(const LLMRequest& req, const std::v
   if (tried.size() > (size_t)LIG_MAX_EXCLUDED)
     return Errorf(InvalidArgument, "ScheduleRetryWithFallbacks: " + std::to_string(tried.size()) +
                                        " tried pods (at most " + std::to_string(LIG_MAX_EXCLUDED) + ")");
-  if (opt_.load_feedback_window > 0)
-    return Errorf(InvalidArgument, "ScheduleRetryWithFallbacks: not defined under load_feedback_window (the picks "
-                                   "come from the feedback chain's copy of the snapshot, these would not)");
+  if (opt_.load_feedback_window > 0 && !(opt_.feedback_retries && opt_.feedback_fallbacks))
+    return Errorf(InvalidArgument, "ScheduleRetryWithFallbacks: not defined under load_feedback_window without "
+                                   "feedback_retries and feedback_fallbacks (the picks come from the feedback "
+                                   "chain's copy of the snapshot, these would not)");
   if (group_)
     return Errorf(InvalidArgument, "ScheduleRetryWithFallbacks: a scheduler over several devices has no retry call");
   std::vector<backend::Pod> ranked;
@@ -699,8 +700,8 @@ void Scheduler::Flush(std::vector<Waiter*>& all) {
 
 // The retry lane: one lig_schedule_batch_excluding call per max_batch waiters (under
 // load_feedback_window, lig_schedule_batch_feedback_chain_excluding; with a ScheduleRetryWithFallbacks
-// caller among them, lig_schedule_batch_excluding_fallbacks at the largest n asked, whose picks are the
-// same).  Each waiter's tried pods are
+// caller among them, lig_schedule_batch_[feedback_chain_]excluding_fallbacks at the largest n asked,
+// whose picks, and under the chain whose windows, are the same).  Each waiter's tried pods are
 // matched by value against the captured snapshot; its row holds their indices, -1 padded to the
 // widest row of the call.  Every waiter takes a rand_key; under the chain a waiter refused on the
 // host is left out of the call, since its pick would load a pod and shift every later window.
@@ -717,7 +718,7 @@ void Scheduler::FlushRetries(std::vector<Waiter*>& batch) {
   size_t done = 0;
   while (done < batch.size()) {
     const int n = (int)std::min(batch.size() - done, (size_t)opt_.max_batch);
-    int nf = 0;   // ScheduleRetryWithFallbacks callers (never under the chain): the largest n asked
+    int nf = 0;   // ScheduleRetryWithFallbacks callers: the largest n asked
     for (int i = 0; i < n; ++i) nf = std::max(nf, batch[done + i]->fallbacks);
     std::shared_ptr<const Snapshot> snap;
     int rc = 0, width = 1, k = 0;
@@ -758,9 +759,12 @@ void Scheduler::FlushRetries(std::vector<Waiter*>& batch) {
         ++k;
       }
       if (W > 0) {
-        rc = k > 0 ? lig_schedule_batch_feedback_chain_excluding(ctx_, snap->epoch, seed_, h_reqs_, k, h_excluded_,
-                                                                 width, h_picks_, W, nullptr)
-                   : 0;
+        rc = k == 0   ? 0
+             : nf > 0 ? lig_schedule_batch_feedback_chain_excluding_fallbacks(ctx_, snap->epoch, seed_, h_reqs_, k,
+                                                                              h_excluded_, width, h_picks_, nf,
+                                                                              h_fallbacks_, W, nullptr)
+                      : lig_schedule_batch_feedback_chain_excluding(ctx_, snap->epoch, seed_, h_reqs_, k, h_excluded_,
+                                                                    width, h_picks_, W, nullptr);
         if (rc == 0) CountFeedback(snap->epoch, k);
       } else if (nf > 0) {
         rc = lig_schedule_batch_excluding_fallbacks(ctx_, snap->epoch, seed_, h_reqs_, n, h_excluded_, width, h_picks_,
@@ -773,9 +777,10 @@ void Scheduler::FlushRetries(std::vector<Waiter*>& batch) {
       stats_.stale_retries++;
     }
     if (failure.ok() && rc != 0)
-      failure = LigFailure(W > 0    ? "lig_schedule_batch_feedback_chain_excluding"
-                           : nf > 0 ? "lig_schedule_batch_excluding_fallbacks"
-                                    : "lig_schedule_batch_excluding");
+      failure = LigFailure(W > 0 && nf > 0 ? "lig_schedule_batch_feedback_chain_excluding_fallbacks"
+                           : W > 0         ? "lig_schedule_batch_feedback_chain_excluding"
+                           : nf > 0        ? "lig_schedule_batch_excluding_fallbacks"
+                                           : "lig_schedule_batch_excluding");
     for (int i = 0; i < n; ++i) {
       Waiter* w = batch[done + i];
       const lig_pick* pk = failure.ok() && slot[(size_t)i] >= 0 ? &h_picks_[slot[(size_t)i]] : nullptr;

@@ -161,13 +161,15 @@ struct Options {
   // survivors in the chain's load-adjusted tables, the set the pick itself drew from.  Picks and
   // feedback windows are the same with or without it.  Off by default only because those calls have
   // always been refused under feedback with InvalidArgument and that refusal is relied upon; without
-  // it they still are.  No effect without load_feedback_window.
+  // it they still are.  No effect without load_feedback_window.  Together with feedback_retries it
+  // also lets ScheduleRetryWithFallbacks run under the chain (see there).
   bool feedback_fallbacks = false;
   // With load_feedback_window > 0: let ScheduleRetry run as feedback-chain calls
   // (lig_schedule_batch_feedback_chain_excluding): a retry is scheduled on the chain's load-adjusted
   // copy without the pods it tried, and its pick counts toward the chain's windows like any other.
   // Off by default because ScheduleRetry has always been refused under feedback with InvalidArgument;
-  // without it, it still is.  No effect without load_feedback_window.
+  // without it, it still is.  No effect without load_feedback_window.  Together with
+  // feedback_fallbacks it also lets ScheduleRetryWithFallbacks run under the chain (see there).
   bool feedback_retries = false;
 };
 
@@ -242,9 +244,13 @@ class Scheduler {
   // attempts.  Goes through the retry lane like ScheduleRetry: a flush whose retry lane holds any such
   // caller makes one lig_schedule_batch_excluding_fallbacks call at the largest n asked in it, and plain
   // ScheduleRetry callers in it get the same picks.  Never through the doorbell; counted in
-  // Stats::retry_scheduled.  Errors are Schedule's.  InvalidArgument for n outside
-  // [1, LIG_MAX_FALLBACKS], more than LIG_MAX_EXCLUDED tried pods, load_feedback_window > 0 (there is
-  // no feedback-chain form of the call, whatever Options::feedback_retries says) and several devices.
+  // Stats::retry_scheduled.  Errors are Schedule's.  With load_feedback_window > 0 and both
+  // Options::feedback_retries and Options::feedback_fallbacks, that call is
+  // lig_schedule_batch_feedback_chain_excluding_fallbacks in place of the chain retry call: same picks
+  // and windows (rows add no load), rows from the reduced pool of the chain's load-adjusted copy, and a
+  // waiter refused on the host is left out of it.  InvalidArgument for n outside [1, LIG_MAX_FALLBACKS],
+  // more than LIG_MAX_EXCLUDED tried pods, load_feedback_window > 0 without both of those options, and
+  // several devices.
   Status ScheduleRetryWithFallbacks(const LLMRequest& req, const std::vector<backend::Pod>& tried, int n,
                                     std::vector<backend::Pod>* pods);
 

@@ -40,7 +40,8 @@ ligh_scheduler* ligh_scheduler_new_tree(ligh_provider*, int device, const int* d
 /* ligh_scheduler_new_tree plus Options::load_feedback_window (0 = off; > 0 flushes through
  * lig_schedule_batch_feedback_chain; refused with several devices or use_doorbell) and
  * Options::feedback_fallbacks (nonzero: the *WithFallbacks calls run under the chain) and
- * Options::feedback_retries (nonzero: ScheduleRetry runs under the chain). */
+ * Options::feedback_retries (nonzero: ScheduleRetry runs under the chain; with both nonzero,
+ * ScheduleRetryWithFallbacks does too). */
 ligh_scheduler* ligh_scheduler_new_feedback(ligh_provider*, int device, const int* devices, int n_devices,
                                             int max_pods, int max_adapters, int max_batch, int flush_size,
                                             int batch_window_us, int refresh_interval_ms, uint64_t seed,

@@ -1048,6 +1048,10 @@ static int create_impl(lig_ctx* c, int device, int max_pods, int max_adapters, i
   CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_count_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_count_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_count_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_count_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   const size_t need = scratch_bytes(words_for(max_pods)) > build_fixed_bytes(words_for(max_pods))
                           ? scratch_bytes(words_for(max_pods)) : build_fixed_bytes(words_for(max_pods));
   if (need > c->smem_optin)
@@ -2557,17 +2561,46 @@ struct FbReqs {
   int16_t* fallbacks = nullptr;          //   fallbacks + i * n_fallbacks
   int n_fallbacks = 0;
   bool retry = false;                    // a chain retry call: request i excludes the pods of
-  const int16_t* excluded = nullptr;     //   excluded + i * n_excluded
-  int n_excluded = 0;
+  const int16_t* excluded = nullptr;     //   excluded + i * n_excluded (with rows: a chain retry
+  int n_excluded = 0;                    //   call with fallback rows)
   size_t in_bytes() const { return models ? sizeof(uint32_t) : sizeof(lig_req); }
   size_t out_bytes() const { return models ? sizeof(lig_mpick) : sizeof(lig_pick); }
 };
 
+// Launch the chain segment of a retry call with fallback rows: x (R >= 1, device-visible, aligned
+// pointers) over the chain's scratch slot fs on st, with the scan's launch shape and the chain's tree
+// and thresholds; each LIG_OK pick is counted into the open window.  The caller checks the launch.
+static void launch_excluding_fallback_count(const lig_ctx* c, const Slot& fs, const FbRun& run,
+                                            const ExcludingCall& x, int n_fallbacks, int16_t* fallbacks,
+                                            cudaStream_t st) {
+  static const FilterTree kNoTree{};
+  const ScanShape sh = scan_shape(c, fs, x.R);
+  const SnapView v = view_of(fs);
+  const FilterTree& t = run.tree ? *run.tree : kNoTree;
+  const int4* in = reinterpret_cast<const int4*>(x.reqs);
+  int2* out = reinterpret_cast<int2*>(x.out);
+  auto launch = [&](auto staged, auto caller_tree) {
+    constexpr bool kS = decltype(staged)::value, kT = decltype(caller_tree)::value;
+    lig_schedule_excluding_fallback_count_kernel<kS, kT><<<sh.grid, kCtaThreads, sh.smem, st>>>(
+        v, run.thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, n_fallbacks, fallbacks, c->d_fb_hist);
+  };
+  using Y = std::true_type;
+  using N = std::false_type;
+  if (run.tree) {
+    if (sh.staged) launch(Y{}, Y{});
+    else launch(N{}, Y{});
+  } else {
+    if (sh.staged) launch(Y{}, N{});
+    else launch(N{}, N{});
+  }
+}
+
 // Schedule R requests through the window sequence: each segment is the rest of the open window or
 // of the call, whichever is shorter; one fused pick + count launch per segment (pick + row + count
 // when the call asked for rows); a filled window is closed at once, its tables are rebuilt only
-// when the next segment needs them.  A retry segment walks the tree over the scratch's pod columns
-// and reads no class table: it leaves them stale, so a later table-reading segment rebuilds once.
+// when the next segment needs them.  A retry segment (with or without rows) walks the tree over the
+// scratch's pod columns and reads no class table: it leaves them stale, so a later table-reading
+// segment rebuilds once.
 static int fb_schedule(lig_ctx* c, FbRun& run, uint64_t seed, const FbReqs& rq, int R, cudaStream_t st) {
   Slot& fs = c->fb_scratch;
   for (int pos = 0; pos < R;) {
@@ -2585,7 +2618,12 @@ static int fb_schedule(lig_ctx* c, FbRun& run, uint64_t seed, const FbReqs& rq, 
     void* out = static_cast<unsigned char*>(rq.out) + (size_t)pos * rq.out_bytes();
     const int grid = (n + kPickThreads * kCountPerThread - 1) / (kPickThreads * kCountPerThread);
     const uint4* fcls = reinterpret_cast<const uint4*>(fs.d_cls);
-    if (rq.retry) {
+    if (rq.retry && rq.rows) {
+      const ExcludingCall x{seed, static_cast<const lig_req*>(in), n, static_cast<lig_pick*>(out), rq.n_excluded,
+                            rq.excluded + (size_t)pos * (size_t)rq.n_excluded};
+      launch_excluding_fallback_count(c, fs, run, x, rq.n_fallbacks,
+                                      rq.fallbacks + (size_t)pos * (size_t)rq.n_fallbacks, st);
+    } else if (rq.retry) {
       const ExcludingCall x{seed, static_cast<const lig_req*>(in), n, static_cast<lig_pick*>(out), rq.n_excluded,
                             rq.excluded + (size_t)pos * (size_t)rq.n_excluded};
       launch_excluding(c, fs, run.thr, run.tree, x, c->d_fb_hist, st);
@@ -2763,7 +2801,8 @@ static int chain_admit(lig_ctx* c, const char* fn) {
   return fb_alloc_scratch(c);
 }
 
-// The row arguments of a chain fallback or retry call; 0 for a plain chain call.
+// The row arguments of a chain fallback or retry call, both sets for a retry call with fallback rows;
+// 0 for a plain chain call.
 static int chain_rows_check(const char* fn, const FbReqs& rq, int R) {
   if (rq.retry) {
     if (rq.n_excluded < 1 || rq.n_excluded > LIG_MAX_EXCLUDED)
@@ -2976,6 +3015,27 @@ int lig_schedule_batch_feedback_chain_excluding_device(lig_ctx* c, uint64_t epoc
   return chain_device(c, "lig_schedule_batch_feedback_chain_excluding_device", epoch, seed,
                       with_excluded(descriptor_reqs(d_reqs, d_out), d_excluded, n_excluded), R, window, d_loads,
                       stream);
+}
+
+int lig_schedule_batch_feedback_chain_excluding_fallbacks(lig_ctx* c, uint64_t epoch, uint64_t seed,
+                                                          const lig_req* reqs, int R, const int16_t* excluded,
+                                                          int n_excluded, lig_pick* out, int n_fallbacks,
+                                                          int16_t* fallbacks, int window, int32_t* loads) {
+  return chain_host(c, "lig_schedule_batch_feedback_chain_excluding_fallbacks", epoch, seed,
+                    with_rows(with_excluded(descriptor_reqs(reqs, out), excluded, n_excluded), n_fallbacks, fallbacks),
+                    R, window, loads);
+}
+
+int lig_schedule_batch_feedback_chain_excluding_fallbacks_device(lig_ctx* c, uint64_t epoch, uint64_t seed,
+                                                                 const lig_req* d_reqs, int R,
+                                                                 const int16_t* d_excluded, int n_excluded,
+                                                                 lig_pick* d_out, int n_fallbacks,
+                                                                 int16_t* d_fallbacks, int window,
+                                                                 int32_t* d_loads, void* stream) {
+  return chain_device(c, "lig_schedule_batch_feedback_chain_excluding_fallbacks_device", epoch, seed,
+                      with_rows(with_excluded(descriptor_reqs(d_reqs, d_out), d_excluded, n_excluded), n_fallbacks,
+                                d_fallbacks),
+                      R, window, d_loads, stream);
 }
 
 int lig_feedback_chain_reset(lig_ctx* c) {

@@ -3086,4 +3086,94 @@ lig_schedule_excluding_fallback_kernel(SnapView s, Thr thr, const __grid_constan
   }
 }
 
+// The chain segment of lig_schedule_batch_feedback_chain_excluding_fallbacks:
+// lig_schedule_excluding_fallback_kernel's walk, pick and row, step for step, on the chain's private
+// copy with the tree and thresholds the chain started with, plus lig_schedule_excluding_count_kernel's
+// count: lane 0 adds each LIG_OK pick to the open window's histogram (row entries add no load).  A
+// separate body, for the reason given at lig_schedule_excluding_count_kernel.
+template <bool kStaged, bool kTree>
+__global__ void __launch_bounds__(kCtaThreads)
+lig_schedule_excluding_fallback_count_kernel(SnapView s, Thr thr, const __grid_constant__ FilterTree tree,
+                                             const int4* reqs, const int16_t* excluded, int n_excluded, int2* out,
+                                             int R, uint64_t seed, int n_fallbacks, int16_t* fallbacks,
+                                             int* __restrict__ hist) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint32_t* X = reinterpret_cast<uint32_t*>(smem) + (size_t)warp * 3 * s.W;
+  uint32_t* T = X + s.W;
+  uint32_t* H = T + s.W;
+  Fields f{s.kv, s.q, s.n_active, s.max_active};
+  if constexpr (kStaged) {
+    f = stage_fields(s, smem + scratch_bytes(s.W));
+    __syncthreads();
+  }
+  for (int i = blockIdx.x * kWarpsPerCta + warp; i < R; i += gridDim.x * kWarpsPerCta) {
+    const int4 r = reqs[i];
+    const int ex = lane < n_excluded ? excluded[(size_t)i * n_excluded + lane] : -1;
+    const bool critical = ((uint32_t)r.y & LIG_REQ_CRITICAL) != 0;
+    const uint64_t key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
+    const uint32_t* Hrow = stage_adapter_row(s, r.x, H, lane);
+    for (int w = lane; w < s.W; w += 32) {
+      const int rem = s.P - w * 32;
+      T[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
+    }
+    __syncwarp();
+    if (ex >= 0 && ex < s.P) atomicAnd(T + (ex >> 5), ~(1u << (ex & 31)));
+    __syncwarp();
+    uint32_t n = 0;
+    for (int w = lane; w < s.W; w += 32) n += __popc(T[w]);
+    n = __reduce_add_sync(kFull, n);
+    EvalResult e;
+    if constexpr (kTree)
+      e = tree_walk_warp<kStaged, true>(f, tree.nodes, Hrow, critical, s.P, s.W, T, X, lane, n);
+    else
+      e = tree_eval_warp<kStaged, true>(f, Hrow, critical, thr, s.P, s.W, X, T, lane, n);
+    int pod = -1;
+    int16_t mine = -1;                 // row entry lane + 1
+    if (e.n > 0) {
+      uint32_t incl = 0;
+      const int groups = (s.W + 31) >> 5;
+      for (int g = 0; g < groups; ++g) {
+        const int w = g * 32 + lane;
+        const uint32_t cg = __reduce_add_sync(kFull, w < s.W ? __popc(e.mask[w]) : 0u);
+        if (lane == g) incl = cg;
+      }
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t t = __shfl_up_sync(kFull, incl, d);
+        if (lane >= d) incl += t;
+      }
+      uint64_t state = seed ^ key;
+      uint32_t pos[LIG_MAX_FALLBACKS], val[LIG_MAX_FALLBACKS];
+      pos[0] = int31n_next(state, e.n);
+      val[0] = 0u;
+      pod = warp_select_survivor(e.mask, s.W, incl, pos[0], lane);
+      const uint32_t m = e.status == (uint32_t)LIG_OK ? min(e.n, (uint32_t)n_fallbacks + 1u) : 0u;
+#pragma unroll
+      for (int j = 1; j <= LIG_MAX_FALLBACKS; ++j) {
+        if ((uint32_t)j >= m) break;
+        const uint32_t rj = (uint32_t)j + int31n_next(state, e.n - (uint32_t)j);
+        uint32_t a = (uint32_t)j, b = rj;
+#pragma unroll
+        for (int k = 0; k < j; ++k) {
+          if (pos[k] == (uint32_t)j) a = val[k];
+          if (pos[k] == rj) b = val[k];
+        }
+        const int p = warp_select_survivor(e.mask, s.W, incl, b, lane);
+        if (lane == j - 1) mine = (int16_t)p;
+        if (j < LIG_MAX_FALLBACKS) {
+          pos[j] = rj;
+          val[j] = a;
+        }
+      }
+    }
+    if (lane == 0) {
+      out[i] = make_int2(pod, (int)(e.status | (e.n << 16)));
+      if (pod >= 0) atomicAdd(hist + pod, 1);   // pod >= 0 only for LIG_OK
+    }
+    if (lane < n_fallbacks) fallbacks[(size_t)i * (size_t)n_fallbacks + lane] = mine;
+    __syncwarp();
+  }
+}
+
 }  // namespace lig

@@ -386,6 +386,41 @@ class Engine:
             self._ctx, epoch, seed, d_reqs or None, R, d_excluded or None, n_excluded, d_out or None, window,
             d_loads or None, stream or None))
 
+    def schedule_batch_feedback_chain_excluding_fallbacks(self, epoch: int, seed: int, reqs: np.ndarray,
+                                                          excluded: np.ndarray, n: int, window: int,
+                                                          loads: Optional[np.ndarray] = None):
+        """lig_schedule_batch_feedback_chain_excluding_fallbacks: (picks, int16 fallbacks of shape (R, n)); the
+        picks and loads are schedule_batch_feedback_chain_excluding's, row i ranks request i's reduced
+        survivor set on the chain's copy as schedule_batch_excluding_fallbacks ranks it on the epoch."""
+        assert reqs.dtype == REQ_DTYPE and reqs.flags.c_contiguous
+        assert excluded.dtype == np.int16 and excluded.flags.c_contiguous and excluded.ndim == 2
+        R = int(reqs.shape[0])
+        assert excluded.shape[0] == R
+        out = np.empty(R, dtype=PICK_DTYPE)
+        rows = np.empty((R, max(n, 0)), dtype=np.int16)
+        if loads is not None:
+            assert loads.dtype == np.int32 and loads.flags.c_contiguous
+        N.check(self._lib.lig_schedule_batch_feedback_chain_excluding_fallbacks(
+            self._ctx, epoch, seed, _ptr(reqs), R, _ptr(excluded), int(excluded.shape[1]), _ptr(out), n, _ptr(rows),
+            window, _ptr(loads) if loads is not None else None))
+        return out, rows
+
+    def schedule_batch_feedback_chain_excluding_fallbacks_ptr(self, epoch: int, seed: int, h_reqs: int, R: int,
+                                                              h_excluded: int, n_excluded: int, h_out: int, n: int,
+                                                              h_fallbacks: int, window: int, h_loads: int = 0) -> None:
+        N.check(self._lib.lig_schedule_batch_feedback_chain_excluding_fallbacks(
+            self._ctx, epoch, seed, h_reqs or None, R, h_excluded or None, n_excluded, h_out or None, n,
+            h_fallbacks or None, window, h_loads or None))
+
+    def schedule_batch_feedback_chain_excluding_fallbacks_device(self, epoch: int, seed: int, d_reqs: int, R: int,
+                                                                 d_excluded: int, n_excluded: int, d_out: int, n: int,
+                                                                 d_fallbacks: int, window: int, d_loads: int = 0,
+                                                                 stream: int = 0) -> None:
+        """Device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_batch_feedback_chain_excluding_fallbacks_device(
+            self._ctx, epoch, seed, d_reqs or None, R, d_excluded or None, n_excluded, d_out or None, n,
+            d_fallbacks or None, window, d_loads or None, stream or None))
+
     def schedule_models_batch_fallbacks(self, epoch: int, seed: int, model_ids: np.ndarray, n: int,
                                         first_index: int = 0):
         """lig_schedule_models_batch_fallbacks: (picks, int16 fallbacks (R, n)), the picks those of

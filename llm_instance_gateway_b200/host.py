@@ -162,7 +162,7 @@ class HostScheduler:
             # Options::filter (a scheduling.Filter chart or a node table),
             # Options::load_feedback_window (load feedback carried across flushes, 0 = off) and
             # Options::feedback_fallbacks / feedback_retries (the *WithFallbacks calls and ScheduleRetry
-            # under that feedback)
+            # under that feedback; with both, ScheduleRetryWithFallbacks too)
             from .engine import _node_table
             nodes, n = _node_table(filter)
             devs = list(devices) if devices is not None else []
@@ -232,7 +232,8 @@ class HostScheduler:
     def ScheduleRetryWithFallbacks(self, resolved: str, critical: bool, tried: Sequence[Pod], n: int
                                    ) -> Tuple[int, List[str], str]:  # noqa: N802
         """Scheduler::ScheduleRetryWithFallbacks: ScheduleRetry plus up to n fallback pods of the same reduced
-        pool: (gRPC code, pod names [pick, fallbacks in retry order], error)."""
+        pool: (gRPC code, pod names [pick, fallbacks in retry order], error).  Under load_feedback_window it
+        needs both feedback_retries and feedback_fallbacks, and then runs on the feedback chain."""
         cap = 64 * 1024
         names, err, k = C.create_string_buffer(cap), C.create_string_buffer(512), C.c_int(0)
         code = self._lib.ligh_schedule_retry_with_fallbacks(self._s, resolved.encode(), int(critical),

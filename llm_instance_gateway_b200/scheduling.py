@@ -24,8 +24,9 @@ schedule a request again without the pods it already tried, as Schedule would on
 (lig_schedule_batch_excluding); under load_feedback_window they need ``feedback_retries=True`` and then run as
 feedback-chain calls.  ``ScheduleRetryWithFallbacks`` / ``ScheduleBatchRetryWithFallbacks`` return the retry's
 pick followed by up to n more distinct survivors of the reduced pool (lig_schedule_batch_excluding_fallbacks), so
-one call serves several attempts; they have no feedback-chain form.  There is no CPU path here: without liblig.so or without a CUDA device construction
-fails.
+one call serves several attempts; under load_feedback_window they need both ``feedback_retries=True`` and
+``feedback_fallbacks=True`` and then run as feedback-chain calls whose rows rank the chain's reduced pool.  There is
+no CPU path here: without liblig.so or without a CUDA device construction fails.
 """
 from __future__ import annotations
 
@@ -490,15 +491,23 @@ class Scheduler:
         (pods, error) per request, pods[0] the pod ScheduleBatchRetry would have returned, then distinct
         survivors of the same reduced pool in the order a proxy should try them, none of them tried.
         Tried pods, the rand_key sequence and errors as ScheduleBatchRetry.  ValueError for n outside
-        [1, LIG_MAX_FALLBACKS], more than LIG_MAX_EXCLUDED tried pods, and under load_feedback_window
-        (there is no feedback-chain form of this call)."""
-        if self._window:
-            raise ValueError("retries with fallbacks are not defined under load_feedback_window: the picks come "
-                             "from the feedback chain's load-adjusted copy of the snapshot, these would not")
+        [1, LIG_MAX_FALLBACKS] and more than LIG_MAX_EXCLUDED tried pods.  Under load_feedback_window the
+        call is a feedback-chain call (lig_schedule_batch_feedback_chain_excluding_fallbacks: the picks and
+        loads are ScheduleBatchRetry's chain call's, the rows rank the reduced pool of the chain's
+        load-adjusted copy) when the scheduler was built with both feedback_retries=True and
+        feedback_fallbacks=True, and raises ValueError otherwise."""
+        if self._window and not (self._feedback_retries and self._feedback_fallbacks):
+            raise ValueError("retries with fallbacks are not defined under load_feedback_window without "
+                             "feedback_retries and feedback_fallbacks: the picks come from the feedback chain's "
+                             "load-adjusted copy of the snapshot, these would not")
         if not 1 <= n <= N.LIG_MAX_FALLBACKS:
             raise ValueError(f"n must be in [1, {N.LIG_MAX_FALLBACKS}], got {n}")
         snap, arr, excluded = self._retry_batch(reqs, tried_lists)
-        picks, rows = self._engine.schedule_batch_excluding_fallbacks(self._epoch, self._seed, arr, excluded, n)
+        if self._window:
+            picks, rows = self._engine.schedule_batch_feedback_chain_excluding_fallbacks(
+                self._epoch, self._seed, arr, excluded, n, self._window)
+        else:
+            picks, rows = self._engine.schedule_batch_excluding_fallbacks(self._epoch, self._seed, arr, excluded, n)
         return [([snap.pods[int(pk["pod_idx"])]] + [snap.pods[int(p)] for p in row if p >= 0], None)
                 if pk["status"] == N.LIG_OK else ([], _schedule_error(int(pk["status"])))
                 for pk, row in zip(picks, rows)]
@@ -596,6 +605,10 @@ def NewScheduler(pmp: PodMetricsProvider, filter: Optional[Filter] = None, load_
     feedback_retries: under load_feedback_window, let ScheduleRetry / ScheduleBatchRetry run as chain calls
     (lig_schedule_batch_feedback_chain_excluding): each retry is scheduled on the chain's load-adjusted copy
     without the pods it tried, and its pick loads the chain like any other; without it they raise
-    ValueError there, as they always have."""
+    ValueError there, as they always have.
+    With both feedback_fallbacks and feedback_retries, ScheduleRetryWithFallbacks /
+    ScheduleBatchRetryWithFallbacks run as chain calls too
+    (lig_schedule_batch_feedback_chain_excluding_fallbacks); with either one alone they raise ValueError
+    under load_feedback_window."""
     return Scheduler(pmp, filter=filter, load_feedback_window=load_feedback_window,
                      feedback_fallbacks=feedback_fallbacks, feedback_retries=feedback_retries, **kw)
