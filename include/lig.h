@@ -236,6 +236,41 @@ int lig_update_snapshot(lig_ctx* ctx, uint64_t new_epoch, uint64_t base_epoch, i
                         const uint16_t* n_active, const uint16_t* max_active,
                         const int32_t* adapter_offsets, const int32_t* adapter_ids);
 
+/* ---- outlier ejection: schedule as if some pods had left the provider ----------------------------
+ * A proxy that finds a pod refusing connections can keep it out of every later pick until it lets it
+ * back, without waiting for the pod to leave the provider (readiness probes take seconds, and a dead
+ * pod's scrape fails, so the provider keeps its last, often attractive, metrics).
+ *
+ * `new_epoch` becomes `base_epoch`'s snapshot (which must be resident and stays so, untouched) with
+ * pod_idx[0 .. n) left out of the pool.  It keeps base's metric columns, bitmap, P, A and pod order.
+ * On it, every call returns byte for byte what it returns on an epoch uploaded from the literally
+ * reduced snapshot (the kept pods' columns in order, the ejected pods' bitmap columns dropped, A
+ * unchanged), built with the filter tree and thresholds in force at this call, with every pod index
+ * of the results (pod_idx, survivor lists, fallback rows, loads) mapped back to base's order.  The
+ * mapping keeps order, so picks, rankings and lists keep their definitions.  That covers the plain,
+ * queue, persistent and model-id picks, the doorbell, lig_filter_*, lig_read_class, the fallback
+ * calls, the in-batch feedback call and every chain call (the chain's private copy carries the
+ * pool: an ejected pod gets no pick and a load of 0).  A retry's pool is the epoch's pool minus the
+ * request's row; a row entry that names an ejected pod leaves out nothing more.  Ejecting every pod
+ * is legal: every call then gets the tree's answer for an empty slice (under the built-in tree
+ * LIG_DROP for every request, as for an empty retry pool).
+ *
+ * The set carried by an epoch: the listed set REPLACES base's (n = 0 derives an epoch with every pod
+ * back); lig_update_snapshot from an ejected base keeps base's set; full uploads
+ * (lig_upload_snapshot[_async|_device], lig_comm_*, lig_group_upload_snapshot) start with none;
+ * lig_set_thresholds rebuilds keep it.  Like every snapshot writer, the new epoch has no model
+ * table until lig_upload_models.  The direct scan (lig_schedule_scan[_device]) returns
+ * LIG_ERR_INVALID for an epoch with ejected pods.  Ranks of a communicator eject the same pods each
+ * on its own ctx.
+ *
+ * Only the pool mask crosses PCIe: the base blob is copied device-to-device and the class tables are
+ * rebuilt from the pool.  Blocks like lig_update_snapshot, takes the upload lock and waits for the
+ * readers of the slot it overwrites.  Refused with nothing written, both resident epochs as they
+ * were: LIG_ERR_INVALID for new_epoch == base_epoch, n < 0, n > P, a null list with n > 0, an index
+ * outside [0, P) or listed twice, and when base is the slot the new epoch would overwrite (the rule
+ * of lig_update_snapshot); LIG_ERR_STALE_EPOCH / LIG_ERR_NO_SNAPSHOT when base is not resident. */
+int lig_eject_pods(lig_ctx* ctx, uint64_t new_epoch, uint64_t base_epoch, const int32_t* pod_idx, int n);
+
 /* Same, but the packed blob is already in HBM (e.g. the receive buffer of an NCCL broadcast of
  * the snapshot).  The blob is copied into the ctx on `stream` (a cudaStream_t, may be NULL =
  * legacy default stream); table build is enqueued on the same stream, nothing is synchronised.

@@ -58,6 +58,7 @@ EXPORTED_SYMBOLS = (
     "lig_schedule_batch_excluding_fallbacks", "lig_schedule_batch_excluding_fallbacks_device",
     "lig_schedule_batch_feedback_chain_excluding_fallbacks",
     "lig_schedule_batch_feedback_chain_excluding_fallbacks_device",
+    "lig_eject_pods",
 )
 
 
@@ -194,6 +195,7 @@ def load() -> C.CDLL:
     lib.lig_schedule_batch_feedback_chain_excluding_fallbacks_device.argtypes = [vp, u64, u64, vp, i32, vp, i32, vp,
                                                                                  i32, vp, i32, vp, vp]
     lib.lig_update_snapshot.argtypes = [vp, u64, u64, i32, vp, vp, vp, vp, vp, vp, vp]
+    lib.lig_eject_pods.argtypes = [vp, u64, u64, vp, i32]
     lib.lig_pick_kernel_info.argtypes = [vp, u64, C.c_char_p, i32, C.POINTER(i32), C.POINTER(i32),
                                          C.POINTER(i32), C.POINTER(i32)]
     lib.lig_last_pick_launch.argtypes = [vp, C.POINTER(LigLaunchInfo)]

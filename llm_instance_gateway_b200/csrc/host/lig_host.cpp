@@ -7,6 +7,7 @@
 #include <cstdio>
 #include <cstring>
 #include <random>
+#include <unordered_set>
 
 #include "../../../include/lig.h"
 
@@ -262,41 +263,24 @@ Status Scheduler::RefreshImpl(const std::shared_ptr<const ModelList>& models) {
                                                 ma16.data(), bitmap.data());
     if (rc != 0) return LigFailure(group_ ? "lig_group_upload_snapshot" : "lig_upload_snapshot");
   }
-  // The model table goes into the new epoch before the epoch is published, so a flush that captures
-  // the epoch always finds the table its names were mapped against.
-  if (models) {
-    PackedModelTable& t = packed_models_;
-    if (t.list != models || t.adapter_ids != snap->adapter_ids) {
-      const size_t n = models->models.size();
-      t.target_offsets.assign(n + 1, 0);
-      t.target_adapter_ids.clear();
-      t.target_weights.clear();
-      t.self_adapter_ids.resize(n);
-      t.critical.resize(n);
-      // a name no pod lists, or one interned after this epoch's table (>= A), is id A: no pod matches
-      auto intern = [&](const std::string& name) {
-        auto it = snap->adapter_ids->find(name);
-        return (it == snap->adapter_ids->end() || it->second >= A) ? A : it->second;
-      };
-      for (size_t m = 0; m < n; ++m) {
-        const backend::InferenceModel& im = *models->models[m];
-        t.critical[m] = im.Critical ? 1 : 0;
-        t.self_adapter_ids[m] = intern(im.ModelName);
-        if (models->present[m])
-          for (const backend::TargetModel& tm : im.TargetModels) {
-            t.target_adapter_ids.push_back(intern(tm.Name));
-            t.target_weights.push_back(tm.Weight);
-          }
-        t.target_offsets[m + 1] = (int32_t)t.target_adapter_ids.size();
-      }
-      t.list = models;
-      t.adapter_ids = snap->adapter_ids;
+  // The ejected set: a delta epoch inherits its base's; when that is not the set EjectPods asks for on
+  // this tick's pods (a full upload has none, or the pods moved), one more epoch is derived from it.
+  snap->ejected = used_delta ? prev_ejected_ : std::vector<int32_t>{};
+  bool derived = false;
+  {
+    std::vector<int32_t> want = EjectedIndices(snap->pods);
+    if (want != snap->ejected) {
+      const uint64_t e = next_epoch_++;
+      if (lig_eject_pods(ctx_, e, snap->epoch, want.data(), (int)want.size()) != 0) return LigFailure("lig_eject_pods");
+      snap->epoch = e;
+      snap->ejected = std::move(want);
+      derived = true;
     }
-    if (lig_upload_models(ctx_, snap->epoch, (int)models->models.size(), t.target_offsets.data(),
-                          t.target_adapter_ids.data(), t.target_weights.data(), t.critical.data(),
-                          t.self_adapter_ids.data(), models->present.data()) != 0)
-      return LigFailure("lig_upload_models");
   }
+  // The model table goes into the published epoch before it is published, so a flush that captures
+  // the epoch always finds the table its names were mapped against.
+  if (models)
+    if (Status st = UploadModelTable(*snap, models); !st.ok()) return st;
   snap->models = models;
   prev_kv_ = kv;
   prev_q_ = q32;
@@ -305,6 +289,8 @@ Status Scheduler::RefreshImpl(const std::shared_ptr<const ModelList>& models) {
   prev_A_ = A;
   reset_base.base = nullptr;
   prev_epoch_ = snap->epoch;
+  prev_ejected_ = snap->ejected;
+  const uint64_t n_ejected = snap->ejected.size();
   {
     std::lock_guard<std::mutex> lk(snap_mu_);
     snap_ = std::move(snap);
@@ -315,8 +301,93 @@ Status Scheduler::RefreshImpl(const std::shared_ptr<const ModelList>& models) {
   stats_.delta_refreshes += used_delta ? 1 : 0;
   stats_.last_dirty_pods = comparable ? dirty.size() : (uint64_t)P;
   stats_.excluded_pods = excluded;
+  stats_.ejected_pods = n_ejected;
+  stats_.eject_publishes += derived ? 1 : 0;
   stats_.last_pack_us = std::chrono::duration<double, std::micro>(t_packed - t_begin).count();
   stats_.last_upload_us = std::chrono::duration<double, std::micro>(t_done - t_packed).count();
+  return Status{};
+}
+
+Status Scheduler::UploadModelTable(const Snapshot& snap, const std::shared_ptr<const ModelList>& models) {
+  const int A = snap.A;
+  PackedModelTable& t = packed_models_;
+  if (t.list != models || t.adapter_ids != snap.adapter_ids) {
+    const size_t n = models->models.size();
+    t.target_offsets.assign(n + 1, 0);
+    t.target_adapter_ids.clear();
+    t.target_weights.clear();
+    t.self_adapter_ids.resize(n);
+    t.critical.resize(n);
+    // a name no pod lists, or one interned after this epoch's table (>= A), is id A: no pod matches
+    auto intern = [&](const std::string& name) {
+      auto it = snap.adapter_ids->find(name);
+      return (it == snap.adapter_ids->end() || it->second >= A) ? A : it->second;
+    };
+    for (size_t m = 0; m < n; ++m) {
+      const backend::InferenceModel& im = *models->models[m];
+      t.critical[m] = im.Critical ? 1 : 0;
+      t.self_adapter_ids[m] = intern(im.ModelName);
+      if (models->present[m])
+        for (const backend::TargetModel& tm : im.TargetModels) {
+          t.target_adapter_ids.push_back(intern(tm.Name));
+          t.target_weights.push_back(tm.Weight);
+        }
+      t.target_offsets[m + 1] = (int32_t)t.target_adapter_ids.size();
+    }
+    t.list = models;
+    t.adapter_ids = snap.adapter_ids;
+  }
+  if (lig_upload_models(ctx_, snap.epoch, (int)models->models.size(), t.target_offsets.data(),
+                        t.target_adapter_ids.data(), t.target_weights.data(), t.critical.data(),
+                        t.self_adapter_ids.data(), models->present.data()) != 0)
+    return LigFailure("lig_upload_models");
+  return Status{};
+}
+
+std::vector<int32_t> Scheduler::EjectedIndices(const std::vector<backend::Pod>& pods) const {
+  std::vector<int32_t> idx;
+  if (ejected_.empty()) return idx;
+  std::unordered_set<std::string> gone;                 // Name + '\0' + Address, as the retry lane matches
+  for (const backend::Pod& p : ejected_) gone.insert(p.Name + '\0' + p.Address);
+  for (size_t p = 0; p < pods.size(); ++p)
+    if (gone.count(pods[p].Name + '\0' + pods[p].Address)) idx.push_back((int32_t)p);
+  return idx;
+}
+
+Status Scheduler::EjectPods(const std::vector<backend::Pod>& pods) {
+  if (group_)
+    return Errorf(InvalidArgument, "EjectPods: a scheduler over several devices has no ejection call (lig_group)");
+  std::lock_guard<std::mutex> rk(refresh_mu_);
+  ejected_ = pods;
+  std::shared_ptr<const Snapshot> cur;
+  {
+    std::lock_guard<std::mutex> lk(snap_mu_);
+    cur = snap_;
+  }
+  if (!cur) return Status{};                            // the first refresh applies the set
+  std::vector<int32_t> want = EjectedIndices(cur->pods);
+  if (want != cur->ejected) {
+    // derived from the published epoch, the newest resident one: the slot it overwrites is the other
+    auto snap = std::make_shared<Snapshot>(*cur);
+    snap->epoch = next_epoch_++;
+    if (lig_eject_pods(ctx_, snap->epoch, cur->epoch, want.data(), (int)want.size()) != 0)
+      return LigFailure("lig_eject_pods");
+    if (snap->models)
+      if (Status st = UploadModelTable(*snap, snap->models); !st.ok()) return st;
+    snap->ejected = std::move(want);
+    if (prev_epoch_ == cur->epoch) {                    // same columns: the next delta starts from it
+      prev_epoch_ = snap->epoch;
+      prev_ejected_ = snap->ejected;
+    }
+    const uint64_t n = snap->ejected.size();
+    {
+      std::lock_guard<std::mutex> lk(snap_mu_);
+      snap_ = std::move(snap);
+    }
+    std::lock_guard<std::mutex> sk(stats_mu_);
+    stats_.ejected_pods = n;
+    stats_.eject_publishes++;
+  }
   return Status{};
 }
 

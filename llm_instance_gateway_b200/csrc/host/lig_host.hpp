@@ -189,6 +189,8 @@ struct Stats {
   uint64_t model_batches = 0;      // device calls issued for model-id requests
   uint64_t fallback_scheduled = 0; // ScheduleWithFallbacks and ScheduleModelWithFallbacks calls completed
   uint64_t retry_scheduled = 0;    // ScheduleRetry and ScheduleRetryWithFallbacks calls completed
+  uint64_t ejected_pods = 0;       // pods of the current snapshot left out of the pool (EjectPods)
+  uint64_t eject_publishes = 0;    // epochs derived with lig_eject_pods and published
   double last_pack_us = 0;     // last Refresh: provider slice -> columns + bitmap (host)
   double last_upload_us = 0;   // last Refresh: lig_upload_snapshot (H2D + class tables)
   double max_device_call_us = 0;   // slowest single lig_schedule_batch call (launch + kernel + synchronise)
@@ -308,6 +310,15 @@ class Scheduler {
   // previous epoch for scheduling but not as a delta base: the per-pod memo has already moved to the
   // refused tick, so the next refresh uploads in full.
   Status Refresh();
+
+  // Outlier ejection: schedule as if `pods` had left the provider, until a later call lets them back.
+  // `pods` is the complete ejected set (an empty list lets every pod back), matched by value (Name +
+  // Address) against the snapshot; pods it does not hold are ignored.  Before it returns, a derived
+  // epoch (lig_eject_pods, with the model table when a list is set) is published, so every Schedule*
+  // call that starts after the return avoids the ejected pods.  Every later refresh keeps them out: a
+  // delta tick inherits the set, and after a full upload (or when the pods' positions moved) one more
+  // epoch is derived and published.  Single device only (InvalidArgument otherwise).
+  Status EjectPods(const std::vector<backend::Pod>& pods);
  private:
   struct ModelList;
   Status RefreshImpl(const std::shared_ptr<const ModelList>& models);
@@ -329,6 +340,7 @@ class Scheduler {
     std::shared_ptr<const InternTable> adapter_ids;   // shared between snapshots until a name is added
     std::vector<backend::Pod> pods;
     std::shared_ptr<const ModelList> models;          // the list this epoch's model table was packed from
+    std::vector<int32_t> ejected;                     // pods left out of this epoch's pool (ascending)
   };
   // The list SetInferenceModels accepted: dense model id -> InferenceModel, and the name map.
   struct ModelList {
@@ -336,6 +348,10 @@ class Scheduler {
     std::unordered_map<std::string, uint32_t> ids;    // Spec.ModelName -> model id
     std::vector<uint8_t> present;                     // 0: weights sum to <= 0, no target can be drawn
   };
+  // EjectPods' set as indices into `pods` (ascending); caller holds refresh_mu_
+  std::vector<int32_t> EjectedIndices(const std::vector<backend::Pod>& pods) const;
+  // pack (when the list or the adapter ids changed) and upload the model table into snap.epoch
+  Status UploadModelTable(const Snapshot& snap, const std::shared_ptr<const ModelList>& models);
   // The last model table packed for lig_upload_models, reused while neither the list nor the
   // adapter-id table changed (guarded by refresh_mu_).
   struct PackedModelTable {
@@ -357,6 +373,8 @@ class Scheduler {
   std::vector<uint16_t> prev_na_, prev_ma_;
   int prev_A_ = -1;
   uint64_t prev_epoch_ = 0;
+  std::vector<int32_t> prev_ejected_;         // the pods prev_epoch_ left out: a delta from it inherits them
+  std::vector<backend::Pod> ejected_;         // EjectPods' set (guarded by refresh_mu_)
   std::atomic<uint64_t> model_draws_{0};
   std::shared_ptr<InternTable> intern_;
   std::vector<PodMemo> memo_;

@@ -335,6 +335,21 @@ int ligh_schedule_retry_with_fallbacks(ligh_scheduler* s, const char* resolved, 
 
 uint64_t ligh_retry_scheduled(ligh_scheduler* s) { return s->sched->stats().retry_scheduled; }
 
+int ligh_eject_pods(ligh_scheduler* s, const char* const* names, const char* const* addrs, int n, char* err,
+                    int err_cap) {
+  std::vector<backend::Pod> pods;
+  for (int i = 0; i < n; ++i) pods.push_back(backend::Pod{names[i] ? names[i] : "", addrs[i] ? addrs[i] : ""});
+  scheduling::Status st = s->sched->EjectPods(pods);
+  if (!st.ok()) put(err, err_cap, st.message);
+  return st.code;
+}
+
+void ligh_eject_stats(ligh_scheduler* s, uint64_t out[2]) {
+  scheduling::Stats st = s->sched->stats();
+  out[0] = st.ejected_pods;
+  out[1] = st.eject_publishes;
+}
+
 int ligh_filter(ligh_scheduler* s, const char* resolved, int critical, char* names, int names_cap, int* n_pods,
                 char* err, int err_cap) {
   scheduling::LLMRequest req;

@@ -73,6 +73,11 @@ int ligh_schedule_retry_with_fallbacks(ligh_scheduler*, const char* resolved_tar
                                        const char* const* tried_names, const char* const* tried_addrs, int n_tried,
                                        int n, char* names, int names_cap, int* n_pods, char* err, int err_cap);
 uint64_t ligh_retry_scheduled(ligh_scheduler*);      /* Stats::retry_scheduled */
+/* Scheduler::EjectPods: the complete ejected set as n (name, address) pairs (n = 0 lets every pod back);
+ * returns the gRPC code, err receives the refusal. */
+int ligh_eject_pods(ligh_scheduler*, const char* const* names, const char* const* addrs, int n, char* err,
+                    int err_cap);
+void ligh_eject_stats(ligh_scheduler*, uint64_t out[2]);  /* Stats::ejected_pods, Stats::eject_publishes */
 int ligh_refresh(ligh_scheduler*, char* err, int err_cap);
 /* several GPUs behind one scheduler (lig_group_*) */
 ligh_scheduler* ligh_scheduler_new_devices(ligh_provider*, const int* devices, int n_devices, int max_pods,

@@ -109,6 +109,10 @@ struct Slot {
   uint64_t stamp = 0;               // upload order, to pick the slot to overwrite
   bool caller_tree = false;         // tables built with a caller filter tree (thresholds do not apply)
   FilterTree tree{};                // that tree (caller_tree only): the retry walk runs the epoch's own tree
+  // lig_eject_pods: the epoch's pool, W words (bit p = pod p is in it), read only when n_ejected > 0.
+  // Every class-table build and retry walk of the slot starts from it instead of every pod.
+  uint32_t* d_pool = nullptr;
+  int n_ejected = 0;
 };
 
 constexpr int kLanes = 8;   // streams of the host-buffer path; also the queue streams
@@ -277,12 +281,15 @@ int note_reader(Slot& s, cudaStream_t st) {
   return 0;
 }
 
-// The direct scan restates the built-in tree only: it refuses an epoch whose class tables a caller
-// filter tree built (lig_read_class reads those survivor sets).
+// The direct scan restates the built-in tree over every pod only: it refuses an epoch whose class
+// tables a caller filter tree built (lig_read_class reads those survivor sets) or that has ejected pods.
 int check_scannable(const Slot& s, uint64_t epoch) {
   if (s.caller_tree)
     return fail(LIG_ERR_INVALID, "direct scan: epoch %llu was built with a caller filter tree; the scan "
                                  "walks the built-in tree only", (unsigned long long)epoch);
+  if (s.n_ejected > 0)
+    return fail(LIG_ERR_INVALID, "direct scan: epoch %llu has ejected pods; the scan walks every pod",
+                (unsigned long long)epoch);
   return 0;
 }
 
@@ -305,6 +312,9 @@ int launch_class_build(lig_ctx* c, Slot& s, cudaStream_t stream, const FilterTre
   const Thr th = thr ? *thr : thr_of(c);
   const int n_classes = 2 * (s.A + 1);
   const int W = s.W > 0 ? s.W : 1;
+  // an epoch with ejected pods builds from its pool (the pool forms of the three builds)
+  const bool pooled = s.n_ejected > 0;
+  const int n_pool = s.P - s.n_ejected;
   s.caller_tree = tree != nullptr;
   if (tree) {
     s.tree = *tree;
@@ -313,12 +323,20 @@ int launch_class_build(lig_ctx* c, Slot& s, cudaStream_t stream, const FilterTre
     const size_t smem = tree_fixed_bytes(W) + (staged ? staged_bytes(W) : 0);
     int per_sm = 0;
     CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(
-        &per_sm, staged ? lig_class_build_tree_kernel<true> : lig_class_build_tree_kernel<false>, kCtaThreads, smem));
+        &per_sm, pooled ? (staged ? lig_class_build_tree_kernel<true, true> : lig_class_build_tree_kernel<false, true>)
+                        : (staged ? lig_class_build_tree_kernel<true> : lig_class_build_tree_kernel<false>),
+        kCtaThreads, smem));
     int grid = (n_classes + kWarpsPerCta - 1) / kWarpsPerCta;
     if (grid > c->sm_count * (per_sm > 0 ? per_sm : 1)) grid = c->sm_count * (per_sm > 0 ? per_sm : 1);
     const CompactOut co{s.d_ctab, s.d_counters, s.ctab_pool_capacity, s.d_hdr_alias, nullptr};
     const int stride = s.P > 0 ? s.P : 1;
-    if (staged)
+    if (pooled && staged)
+      lig_class_build_tree_kernel<true, true><<<grid, kCtaThreads, smem, stream>>>(v, *tree, s.d_cls, s.d_lists, stride, co,
+                                                                                  s.d_pool, n_pool);
+    else if (pooled)
+      lig_class_build_tree_kernel<false, true><<<grid, kCtaThreads, smem, stream>>>(v, *tree, s.d_cls, s.d_lists, stride, co,
+                                                                                   s.d_pool, n_pool);
+    else if (staged)
       lig_class_build_tree_kernel<true><<<grid, kCtaThreads, smem, stream>>>(v, *tree, s.d_cls, s.d_lists, stride, co);
     else
       lig_class_build_tree_kernel<false><<<grid, kCtaThreads, smem, stream>>>(v, *tree, s.d_cls, s.d_lists, stride, co);
@@ -347,15 +365,26 @@ int launch_class_build(lig_ctx* c, Slot& s, cudaStream_t stream, const FilterTre
     dbg[7] = 0;
   }
   const CompactOut co{s.d_ctab, s.d_counters, s.ctab_pool_capacity, s.d_hdr_alias, dbg};
+  // an empty pool takes the general build's early path (every class LIG_DROP)
   const bool fast = c->fast_build && s.P > 0 && W <= kFastMaxWords &&
-                    fast_fixed_bytes(W) + staged_bytes(W) <= c->smem_optin;
+                    fast_fixed_bytes(W) + staged_bytes(W) <= c->smem_optin && (!pooled || n_pool > 0);
   if (fast) {
     // pools of up to 4096 pods: register-resident shared stages, one class per warp up to
     // 8 * SMs adapters, several per warp (round-robin) beyond
     int fgrid = (n_classes + kBuildWarps - 1) / kBuildWarps;
     if (fgrid > c->sm_count) fgrid = c->sm_count;
-    lig_class_build_fast_kernel<<<fgrid, kBuildThreads, fast_fixed_bytes(W) + staged_bytes(W), stream>>>(
-        v, th, s.d_cls, s.d_lists, stride, co);
+    if (pooled)
+      lig_class_build_fast_kernel<true><<<fgrid, kBuildThreads, fast_fixed_bytes(W) + staged_bytes(W), stream>>>(
+          v, th, s.d_cls, s.d_lists, stride, co, s.d_pool, n_pool);
+    else
+      lig_class_build_fast_kernel<<<fgrid, kBuildThreads, fast_fixed_bytes(W) + staged_bytes(W), stream>>>(
+          v, th, s.d_cls, s.d_lists, stride, co);
+  } else if (pooled && staged) {
+    lig_class_build_kernel<true, true><<<grid, kBuildThreads, smem, stream>>>(v, th, s.d_cls, s.d_lists, stride, co,
+                                                                             s.d_pool, n_pool);
+  } else if (pooled) {
+    lig_class_build_kernel<false, true><<<grid, kBuildThreads, smem, stream>>>(v, th, s.d_cls, s.d_lists, stride, co,
+                                                                              s.d_pool, n_pool);
   } else if (staged) {
     lig_class_build_kernel<true><<<grid, kBuildThreads, smem, stream>>>(v, th, s.d_cls, s.d_lists, stride, co);
   } else {
@@ -863,6 +892,8 @@ int begin_write(lig_ctx* c, uint64_t epoch, int P, int A, cudaStream_t stream, b
     Slot& s = victim_slot(c, epoch);
     s.valid = false;                       // evicted: schedule calls on its old epoch now get STALE_EPOCH
     s.models_valid = false;                // the model table is interned against the old snapshot
+    s.n_ejected = 0;                       // full uploads start with every pod; lig_update_snapshot and
+                                           // lig_eject_pods set the set after begin_write
     rc = wait_readers(s, st);              // batches still reading the old content
     if (!rc && cudaStreamWaitEvent(st, s.ready, 0) != cudaSuccess)   // an earlier device-side upload of this slot
       rc = fail(LIG_ERR_CUDA, "cudaStreamWaitEvent failed");
@@ -990,6 +1021,7 @@ static int alloc_slot(lig_ctx* c, Slot& s) {
     CUDA_TRY(cudaMalloc(&s.d_counters, 2 * sizeof(uint32_t)));
     CUDA_TRY(cudaMemset(s.d_counters, 0, 2 * sizeof(uint32_t)));
   }
+  CUDA_TRY(cudaMalloc(&s.d_pool, (size_t)(words_for(c->max_pods) > 0 ? words_for(c->max_pods) : 1) * sizeof(uint32_t)));
   CUDA_TRY(cudaHostAlloc(&s.h_blob, l.total, cudaHostAllocDefault));
   CUDA_TRY(cudaEventCreateWithFlags(&s.ready, cudaEventDisableTiming));
   CUDA_TRY(cudaEventCreateWithFlags(&s.models_ready, cudaEventDisableTiming));
@@ -1003,6 +1035,7 @@ static void free_slot(Slot& s) {
   cudaFree(s.d_lists);
   cudaFree(s.d_ctab);
   cudaFree(s.d_counters);
+  cudaFree(s.d_pool);
   cudaFree(s.d_mtab);
   if (s.h_mtab) cudaFreeHost(s.h_mtab);
   if (s.models_ready) cudaEventDestroy(s.models_ready);
@@ -1029,9 +1062,15 @@ static int create_impl(lig_ctx* c, int device, int max_pods, int max_adapters, i
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_class_build_kernel<false>,
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  CUDA_TRY(cudaFuncSetAttribute(lig_class_build_fast_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_class_build_fast_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_class_build_tree_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_class_build_tree_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  // the pool forms (epochs derived by lig_eject_pods)
+  CUDA_TRY(cudaFuncSetAttribute(lig_class_build_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_class_build_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_class_build_fast_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_class_build_tree_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  CUDA_TRY(cudaFuncSetAttribute(lig_class_build_tree_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_scan_kernel<true>,
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_scan_kernel<false>,
@@ -1052,6 +1091,17 @@ static int create_impl(lig_ctx* c, int device, int max_pods, int max_adapters, i
   CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_count_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_count_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_count_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  const void* pool_forms[] = {   // the pool forms of the four retry kernels, every (staged, tree)
+      (const void*)lig_schedule_excluding_kernel<true, false, true>, (const void*)lig_schedule_excluding_kernel<false, false, true>,
+      (const void*)lig_schedule_excluding_kernel<true, true, true>, (const void*)lig_schedule_excluding_kernel<false, true, true>,
+      (const void*)lig_schedule_excluding_count_kernel<true, false, true>, (const void*)lig_schedule_excluding_count_kernel<false, false, true>,
+      (const void*)lig_schedule_excluding_count_kernel<true, true, true>, (const void*)lig_schedule_excluding_count_kernel<false, true, true>,
+      (const void*)lig_schedule_excluding_fallback_kernel<true, false, true>, (const void*)lig_schedule_excluding_fallback_kernel<false, false, true>,
+      (const void*)lig_schedule_excluding_fallback_kernel<true, true, true>, (const void*)lig_schedule_excluding_fallback_kernel<false, true, true>,
+      (const void*)lig_schedule_excluding_fallback_count_kernel<true, false, true>, (const void*)lig_schedule_excluding_fallback_count_kernel<false, false, true>,
+      (const void*)lig_schedule_excluding_fallback_count_kernel<true, true, true>, (const void*)lig_schedule_excluding_fallback_count_kernel<false, true, true>,
+  };
+  for (const void* fn : pool_forms) CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   const size_t need = scratch_bytes(words_for(max_pods)) > build_fixed_bytes(words_for(max_pods))
                           ? scratch_bytes(words_for(max_pods)) : build_fixed_bytes(words_for(max_pods));
   if (need > c->smem_optin)
@@ -1399,6 +1449,12 @@ int lig_update_snapshot(lig_ctx* c, uint64_t new_epoch, uint64_t base_epoch, int
     if (cudaMemcpyAsync(w.d_blob, base->d_blob, w.bytes, cudaMemcpyDeviceToDevice, w.stream) != cudaSuccess)
       return bail(fail(LIG_ERR_CUDA, "base snapshot copy failed"));
     if (int rc = note_reader(*base, w.stream)) return bail(rc);     // a later overwrite of the base waits for this copy
+    Slot& ns = *static_cast<Slot*>(w.slot);
+    ns.n_ejected = base->n_ejected;                                   // the delta keeps base's ejected pods
+    if (base->n_ejected > 0 &&
+        cudaMemcpyAsync(ns.d_pool, base->d_pool, (size_t)ns.W * sizeof(uint32_t), cudaMemcpyDeviceToDevice,
+                        w.stream) != cudaSuccess)
+      return bail(fail(LIG_ERR_CUDA, "base pool copy failed"));
   }
   if (n_dirty > 0) {
     unsigned char* h = c->h_delta;     // the previous delta upload synchronised before returning
@@ -1423,6 +1479,62 @@ int lig_update_snapshot(lig_ctx* c, uint64_t new_epoch, uint64_t base_epoch, int
         reinterpret_cast<uint32_t*>(w.d_blob + l.bitmap), P, A, words_for(P));
     if (cudaGetLastError() != cudaSuccess) return bail(fail(LIG_ERR_CUDA, "delta kernel launch failed"));
     c->launches++;
+  }
+  if (int rc = ligi::enqueue_build(c, &w)) return bail(rc);
+  return ligi::finish_write(c, &w, true);
+}
+
+int lig_eject_pods(lig_ctx* c, uint64_t new_epoch, uint64_t base_epoch, const int32_t* pod_idx, int n) {
+  if (!c || n < 0 || (n > 0 && !pod_idx)) return fail(LIG_ERR_INVALID, "lig_eject_pods: bad argument");
+  if (new_epoch == base_epoch) return fail(LIG_ERR_INVALID, "lig_eject_pods: new_epoch == base_epoch");
+  int P = 0, A = 0;
+  {
+    std::lock_guard<std::mutex> lk(c->mu);
+    Slot* b = nullptr;
+    if (int rc = resolve_slot(c, base_epoch, &b)) return rc;
+    P = b->P;
+    A = b->A;
+    if (&victim_slot(c, new_epoch) == b)   // the rule of lig_update_snapshot
+      return fail(LIG_ERR_INVALID, "base epoch %llu is the slot epoch %llu would overwrite",
+                  (unsigned long long)base_epoch, (unsigned long long)new_epoch);
+  }
+  if (n > P) return fail(LIG_ERR_INVALID, "lig_eject_pods: n=%d exceeds P=%d", n, P);
+  // the pool: every pod of [0, P) but the listed ones; refused before the writer lock, so a refused
+  // call leaves both resident epochs untouched
+  const int W = words_for(P);
+  std::vector<uint32_t> pool((size_t)W, 0u);
+  for (int w = 0; w < W; ++w) {
+    const int rem = P - w * 32;
+    pool[(size_t)w] = rem >= 32 ? 0xffffffffu : ((1u << rem) - 1u);
+  }
+  for (int i = 0; i < n; ++i) {
+    const int p = pod_idx[i];
+    if (p < 0 || p >= P) return fail(LIG_ERR_INVALID, "ejected pod index %d outside [0, %d)", p, P);
+    const uint32_t bit = 1u << (p & 31);
+    if (!(pool[(size_t)(p >> 5)] & bit)) return fail(LIG_ERR_INVALID, "ejected pod index %d listed twice", p);
+    pool[(size_t)(p >> 5)] &= ~bit;
+  }
+  ligi::SnapshotWrite w;
+  if (int rc = ligi::begin_write(c, new_epoch, P, A, nullptr, true, &w)) return rc;
+  auto bail = [&](int rc) { ligi::abort_write(c, &w); return rc; };
+  Slot& ns = *static_cast<Slot*>(w.slot);
+  {
+    std::lock_guard<std::mutex> lk(c->mu);
+    Slot* base = nullptr;
+    if (int rc = resolve_slot(c, base_epoch, &base)) return bail(rc);
+    if (base == &ns) return bail(fail(LIG_ERR_INVALID, "base epoch was evicted meanwhile"));
+    if (cudaStreamWaitEvent(w.stream, base->ready, 0) != cudaSuccess) return bail(fail(LIG_ERR_CUDA, "cudaStreamWaitEvent failed"));
+    if (cudaMemcpyAsync(w.d_blob, base->d_blob, w.bytes, cudaMemcpyDeviceToDevice, w.stream) != cudaSuccess)
+      return bail(fail(LIG_ERR_CUDA, "base snapshot copy failed"));
+    if (int rc = note_reader(*base, w.stream)) return bail(rc);     // a later overwrite of the base waits for this copy
+  }
+  // the pool mask (W words, not the blob) crosses PCIe through the slot's pinned staging, which
+  // begin_write found free
+  ns.n_ejected = n;
+  if (n > 0) {
+    memcpy(w.h_blob, pool.data(), (size_t)W * sizeof(uint32_t));
+    if (cudaMemcpyAsync(ns.d_pool, w.h_blob, (size_t)W * sizeof(uint32_t), cudaMemcpyHostToDevice, w.stream) != cudaSuccess)
+      return bail(fail(LIG_ERR_CUDA, "pool mask copy failed"));
   }
   if (int rc = ligi::enqueue_build(c, &w)) return bail(rc);
   return ligi::finish_write(c, &w, true);
@@ -2227,9 +2339,15 @@ static void launch_excluding(const lig_ctx* c, const Slot& s, const Thr& thr, co
   int2* out = reinterpret_cast<int2*>(x.out);
   auto launch = [&](auto staged, auto caller_tree) {
     constexpr bool kS = decltype(staged)::value, kT = decltype(caller_tree)::value;
-    if (hist)
+    if (hist && s.n_ejected > 0)
+      lig_schedule_excluding_count_kernel<kS, kT, true><<<sh.grid, kCtaThreads, sh.smem, st>>>(
+          v, thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, hist, s.d_pool);
+    else if (hist)
       lig_schedule_excluding_count_kernel<kS, kT><<<sh.grid, kCtaThreads, sh.smem, st>>>(
           v, thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, hist);
+    else if (s.n_ejected > 0)
+      lig_schedule_excluding_kernel<kS, kT, true><<<sh.grid, kCtaThreads, sh.smem, st>>>(
+          v, thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, s.d_pool);
     else
       lig_schedule_excluding_kernel<kS, kT><<<sh.grid, kCtaThreads, sh.smem, st>>>(
           v, thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed);
@@ -2358,8 +2476,12 @@ static int enqueue_excluding_fallbacks(lig_ctx* c, Slot& s, const ExcludingCall&
   int2* out = reinterpret_cast<int2*>(x.out);
   auto launch = [&](auto staged, auto caller_tree) {
     constexpr bool kS = decltype(staged)::value, kT = decltype(caller_tree)::value;
-    lig_schedule_excluding_fallback_kernel<kS, kT><<<sh.grid, kCtaThreads, sh.smem, st>>>(
-        v, thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, n_fallbacks, fallbacks);
+    if (s.n_ejected > 0)
+      lig_schedule_excluding_fallback_kernel<kS, kT, true><<<sh.grid, kCtaThreads, sh.smem, st>>>(
+          v, thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, n_fallbacks, fallbacks, s.d_pool);
+    else
+      lig_schedule_excluding_fallback_kernel<kS, kT><<<sh.grid, kCtaThreads, sh.smem, st>>>(
+          v, thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, n_fallbacks, fallbacks);
   };
   using Y = std::true_type;
   using N = std::false_type;
@@ -2523,7 +2645,10 @@ static int fb_copy_epoch(lig_ctx* c, Slot* s, cudaStream_t st) {
   fs.P = s->P;
   fs.A = s->A;
   fs.W = s->W;
+  fs.n_ejected = s->n_ejected;                              // the private copy carries the pool
   CUDA_TRY(cudaMemcpyAsync(fs.d_blob, s->d_blob, layout_for(s->P, s->A).total, cudaMemcpyDeviceToDevice, st));
+  if (s->n_ejected > 0)
+    CUDA_TRY(cudaMemcpyAsync(fs.d_pool, s->d_pool, (size_t)s->W * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
   if (fs.P > 0) CUDA_TRY(cudaMemsetAsync(c->d_fb_hist, 0, (size_t)fs.P * sizeof(int32_t), st));
   return note_reader(*s, st);
 }
@@ -2581,8 +2706,13 @@ static void launch_excluding_fallback_count(const lig_ctx* c, const Slot& fs, co
   int2* out = reinterpret_cast<int2*>(x.out);
   auto launch = [&](auto staged, auto caller_tree) {
     constexpr bool kS = decltype(staged)::value, kT = decltype(caller_tree)::value;
-    lig_schedule_excluding_fallback_count_kernel<kS, kT><<<sh.grid, kCtaThreads, sh.smem, st>>>(
-        v, run.thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, n_fallbacks, fallbacks, c->d_fb_hist);
+    if (fs.n_ejected > 0)
+      lig_schedule_excluding_fallback_count_kernel<kS, kT, true><<<sh.grid, kCtaThreads, sh.smem, st>>>(
+          v, run.thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, n_fallbacks, fallbacks, c->d_fb_hist,
+          fs.d_pool);
+    else
+      lig_schedule_excluding_fallback_count_kernel<kS, kT><<<sh.grid, kCtaThreads, sh.smem, st>>>(
+          v, run.thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, n_fallbacks, fallbacks, c->d_fb_hist);
   };
   using Y = std::true_type;
   using N = std::false_type;

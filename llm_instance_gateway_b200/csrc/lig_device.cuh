@@ -722,10 +722,13 @@ __device__ __forceinline__ void seal_compact(const CompactOut& co, int n_classes
   }
 }
 
-template <bool kStaged>
+// kPool (an epoch derived by lig_eject_pods): the tree's input is not every pod but the n_pool pods
+// set in `pool` (W words, global memory); an ejected pod is treated like a padding pod.
+template <bool kStaged, bool kPool = false>
 __global__ void __launch_bounds__(kBuildThreads)
 lig_class_build_kernel(SnapView s, Thr thr, ClassEntry* __restrict__ cls,
-                       uint16_t* __restrict__ lists, int list_stride, CompactOut co) {
+                       uint16_t* __restrict__ lists, int list_stride, CompactOut co,
+                       const uint32_t* __restrict__ pool = nullptr, int n_pool = 0) {
   extern __shared__ __align__(16) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int P = s.P, W = s.W, A = s.A;
@@ -754,7 +757,7 @@ lig_class_build_kernel(SnapView s, Thr thr, ClassEntry* __restrict__ cls,
   // the last CTA to finish seals the blob: total size, or 0 when the pool overflowed
   auto seal = [&](uint32_t fixed_entries) { seal_compact(co, n_classes, fixed_entries); };
 
-  if (P == 0) {   // critical: predicate node errs on an empty pool -> sheddable branch -> drop
+  if (kPool ? n_pool == 0 : P == 0) {   // critical: predicate node errs on an empty pool -> sheddable branch -> drop
     for (int c = blockIdx.x * kBuildThreads + threadIdx.x; c < n_classes; c += gridDim.x * kBuildThreads) {
       const ClassEntry e = make_entry(0u, (uint32_t)LIG_DROP, none);
       cls[c] = e;
@@ -772,7 +775,7 @@ lig_class_build_kernel(SnapView s, Thr thr, ClassEntry* __restrict__ cls,
   for (int w = warp; w < W; w += kBuildWarps) {
     const int p = w * 32 + lane;
     bool room = false, low = false, shed = false;
-    if (p < P) {
+    if (kPool ? ((pool[w] >> lane) & 1u) != 0 : p < P) {
       const long long qq = ldq(p);
       room = has_room<kStaged>(f, p);                                     // filter.go:175-177
       low = qq < thr.q_lora;                                              // scheduler.go:58-60
@@ -812,7 +815,7 @@ lig_class_build_kernel(SnapView s, Thr thr, ClassEntry* __restrict__ cls,
     __syncthreads();
   } else {
     // low-queue filter failed: all pods -> least queuing -> low cost LoRA -> least KV  scheduler.go:71,35-46
-    uint32_t ny = blk_pred_pass(TMP, nullptr, P, W, sh, warp, lane, [&](int) { return true; });
+    uint32_t ny = blk_pred_pass(TMP, kPool ? pool : nullptr, P, W, sh, warp, lane, [&](int) { return true; });
     ny = blk_least_queuing<kStaged>(f, TMP, W, ny, sh, warp, lane);
     uint32_t nz = 0;
     for (int w = warp; w < W; w += kBuildWarps) {
@@ -981,9 +984,13 @@ __device__ __forceinline__ void compact_mask_to_two_lists(const uint32_t* X, int
   }
 }
 
+// kPool: as in lig_class_build_kernel, for a non-empty pool (an empty one takes the general build's
+// early path).
+template <bool kPool = false>
 __global__ void __launch_bounds__(kBuildThreads)
 lig_class_build_fast_kernel(SnapView s, Thr thr, ClassEntry* __restrict__ cls, uint16_t* __restrict__ lists,
-                            int list_stride, CompactOut co) {
+                            int list_stride, CompactOut co, const uint32_t* __restrict__ pool = nullptr,
+                            int n_pool = 0) {
   extern __shared__ __align__(16) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int P = s.P, W = s.W, A = s.A;
@@ -1033,7 +1040,7 @@ lig_class_build_fast_kernel(SnapView s, Thr thr, ClassEntry* __restrict__ cls, u
     const int p = w * 32 + lane;
     q[j] = 0;
     kv[j] = 0.0;
-    if (w < W && p < P) {
+    if (w < W && (kPool ? ((pool[w] >> lane) & 1u) != 0 : p < P)) {
       q[j] = f.q[p];
       kv[j] = f.kv[p];
       valid |= 1u << j;
@@ -1071,7 +1078,7 @@ lig_class_build_fast_kernel(SnapView s, Thr thr, ClassEntry* __restrict__ cls, u
   // critical side, start set:  low-queue pods that can accept the adapter, else all low-queue pods
   // (scheduler.go:58-69); no low-queue pod at all: every pod (scheduler.go:71)
   uint32_t tc = n_low > 0 ? (n_low_room > 0 ? (low & room) : low) : valid;
-  uint32_t n_tc = n_low > 0 ? (n_low_room > 0 ? n_low_room : n_low) : (uint32_t)P;
+  uint32_t n_tc = n_low > 0 ? (n_low_room > 0 ? n_low_room : n_low) : (uint32_t)(kPool ? n_pool : P);
   // sheddable side, start set: pods with capacity (scheduler.go:74-79); empty -> drop
   uint32_t ts = shed;
   uint32_t n_ts = n_shed;
@@ -1348,10 +1355,12 @@ __device__ __forceinline__ EvalResult tree_walk_warp(const Fields& f, const lig_
   }
 }
 
-template <bool kStaged>
+// kPool: the root's input is the n_pool pods set in `pool` (as in lig_class_build_kernel).
+template <bool kStaged, bool kPool = false>
 __global__ void __launch_bounds__(kCtaThreads)
 lig_class_build_tree_kernel(SnapView s, const __grid_constant__ FilterTree tree, ClassEntry* __restrict__ cls,
-                            uint16_t* __restrict__ lists, int list_stride, CompactOut co) {
+                            uint16_t* __restrict__ lists, int list_stride, CompactOut co,
+                            const uint32_t* __restrict__ pool = nullptr, int n_pool = 0) {
   extern __shared__ __align__(16) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int P = s.P, W = s.W, A = s.A;
@@ -1382,7 +1391,14 @@ lig_class_build_tree_kernel(SnapView s, const __grid_constant__ FilterTree tree,
     const bool critical = c >= A + 1;
     const int a = critical ? c - (A + 1) : c;
     const uint32_t* Hrow = stage_adapter_row(s, a, H, lane);     // nullptr for a == A
-    const EvalResult r = tree_walk_warp<kStaged>(f, nodes, Hrow, critical, P, W, M0, M1, lane);
+    EvalResult r;
+    if constexpr (kPool) {
+      for (int w = lane; w < W; w += 32) M0[w] = __ldg(pool + w);
+      __syncwarp();
+      r = tree_walk_warp<kStaged, true>(f, nodes, Hrow, critical, P, W, M0, M1, lane, (uint32_t)n_pool);
+    } else {
+      r = tree_walk_warp<kStaged>(f, nodes, Hrow, critical, P, W, M0, M1, lane);
+    }
     const uint32_t off = (uint32_t)c * (uint32_t)list_stride;
     uint32_t coff = 0;                   // the class's list in the compact pool (0 = the sentinel)
     if (r.n) {
@@ -2859,10 +2875,14 @@ lig_scan_kernel(SnapView s, Thr thr, const int4* __restrict__ reqs, int2* __rest
 // shared-memory atomicAnd, so a duplicate clears nothing twice, and entries outside [0, P) clear
 // nothing.  The walk starts from that mask: the built-in tree, or (kTree) the caller tree that built
 // the epoch.  Requests and rows are read with plain loads: they may be page-locked host memory.
-template <bool kStaged, bool kTree>
+// kPool (an epoch derived by lig_eject_pods, here and in the three kernels below): the mask starts from
+// the epoch's pool words instead of every pod.  The pool pointer of the two resident kernels is not
+// __restrict__: with it, ptxas allocated the registers of their kPool = false forms differently.
+template <bool kStaged, bool kTree, bool kPool = false>
 __global__ void __launch_bounds__(kCtaThreads)
 lig_schedule_excluding_kernel(SnapView s, Thr thr, const __grid_constant__ FilterTree tree, const int4* reqs,
-                              const int16_t* excluded, int n_excluded, int2* out, int R, uint64_t seed) {
+                              const int16_t* excluded, int n_excluded, int2* out, int R, uint64_t seed,
+                              const uint32_t* pool = nullptr) {
   extern __shared__ __align__(16) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint32_t* X = reinterpret_cast<uint32_t*>(smem) + (size_t)warp * 3 * s.W;
@@ -2879,9 +2899,13 @@ lig_schedule_excluding_kernel(SnapView s, Thr thr, const __grid_constant__ Filte
     const bool critical = ((uint32_t)r.y & LIG_REQ_CRITICAL) != 0;
     const uint64_t key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
     const uint32_t* Hrow = stage_adapter_row(s, r.x, H, lane);
-    for (int w = lane; w < s.W; w += 32) {   // the request's pool: every pod ...
-      const int rem = s.P - w * 32;
-      T[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
+    for (int w = lane; w < s.W; w += 32) {   // the request's pool: every pod (kPool: of the epoch's pool) ...
+      if constexpr (kPool) {
+        T[w] = pool[w];
+      } else {
+        const int rem = s.P - w * 32;
+        T[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
+      }
     }
     __syncwarp();
     if (ex >= 0 && ex < s.P) atomicAnd(T + (ex >> 5), ~(1u << (ex & 31)));   // ... but the excluded
@@ -2916,11 +2940,11 @@ lig_schedule_excluding_kernel(SnapView s, Thr thr, const __grid_constant__ Filte
 // as in count_window_picks).  A separate body, not a shared __forceinline__ one or a template flag
 // on the resident kernel: both of those change ptxas's register allocation of the resident
 // caller-tree forms (a 16-byte stack frame appears in the staged one).
-template <bool kStaged, bool kTree>
+template <bool kStaged, bool kTree, bool kPool = false>
 __global__ void __launch_bounds__(kCtaThreads)
 lig_schedule_excluding_count_kernel(SnapView s, Thr thr, const __grid_constant__ FilterTree tree, const int4* reqs,
                                     const int16_t* excluded, int n_excluded, int2* out, int R, uint64_t seed,
-                                    int* __restrict__ hist) {
+                                    int* __restrict__ hist, const uint32_t* __restrict__ pool = nullptr) {
   extern __shared__ __align__(16) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint32_t* X = reinterpret_cast<uint32_t*>(smem) + (size_t)warp * 3 * s.W;
@@ -2938,8 +2962,12 @@ lig_schedule_excluding_count_kernel(SnapView s, Thr thr, const __grid_constant__
     const uint64_t key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
     const uint32_t* Hrow = stage_adapter_row(s, r.x, H, lane);
     for (int w = lane; w < s.W; w += 32) {
-      const int rem = s.P - w * 32;
-      T[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
+      if constexpr (kPool) {
+        T[w] = pool[w];
+      } else {
+        const int rem = s.P - w * 32;
+        T[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
+      }
     }
     __syncwarp();
     if (ex >= 0 && ex < s.P) atomicAnd(T + (ex >> 5), ~(1u << (ex & 31)));
@@ -3004,11 +3032,11 @@ __device__ __forceinline__ int warp_select_survivor(const uint32_t* M, int W, ui
 // whole warp (warp_select_survivor) rather than by the retry's serial W-word loop.  Lane j-1 keeps
 // entry j and the row is stored by lanes 0 .. n_fallbacks-1.  A separate body, for the reason given
 // at lig_schedule_excluding_count_kernel.
-template <bool kStaged, bool kTree>
+template <bool kStaged, bool kTree, bool kPool = false>
 __global__ void __launch_bounds__(kCtaThreads)
 lig_schedule_excluding_fallback_kernel(SnapView s, Thr thr, const __grid_constant__ FilterTree tree, const int4* reqs,
                                        const int16_t* excluded, int n_excluded, int2* out, int R, uint64_t seed,
-                                       int n_fallbacks, int16_t* fallbacks) {
+                                       int n_fallbacks, int16_t* fallbacks, const uint32_t* pool = nullptr) {
   extern __shared__ __align__(16) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint32_t* X = reinterpret_cast<uint32_t*>(smem) + (size_t)warp * 3 * s.W;
@@ -3026,8 +3054,12 @@ lig_schedule_excluding_fallback_kernel(SnapView s, Thr thr, const __grid_constan
     const uint64_t key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
     const uint32_t* Hrow = stage_adapter_row(s, r.x, H, lane);
     for (int w = lane; w < s.W; w += 32) {
-      const int rem = s.P - w * 32;
-      T[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
+      if constexpr (kPool) {
+        T[w] = pool[w];
+      } else {
+        const int rem = s.P - w * 32;
+        T[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
+      }
     }
     __syncwarp();
     if (ex >= 0 && ex < s.P) atomicAnd(T + (ex >> 5), ~(1u << (ex & 31)));
@@ -3091,12 +3123,12 @@ lig_schedule_excluding_fallback_kernel(SnapView s, Thr thr, const __grid_constan
 // copy with the tree and thresholds the chain started with, plus lig_schedule_excluding_count_kernel's
 // count: lane 0 adds each LIG_OK pick to the open window's histogram (row entries add no load).  A
 // separate body, for the reason given at lig_schedule_excluding_count_kernel.
-template <bool kStaged, bool kTree>
+template <bool kStaged, bool kTree, bool kPool = false>
 __global__ void __launch_bounds__(kCtaThreads)
 lig_schedule_excluding_fallback_count_kernel(SnapView s, Thr thr, const __grid_constant__ FilterTree tree,
                                              const int4* reqs, const int16_t* excluded, int n_excluded, int2* out,
                                              int R, uint64_t seed, int n_fallbacks, int16_t* fallbacks,
-                                             int* __restrict__ hist) {
+                                             int* __restrict__ hist, const uint32_t* __restrict__ pool = nullptr) {
   extern __shared__ __align__(16) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint32_t* X = reinterpret_cast<uint32_t*>(smem) + (size_t)warp * 3 * s.W;
@@ -3114,8 +3146,12 @@ lig_schedule_excluding_fallback_count_kernel(SnapView s, Thr thr, const __grid_c
     const uint64_t key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
     const uint32_t* Hrow = stage_adapter_row(s, r.x, H, lane);
     for (int w = lane; w < s.W; w += 32) {
-      const int rem = s.P - w * 32;
-      T[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
+      if constexpr (kPool) {
+        T[w] = pool[w];
+      } else {
+        const int rem = s.P - w * 32;
+        T[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
+      }
     }
     __syncwarp();
     if (ex >= 0 && ex < s.P) atomicAnd(T + (ex >> 5), ~(1u << (ex & 31)));

@@ -81,6 +81,12 @@ class Engine:
              np.ascontiguousarray(adapter_ids, dtype=np.int32)]
         N.check(self._lib.lig_update_snapshot(self._ctx, new_epoch, base_epoch, len(a[0]), *[_ptr(x) for x in a]))
 
+    def eject_pods(self, new_epoch: int, base_epoch: int, pod_idx) -> None:
+        """lig_eject_pods: new_epoch is base_epoch's snapshot scheduled without the pods `pod_idx` (the
+        complete ejected set; empty = every pod back)."""
+        idx = np.ascontiguousarray(pod_idx, dtype=np.int32)
+        N.check(self._lib.lig_eject_pods(self._ctx, new_epoch, base_epoch, _ptr(idx), len(idx)))
+
     def upload_snapshot_device(self, epoch: int, P: int, A: int, d_blob: int, stream: int = 0) -> None:
         N.check(self._lib.lig_upload_snapshot_device(self._ctx, epoch, P, A, d_blob, stream or None))
 

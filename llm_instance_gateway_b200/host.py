@@ -30,6 +30,7 @@ EXPORTED_SYMBOLS = (
     "ligh_scheduler_set_models", "ligh_schedule_model_device", "ligh_model_stats", "ligh_schedule_models_concurrent",
     "ligh_filter", "ligh_schedule_with_fallbacks", "ligh_fallback_scheduled", "ligh_schedule_model_with_fallbacks",
     "ligh_schedule_retry", "ligh_retry_scheduled", "ligh_schedule_retry_with_fallbacks",
+    "ligh_eject_pods", "ligh_eject_stats",
 )
 
 _lib = None
@@ -89,6 +90,9 @@ def load() -> C.CDLL:
     lib.ligh_schedule_retry_with_fallbacks.argtypes = [vp, C.c_char_p, i32, cpp, cpp, i32, i32, C.c_char_p, i32,
                                                        C.POINTER(i32), C.c_char_p, i32]
     lib.ligh_retry_scheduled.argtypes = [vp]
+    lib.ligh_eject_pods.argtypes = [vp, cpp, cpp, i32, C.c_char_p, i32]
+    lib.ligh_eject_stats.argtypes = [vp, vp]
+    lib.ligh_eject_stats.restype = None
     lib.ligh_retry_scheduled.restype = u64
     lib.ligh_fallback_scheduled.restype = u64
     lib.ligh_stats.argtypes = [vp, vp]
@@ -254,6 +258,15 @@ class HostScheduler:
         pods = names.value.decode().split("\n") if k.value else []
         return code, resolved.value.decode(), pods, err.value.decode("utf-8", "replace") if code != GRPC_OK else ""
 
+    def EjectPods(self, pods: Sequence[Pod]) -> None:  # noqa: N802
+        """Scheduler::EjectPods: schedule as if `pods` (the complete set, matched by value; empty = every
+        pod back) had left the provider, from the return on and across refreshes."""
+        err = C.create_string_buffer(512)
+        code = self._lib.ligh_eject_pods(self._s, _strs([p.Name for p in pods]), _strs([p.Address for p in pods]),
+                                         len(pods), err, 512)
+        if code != GRPC_OK:
+            raise HostSchedulerError(err.value.decode("utf-8", "replace"))
+
     def Refresh(self) -> None:  # noqa: N802
         err = C.create_string_buffer(512)
         if self._lib.ligh_refresh(self._s, err, 512) != 0:
@@ -266,12 +279,15 @@ class HostScheduler:
         self._lib.ligh_feedback_stats(self._s, fb)
         ms = (C.c_uint64 * 2)()
         self._lib.ligh_model_stats(self._s, ms)
+        ej = (C.c_uint64 * 2)()
+        self._lib.ligh_eject_stats(self._s, ej)
         return dict(zip(("scheduled", "batches", "max_batch", "refreshes", "stale_retries", "failed_refreshes",
                          "excluded_pods", "delta_refreshes", "last_dirty_pods", "feedback_windows",
                          "feedback_restarts", "model_scheduled", "model_batches", "fallback_scheduled",
-                         "retry_scheduled"),
+                         "retry_scheduled", "ejected_pods", "eject_publishes"),
                         map(int, list(out) + list(fb) + list(ms) + [self._lib.ligh_fallback_scheduled(self._s),
-                                                                    self._lib.ligh_retry_scheduled(self._s)])))
+                                                                    self._lib.ligh_retry_scheduled(self._s)] +
+                            list(ej))))
 
     def ScheduleModel(self, datastore: "HostDataStore", model: str):  # noqa: N802
         """resolve (FetchModelData + RandomWeightedDraw + IsCritical) + Schedule: (code, resolved, pod, err)."""

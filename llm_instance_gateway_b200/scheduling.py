@@ -215,6 +215,8 @@ class Scheduler:
         self._models: Optional[List[InferenceModel]] = None          # SetInferenceModels' list
         self._packed_models: Optional[PackedModels] = None           # that list packed for self._epoch
         self._model_index = 0                # first_index of the next model-id call
+        self._ejected: List[Pod] = []        # EjectPods' set
+        self._ejected_idx: List[int] = []    # its pods in the published epoch
         self._rng = random.Random(seed)      # the Go global source is auto-seeded (scheduler.go:120)
         self._seed = self._rng.getrandbits(64)
 
@@ -235,11 +237,41 @@ class Scheduler:
         self._uploaded += 1
         self._engine.upload_snapshot(self._uploaded, snap)
         packed = pack_models(models, snap) if models is not None else None
-        if packed is not None:
+        self._epoch, self._snap, self._packed_models, self._ejected_idx = self._uploaded, snap, packed, []
+        idx = self._ejected_indices()
+        if idx:                              # a full upload has every pod: derive once more
+            self._derive(idx)
+        elif packed is not None:
             self._engine.upload_models(self._uploaded, packed)
-        self._epoch, self._snap, self._packed_models = self._uploaded, snap, packed
         self._version = self._provider_version()
         return snap
+
+    def _ejected_indices(self) -> List[int]:
+        gone = set(self._ejected)
+        return [p for p, pod in enumerate(self._snap.pods) if pod in gone] if gone else []
+
+    def _derive(self, idx: List[int]) -> None:
+        """Publish an epoch derived from the published one (the newest resident epoch) without `idx`,
+        with the model table when a list is set."""
+        self._uploaded += 1
+        self._engine.eject_pods(self._uploaded, self._epoch, idx)
+        if self._packed_models is not None:
+            self._engine.upload_models(self._uploaded, self._packed_models)
+        self._epoch, self._ejected_idx = self._uploaded, idx
+
+    def EjectPods(self, pods: Sequence[Pod]) -> None:
+        """Schedule as if `pods` had left the provider (lig_eject_pods), until a later call lets them
+        back.  `pods` is the complete ejected set (empty: every pod back), matched by value against the
+        snapshot; pods it does not hold are ignored.  Before the return a derived epoch is published
+        (with the model table when a list is set), so every later call avoids them; every Refresh
+        derives again from its new snapshot.  Publishing an epoch restarts the load-feedback chain."""
+        self._ejected = list(pods)
+        before = self._epoch
+        self._current()                      # a refresh here already applies the new set
+        if self._epoch == before:
+            idx = self._ejected_indices()
+            if idx != self._ejected_idx:
+                self._derive(idx)
 
     def SetInferenceModels(self, models: Sequence[InferenceModel]) -> None:
         """The InferenceModels ScheduleModel resolves against (of two with one ModelName the later
@@ -524,7 +556,9 @@ class Scheduler:
         """The survivors of `req` against the scraped snapshot.  With load_feedback_window set this
         is still the scraped epoch: the queue sizes the feedback chain has added are not in it."""
         snap = self._current()
-        if self._filter is not None:         # the class table holds the caller tree's survivor set
+        # the class table holds the caller tree's survivor set, and the pool's: the direct scan walks
+        # the built-in tree over every pod
+        if self._filter is not None or self._ejected_idx:
             st, _, lst = self._engine.read_class(self._epoch, req.Critical, snap.adapter_id(req.ResolvedTargetModel),
                                                  snap.P)
             if st == N.LIG_DROP:
