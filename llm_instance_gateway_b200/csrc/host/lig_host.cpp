@@ -43,6 +43,15 @@ inline uint64_t splitmix_next(uint64_t& s) {
   return z ^ (z >> 31);
 }
 
+// A stale epoch is re-resolved and tried again up to this many attempts in all (AwaitPublication).
+constexpr int kStaleAttempts = 4;
+
+template <class F>
+struct OnExit {
+  F f;
+  ~OnExit() { f(); }
+};
+
 }  // namespace
 
 Status NewScheduler(std::shared_ptr<PodMetricsProvider> pmp, const Options& opt,
@@ -121,8 +130,10 @@ Scheduler::~Scheduler() {
 // One pack per refresh tick replaces the per-request AllPodMetrics() of scheduler.go:114-115.
 // A failed refresh keeps the previous snapshot — like a failed scrape keeps stale metrics
 // (backend/provider.go:151-156) — but never silently: it is counted and its reason kept.
+// Its end is counted (FinishWrite): calls refused with a stale epoch meanwhile wait for it.
 Status Scheduler::Refresh() {
   std::lock_guard<std::mutex> rk(refresh_mu_);
+  const OnExit finish{[this] { FinishWrite(); }};
   return RecordRefresh(RefreshImpl(models_));
 }
 
@@ -265,6 +276,8 @@ Status Scheduler::RefreshImpl(const std::shared_ptr<const ModelList>& models) {
   }
   // The ejected set: a delta epoch inherits its base's; when that is not the set EjectPods asks for on
   // this tick's pods (a full upload has none, or the pods moved), one more epoch is derived from it.
+  // That derive evicts the published epoch until snap_ moves on; calls refused meanwhile wait for the
+  // end of this write (AwaitPublication) before they re-resolve.
   snap->ejected = used_delta ? prev_ejected_ : std::vector<int32_t>{};
   bool derived = false;
   {
@@ -358,6 +371,7 @@ Status Scheduler::EjectPods(const std::vector<backend::Pod>& pods) {
   if (group_)
     return Errorf(InvalidArgument, "EjectPods: a scheduler over several devices has no ejection call (lig_group)");
   std::lock_guard<std::mutex> rk(refresh_mu_);
+  const OnExit finish{[this] { FinishWrite(); }};
   ejected_ = pods;
   std::shared_ptr<const Snapshot> cur;
   {
@@ -428,6 +442,7 @@ Status Scheduler::SetInferenceModels(std::vector<std::shared_ptr<const backend::
   }
   std::shared_ptr<const ModelList> next = std::move(list);
   std::lock_guard<std::mutex> rk(refresh_mu_);
+  const OnExit finish{[this] { FinishWrite(); }};
   Status st = RecordRefresh(RefreshImpl(next));
   if (st.ok()) models_ = std::move(next);
   return st;
@@ -555,10 +570,12 @@ Status Scheduler::Filter(const LLMRequest& req, std::vector<backend::Pod>* pods)
   std::vector<uint16_t> list;
   std::shared_ptr<const Snapshot> snap;
   int rc = 0;
-  for (int attempt = 0; attempt < 4; ++attempt) {
+  uint64_t writes_seen = 0;
+  for (int attempt = 0; attempt < kStaleAttempts; ++attempt) {
     {
       std::lock_guard<std::mutex> lk(snap_mu_);
       snap = snap_;
+        writes_seen = writes_done_;
     }
     if (!snap) return Errorf(Internal, "Filter: no snapshot uploaded yet");
     auto it = snap->adapter_ids->find(req.ResolvedTargetModel);   // interned as in Flush
@@ -566,7 +583,7 @@ Status Scheduler::Filter(const LLMRequest& req, std::vector<backend::Pod>* pods)
     r.flags = req.Critical ? LIG_REQ_CRITICAL : 0u;
     list.resize(std::max<size_t>(snap->pods.size(), 1));   // a survivor list never exceeds P
     rc = lig_filter_batch(ctx_, snap->epoch, seed_, &r, 1, &pick, offsets, list.data(), (int64_t)list.size());
-    if (rc != LIG_ERR_STALE_EPOCH) break;   // two refreshes raced past this call: re-resolve
+    if (!AwaitPublication(rc, writes_seen, attempt)) break;
   }
   if (rc != 0) return LigFailure("lig_filter_batch");
   if (pick.status == LIG_DROP)                                               // scheduler.go:83-89
@@ -576,6 +593,34 @@ Status Scheduler::Filter(const LLMRequest& req, std::vector<backend::Pod>* pods)
   if (pods)
     for (int64_t k = offsets[0]; k < offsets[1]; ++k) pods->push_back(snap->pods[list[(size_t)k]]);
   return Status{};
+}
+
+// Whether a call refused with `rc` is tried again.  LIG_ERR_STALE_EPOCH means its epoch was evicted
+// after it was captured, by a write that may still be in progress: a refresh that derives an ejected
+// set evicts the published epoch before the derived one is published.  Every eviction happens inside
+// Refresh, SetInferenceModels or EjectPods, and each of them counts writes_done_ when it ends, so the
+// call waits until writes_done_ moves past the count it captured with its epoch: for the write in
+// flight only, not for a later one still scraping the provider (a provider that calls back into the
+// scheduler cannot deadlock here).  The last attempt does not wait.  The wait is bounded so that a
+// refusal no write of this scheduler caused cannot hold a flush for good.
+bool Scheduler::AwaitPublication(int rc, uint64_t writes_seen, int attempt) {
+  if (rc != LIG_ERR_STALE_EPOCH) return false;
+  {
+    std::lock_guard<std::mutex> sk(stats_mu_);
+    stats_.stale_retries++;
+  }
+  if (attempt + 1 >= kStaleAttempts) return false;
+  std::unique_lock<std::mutex> lk(snap_mu_);
+  writes_cv_.wait_for(lk, std::chrono::seconds(1), [&] { return writes_done_ != writes_seen; });
+  return true;
+}
+
+void Scheduler::FinishWrite() {
+  {
+    std::lock_guard<std::mutex> lk(snap_mu_);
+    writes_done_++;
+  }
+  writes_cv_.notify_all();
 }
 
 // Queue the waiter for the batcher and block until its result is published.
@@ -687,10 +732,12 @@ void Scheduler::Flush(std::vector<Waiter*>& all) {
     std::shared_ptr<const Snapshot> snap;
     Status failure;
     int rc = 0;
-    for (int attempt = 0; attempt < 4; ++attempt) {
+    uint64_t writes_seen = 0;
+  for (int attempt = 0; attempt < kStaleAttempts; ++attempt) {
       {
         std::lock_guard<std::mutex> lk(snap_mu_);
         snap = snap_;
+        writes_seen = writes_done_;
       }
       for (int i = 0; i < n; ++i) {
         const LLMRequest& r = *batch[done + i]->req;
@@ -719,9 +766,7 @@ void Scheduler::Flush(std::vector<Waiter*>& all) {
         device_us = call_us;
         device_cpu_us = thread_cpu_us() - cpu_t0;
       }
-      if (rc != LIG_ERR_STALE_EPOCH) break;   // two refreshes raced past this batch: re-resolve
-      std::lock_guard<std::mutex> sk(stats_mu_);
-      stats_.stale_retries++;
+      if (!AwaitPublication(rc, writes_seen, attempt)) break;
     }
     if (rc != 0)
       failure = LigFailure(nf > 0 && opt_.load_feedback_window > 0 ? "lig_schedule_batch_feedback_chain_fallbacks"
@@ -793,10 +838,12 @@ void Scheduler::FlushRetries(std::vector<Waiter*>& batch) {
     for (int i = 0; i < n; ++i) nf = std::max(nf, batch[done + i]->fallbacks);
     std::shared_ptr<const Snapshot> snap;
     int rc = 0, width = 1, k = 0;
-    for (int attempt = 0; failure.ok() && attempt < 4; ++attempt) {
+    uint64_t writes_seen = 0;
+    for (int attempt = 0; failure.ok() && attempt < kStaleAttempts; ++attempt) {
       {
         std::lock_guard<std::mutex> lk(snap_mu_);
         snap = snap_;
+        writes_seen = writes_done_;
       }
       std::unordered_map<std::string, std::vector<int16_t>> where;   // Name + '\0' + Address -> pod indices
       for (size_t p = 0; p < snap->pods.size(); ++p)
@@ -843,9 +890,7 @@ void Scheduler::FlushRetries(std::vector<Waiter*>& batch) {
       } else {
         rc = lig_schedule_batch_excluding(ctx_, snap->epoch, seed_, h_reqs_, n, h_excluded_, width, h_picks_);
       }
-      if (rc != LIG_ERR_STALE_EPOCH) break;   // two refreshes raced past this batch: re-resolve
-      std::lock_guard<std::mutex> sk(stats_mu_);
-      stats_.stale_retries++;
+      if (!AwaitPublication(rc, writes_seen, attempt)) break;
     }
     if (failure.ok() && rc != 0)
       failure = LigFailure(W > 0 && nf > 0 ? "lig_schedule_batch_feedback_chain_excluding_fallbacks"
@@ -897,10 +942,12 @@ void Scheduler::FlushModels(std::vector<Waiter*>& batch) {
     std::shared_ptr<const Snapshot> snap;
     int rc = 0, k = 0, nf = 0;
     const char* call = "lig_schedule_models_batch";
-    for (int attempt = 0; attempt < 4; ++attempt) {
+    uint64_t writes_seen = 0;
+  for (int attempt = 0; attempt < kStaleAttempts; ++attempt) {
       {
         std::lock_guard<std::mutex> lk(snap_mu_);
         snap = snap_;
+        writes_seen = writes_done_;
       }
       const ModelList* list = snap->models.get();
       k = 0;
@@ -945,9 +992,7 @@ void Scheduler::FlushModels(std::vector<Waiter*>& batch) {
         rc = lig_schedule_models_batch(ctx_, snap->epoch, seed_, model_index_, h_model_ids_, k, h_mpicks_);
       }
       if (rc == 0 && W > 0) CountFeedback(snap->epoch, k);
-      if (rc != LIG_ERR_STALE_EPOCH) break;
-      std::lock_guard<std::mutex> sk(stats_mu_);
-      stats_.stale_retries++;
+      if (!AwaitPublication(rc, writes_seen, attempt)) break;
     }
     if (k > 0) model_index_ += (uint64_t)k;
     const Status failure = rc != 0 ? LigFailure(call) : Status{};

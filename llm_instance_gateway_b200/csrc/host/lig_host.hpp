@@ -178,7 +178,7 @@ struct Stats {
   uint64_t batches = 0;        // lig_schedule_batch calls issued
   uint64_t max_batch = 0;      // largest batch flushed
   uint64_t refreshes = 0;      // snapshots uploaded
-  uint64_t stale_retries = 0;  // batches re-resolved after LIG_ERR_STALE_EPOCH
+  uint64_t stale_retries = 0;  // batches and Filter calls re-resolved after LIG_ERR_STALE_EPOCH
   uint64_t delta_refreshes = 0;    // refreshes that went through lig_update_snapshot (dirty pods only)
   uint64_t last_dirty_pods = 0;    // pods whose metrics changed at the last refresh
   uint64_t failed_refreshes = 0;   // Refresh() calls that kept the previous snapshot (see last_refresh_error)
@@ -403,6 +403,8 @@ class Scheduler {
   void FlushModels(std::vector<Waiter*>& batch);
   void FlushRetries(std::vector<Waiter*>& batch);
   void CountFeedback(uint64_t epoch, int n);
+  bool AwaitPublication(int rc, uint64_t writes_seen, int attempt);
+  void FinishWrite();
   Status CheckFallbacks(const char* fn, int n) const;
 
   std::shared_ptr<PodMetricsProvider> pmp_;
@@ -425,6 +427,10 @@ class Scheduler {
 
   mutable std::mutex snap_mu_;
   std::shared_ptr<const Snapshot> snap_;
+  // Refresh, SetInferenceModels and EjectPods calls finished, published or not (guarded by snap_mu_);
+  // a call refused with a stale epoch waits on writes_cv_ for the next one (AwaitPublication)
+  uint64_t writes_done_ = 0;
+  std::condition_variable writes_cv_;
   uint64_t next_epoch_ = 1;
   std::mutex refresh_mu_;
 

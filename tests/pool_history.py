@@ -325,6 +325,48 @@ UNITS = ("qkv_boundary", "qkv_past", "qkv_most", "swap", "add_remove", "new_name
          "join_leave", "unrepresentable", "refused", "kv_bits", "max_active")
 
 
+NOT_IN_POOL = Pod("pod-never", "address-never")
+
+
+def affected(history: Sequence[Tick], t: int) -> List[Pod]:
+    """The pods of the slice before tick t that tick t changes by its kind: renamed away (rename),
+    at a new index (reorder), gone (join_leave), or no longer representable (unrepresentable)."""
+    kind, prev, cur = history[t].kind, history[t - 1].pods, history[t].pods
+    now = [p.Pod for p in cur]
+    if kind in ("rename", "join_leave"):
+        return [p.Pod for p in prev if p.Pod not in now]
+    if kind == "reorder":
+        return [p.Pod for i, p in enumerate(prev) if now.index(p.Pod) != i]
+    if kind == "unrepresentable":
+        return [p.Pod for p in cur if not representable(p)]
+    return []
+
+
+def eject_schedule(history: Sequence[Tick], seed: int) -> Dict[int, List[Pod]]:
+    """{tick: the complete set Scheduler::EjectPods is called with after that tick's refresh}.
+
+    The set in force at a rename, reorder, join_leave and unrepresentable tick holds up to two of the
+    pods that tick changes (ejected the tick before), a kept pod at random and a pod that is in no
+    slice.  Once, the whole pool is ejected, and at the next tick the empty set lifts every pod; a
+    non-empty set is in force again from the tick after that on, so the sets change across ticks of
+    every kind."""
+    rng = np.random.default_rng(seed)
+    pools = expected_pools(history)
+    out: Dict[int, List[Pod]] = {}
+    for kind in ("rename", "reorder", "join_leave", "unrepresentable"):
+        t = [tk.kind for tk in history].index(kind)
+        hit = affected(history, t)
+        hit = [hit[i] for i in sorted(rng.choice(len(hit), size=min(2, len(hit)), replace=False))]
+        other = pools[t - 1][int(rng.integers(0, len(pools[t - 1])))].Pod
+        out[t - 1] = sorted(set(out.get(t - 1, [])) | set(hit) | {other, NOT_IN_POOL}, key=lambda p: p.Name)
+    free = [t for t in range(len(history) - 2) if not {t, t + 1, t + 2} & set(out)]
+    whole = free[int(rng.integers(0, len(free)))]
+    out[whole] = [p.Pod for p in pools[whole]]
+    out[whole + 1] = []
+    out[whole + 2] = [pools[whole + 2][0].Pod, NOT_IN_POOL]
+    return dict(sorted(out.items()))
+
+
 def make_history(P: int, seed: int, sets: Optional[SurvivorSets] = None) -> List[Tick]:
     """A seeded history over a pool of P pods for a scheduler with max_pods = P and max_adapters =
     MAX_ADAPTERS.  With `sets`, every swap (also the one of a refused tick) changes at least one

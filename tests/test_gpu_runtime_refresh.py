@@ -21,6 +21,7 @@ The regression tests replay a refused tick that swapped a pod's adapter names: t
 must not leave that pod's old bitmap row on the device.
 """
 import functools
+import threading
 
 import numpy as np
 import pytest
@@ -172,14 +173,37 @@ def probes_for(pools, t, seen):
 @pytest.mark.parametrize("doorbell", [False, True], ids=["launch", "doorbell"])
 @pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
 def test_runtime_follows_pool_history(case, doorbell):
+    follow_history(case, doorbell, eject=False)
+
+
+EJECT_CASES = [c for c in CASES if c[0] in ("p1", "p33", "p1000", "p5000", "drop_tree", "no_pods_tree")]
+
+
+@pytest.mark.parametrize("doorbell", [False, True], ids=["launch", "doorbell"])
+@pytest.mark.parametrize("case", EJECT_CASES, ids=[c[0] for c in EJECT_CASES])
+def test_runtime_follows_pool_history_with_ejections(case, doorbell):
+    """The same history with EjectPods called at the ticks of pool_history.eject_schedule: every
+    check runs on the expected pool without the ejected pods (by value), ejected_pods counts the
+    ejected pods in that pool, and eject_publishes moves exactly where an epoch is derived: an
+    EjectPods whose pods sit at other indices than the published epoch's set, a full upload with any
+    ejected pod in the pool, and a delta whose ejected pods are not its base's (renamed pods)."""
+    follow_history(case, doorbell, eject=True)
+
+
+def follow_history(case, doorbell, eject):
     _, P, tree = case
     hist = history(P, tree)
     pools = PH.expected_pools(hist)
+    ejections = PH.eject_schedule(hist, seed=P) if eject else {}
     rt = Runtime(hist, P, tree, doorbell, seed=1000 + P + (tree or 0))
     try:
         refreshes = 2 if rt.lists else 1      # NewScheduler's refresh, and SetInferenceModels'
-        failed = delta = excluded = 0
+        failed = delta = excluded = publishes = deltas_seen = 0
         seen, last_ok = set(), True
+        gone, ejected = set(), []             # EjectPods' set, and its indices in the published pool
+
+        def indices(pool):
+            return [i for i, p in enumerate(pool) if p.Pod in gone]
         for t, tick in enumerate(hist):
             where = (t, tick.kind)
             if t:
@@ -201,21 +225,35 @@ def test_runtime_follows_pool_history(case, doorbell):
             else:
                 failed += 1
             st = rt.s.stats()
+            if t and tick.published:          # a delta inherits its base's set, a full upload has none
+                used_delta = st["delta_refreshes"] > deltas_seen
+                publishes += (indices(pools[t]) != ejected) if used_delta else bool(indices(pools[t]))
+                ejected = indices(pools[t])
+            deltas_seen = st["delta_refreshes"]
+            if t in ejections:
+                rt.s.EjectPods(ejections[t])
+                gone = set(ejections[t])
+                publishes += indices(pools[t]) != ejected
+                ejected = indices(pools[t])
+                st = rt.s.stats()
+            assert (st["eject_publishes"], st["ejected_pods"]) == (publishes, len(ejected)), (where, st)
             if t and tick.kind in ("qkv_boundary", "rename") and last_ok:
                 delta += 1                            # at most P // 4 dirty pods, nothing else changed
             assert (st["refreshes"], st["failed_refreshes"], st["excluded_pods"]) == (refreshes, failed, excluded), \
                 (where, st)
             seen |= PH.names_of(tick.kept())
-            want = rt.check_survivors(pools[t], probes_for(pools, t, seen), where)
+            pool = [p for p in pools[t] if p.Pod not in gone]
+            want = rt.check_survivors(pool, probes_for(pools, t, seen), where)
             rt.check_picks(want, where)
             if rt.lists:
-                rt.check_models(pools[t], where)
+                rt.check_models(pool, where)
             if t and (tick.kind in ("qkv_boundary", "rename", "qkv_past", "qkv_most", "after_refusal")):
                 assert st["delta_refreshes"] == delta, (where, st)
             delta = st["delta_refreshes"]
             last_ok = tick.published
         st = rt.s.stats()
         assert st["stale_retries"] == 0 and st["delta_refreshes"] >= 3, st
+        assert publishes >= (4 if eject else 0), publishes
     finally:
         rt.close()
 
@@ -265,3 +303,83 @@ def test_refused_refresh_leaves_no_stale_adapter_row_at(swapped):
     """The same on 40 pods (the last bitmap word holds pods 32..39) with the swap on the first pod,
     the last pod and a pod inside the ragged last word."""
     refuse_then_return(40, swapped)
+
+
+def test_refresh_that_derives_under_concurrent_callers():
+    """A refresh that derives (a full upload with ejected pods) evicts the published epoch while it
+    derives the next one: calls that captured it get LIG_ERR_STALE_EPOCH and must wait for the
+    publication instead of spending their attempts at once.  Two slices hold the same 40 pods; the
+    second rotates the 3 ejected pods among their own positions and reverses the kept pods among
+    theirs, so every tick is a full upload that derives, and an ejected pod is at the same index in
+    either slice."""
+    names = ("a", "b", "c")
+    gone_at = [0, 17, 33]
+    pods = [pod(i, names) for i in range(40)]
+    for i, pm in enumerate(pods):                            # distinct metrics: every moved pod is dirty
+        pm.Metrics.WaitingQueueSize = i % 4
+        pm.Metrics.KVCacheUsagePercent = 0.01 * i
+    kept_at = [i for i in range(40) if i not in gone_at]
+    other = list(pods)
+    for a, b in zip(gone_at, gone_at[1:] + gone_at[:1]):
+        other[b] = pods[a]
+    for a, b in zip(kept_at, kept_at[::-1]):
+        other[b] = pods[a]
+    slices = [pods, other]
+    gone = {pods[i].Pod for i in gone_at}
+    assert {other[i].Pod for i in gone_at} == gone
+    sets = PH.survivor_sets(None)
+    for s_ in slices:                                        # every class keeps a survivor
+        for (name, crit), (rc, surv) in sets([p for p in s_ if p.Pod not in gone], list(names)).items():
+            assert rc == N.LIG_OK and surv, (name, crit)
+    models = [im(f"model-{n}", CRITICAL, [(n, 1)]) for n in names]
+    prov = H.HostProvider(pods)
+    s = H.HostScheduler(prov, max_pods=40, max_adapters=8, max_batch=256, batch_window_us=20, seed=5)
+    ds = H.HostDataStore(models)
+    errors, stop = [], [False]
+    try:
+        s.set_inference_models(ds)
+        s.EjectPods([pods[i].Pod for i in gone_at])
+        before = s.stats()
+        ticks = [0]
+
+        def refresher():
+            while not stop[0] or ticks[0] < 200:
+                ticks[0] += 1
+                prov.set_pods(slices[ticks[0] % 2])
+                s.Refresh()
+
+        def caller():                                        # keeps the errors and ejected picks
+            while not stop[0]:
+                code, got, err = s.Schedule("m", "a", True)
+                if code != H.GRPC_OK or got in gone:
+                    errors.append(err or f"ejected pod {got}")
+        threads = [threading.Thread(target=refresher), threading.Thread(target=caller)]
+        for t in threads:
+            t.start()
+        try:
+            res = {}
+            workers = [threading.Thread(target=lambda: res.update(d=s.schedule_concurrent(16, 200, list(names),
+                                                                                         [False, True, False]))),
+                       threading.Thread(target=lambda: res.update(m=s.schedule_models_concurrent(
+                           16, 200, [f"model-{n}" for n in names])))]
+            for w in workers:
+                w.start()
+            for w in workers:
+                w.join()
+        finally:
+            stop[0] = True
+            for t in threads:
+                t.join()
+        st = s.stats()
+        (dcodes, dpods), (mcodes, mpods, _) = res["d"], res["m"]
+        info = (st["stale_retries"], errors[:1], int((dcodes != H.GRPC_OK).sum()), int((mcodes != H.GRPC_OK).sum()), st)
+        assert (dcodes == H.GRPC_OK).all() and (mcodes == H.GRPC_OK).all() and not errors, info
+        assert not set(gone_at) & (set(dpods.tolist()) | set(mpods.tolist())), info
+        assert st["failed_refreshes"] == 0 and ticks[0] >= 200, info
+        assert st["eject_publishes"] - before["eject_publishes"] == st["refreshes"] - before["refreshes"], info
+        assert st["refreshes"] - before["refreshes"] == ticks[0] and st["ejected_pods"] == 3, info
+    finally:
+        stop[0] = True
+        s.close()
+        ds.close()
+        prov.close()

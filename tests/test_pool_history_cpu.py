@@ -83,6 +83,31 @@ def test_history_holds_every_kind_and_every_kind_does_its_change(case):
             assert pairs and all(min(max(x, 0), 65535) == min(max(y, 0), 65535) for x, y in pairs)
 
 
+@pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
+def test_eject_schedule_holds_every_situation(case):
+    """The ejected sets of tests/test_gpu_runtime_refresh.py: across the history, the set in force
+    at a rename, reorder, join_leave and unrepresentable tick holds a pod that tick changes; a set
+    names a pod that is in no slice; one set is the whole pool, and the empty set lifts it."""
+    _, P, tree = case
+    hist = case_history(P, tree, seed=P + 7 * (tree or 0))
+    pools = PH.expected_pools(hist)
+    sched = PH.eject_schedule(hist, seed=P)
+    assert sched == PH.eject_schedule(hist, seed=P)
+    seen, active = set(), []
+    for t, tick in enumerate(hist):
+        if t and set(active) & set(PH.affected(hist, t)):
+            seen.add(tick.kind)
+        if t in sched:
+            new = sched[t]
+            pool = {p.Pod for p in pools[t]}
+            seen |= {"not_in_pool"} if set(new) - pool else set()
+            seen |= {"whole_pool"} if pool <= set(new) else set()
+            seen |= {"lifted"} if active and not new else set()
+            active = new
+    want = {"rename", "reorder", "join_leave", "unrepresentable", "not_in_pool", "whole_pool", "lifted"}
+    assert seen == (want - {"reorder"} if P == 1 else want), seen      # one pod cannot move
+
+
 @pytest.mark.parametrize("case", [c for c in CASES if not (c[1] == 1 and c[2] is None)],
                          ids=[c[0] for c in CASES if not (c[1] == 1 and c[2] is None)])
 def test_swaps_and_refusals_change_survivor_sets(case):
