@@ -604,6 +604,53 @@ int lig_schedule_batch_excluding_fallbacks_device(lig_ctx* ctx, uint64_t epoch, 
                                                   int R, const int16_t* d_excluded, int n_excluded, lig_pick* d_out,
                                                   int n_fallbacks, int16_t* d_fallbacks, void* stream);
 
+/* ---- model-id retries: keep the drawn target, resolve on the device ------------------------------
+ * A model-id request that needs a retry already went out rewritten to its drawn target, so a retry
+ * must not draw again (a second draw could move it to another adapter and count it twice against
+ * the traffic split).  These calls take the target index the first attempt returned
+ * (lig_mpick.target_idx) and resolve it without a draw, so a caller of lig_schedule_models_batch
+ * never interns adapter names or looks up criticality on the host to retry.
+ *
+ * The definition.  Request i is model_ids[i], targets[i] (a target_idx returned earlier), the
+ * excluded row excluded[i * n_excluded ..) in the format and with the rules of
+ * lig_schedule_batch_excluding, and rand_key = first_index + i (mod 2^64).  Fixed-target resolve
+ * against E's model table as it stands at the call (no draw; LIG_DRAW_DOMAIN is not used): the
+ * request is LIG_NO_MODEL when m >= n_models, present[m] == 0, the model has no TargetModels and
+ * t != 255, or it has TargetModels and t >= their count.  Otherwise adapter_id = self_adapter_ids[m]
+ * when t == 255, else target_adapter_ids[offset[m] + t], and Critical = critical[m].  out[i] is
+ * lig_schedule_batch_excluding's pick for the descriptor {adapter_id, Critical, rand_key}, packed as
+ * a lig_mpick {pod_idx, status, target_idx = t}; a LIG_NO_MODEL request gets {-1, LIG_NO_MODEL, 255}.
+ * The pool, the tree, an ejected epoch's pool and the statuses are the descriptor retry's.  The
+ * _fallbacks forms add lig_schedule_batch_excluding_fallbacks's row over the reduced survivor set;
+ * a request that is not LIG_OK gets a row of -1.  The table re-interns target names at every
+ * upload, so a target index stays valid across a refresh that gives adapters new ids.
+ * So, with the target_idx values lig_schedule_models_batch[_fallbacks] returned for the same
+ * (seed, first_index) and rows that exclude nothing, out and the rows are that call's byte for byte
+ * (the pick stream seed ^ rand_key does not depend on the draw), and a model retry equals the
+ * descriptor retry on host-built descriptors.
+ *
+ * Refused for every reason the descriptor counterpart is refused, with LIG_ERR_NO_SNAPSHOT when E
+ * has no model table and LIG_ERR_INVALID for a null `targets` when R > 0; a bad id or target is
+ * data (LIG_NO_MODEL), not a refusal.  Ordered behind the table's upload, both forms register as
+ * readers of E's slot.  Host forms stage pageable or misaligned buffers; device forms refuse buffers
+ * not aligned to their element (ids 4, picks 4, rows 2). */
+int lig_schedule_models_batch_excluding(lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                                        const uint32_t* model_ids, const uint8_t* targets, int R,
+                                        const int16_t* excluded, int n_excluded, lig_mpick* out);
+int lig_schedule_models_batch_excluding_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                                               const uint32_t* d_model_ids, const uint8_t* d_targets, int R,
+                                               const int16_t* d_excluded, int n_excluded, lig_mpick* d_out,
+                                               void* stream);
+int lig_schedule_models_batch_excluding_fallbacks(lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                                                  const uint32_t* model_ids, const uint8_t* targets, int R,
+                                                  const int16_t* excluded, int n_excluded, lig_mpick* out,
+                                                  int n_fallbacks, int16_t* fallbacks);
+int lig_schedule_models_batch_excluding_fallbacks_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed,
+                                                         uint64_t first_index, const uint32_t* d_model_ids,
+                                                         const uint8_t* d_targets, int R, const int16_t* d_excluded,
+                                                         int n_excluded, lig_mpick* d_out, int n_fallbacks,
+                                                         int16_t* d_fallbacks, void* stream);
+
 /* ---- in-batch load feedback (opt-in; the default path never mutates the snapshot) ----------------
  * The reference schedules every request against the scraped metrics as they are
  * (scheduler.go:113-122 never writes them), so all requests of one class that arrive inside a
@@ -790,6 +837,38 @@ int lig_schedule_batch_feedback_chain_excluding_fallbacks_device(lig_ctx* ctx, u
                                                                  lig_pick* d_out, int n_fallbacks,
                                                                  int16_t* d_fallbacks, int window,
                                                                  int32_t* d_loads, void* stream);
+/* Model-id retries under the chain: the model-id retries above (fixed-target resolve, then the
+ * descriptor's retry) as chain calls in every respect.  The requests join the chain's sequence and
+ * windows, and calls of every kind (descriptor and model, plain, fallback and retry) may alternate.
+ * The walk uses the chain's private copy and the tree and thresholds the chain started with.  Only a
+ * LIG_OK pick adds load; LIG_NO_MODEL, DROP, EMPTY and NO_PODS_LEFT count toward the window's length
+ * and add none, and row entries add none.  The model table is read from E's resident slot, as
+ * lig_schedule_models_batch_feedback_chain reads it.  So with the target_idx values the plain model
+ * chain call returned at the same positions and rows that exclude nothing, picks, rows and loads are
+ * that call's byte for byte.  Refused, leaving the chain exactly as it was, for every reason the
+ * descriptor chain retry calls are refused, with LIG_ERR_NO_SNAPSHOT when E has no model table, and
+ * with LIG_ERR_INVALID for a null `targets` when R > 0.  Host forms stage pageable targets in
+ * stream-ordered device memory, as they stage excluded rows. */
+int lig_schedule_models_batch_feedback_chain_excluding(lig_ctx* ctx, uint64_t epoch, uint64_t seed,
+                                                       uint64_t first_index, const uint32_t* model_ids,
+                                                       const uint8_t* targets, int R, const int16_t* excluded,
+                                                       int n_excluded, lig_mpick* out, int window, int32_t* loads);
+int lig_schedule_models_batch_feedback_chain_excluding_device(lig_ctx* ctx, uint64_t epoch, uint64_t seed,
+                                                              uint64_t first_index, const uint32_t* d_model_ids,
+                                                              const uint8_t* d_targets, int R,
+                                                              const int16_t* d_excluded, int n_excluded,
+                                                              lig_mpick* d_out, int window, int32_t* d_loads,
+                                                              void* stream);
+int lig_schedule_models_batch_feedback_chain_excluding_fallbacks(lig_ctx* ctx, uint64_t epoch, uint64_t seed,
+                                                                 uint64_t first_index, const uint32_t* model_ids,
+                                                                 const uint8_t* targets, int R,
+                                                                 const int16_t* excluded, int n_excluded,
+                                                                 lig_mpick* out, int n_fallbacks, int16_t* fallbacks,
+                                                                 int window, int32_t* loads);
+int lig_schedule_models_batch_feedback_chain_excluding_fallbacks_device(
+    lig_ctx* ctx, uint64_t epoch, uint64_t seed, uint64_t first_index, const uint32_t* d_model_ids,
+    const uint8_t* d_targets, int R, const int16_t* d_excluded, int n_excluded, lig_mpick* d_out, int n_fallbacks,
+    int16_t* d_fallbacks, int window, int32_t* d_loads, void* stream);
 /* The next chain call starts a new chain. */
 int lig_feedback_chain_reset(lig_ctx* ctx);
 

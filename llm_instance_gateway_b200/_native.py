@@ -59,6 +59,11 @@ EXPORTED_SYMBOLS = (
     "lig_schedule_batch_feedback_chain_excluding_fallbacks",
     "lig_schedule_batch_feedback_chain_excluding_fallbacks_device",
     "lig_eject_pods",
+    "lig_schedule_models_batch_excluding", "lig_schedule_models_batch_excluding_device",
+    "lig_schedule_models_batch_excluding_fallbacks", "lig_schedule_models_batch_excluding_fallbacks_device",
+    "lig_schedule_models_batch_feedback_chain_excluding", "lig_schedule_models_batch_feedback_chain_excluding_device",
+    "lig_schedule_models_batch_feedback_chain_excluding_fallbacks",
+    "lig_schedule_models_batch_feedback_chain_excluding_fallbacks_device",
 )
 
 
@@ -194,6 +199,21 @@ def load() -> C.CDLL:
                                                                           vp, i32, vp]
     lib.lig_schedule_batch_feedback_chain_excluding_fallbacks_device.argtypes = [vp, u64, u64, vp, i32, vp, i32, vp,
                                                                                  i32, vp, i32, vp, vp]
+    # model-id retries: the descriptor counterpart's arguments with first_index, model_ids, targets
+    lib.lig_schedule_models_batch_excluding.argtypes = [vp, u64, u64, u64, vp, vp, i32, vp, i32, vp]
+    lib.lig_schedule_models_batch_excluding_device.argtypes = [vp, u64, u64, u64, vp, vp, i32, vp, i32, vp, vp]
+    lib.lig_schedule_models_batch_excluding_fallbacks.argtypes = [vp, u64, u64, u64, vp, vp, i32, vp, i32, vp, i32,
+                                                                  vp]
+    lib.lig_schedule_models_batch_excluding_fallbacks_device.argtypes = [vp, u64, u64, u64, vp, vp, i32, vp, i32, vp,
+                                                                         i32, vp, vp]
+    lib.lig_schedule_models_batch_feedback_chain_excluding.argtypes = [vp, u64, u64, u64, vp, vp, i32, vp, i32, vp,
+                                                                       i32, vp]
+    lib.lig_schedule_models_batch_feedback_chain_excluding_device.argtypes = [vp, u64, u64, u64, vp, vp, i32, vp,
+                                                                              i32, vp, i32, vp, vp]
+    lib.lig_schedule_models_batch_feedback_chain_excluding_fallbacks.argtypes = [vp, u64, u64, u64, vp, vp, i32, vp,
+                                                                                 i32, vp, i32, vp, i32, vp]
+    lib.lig_schedule_models_batch_feedback_chain_excluding_fallbacks_device.argtypes = [
+        vp, u64, u64, u64, vp, vp, i32, vp, i32, vp, i32, vp, i32, vp, vp]
     lib.lig_update_snapshot.argtypes = [vp, u64, u64, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.lig_eject_pods.argtypes = [vp, u64, u64, vp, i32]
     lib.lig_pick_kernel_info.argtypes = [vp, u64, C.c_char_p, i32, C.POINTER(i32), C.POINTER(i32),

@@ -560,6 +560,55 @@ Status Scheduler::ScheduleModelWithFallbacks(const std::string& model, int n, st
   return w.status;
 }
 
+Status Scheduler::ScheduleModelRetry(const std::string& model, const std::string& resolvedTargetModel,
+                                     const std::vector<backend::Pod>& tried, backend::Pod* targetPod) {
+  if (tried.size() > (size_t)LIG_MAX_EXCLUDED)
+    return Errorf(InvalidArgument, "ScheduleModelRetry: " + std::to_string(tried.size()) + " tried pods (at most " +
+                                       std::to_string(LIG_MAX_EXCLUDED) + ")");
+  if (opt_.load_feedback_window > 0 && !opt_.feedback_retries)
+    return Errorf(InvalidArgument, "ScheduleModelRetry: not defined under load_feedback_window without "
+                                   "feedback_retries (the picks come from the feedback chain's copy of the "
+                                   "snapshot, a retry would not)");
+  if (group_)
+    return Errorf(InvalidArgument, "ScheduleModelRetry: a scheduler over several devices has no retry call");
+  Waiter w;
+  w.model = &model;
+  w.target = &resolvedTargetModel;
+  w.tried = &tried;
+  Submit(w);
+  if (w.status.ok() && targetPod) *targetPod = std::move(w.pod);
+  return w.status;
+}
+
+Status Scheduler::ScheduleModelRetryWithFallbacks(const std::string& model, const std::string& resolvedTargetModel,
+                                                  const std::vector<backend::Pod>& tried, int n,
+                                                  std::vector<backend::Pod>* pods) {
+  if (pods) pods->clear();
+  if (n < 1 || n > LIG_MAX_FALLBACKS)
+    return Errorf(InvalidArgument, "ScheduleModelRetryWithFallbacks: n=" + std::to_string(n) + " outside [1, " +
+                                       std::to_string(LIG_MAX_FALLBACKS) + "]");
+  if (tried.size() > (size_t)LIG_MAX_EXCLUDED)
+    return Errorf(InvalidArgument, "ScheduleModelRetryWithFallbacks: " + std::to_string(tried.size()) +
+                                       " tried pods (at most " + std::to_string(LIG_MAX_EXCLUDED) + ")");
+  if (opt_.load_feedback_window > 0 && !(opt_.feedback_retries && opt_.feedback_fallbacks))
+    return Errorf(InvalidArgument, "ScheduleModelRetryWithFallbacks: not defined under load_feedback_window without "
+                                   "feedback_retries and feedback_fallbacks (the picks come from the feedback "
+                                   "chain's copy of the snapshot, these would not)");
+  if (group_)
+    return Errorf(InvalidArgument,
+                  "ScheduleModelRetryWithFallbacks: a scheduler over several devices has no retry call");
+  std::vector<backend::Pod> ranked;
+  Waiter w;
+  w.model = &model;
+  w.target = &resolvedTargetModel;
+  w.tried = &tried;
+  w.fallbacks = n;
+  w.pods = &ranked;
+  Submit(w);
+  if (w.status.ok() && pods) *pods = std::move(ranked);
+  return w.status;
+}
+
 Status Scheduler::Filter(const LLMRequest& req, std::vector<backend::Pod>* pods) {
   if (group_)
     return Errorf(InvalidArgument, "Filter: a scheduler over several devices has no survivor-list call");
@@ -713,7 +762,9 @@ void Scheduler::Flush(std::vector<Waiter*>& all) {
   desc_lane_.clear();
   model_lane_.clear();
   retry_lane_.clear();
-  for (Waiter* w : all) (w->model ? model_lane_ : w->tried ? retry_lane_ : desc_lane_).push_back(w);
+  model_retry_lane_.clear();
+  for (Waiter* w : all)
+    (w->model ? (w->tried ? model_retry_lane_ : model_lane_) : w->tried ? retry_lane_ : desc_lane_).push_back(w);
   std::vector<Waiter*>& batch = desc_lane_;
   size_t done = 0;
   const auto flush_t0 = std::chrono::steady_clock::now();
@@ -804,6 +855,7 @@ void Scheduler::Flush(std::vector<Waiter*>& all) {
   }
   FlushRetries(retry_lane_);
   FlushModels(model_lane_);
+  FlushModelRetries(model_retry_lane_);
   const double flush_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - flush_t0).count();
   std::lock_guard<std::mutex> sk(stats_mu_);
   if (device_us > stats_.max_device_call_us) {
@@ -812,6 +864,23 @@ void Scheduler::Flush(std::vector<Waiter*>& all) {
     stats_.slowest_call_batch = stats_.batches ? stats_.batches - 1 : 0;
   }
   stats_.max_flush_us = std::max(stats_.max_flush_us, flush_us);
+}
+
+void Scheduler::TriedRows(const Snapshot& snap, Waiter* const* batch, int n, std::vector<std::vector<int16_t>>* rows,
+                          int* width) {
+  std::unordered_map<std::string, std::vector<int16_t>> where;   // Name + '\0' + Address -> pod indices
+  for (size_t p = 0; p < snap.pods.size(); ++p) where[snap.pods[p].Name + '\0' + snap.pods[p].Address].push_back((int16_t)p);
+  rows->assign((size_t)n, {});
+  *width = 1;
+  for (int i = 0; i < n; ++i) {
+    std::vector<int16_t>& row = (*rows)[(size_t)i];
+    for (const backend::Pod& t : *batch[i]->tried) {
+      auto it = where.find(t.Name + '\0' + t.Address);
+      if (it != where.end()) row.insert(row.end(), it->second.begin(), it->second.end());
+    }
+    // only pods listed more than once in the slice get past 32: that caller is refused
+    if ((int)row.size() <= LIG_MAX_EXCLUDED) *width = std::max(*width, (int)row.size());
+  }
 }
 
 // The retry lane: one lig_schedule_batch_excluding call per max_batch waiters (under
@@ -845,20 +914,7 @@ void Scheduler::FlushRetries(std::vector<Waiter*>& batch) {
         snap = snap_;
         writes_seen = writes_done_;
       }
-      std::unordered_map<std::string, std::vector<int16_t>> where;   // Name + '\0' + Address -> pod indices
-      for (size_t p = 0; p < snap->pods.size(); ++p)
-        where[snap->pods[p].Name + '\0' + snap->pods[p].Address].push_back((int16_t)p);
-      rows.assign((size_t)n, {});
-      width = 1;
-      for (int i = 0; i < n; ++i) {
-        std::vector<int16_t>& row = rows[(size_t)i];
-        for (const backend::Pod& t : *batch[done + i]->tried) {
-          auto it = where.find(t.Name + '\0' + t.Address);
-          if (it != where.end()) row.insert(row.end(), it->second.begin(), it->second.end());
-        }
-        // only pods listed more than once in the slice get past 32: that caller is refused below
-        if ((int)row.size() <= LIG_MAX_EXCLUDED) width = std::max(width, (int)row.size());
-      }
+      TriedRows(*snap, batch.data() + done, n, &rows, &width);
       slot.assign((size_t)n, -1);
       k = 0;
       for (int i = 0; i < n; ++i) {
@@ -932,6 +988,35 @@ void Scheduler::FlushRetries(std::vector<Waiter*>& batch) {
   }
 }
 
+// A model request's result from its device pick (and row), with ScheduleModel's errors.
+static constexpr const char* kModelPrefix = "failed to find target pod: ";            // request.go:73-75
+
+template <class Snap, class W>
+static void ModelPickResult(const Snap& snap, const backend::InferenceModel& im, const lig_mpick& pk, const int16_t* row,
+                            W* w) {
+  const std::string prefix = kModelPrefix;
+  if (pk.status == LIG_OK) {
+    w->pod = snap.pods[(size_t)pk.pod_idx];
+    if (w->fallbacks > 0) {
+      w->pods->push_back(w->pod);
+      for (int f = 0; f < w->fallbacks && row[f] >= 0; ++f) w->pods->push_back(snap.pods[(size_t)row[f]]);
+    }
+  } else if (pk.status == LIG_DROP) {
+    w->status = Errorf(ResourceExhausted, prefix + "failed to apply filter, resulted 0 pods, this should never "
+                                                   "happen: " + kDropInner);
+  } else if (pk.status == LIG_NO_PODS_LEFT) {
+    w->status = Errorf(Unknown, prefix + "failed to apply filter, resulted 0 pods, this should never happen: "
+                                         "no pods left");
+  } else if (pk.status == LIG_EMPTY) {
+    w->status = Errorf(Unknown, prefix + "failed to apply filter, resulted 0 pods, this should never happen: "
+                                         "%!w(<nil>)");
+  } else {   // LIG_NO_MODEL: absent models and targets are answered on the host and never sent
+    w->status = Errorf(Internal, prefix + "rpc error: code = Internal desc = model id " +
+                                     std::to_string(w->model_id) + " (" + im.ModelName +
+                                     ") has no model entry on the device");
+  }
+}
+
 // The model-id lane: names are mapped to ids against the captured epoch's list; names the host can
 // answer from that list alone never reach the device.  Request k that reaches the device has
 // rand_key = model_index_ + k; a stale-epoch retry maps again and reuses the same first_index.
@@ -996,7 +1081,7 @@ void Scheduler::FlushModels(std::vector<Waiter*>& batch) {
     }
     if (k > 0) model_index_ += (uint64_t)k;
     const Status failure = rc != 0 ? LigFailure(call) : Status{};
-    const std::string prefix = "failed to find target pod: ";                        // request.go:73-75
+    const std::string prefix = kModelPrefix;
     for (int i = 0, j = 0; i < n; ++i) {
       Waiter* w = batch[done + i];
       if (w->model_id < 0) continue;
@@ -1010,31 +1095,141 @@ void Scheduler::FlushModels(std::vector<Waiter*>& batch) {
       const backend::InferenceModel& im = *snap->models->models[(size_t)w->model_id];
       // 255: TargetModels is empty and the requested name passes through (request.go:47)
       w->resolved = pk.target_idx == 255 ? *w->model : im.TargetModels[pk.target_idx].Name;
-      if (pk.status == LIG_OK) {
-        w->pod = snap->pods[(size_t)pk.pod_idx];
-        if (w->fallbacks > 0) {
-          w->pods->push_back(w->pod);
-          for (int f = 0; f < w->fallbacks && row[f] >= 0; ++f) w->pods->push_back(snap->pods[(size_t)row[f]]);
-        }
-      } else if (pk.status == LIG_DROP) {
-        w->status = Errorf(ResourceExhausted, prefix + "failed to apply filter, resulted 0 pods, this should never "
-                                                       "happen: " + kDropInner);
-      } else if (pk.status == LIG_NO_PODS_LEFT) {
-        w->status = Errorf(Unknown, prefix + "failed to apply filter, resulted 0 pods, this should never happen: "
-                                             "no pods left");
-      } else if (pk.status == LIG_EMPTY) {
-        w->status = Errorf(Unknown, prefix + "failed to apply filter, resulted 0 pods, this should never happen: "
-                                             "%!w(<nil>)");
-      } else {   // LIG_NO_MODEL: absent models are answered on the host and never sent
-        w->status = Errorf(Internal, prefix + "rpc error: code = Internal desc = model id " +
-                                         std::to_string(w->model_id) + " (" + im.ModelName +
-                                         ") has no model entry on the device");
-      }
+      ModelPickResult(*snap, im, pk, row, w);
     }
     {
       std::lock_guard<std::mutex> sk(stats_mu_);
       stats_.model_scheduled += (uint64_t)n;
       for (int i = 0; i < n; ++i) stats_.fallback_scheduled += batch[done + i]->fallbacks > 0 ? 1 : 0;
+      stats_.model_batches += k > 0 ? 1 : 0;
+    }
+    for (int i = 0; i < n; ++i) {
+      Waiter* w = batch[done + i];
+      w->done.store(1, std::memory_order_release);
+      w->done.notify_one();
+      w->done.store(2, std::memory_order_release);   // last access: the caller may now destroy *w
+    }
+    done += (size_t)n;
+  }
+}
+
+// The model-retry lane: per max_batch waiters, names are mapped against the captured epoch's list (the
+// model to its id, the resolved target to its index, 255 for a model without TargetModels), tried pods
+// to their indices; waiters the host can answer never reach the device and take no rand_key.  Request k
+// that reaches the device has rand_key = model_index_ + k.  One lig_schedule_models_batch_excluding call
+// (with fallback rows at the largest n asked when any caller wants them; under load_feedback_window the
+// chain forms); a stale-epoch retry maps again and reuses the same first_index.
+void Scheduler::FlushModelRetries(std::vector<Waiter*>& batch) {
+  if (batch.empty()) return;
+  Status failure;
+  if (!h_excluded_) {
+    h_excluded_ = static_cast<int16_t*>(lig_host_alloc((size_t)opt_.max_batch * LIG_MAX_EXCLUDED * sizeof(int16_t)));
+    if (!h_excluded_) failure = LigFailure("lig_host_alloc");
+  }
+  model_targets_.resize((size_t)opt_.max_batch);
+  std::vector<std::vector<int16_t>> rows;
+  const int W = opt_.load_feedback_window;
+  size_t done = 0;
+  while (done < batch.size()) {
+    const int n = (int)std::min(batch.size() - done, (size_t)opt_.max_batch);
+    std::shared_ptr<const Snapshot> snap;
+    int rc = 0, k = 0, nf = 0, width = 1;
+    bool mapped = false;   // the waiters were mapped against a snapshot (host answers are in place)
+    const char* call = "lig_schedule_models_batch_excluding";
+    uint64_t writes_seen = 0;
+    for (int attempt = 0; failure.ok() && attempt < kStaleAttempts; ++attempt) {
+      {
+        std::lock_guard<std::mutex> lk(snap_mu_);
+        snap = snap_;
+        writes_seen = writes_done_;
+      }
+      const ModelList* list = snap->models.get();
+      TriedRows(*snap, batch.data() + done, n, &rows, &width);
+      mapped = true;
+      k = 0;
+      nf = 0;
+      for (int i = 0; i < n; ++i) {
+        Waiter* w = batch[done + i];
+        w->model_id = -1;
+        auto it = list ? list->ids.find(*w->model) : decltype(list->ids)::const_iterator{};
+        if (!list || it == list->ids.end()) {                                       // request.go:42-45
+          w->status = Errorf(Unknown, "error finding a model object in InferenceModel for input " + *w->model);
+          continue;
+        }
+        if (!list->present[it->second]) {                                           // request.go:48-51
+          w->status = Errorf(Unknown, "error getting target model name for model " +
+                                          list->models[it->second]->ModelName);
+          continue;
+        }
+        const backend::InferenceModel& im = *list->models[it->second];
+        int t = -1;
+        if (im.TargetModels.empty()) {
+          if (*w->target == *w->model) t = 255;                                      // request.go:47
+        } else {
+          for (size_t j = 0; j < im.TargetModels.size() && t < 0; ++j)
+            if (im.TargetModels[j].Name == *w->target) t = (int)j;
+        }
+        if (t < 0) {
+          w->status = Errorf(InvalidArgument, "ScheduleModelRetry: " + *w->target + " is not a target model of " +
+                                                  *w->model);
+          continue;
+        }
+        const std::vector<int16_t>& ex = rows[(size_t)i];
+        if (ex.size() > (size_t)LIG_MAX_EXCLUDED) {
+          w->status = Errorf(InvalidArgument, "ScheduleModelRetry: the tried pods match more than " +
+                                                  std::to_string(LIG_MAX_EXCLUDED) + " pods of the snapshot");
+          continue;
+        }
+        w->model_id = it->second;
+        w->status = Status{};   // a retry may map a name the previous epoch answered on the host
+        w->resolved = *w->target;
+        h_model_ids_[k] = it->second;
+        model_targets_[(size_t)k] = (uint8_t)t;
+        int16_t* row = h_excluded_ + (size_t)k * (size_t)width;
+        for (int j = 0; j < width; ++j) row[j] = j < (int)ex.size() ? ex[(size_t)j] : (int16_t)-1;
+        nf = std::max(nf, w->fallbacks);   // rows only for the requests the device sees
+        ++k;
+      }
+      if (k == 0) break;
+      if (nf > 0 && W > 0) {
+        call = "lig_schedule_models_batch_feedback_chain_excluding_fallbacks";
+        rc = lig_schedule_models_batch_feedback_chain_excluding_fallbacks(
+            ctx_, snap->epoch, seed_, model_index_, h_model_ids_, model_targets_.data(), k, h_excluded_, width,
+            h_mpicks_, nf, h_fallbacks_, W, nullptr);
+      } else if (nf > 0) {
+        call = "lig_schedule_models_batch_excluding_fallbacks";
+        rc = lig_schedule_models_batch_excluding_fallbacks(ctx_, snap->epoch, seed_, model_index_, h_model_ids_,
+                                                           model_targets_.data(), k, h_excluded_, width, h_mpicks_, nf,
+                                                           h_fallbacks_);
+      } else if (W > 0) {
+        call = "lig_schedule_models_batch_feedback_chain_excluding";
+        rc = lig_schedule_models_batch_feedback_chain_excluding(ctx_, snap->epoch, seed_, model_index_, h_model_ids_,
+                                                                model_targets_.data(), k, h_excluded_, width,
+                                                                h_mpicks_, W, nullptr);
+      } else {
+        rc = lig_schedule_models_batch_excluding(ctx_, snap->epoch, seed_, model_index_, h_model_ids_,
+                                                 model_targets_.data(), k, h_excluded_, width, h_mpicks_);
+      }
+      if (rc == 0 && W > 0) CountFeedback(snap->epoch, k);
+      if (!AwaitPublication(rc, writes_seen, attempt)) break;
+    }
+    if (k > 0) model_index_ += (uint64_t)k;
+    if (failure.ok() && rc != 0) failure = LigFailure(call);
+    for (int i = 0, j = 0; i < n; ++i) {
+      Waiter* w = batch[done + i];
+      if (mapped && w->model_id < 0) continue;
+      if (!failure.ok()) {
+        w->status = failure;
+        if (w->model_id >= 0) w->status.message = kModelPrefix + w->status.message;
+        continue;
+      }
+      const int16_t* row = h_fallbacks_ + (size_t)j * (size_t)nf;
+      const lig_mpick& pk = h_mpicks_[j++];
+      ModelPickResult(*snap, *snap->models->models[(size_t)w->model_id], pk, row, w);
+    }
+    {
+      std::lock_guard<std::mutex> sk(stats_mu_);
+      stats_.retry_scheduled += (uint64_t)n;
       stats_.model_batches += k > 0 ? 1 : 0;
     }
     for (int i = 0; i < n; ++i) {

@@ -188,7 +188,7 @@ struct Stats {
   uint64_t model_scheduled = 0;    // ScheduleModel(model, ...) calls completed (host-answered ones included)
   uint64_t model_batches = 0;      // device calls issued for model-id requests
   uint64_t fallback_scheduled = 0; // ScheduleWithFallbacks and ScheduleModelWithFallbacks calls completed
-  uint64_t retry_scheduled = 0;    // ScheduleRetry and ScheduleRetryWithFallbacks calls completed
+  uint64_t retry_scheduled = 0;    // ScheduleRetry, ScheduleModelRetry and their WithFallbacks calls completed
   uint64_t ejected_pods = 0;       // pods of the current snapshot left out of the pool (EjectPods)
   uint64_t eject_publishes = 0;    // epochs derived with lig_eject_pods and published
   double last_pack_us = 0;     // last Refresh: provider slice -> columns + bitmap (host)
@@ -236,7 +236,7 @@ class Scheduler {
   // LIG_MAX_EXCLUDED (32) tried pods, with load_feedback_window > 0 unless Options::feedback_retries
   // (then the flush's retries make one lig_schedule_batch_feedback_chain_excluding call instead, and a
   // waiter refused on the host is left out of it, so it loads no pod) and with several devices.  A handler that used
-  // ScheduleModel builds req from the resolved target model it got back and the model's criticality.
+  // ScheduleModel retries with ScheduleModelRetry.
   Status ScheduleRetry(const LLMRequest& req, const std::vector<backend::Pod>& tried, backend::Pod* targetPod);
 
   // ScheduleRetry plus up to n fallback endpoints (1 <= n <= LIG_MAX_FALLBACKS): fills *pods with the
@@ -293,6 +293,33 @@ class Scheduler {
   // the doorbell.  Refused like ScheduleWithFallbacks.
   Status ScheduleModelWithFallbacks(const std::string& model, int n, std::string* resolvedTargetModel,
                                     std::vector<backend::Pod>* pods);
+
+  // The retry of a ScheduleModel(model, ...) request without the pods it tried, keeping the target it
+  // drew: resolvedTargetModel is the name ScheduleModel returned, so the retry does not draw again (the
+  // body went out rewritten to it).  At flush time, against the captured epoch's list, the batcher maps
+  // model to its id and resolvedTargetModel to the first TargetModels entry of that name, or, for a
+  // model without TargetModels, to its own name; the device resolves that target and schedules as
+  // ScheduleRetry does (lig_schedule_models_batch_excluding).  Tried pods are matched by value as in
+  // ScheduleRetry.  Answered on the host, with no rand_key and no place in a feedback window: an
+  // unknown model or one whose weights sum to <= 0 with ScheduleModel's Unknown errors, a name that is
+  // not a target of the model in the current list and tried pods matching more than LIG_MAX_EXCLUDED
+  // pods of the snapshot with InvalidArgument.  Requests that reach the device take their rand_keys
+  // from ScheduleModel's sequence, after the flush's ScheduleModel requests.  Other errors are
+  // ScheduleModel's.  Never through the doorbell; counted in Stats::retry_scheduled, its device calls
+  // in Stats::model_batches.  InvalidArgument for more than LIG_MAX_EXCLUDED tried pods, with
+  // load_feedback_window > 0 unless Options::feedback_retries (then the call is
+  // lig_schedule_models_batch_feedback_chain_excluding), and with several devices.
+  Status ScheduleModelRetry(const std::string& model, const std::string& resolvedTargetModel,
+                            const std::vector<backend::Pod>& tried, backend::Pod* targetPod);
+
+  // ScheduleModelRetry plus up to n fallback endpoints (1 <= n <= LIG_MAX_FALLBACKS), as
+  // ScheduleRetryWithFallbacks adds them to ScheduleRetry: a flush whose model-retry lane holds any such
+  // caller makes one lig_schedule_models_batch[_feedback_chain]_excluding_fallbacks call at the largest
+  // n asked.  Under load_feedback_window it needs both Options::feedback_retries and
+  // Options::feedback_fallbacks; refused otherwise like ScheduleModelRetry.
+  Status ScheduleModelRetryWithFallbacks(const std::string& model, const std::string& resolvedTargetModel,
+                                         const std::vector<backend::Pod>& tried, int n,
+                                         std::vector<backend::Pod>* pods);
 
   // Replace the InferenceModels that ScheduleModel(model, ...) resolves against; of two models
   // with one ModelName the later wins (the reference's datastore is a map).  Publishes a new epoch
@@ -389,6 +416,7 @@ class Scheduler {
     int fallbacks = 0;           // *WithFallbacks: the n asked for (0: Schedule / ScheduleModel)
     std::vector<backend::Pod>* pods = nullptr;   // *WithFallbacks: receives the pick and its row
     const std::vector<backend::Pod>* tried = nullptr;   // ScheduleRetry: the pods to leave out
+    const std::string* target = nullptr;   // ScheduleModelRetry: the resolved target model to keep
     int64_t model_id = -1;       // flush-time id in the captured epoch's table; -1: answered on the host
     std::string resolved;        // model requests: the resolved target model
     Status status;
@@ -402,6 +430,11 @@ class Scheduler {
   void Flush(std::vector<Waiter*>& batch);
   void FlushModels(std::vector<Waiter*>& batch);
   void FlushRetries(std::vector<Waiter*>& batch);
+  void FlushModelRetries(std::vector<Waiter*>& batch);
+  // The tried pods of batch[0 .. n) as indices into snap.pods, matched by value; *width is the widest
+  // row of at most LIG_MAX_EXCLUDED entries (at least 1)
+  static void TriedRows(const Snapshot& snap, Waiter* const* batch, int n, std::vector<std::vector<int16_t>>* rows,
+                        int* width);
   void CountFeedback(uint64_t epoch, int n);
   bool AwaitPublication(int rc, uint64_t writes_seen, int attempt);
   void FinishWrite();
@@ -417,7 +450,9 @@ class Scheduler {
   uint32_t* h_model_ids_ = nullptr;   // pinned, max_batch entries each: the model-id lane
   lig_mpick* h_mpicks_ = nullptr;
   uint64_t model_index_ = 0;          // first_index of the next model-id device call
-  std::vector<Waiter*> desc_lane_, model_lane_, retry_lane_;   // a flush split by kind (batcher thread only)
+  std::vector<Waiter*> desc_lane_, model_lane_, retry_lane_, model_retry_lane_;   // a flush split by kind
+                                                                                  // (batcher thread only)
+  std::vector<uint8_t> model_targets_;   // the model-retry lane's target indices (batcher thread only)
   int16_t* h_excluded_ = nullptr;     // pinned, max_batch x LIG_MAX_EXCLUDED rows (first retry flush)
   uint64_t seed_ = 0;
   uint64_t rng_state_ = 0;

@@ -335,6 +335,42 @@ int ligh_schedule_retry_with_fallbacks(ligh_scheduler* s, const char* resolved, 
 
 uint64_t ligh_retry_scheduled(ligh_scheduler* s) { return s->sched->stats().retry_scheduled; }
 
+int ligh_schedule_model_retry(ligh_scheduler* s, const char* model, const char* resolved,
+                              const char* const* tried_names, const char* const* tried_addrs, int n_tried, char* name,
+                              int name_cap, char* addr, int addr_cap, char* err, int err_cap) {
+  std::vector<backend::Pod> tried;
+  for (int i = 0; i < n_tried; ++i)
+    tried.push_back(backend::Pod{tried_names[i] ? tried_names[i] : "", tried_addrs[i] ? tried_addrs[i] : ""});
+  backend::Pod pod;
+  scheduling::Status st =
+      s->sched->ScheduleModelRetry(std::string(model ? model : ""), std::string(resolved ? resolved : ""), tried, &pod);
+  if (st.ok()) {
+    put(name, name_cap, pod.Name);
+    put(addr, addr_cap, pod.Address);
+  } else {
+    put(err, err_cap, st.message);
+  }
+  return st.code;
+}
+
+int ligh_schedule_model_retry_with_fallbacks(ligh_scheduler* s, const char* model, const char* resolved,
+                                             const char* const* tried_names, const char* const* tried_addrs,
+                                             int n_tried, int n, char* names, int names_cap, int* n_pods, char* err,
+                                             int err_cap) {
+  std::vector<backend::Pod> tried;
+  for (int i = 0; i < n_tried; ++i)
+    tried.push_back(backend::Pod{tried_names[i] ? tried_names[i] : "", tried_addrs[i] ? tried_addrs[i] : ""});
+  std::vector<backend::Pod> pods;
+  scheduling::Status st = s->sched->ScheduleModelRetryWithFallbacks(
+      std::string(model ? model : ""), std::string(resolved ? resolved : ""), tried, n, &pods);
+  std::string joined;
+  for (size_t i = 0; i < pods.size(); ++i) joined += (i ? "\n" : "") + pods[i].Name;
+  if (n_pods) *n_pods = (int)pods.size();
+  put(names, names_cap, joined);
+  if (!st.ok()) put(err, err_cap, st.message);
+  return st.code;
+}
+
 int ligh_eject_pods(ligh_scheduler* s, const char* const* names, const char* const* addrs, int n, char* err,
                     int err_cap) {
   std::vector<backend::Pod> pods;

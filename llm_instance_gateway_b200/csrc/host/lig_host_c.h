@@ -73,6 +73,16 @@ int ligh_schedule_retry_with_fallbacks(ligh_scheduler*, const char* resolved_tar
                                        const char* const* tried_names, const char* const* tried_addrs, int n_tried,
                                        int n, char* names, int names_cap, int* n_pods, char* err, int err_cap);
 uint64_t ligh_retry_scheduled(ligh_scheduler*);      /* Stats::retry_scheduled */
+/* Scheduler::ScheduleModelRetry: returns the gRPC code; resolved_target_model is the name the model call
+ * returned; the tried pods as ligh_schedule_retry's. */
+int ligh_schedule_model_retry(ligh_scheduler*, const char* model, const char* resolved_target_model,
+                              const char* const* tried_names, const char* const* tried_addrs, int n_tried, char* name,
+                              int name_cap, char* addr, int addr_cap, char* err, int err_cap);
+/* Scheduler::ScheduleModelRetryWithFallbacks: as ligh_schedule_retry_with_fallbacks, for a model request. */
+int ligh_schedule_model_retry_with_fallbacks(ligh_scheduler*, const char* model, const char* resolved_target_model,
+                                             const char* const* tried_names, const char* const* tried_addrs,
+                                             int n_tried, int n, char* names, int names_cap, int* n_pods, char* err,
+                                             int err_cap);
 /* Scheduler::EjectPods: the complete ejected set as n (name, address) pairs (n = 0 lets every pod back);
  * returns the gRPC code, err receives the refusal. */
 int ligh_eject_pods(ligh_scheduler*, const char* const* names, const char* const* addrs, int n, char* err,

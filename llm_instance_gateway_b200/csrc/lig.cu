@@ -16,6 +16,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
+#include <utility>
 #include <vector>
 
 #include "lig_device.cuh"
@@ -953,6 +954,16 @@ void abort_write(lig_ctx* c, SnapshotWrite*) { c->upload_mu.unlock(); }
 
 }  // namespace ligi
 
+// The dynamic shared-memory limit of every form of the model-id retry kernel: form I has kStaged = bit 0,
+// kTree = bit 1, kPool = bit 2, kRows = bit 3, kCount = bit 4.
+template <size_t... I>
+static int set_models_excluding_smem(int bytes, std::index_sequence<I...>) {
+  const void* forms[] = {(const void*)lig_schedule_models_excluding_kernel<(I & 1) != 0, (I & 2) != 0, (I & 4) != 0,
+                                                                           (I & 8) != 0, (I & 16) != 0>...};
+  for (const void* fn : forms) CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  return 0;
+}
+
 extern "C" {
 
 const char* lig_last_error(void) { return g_err; }
@@ -1102,6 +1113,7 @@ static int create_impl(lig_ctx* c, int device, int max_pods, int max_adapters, i
       (const void*)lig_schedule_excluding_fallback_count_kernel<true, true, true>, (const void*)lig_schedule_excluding_fallback_count_kernel<false, true, true>,
   };
   for (const void* fn : pool_forms) CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+  if (int rc = set_models_excluding_smem(v, std::make_index_sequence<32>{})) return rc;
   const size_t need = scratch_bytes(words_for(max_pods)) > build_fixed_bytes(words_for(max_pods))
                           ? scratch_bytes(words_for(max_pods)) : build_fixed_bytes(words_for(max_pods));
   if (need > c->smem_optin)
@@ -2307,36 +2319,59 @@ int lig_schedule_models_batch_fallbacks_device(lig_ctx* c, uint64_t epoch, uint6
                          stream);
 }
 
-// ---- retry scheduling (lig_schedule_batch_excluding) ---------------------------------------------------
+// ---- retry scheduling (lig_schedule_[models_]batch_excluding) -----------------------------------------
+// One retry call: descriptors in, lig_pick out; or (models) model ids in at the fixed targets
+// targets[i], lig_mpick out, request i with rand_key = first_index + i, resolved against the model
+// table mtab of n_models entries (set where the call is enqueued).
 struct ExcludingCall {
   uint64_t seed;
-  const lig_req* reqs;
+  const void* in;                        // lig_req[R] or uint32_t[R]
   int R;
-  lig_pick* out;
+  void* out;                             // lig_pick[R] or lig_mpick[R]
   int n_excluded;
   const int16_t* excluded;
+  bool models = false;
+  uint64_t first_index = 0;
+  const uint8_t* targets = nullptr;
+  const unsigned char* mtab = nullptr;
+  uint32_t n_models = 0;
+  size_t in_bytes() const { return models ? sizeof(uint32_t) : sizeof(lig_req); }
+  size_t out_bytes() const { return models ? sizeof(lig_mpick) : sizeof(lig_pick); }
   size_t row_bytes() const { return (size_t)n_excluded * sizeof(int16_t); }
 };
 
+static ExcludingCall model_retry(uint64_t seed, uint64_t first_index, const uint32_t* ids, const uint8_t* targets,
+                                 int R, const int16_t* excluded, int n_excluded, lig_mpick* out) {
+  ExcludingCall x{seed, ids, R, out, n_excluded, excluded};
+  x.models = true;
+  x.first_index = first_index;
+  x.targets = targets;
+  return x;
+}
+
 static int excluding_check(const lig_ctx* c, const char* fn, const ExcludingCall& x) {
-  if (!c || x.R < 0 || (x.R > 0 && (!x.reqs || !x.out || !x.excluded)))
+  if (!c || x.R < 0 || (x.R > 0 && (!x.in || !x.out || !x.excluded || (x.models && !x.targets))))
     return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
   if (x.n_excluded < 1 || x.n_excluded > LIG_MAX_EXCLUDED)
     return fail(LIG_ERR_INVALID, "%s: n_excluded=%d outside [1, %d]", fn, x.n_excluded, LIG_MAX_EXCLUDED);
   return 0;
 }
 
-// Launch the retry walk for x (R >= 1, device-visible, aligned pointers) over slot s on st, with the
-// scan's launch shape: `tree` (null = the built-in tree with `thr`); `hist` non-null counts each
-// LIG_OK pick into it (the feedback chain's segment).  The caller checks the launch.
+static int excluding_slot(lig_ctx* c, const ExcludingCall& x, uint64_t epoch, Slot** s) {
+  return x.models ? resolve_models_slot(c, epoch, s) : resolve_slot(c, epoch, s);
+}
+
+// Launch the retry walk for x (descriptors; R >= 1, device-visible, aligned pointers) over slot s on
+// st, with the scan's launch shape: `tree` (null = the built-in tree with `thr`); `hist` non-null
+// counts each LIG_OK pick into it (the feedback chain's segment).  The caller checks the launch.
 static void launch_excluding(const lig_ctx* c, const Slot& s, const Thr& thr, const FilterTree* tree,
                              const ExcludingCall& x, int* hist, cudaStream_t st) {
   static const FilterTree kNoTree{};
   const ScanShape sh = scan_shape(c, s, x.R);
   const SnapView v = view_of(s);
   const FilterTree& t = tree ? *tree : kNoTree;
-  const int4* in = reinterpret_cast<const int4*>(x.reqs);
-  int2* out = reinterpret_cast<int2*>(x.out);
+  const int4* in = static_cast<const int4*>(x.in);
+  int2* out = static_cast<int2*>(x.out);
   auto launch = [&](auto staged, auto caller_tree) {
     constexpr bool kS = decltype(staged)::value, kT = decltype(caller_tree)::value;
     if (hist && s.n_ejected > 0)
@@ -2363,94 +2398,90 @@ static void launch_excluding(const lig_ctx* c, const Slot& s, const Thr& thr, co
   }
 }
 
+// Launch the model-id retry walk for x (models; R >= 1, device-visible, aligned pointers, x.mtab set)
+// over slot s on st, with the scan's launch shape: `tree` as above; a row of n_fallbacks per request
+// when n_fallbacks > 0; `hist` non-null counts each LIG_OK pick into it.  The caller checks the launch.
+static void launch_models_excluding(const lig_ctx* c, const Slot& s, const Thr& thr, const FilterTree* tree,
+                                    const ExcludingCall& x, int n_fallbacks, int16_t* fallbacks, int* hist,
+                                    cudaStream_t st) {
+  static const FilterTree kNoTree{};
+  const ScanShape sh = scan_shape(c, s, x.R);
+  const SnapView v = view_of(s);
+  const FilterTree& t = tree ? *tree : kNoTree;
+  const uint32_t* pool = s.n_ejected > 0 ? s.d_pool : nullptr;
+  auto launch = [&](auto staged, auto caller_tree, auto ejected, auto rows, auto count) {
+    lig_schedule_models_excluding_kernel<decltype(staged)::value, decltype(caller_tree)::value,
+                                         decltype(ejected)::value, decltype(rows)::value, decltype(count)::value>
+        <<<sh.grid, kCtaThreads, sh.smem, st>>>(v, thr, t, static_cast<const uint32_t*>(x.in), x.targets, x.excluded,
+                                                x.n_excluded, static_cast<uint32_t*>(x.out), x.R, x.seed,
+                                                x.first_index, x.mtab, x.n_models, n_fallbacks, fallbacks, hist,
+                                                pool);
+  };
+  using Y = std::true_type;
+  using N = std::false_type;
+  auto with_count = [&](auto... f) { if (hist) launch(f..., Y{}); else launch(f..., N{}); };
+  auto with_rows = [&](auto... f) { if (n_fallbacks > 0) with_count(f..., Y{}); else with_count(f..., N{}); };
+  auto with_pool = [&](auto... f) { if (pool) with_rows(f..., Y{}); else with_rows(f..., N{}); };
+  auto with_tree = [&](auto... f) { if (tree) with_pool(f..., Y{}); else with_pool(f..., N{}); };
+  if (sh.staged) with_tree(Y{});
+  else with_tree(N{});
+}
+
+// The model-id form of x against slot s: ordered behind the slot's model table on st, reading it.
+// Caller holds c->mu.
+static int with_model_table(Slot& s, ExcludingCall* x, cudaStream_t st) {
+  CUDA_TRY(cudaStreamWaitEvent(st, s.models_ready, 0));
+  x->mtab = s.d_mtab;
+  x->n_models = s.n_models;
+  return 0;
+}
+
 // Enqueue the retry kernel for x (R >= 1, device-visible, aligned pointers) against slot s on st,
 // behind the slot's tables, and register st as a reader of the slot.  The walk is the tree that
 // built the slot's tables.  Caller holds c->mu.
 static int enqueue_excluding(lig_ctx* c, Slot& s, const ExcludingCall& x, cudaStream_t st) {
   CUDA_TRY(cudaStreamWaitEvent(st, s.ready, 0));
-  launch_excluding(c, s, thr_of(c), s.caller_tree ? &s.tree : nullptr, x, nullptr, st);
+  if (x.models) {
+    ExcludingCall m = x;
+    if (int rc = with_model_table(s, &m, st)) return rc;
+    launch_models_excluding(c, s, thr_of(c), s.caller_tree ? &s.tree : nullptr, m, 0, nullptr, nullptr, st);
+  } else {
+    launch_excluding(c, s, thr_of(c), s.caller_tree ? &s.tree : nullptr, x, nullptr, st);
+  }
   CUDA_TRY(cudaGetLastError());
   c->launches++;
   return note_reader(s, st);
 }
 
-int lig_schedule_batch_excluding_device(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* d_reqs, int R,
-                                        const int16_t* d_excluded, int n_excluded, lig_pick* d_out, void* stream) {
-  static const char fn[] = "lig_schedule_batch_excluding_device";
-  const ExcludingCall x{seed, d_reqs, R, d_out, n_excluded, d_excluded};
+static int excluding_device(lig_ctx* c, const char* fn, uint64_t epoch, const ExcludingCall& x, void* stream) {
   if (int rc = excluding_check(c, fn, x)) return rc;
-  if (R > 0 && (misaligned(d_reqs, sizeof(lig_req)) || misaligned(d_out, sizeof(lig_pick)) ||
-                misaligned(d_excluded, sizeof(int16_t))))
+  if (x.R > 0 && (misaligned(x.in, x.in_bytes()) || misaligned(x.out, x.out_bytes()) ||
+                  misaligned(x.excluded, sizeof(int16_t))))
     return fail(LIG_ERR_INVALID, "%s: a device buffer is not aligned to its element", fn);
   std::lock_guard<std::mutex> lk(c->mu);
   Slot* s = nullptr;
-  if (int rc = resolve_slot(c, epoch, &s)) return rc;
-  if (R == 0) return 0;
+  if (int rc = excluding_slot(c, x, epoch, &s)) return rc;
+  if (x.R == 0) return 0;
   CUDA_TRY(cudaSetDevice(c->device));
   return enqueue_excluding(c, *s, x, static_cast<cudaStream_t>(stream));
 }
 
-// Host buffers: page-locked, aligned ones are read and written by the kernel in place; the others
-// are staged in stream-ordered HBM and copied on the call's lane.  Blocks until the picks are back.
-int lig_schedule_batch_excluding(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
-                                 const int16_t* excluded, int n_excluded, lig_pick* out) {
-  static const char fn[] = "lig_schedule_batch_excluding";
-  const ExcludingCall x{seed, reqs, R, out, n_excluded, excluded};
-  if (int rc = excluding_check(c, fn, x)) return rc;
-  if (R > c->max_batch) return fail(LIG_ERR_INVALID, "%s: R=%d exceeds max_batch=%d", fn, R, c->max_batch);
-  ExcludingCall d = x;    // the same call with device-visible pointers
-  const size_t in_b = (size_t)R * sizeof(lig_req), out_b = (size_t)R * sizeof(lig_pick);
-  const size_t rows_b = (size_t)R * x.row_bytes();
-  d.reqs = R ? mapped_device_pointer(reqs) : nullptr;
-  d.out = R ? mapped_device_pointer(out) : nullptr;
-  d.excluded = R ? mapped_device_pointer(excluded) : nullptr;
-  // the kernel reads a descriptor with one 16-byte load and stores every pick whole
-  const bool st_in = R && (!d.reqs || misaligned(d.reqs, sizeof(lig_req)));
-  const bool st_out = R && (!d.out || misaligned(d.out, sizeof(lig_pick)));
-  const bool st_rows = R && (!d.excluded || misaligned(d.excluded, sizeof(int16_t)));
-  cudaStream_t st = nullptr;
-  unsigned char* stage = nullptr;
-  {
-    std::lock_guard<std::mutex> lk(c->mu);
-    Slot* s = nullptr;
-    if (int rc = resolve_slot(c, epoch, &s)) return rc;
-    if (R == 0) return 0;
-    CUDA_TRY(cudaSetDevice(c->device));
-    st = c->s_lane[c->next_lane];
-    c->next_lane = (c->next_lane + 1) % kLanes;
-    size_t at = 0, o_in = 0, o_out = 0, o_rows = 0;
-    auto take = [&](bool on, size_t bytes, size_t* o) { if (on) { *o = at; at = (at + bytes + 255) & ~(size_t)255; } };
-    take(st_in, in_b, &o_in);
-    take(st_out, out_b, &o_out);
-    take(st_rows, rows_b, &o_rows);
-    if (at) {
-      CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&stage), at, st));
-      if (st_in) d.reqs = reinterpret_cast<const lig_req*>(stage + o_in);
-      if (st_out) d.out = reinterpret_cast<lig_pick*>(stage + o_out);
-      if (st_rows) d.excluded = reinterpret_cast<const int16_t*>(stage + o_rows);
-    }
-    int rc = 0;
-    if (st_in && cudaMemcpyAsync(const_cast<lig_req*>(d.reqs), reqs, in_b, cudaMemcpyHostToDevice, st) != cudaSuccess)
-      rc = fail(LIG_ERR_CUDA, "%s: staging the requests failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
-    if (!rc && st_rows &&
-        cudaMemcpyAsync(const_cast<int16_t*>(d.excluded), excluded, rows_b, cudaMemcpyHostToDevice, st) != cudaSuccess)
-      rc = fail(LIG_ERR_CUDA, "%s: staging the rows failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
-    if (!rc) rc = enqueue_excluding(c, *s, d, st);
-    if (rc) {
-      if (stage) cudaFreeAsync(stage, st);
-      return rc;
-    }
-  }
-  // the copy back waits for the kernel on the lane; it may block, so not under c->mu
-  cudaError_t e = cudaSuccess;
-  if (st_out) e = cudaMemcpyAsync(out, d.out, out_b, cudaMemcpyDeviceToHost, st);
-  if (stage) cudaFreeAsync(stage, st);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  if (e != cudaSuccess) return fail(LIG_ERR_CUDA, "%s failed on the device: %s", fn, cudaGetErrorString(e));
-  return 0;
+int lig_schedule_batch_excluding_device(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* d_reqs, int R,
+                                        const int16_t* d_excluded, int n_excluded, lig_pick* d_out, void* stream) {
+  return excluding_device(c, "lig_schedule_batch_excluding_device", epoch,
+                          ExcludingCall{seed, d_reqs, R, d_out, n_excluded, d_excluded}, stream);
 }
 
-// ---- retry scheduling with fallback rows (lig_schedule_batch_excluding_fallbacks) ----------------------
+int lig_schedule_models_batch_excluding_device(lig_ctx* c, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                                               const uint32_t* d_model_ids, const uint8_t* d_targets, int R,
+                                               const int16_t* d_excluded, int n_excluded, lig_mpick* d_out,
+                                               void* stream) {
+  return excluding_device(c, "lig_schedule_models_batch_excluding_device", epoch,
+                          model_retry(seed, first_index, d_model_ids, d_targets, R, d_excluded, n_excluded, d_out),
+                          stream);
+}
+
+// ---- retry scheduling with fallback rows (lig_schedule_[models_]batch_excluding_fallbacks) ------------
 // The retry call's arguments plus a row of n_fallbacks int16 per request; every retry rule applies.
 static int excluding_fallbacks_check(const lig_ctx* c, const char* fn, const ExcludingCall& x, int n_fallbacks,
                                      const int16_t* fallbacks) {
@@ -2468,12 +2499,21 @@ static int enqueue_excluding_fallbacks(lig_ctx* c, Slot& s, const ExcludingCall&
                                        int16_t* fallbacks, cudaStream_t st) {
   static const FilterTree kNoTree{};
   CUDA_TRY(cudaStreamWaitEvent(st, s.ready, 0));
+  if (x.models) {
+    ExcludingCall m = x;
+    if (int rc = with_model_table(s, &m, st)) return rc;
+    launch_models_excluding(c, s, thr_of(c), s.caller_tree ? &s.tree : nullptr, m, n_fallbacks, fallbacks, nullptr,
+                            st);
+    CUDA_TRY(cudaGetLastError());
+    c->launches++;
+    return note_reader(s, st);
+  }
   const ScanShape sh = scan_shape(c, s, x.R);
   const SnapView v = view_of(s);
   const FilterTree& t = s.caller_tree ? s.tree : kNoTree;
   const Thr thr = thr_of(c);
-  const int4* in = reinterpret_cast<const int4*>(x.reqs);
-  int2* out = reinterpret_cast<int2*>(x.out);
+  const int4* in = static_cast<const int4*>(x.in);
+  int2* out = static_cast<int2*>(x.out);
   auto launch = [&](auto staged, auto caller_tree) {
     constexpr bool kS = decltype(staged)::value, kT = decltype(caller_tree)::value;
     if (s.n_ejected > 0)
@@ -2497,75 +2537,96 @@ static int enqueue_excluding_fallbacks(lig_ctx* c, Slot& s, const ExcludingCall&
   return note_reader(s, st);
 }
 
-int lig_schedule_batch_excluding_fallbacks_device(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* d_reqs,
-                                                  int R, const int16_t* d_excluded, int n_excluded, lig_pick* d_out,
-                                                  int n_fallbacks, int16_t* d_fallbacks, void* stream) {
-  static const char fn[] = "lig_schedule_batch_excluding_fallbacks_device";
-  const ExcludingCall x{seed, d_reqs, R, d_out, n_excluded, d_excluded};
+static int excluding_fallbacks_device(lig_ctx* c, const char* fn, uint64_t epoch, const ExcludingCall& x,
+                                      int n_fallbacks, int16_t* d_fallbacks, void* stream) {
   if (int rc = excluding_fallbacks_check(c, fn, x, n_fallbacks, d_fallbacks)) return rc;
-  if (R > 0 && (misaligned(d_reqs, sizeof(lig_req)) || misaligned(d_out, sizeof(lig_pick)) ||
-                misaligned(d_excluded, sizeof(int16_t)) || misaligned(d_fallbacks, sizeof(int16_t))))
+  if (x.R > 0 && (misaligned(x.in, x.in_bytes()) || misaligned(x.out, x.out_bytes()) ||
+                  misaligned(x.excluded, sizeof(int16_t)) || misaligned(d_fallbacks, sizeof(int16_t))))
     return fail(LIG_ERR_INVALID, "%s: a device buffer is not aligned to its element", fn);
   std::lock_guard<std::mutex> lk(c->mu);
   Slot* s = nullptr;
-  if (int rc = resolve_slot(c, epoch, &s)) return rc;
-  if (R == 0) return 0;
+  if (int rc = excluding_slot(c, x, epoch, &s)) return rc;
+  if (x.R == 0) return 0;
   CUDA_TRY(cudaSetDevice(c->device));
   return enqueue_excluding_fallbacks(c, *s, x, n_fallbacks, d_fallbacks, static_cast<cudaStream_t>(stream));
 }
 
-// Host buffers, as lig_schedule_batch_excluding handles them: page-locked, aligned ones are read and
-// written by the kernel in place; the others are staged in stream-ordered HBM and copied on the
-// call's lane.  Blocks until the picks and rows are back.
-int lig_schedule_batch_excluding_fallbacks(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
-                                           const int16_t* excluded, int n_excluded, lig_pick* out,
-                                           int n_fallbacks, int16_t* fallbacks) {
-  static const char fn[] = "lig_schedule_batch_excluding_fallbacks";
-  const ExcludingCall x{seed, reqs, R, out, n_excluded, excluded};
-  if (int rc = excluding_fallbacks_check(c, fn, x, n_fallbacks, fallbacks)) return rc;
+int lig_schedule_batch_excluding_fallbacks_device(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* d_reqs,
+                                                  int R, const int16_t* d_excluded, int n_excluded, lig_pick* d_out,
+                                                  int n_fallbacks, int16_t* d_fallbacks, void* stream) {
+  return excluding_fallbacks_device(c, "lig_schedule_batch_excluding_fallbacks_device", epoch,
+                                    ExcludingCall{seed, d_reqs, R, d_out, n_excluded, d_excluded}, n_fallbacks,
+                                    d_fallbacks, stream);
+}
+
+int lig_schedule_models_batch_excluding_fallbacks_device(lig_ctx* c, uint64_t epoch, uint64_t seed,
+                                                         uint64_t first_index, const uint32_t* d_model_ids,
+                                                         const uint8_t* d_targets, int R, const int16_t* d_excluded,
+                                                         int n_excluded, lig_mpick* d_out, int n_fallbacks,
+                                                         int16_t* d_fallbacks, void* stream) {
+  return excluding_fallbacks_device(
+      c, "lig_schedule_models_batch_excluding_fallbacks_device", epoch,
+      model_retry(seed, first_index, d_model_ids, d_targets, R, d_excluded, n_excluded, d_out), n_fallbacks,
+      d_fallbacks, stream);
+}
+
+// The host buffers of a retry call (with rows when n_fallbacks > 0): page-locked, aligned ones are
+// read and written by the kernel in place; the others are staged in stream-ordered HBM and copied on
+// the call's lane.  Blocks until the picks (and rows) are back.
+static int excluding_host(lig_ctx* c, const char* fn, uint64_t epoch, const ExcludingCall& x, int n_fallbacks,
+                          int16_t* fallbacks) {
+  const int R = x.R;
   if (R > c->max_batch) return fail(LIG_ERR_INVALID, "%s: R=%d exceeds max_batch=%d", fn, R, c->max_batch);
   ExcludingCall d = x;    // the same call with device-visible pointers
-  const size_t in_b = (size_t)R * sizeof(lig_req), out_b = (size_t)R * sizeof(lig_pick);
+  const size_t in_b = (size_t)R * x.in_bytes(), out_b = (size_t)R * x.out_bytes();
   const size_t rows_b = (size_t)R * x.row_bytes(), fb_b = (size_t)R * (size_t)n_fallbacks * sizeof(int16_t);
-  d.reqs = R ? mapped_device_pointer(reqs) : nullptr;
-  d.out = R ? mapped_device_pointer(out) : nullptr;
-  d.excluded = R ? mapped_device_pointer(excluded) : nullptr;
-  int16_t* d_fb = R ? mapped_device_pointer(fallbacks) : nullptr;
-  // the kernel reads a descriptor with one 16-byte load and stores every pick whole
-  const bool st_in = R && (!d.reqs || misaligned(d.reqs, sizeof(lig_req)));
-  const bool st_out = R && (!d.out || misaligned(d.out, sizeof(lig_pick)));
+  const size_t tg_b = x.models ? (size_t)R : 0;
+  d.in = R ? mapped_device_pointer(x.in) : nullptr;
+  d.out = R ? mapped_device_pointer(x.out) : nullptr;
+  d.excluded = R ? mapped_device_pointer(x.excluded) : nullptr;
+  d.targets = R && x.models ? mapped_device_pointer(x.targets) : nullptr;
+  int16_t* d_fb = R && n_fallbacks ? mapped_device_pointer(fallbacks) : nullptr;
+  // the kernels read a descriptor with one 16-byte load and store every pick whole
+  const bool st_in = R && (!d.in || misaligned(d.in, x.in_bytes()));
+  const bool st_out = R && (!d.out || misaligned(d.out, x.out_bytes()));
   const bool st_rows = R && (!d.excluded || misaligned(d.excluded, sizeof(int16_t)));
-  const bool st_fb = R && (!d_fb || misaligned(d_fb, sizeof(int16_t)));
+  const bool st_tg = R && x.models && !d.targets;
+  const bool st_fb = R && n_fallbacks && (!d_fb || misaligned(d_fb, sizeof(int16_t)));
   cudaStream_t st = nullptr;
   unsigned char* stage = nullptr;
   {
     std::lock_guard<std::mutex> lk(c->mu);
     Slot* s = nullptr;
-    if (int rc = resolve_slot(c, epoch, &s)) return rc;
+    if (int rc = excluding_slot(c, x, epoch, &s)) return rc;
     if (R == 0) return 0;
     CUDA_TRY(cudaSetDevice(c->device));
     st = c->s_lane[c->next_lane];
     c->next_lane = (c->next_lane + 1) % kLanes;
-    size_t at = 0, o_in = 0, o_out = 0, o_rows = 0, o_fb = 0;
+    size_t at = 0, o_in = 0, o_out = 0, o_rows = 0, o_tg = 0, o_fb = 0;
     auto take = [&](bool on, size_t bytes, size_t* o) { if (on) { *o = at; at = (at + bytes + 255) & ~(size_t)255; } };
     take(st_in, in_b, &o_in);
     take(st_out, out_b, &o_out);
     take(st_rows, rows_b, &o_rows);
+    take(st_tg, tg_b, &o_tg);
     take(st_fb, fb_b, &o_fb);
     if (at) {
       CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&stage), at, st));
-      if (st_in) d.reqs = reinterpret_cast<const lig_req*>(stage + o_in);
-      if (st_out) d.out = reinterpret_cast<lig_pick*>(stage + o_out);
+      if (st_in) d.in = stage + o_in;
+      if (st_out) d.out = stage + o_out;
       if (st_rows) d.excluded = reinterpret_cast<const int16_t*>(stage + o_rows);
+      if (st_tg) d.targets = stage + o_tg;
       if (st_fb) d_fb = reinterpret_cast<int16_t*>(stage + o_fb);
     }
     int rc = 0;
-    if (st_in && cudaMemcpyAsync(const_cast<lig_req*>(d.reqs), reqs, in_b, cudaMemcpyHostToDevice, st) != cudaSuccess)
+    if (st_in && cudaMemcpyAsync(const_cast<void*>(d.in), x.in, in_b, cudaMemcpyHostToDevice, st) != cudaSuccess)
       rc = fail(LIG_ERR_CUDA, "%s: staging the requests failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
     if (!rc && st_rows &&
-        cudaMemcpyAsync(const_cast<int16_t*>(d.excluded), excluded, rows_b, cudaMemcpyHostToDevice, st) != cudaSuccess)
+        cudaMemcpyAsync(const_cast<int16_t*>(d.excluded), x.excluded, rows_b, cudaMemcpyHostToDevice, st) != cudaSuccess)
       rc = fail(LIG_ERR_CUDA, "%s: staging the rows failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
-    if (!rc) rc = enqueue_excluding_fallbacks(c, *s, d, n_fallbacks, d_fb, st);
+    if (!rc && st_tg &&
+        cudaMemcpyAsync(const_cast<uint8_t*>(d.targets), x.targets, tg_b, cudaMemcpyHostToDevice, st) != cudaSuccess)
+      rc = fail(LIG_ERR_CUDA, "%s: staging the targets failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
+    if (!rc) rc = n_fallbacks ? enqueue_excluding_fallbacks(c, *s, d, n_fallbacks, d_fb, st) : enqueue_excluding(c, *s, d, st);
     if (rc) {
       if (stage) cudaFreeAsync(stage, st);
       return rc;
@@ -2573,12 +2634,48 @@ int lig_schedule_batch_excluding_fallbacks(lig_ctx* c, uint64_t epoch, uint64_t 
   }
   // the copies back wait for the kernel on the lane; they may block, so not under c->mu
   cudaError_t e = cudaSuccess;
-  if (st_out) e = cudaMemcpyAsync(out, d.out, out_b, cudaMemcpyDeviceToHost, st);
+  if (st_out) e = cudaMemcpyAsync(x.out, d.out, out_b, cudaMemcpyDeviceToHost, st);
   if (st_fb && e == cudaSuccess) e = cudaMemcpyAsync(fallbacks, d_fb, fb_b, cudaMemcpyDeviceToHost, st);
   if (stage) cudaFreeAsync(stage, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   if (e != cudaSuccess) return fail(LIG_ERR_CUDA, "%s failed on the device: %s", fn, cudaGetErrorString(e));
   return 0;
+}
+
+int lig_schedule_batch_excluding(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
+                                 const int16_t* excluded, int n_excluded, lig_pick* out) {
+  static const char fn[] = "lig_schedule_batch_excluding";
+  const ExcludingCall x{seed, reqs, R, out, n_excluded, excluded};
+  if (int rc = excluding_check(c, fn, x)) return rc;
+  return excluding_host(c, fn, epoch, x, 0, nullptr);
+}
+
+int lig_schedule_models_batch_excluding(lig_ctx* c, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                                        const uint32_t* model_ids, const uint8_t* targets, int R,
+                                        const int16_t* excluded, int n_excluded, lig_mpick* out) {
+  static const char fn[] = "lig_schedule_models_batch_excluding";
+  const ExcludingCall x = model_retry(seed, first_index, model_ids, targets, R, excluded, n_excluded, out);
+  if (int rc = excluding_check(c, fn, x)) return rc;
+  return excluding_host(c, fn, epoch, x, 0, nullptr);
+}
+
+int lig_schedule_batch_excluding_fallbacks(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
+                                           const int16_t* excluded, int n_excluded, lig_pick* out,
+                                           int n_fallbacks, int16_t* fallbacks) {
+  static const char fn[] = "lig_schedule_batch_excluding_fallbacks";
+  const ExcludingCall x{seed, reqs, R, out, n_excluded, excluded};
+  if (int rc = excluding_fallbacks_check(c, fn, x, n_fallbacks, fallbacks)) return rc;
+  return excluding_host(c, fn, epoch, x, n_fallbacks, fallbacks);
+}
+
+int lig_schedule_models_batch_excluding_fallbacks(lig_ctx* c, uint64_t epoch, uint64_t seed, uint64_t first_index,
+                                                  const uint32_t* model_ids, const uint8_t* targets, int R,
+                                                  const int16_t* excluded, int n_excluded, lig_mpick* out,
+                                                  int n_fallbacks, int16_t* fallbacks) {
+  static const char fn[] = "lig_schedule_models_batch_excluding_fallbacks";
+  const ExcludingCall x = model_retry(seed, first_index, model_ids, targets, R, excluded, n_excluded, out);
+  if (int rc = excluding_fallbacks_check(c, fn, x, n_fallbacks, fallbacks)) return rc;
+  return excluding_host(c, fn, epoch, x, n_fallbacks, fallbacks);
 }
 
 int lig_pick_kernel_info(lig_ctx* c, uint64_t epoch, char* name, int name_len, int* grid, int* threads,
@@ -2688,6 +2785,7 @@ struct FbReqs {
   bool retry = false;                    // a chain retry call: request i excludes the pods of
   const int16_t* excluded = nullptr;     //   excluded + i * n_excluded (with rows: a chain retry
   int n_excluded = 0;                    //   call with fallback rows)
+  const uint8_t* targets = nullptr;      // a model-id retry call: request i's fixed target
   size_t in_bytes() const { return models ? sizeof(uint32_t) : sizeof(lig_req); }
   size_t out_bytes() const { return models ? sizeof(lig_mpick) : sizeof(lig_pick); }
 };
@@ -2702,8 +2800,8 @@ static void launch_excluding_fallback_count(const lig_ctx* c, const Slot& fs, co
   const ScanShape sh = scan_shape(c, fs, x.R);
   const SnapView v = view_of(fs);
   const FilterTree& t = run.tree ? *run.tree : kNoTree;
-  const int4* in = reinterpret_cast<const int4*>(x.reqs);
-  int2* out = reinterpret_cast<int2*>(x.out);
+  const int4* in = static_cast<const int4*>(x.in);
+  int2* out = static_cast<int2*>(x.out);
   auto launch = [&](auto staged, auto caller_tree) {
     constexpr bool kS = decltype(staged)::value, kT = decltype(caller_tree)::value;
     if (fs.n_ejected > 0)
@@ -2748,14 +2846,22 @@ static int fb_schedule(lig_ctx* c, FbRun& run, uint64_t seed, const FbReqs& rq, 
     void* out = static_cast<unsigned char*>(rq.out) + (size_t)pos * rq.out_bytes();
     const int grid = (n + kPickThreads * kCountPerThread - 1) / (kPickThreads * kCountPerThread);
     const uint4* fcls = reinterpret_cast<const uint4*>(fs.d_cls);
-    if (rq.retry && rq.rows) {
-      const ExcludingCall x{seed, static_cast<const lig_req*>(in), n, static_cast<lig_pick*>(out), rq.n_excluded,
-                            rq.excluded + (size_t)pos * (size_t)rq.n_excluded};
+    if (rq.retry && rq.models) {
+      ExcludingCall x{seed, in, n, out, rq.n_excluded, rq.excluded + (size_t)pos * (size_t)rq.n_excluded};
+      x.models = true;
+      x.first_index = rq.first_index + (uint64_t)pos;
+      x.targets = rq.targets + pos;
+      x.mtab = rq.mtab;
+      x.n_models = rq.n_models;
+      launch_models_excluding(c, fs, run.thr, run.tree, x, rq.rows ? rq.n_fallbacks : 0,
+                              rq.rows ? rq.fallbacks + (size_t)pos * (size_t)rq.n_fallbacks : nullptr, c->d_fb_hist,
+                              st);
+    } else if (rq.retry && rq.rows) {
+      const ExcludingCall x{seed, in, n, out, rq.n_excluded, rq.excluded + (size_t)pos * (size_t)rq.n_excluded};
       launch_excluding_fallback_count(c, fs, run, x, rq.n_fallbacks,
                                       rq.fallbacks + (size_t)pos * (size_t)rq.n_fallbacks, st);
     } else if (rq.retry) {
-      const ExcludingCall x{seed, static_cast<const lig_req*>(in), n, static_cast<lig_pick*>(out), rq.n_excluded,
-                            rq.excluded + (size_t)pos * (size_t)rq.n_excluded};
+      const ExcludingCall x{seed, in, n, out, rq.n_excluded, rq.excluded + (size_t)pos * (size_t)rq.n_excluded};
       launch_excluding(c, fs, run.thr, run.tree, x, c->d_fb_hist, st);
     } else if (rq.rows) {
       int16_t* rows = rq.fallbacks + (size_t)pos * (size_t)rq.n_fallbacks;
@@ -2937,7 +3043,7 @@ static int chain_rows_check(const char* fn, const FbReqs& rq, int R) {
   if (rq.retry) {
     if (rq.n_excluded < 1 || rq.n_excluded > LIG_MAX_EXCLUDED)
       return fail(LIG_ERR_INVALID, "%s: n_excluded=%d outside [1, %d]", fn, rq.n_excluded, LIG_MAX_EXCLUDED);
-    if (R > 0 && !rq.excluded) return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
+    if (R > 0 && (!rq.excluded || (rq.models && !rq.targets))) return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
   }
   if (!rq.rows) return 0;
   if (rq.n_fallbacks < 1 || rq.n_fallbacks > LIG_MAX_FALLBACKS)
@@ -2953,7 +3059,7 @@ static int chain_device(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t see
   if (int rc = chain_rows_check(fn, rq, R)) return rc;
   if (R > 0 && rq.rows && misaligned(rq.fallbacks, sizeof(int16_t)))
     return fail(LIG_ERR_INVALID, "%s: the row buffer is not 2-byte aligned", fn);
-  if (R > 0 && rq.retry && (misaligned(rq.in, sizeof(lig_req)) || misaligned(rq.out, sizeof(lig_pick)) ||
+  if (R > 0 && rq.retry && (misaligned(rq.in, rq.in_bytes()) || misaligned(rq.out, rq.out_bytes()) ||
                             misaligned(rq.excluded, sizeof(int16_t))))
     return fail(LIG_ERR_INVALID, "%s: a device buffer is not aligned to its element", fn);
   std::lock_guard<std::mutex> fk(c->fb_mu);
@@ -2976,7 +3082,7 @@ static int chain_host(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t seed,
   rq.in = R ? mapped_device_pointer(in) : nullptr;
   rq.out = R ? mapped_device_pointer(out) : nullptr;
   const bool bounce = R > 0 && !(rq.in && rq.out && !(reinterpret_cast<uintptr_t>(rq.in) & (rq.in_bytes() - 1)) &&
-                                 !(rq.retry && misaligned(rq.out, sizeof(lig_pick))));
+                                 !(rq.retry && misaligned(rq.out, rq.out_bytes())));
   std::unique_lock<std::mutex> bk(c->bounce_mu, std::defer_lock);
   if (bounce) {
     bk.lock();
@@ -3011,7 +3117,7 @@ static int chain_host(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t seed,
   if (loads_bounce && !(dev_loads = mapped_device_pointer(c->h_fb_loads)))
     return fail(LIG_ERR_CUDA, "pinned staging buffers are not device-mapped on this platform");
   // retry rows: page-locked, 2-byte aligned ones are read in place, the others staged in
-  // stream-ordered HBM (as lig_schedule_batch_excluding does)
+  // stream-ordered HBM (as lig_schedule_batch_excluding does); so are the targets of a model-id retry
   int16_t* stage = nullptr;
   if (R > 0 && rq.retry) {
     const int16_t* rows = rq.excluded;
@@ -3026,8 +3132,23 @@ static int chain_host(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t seed,
       rq.excluded = stage;
     }
   }
+  uint8_t* stage_tg = nullptr;
+  if (R > 0 && rq.retry && rq.models) {
+    const uint8_t* tg = rq.targets;
+    if (!(rq.targets = mapped_device_pointer(tg))) {
+      cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&stage_tg), (size_t)R, c->s_fb);
+      if (e == cudaSuccess) e = cudaMemcpyAsync(stage_tg, tg, (size_t)R, cudaMemcpyHostToDevice, c->s_fb);
+      if (e != cudaSuccess) {
+        if (stage_tg) cudaFreeAsync(stage_tg, c->s_fb);
+        if (stage) cudaFreeAsync(stage, c->s_fb);
+        return fail(LIG_ERR_CUDA, "%s: staging the targets failed: %s", fn, cudaGetErrorString(e));
+      }
+      rq.targets = stage_tg;
+    }
+  }
   const int rc = chain_call(c, epoch, seed, rq, R, window, dev_loads, c->s_fb);
   if (stage) cudaFreeAsync(stage, c->s_fb);
+  if (stage_tg) cudaFreeAsync(stage_tg, c->s_fb);
   if (rc) return rc;
   const cudaError_t e = cudaStreamSynchronize(c->s_fb);
   if (e != cudaSuccess) {
@@ -3166,6 +3287,57 @@ int lig_schedule_batch_feedback_chain_excluding_fallbacks_device(lig_ctx* c, uin
                       with_rows(with_excluded(descriptor_reqs(d_reqs, d_out), d_excluded, n_excluded), n_fallbacks,
                                 d_fallbacks),
                       R, window, d_loads, stream);
+}
+
+static FbReqs with_targets(FbReqs rq, const uint8_t* targets) {
+  rq.targets = targets;
+  return rq;
+}
+
+int lig_schedule_models_batch_feedback_chain_excluding(lig_ctx* c, uint64_t epoch, uint64_t seed,
+                                                       uint64_t first_index, const uint32_t* model_ids,
+                                                       const uint8_t* targets, int R, const int16_t* excluded,
+                                                       int n_excluded, lig_mpick* out, int window, int32_t* loads) {
+  return chain_host(c, "lig_schedule_models_batch_feedback_chain_excluding", epoch, seed,
+                    with_targets(with_excluded(model_reqs(model_ids, out, first_index), excluded, n_excluded), targets),
+                    R, window, loads);
+}
+
+int lig_schedule_models_batch_feedback_chain_excluding_device(lig_ctx* c, uint64_t epoch, uint64_t seed,
+                                                              uint64_t first_index, const uint32_t* d_model_ids,
+                                                              const uint8_t* d_targets, int R,
+                                                              const int16_t* d_excluded, int n_excluded,
+                                                              lig_mpick* d_out, int window, int32_t* d_loads,
+                                                              void* stream) {
+  return chain_device(c, "lig_schedule_models_batch_feedback_chain_excluding_device", epoch, seed,
+                      with_targets(with_excluded(model_reqs(d_model_ids, d_out, first_index), d_excluded, n_excluded),
+                                   d_targets),
+                      R, window, d_loads, stream);
+}
+
+int lig_schedule_models_batch_feedback_chain_excluding_fallbacks(lig_ctx* c, uint64_t epoch, uint64_t seed,
+                                                                 uint64_t first_index, const uint32_t* model_ids,
+                                                                 const uint8_t* targets, int R,
+                                                                 const int16_t* excluded, int n_excluded,
+                                                                 lig_mpick* out, int n_fallbacks, int16_t* fallbacks,
+                                                                 int window, int32_t* loads) {
+  return chain_host(c, "lig_schedule_models_batch_feedback_chain_excluding_fallbacks", epoch, seed,
+                    with_rows(with_targets(with_excluded(model_reqs(model_ids, out, first_index), excluded, n_excluded),
+                                           targets),
+                              n_fallbacks, fallbacks),
+                    R, window, loads);
+}
+
+int lig_schedule_models_batch_feedback_chain_excluding_fallbacks_device(
+    lig_ctx* c, uint64_t epoch, uint64_t seed, uint64_t first_index, const uint32_t* d_model_ids,
+    const uint8_t* d_targets, int R, const int16_t* d_excluded, int n_excluded, lig_mpick* d_out, int n_fallbacks,
+    int16_t* d_fallbacks, int window, int32_t* d_loads, void* stream) {
+  return chain_device(
+      c, "lig_schedule_models_batch_feedback_chain_excluding_fallbacks_device", epoch, seed,
+      with_rows(with_targets(with_excluded(model_reqs(d_model_ids, d_out, first_index), d_excluded, n_excluded),
+                             d_targets),
+                n_fallbacks, d_fallbacks),
+      R, window, d_loads, stream);
 }
 
 int lig_feedback_chain_reset(lig_ctx* c) {

@@ -3212,4 +3212,134 @@ lig_schedule_excluding_fallback_count_kernel(SnapView s, Thr thr, const __grid_c
   }
 }
 
+// ---- model-id retries (lig_schedule_models_batch[_feedback_chain]_excluding[_fallbacks]) ------------
+// Request i is model ids[i] at the fixed target targets[i] (the target_idx an earlier model call
+// returned), with rand_key = first_index + i.  The warp resolves it without a draw: one broadcast
+// 16-byte gather of the model entry, plus one target record when the model has >= 2 targets.  The
+// request is LIG_NO_MODEL for an id past the table, an absent model, a model without TargetModels
+// and t != 255, or a model with TargetModels and t >= their count.  Otherwise the descriptor
+// {adapter, Critical, rand_key} goes through the walk of lig_schedule_excluding_kernel, step for
+// step; kRows adds the row of lig_schedule_excluding_fallback_kernel, kCount the chain count of
+// lig_schedule_excluding_count_kernel (a LIG_NO_MODEL request writes its result and adds no load).
+// The pick is packed as a lig_mpick with target_idx = t.  The model table is read through the
+// read-only path: every launch is ordered behind the table's upload.  A body of its own, for the
+// reason given at lig_schedule_excluding_count_kernel.
+template <bool kStaged, bool kTree, bool kPool, bool kRows, bool kCount>
+__global__ void __launch_bounds__(kCtaThreads)
+lig_schedule_models_excluding_kernel(SnapView s, Thr thr, const __grid_constant__ FilterTree tree,
+                                     const uint32_t* ids, const uint8_t* targets, const int16_t* excluded,
+                                     int n_excluded, uint32_t* out, int R, uint64_t seed, uint64_t first_index,
+                                     const unsigned char* __restrict__ mtab, uint32_t n_models, int n_fallbacks,
+                                     int16_t* fallbacks, int* __restrict__ hist, const uint32_t* __restrict__ pool) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint32_t* X = reinterpret_cast<uint32_t*>(smem) + (size_t)warp * 3 * s.W;
+  uint32_t* T = X + s.W;
+  uint32_t* H = T + s.W;
+  const uint4* entries = reinterpret_cast<const uint4*>(mtab + sizeof(ModelHeader));
+  const uint2* records = reinterpret_cast<const uint2*>(entries + n_models);
+  Fields f{s.kv, s.q, s.n_active, s.max_active};
+  if constexpr (kStaged) {
+    f = stage_fields(s, smem + scratch_bytes(s.W));
+    __syncthreads();
+  }
+  for (int i = blockIdx.x * kWarpsPerCta + warp; i < R; i += gridDim.x * kWarpsPerCta) {
+    const uint32_t m = ids[i];                 // whole warp reads the same id and target (broadcast)
+    const uint32_t t = targets[i];
+    const int ex = lane < n_excluded ? excluded[(size_t)i * n_excluded + lane] : -1;
+    const uint64_t key = first_index + (uint64_t)i;
+    bool found = false;
+    uint32_t adapter = 0, critical = 0;
+    if (m < n_models) {
+      const uint4 e = __ldg(entries + m);
+      const uint32_t nt = e.x & 0xffu;
+      found = (e.x & kModelPresent) && (nt == 0 ? t == 255u : t < nt);
+      critical = (e.x >> 8) & 1u;
+      adapter = e.w;                           // the own id (nt == 0) or the single target (nt == 1)
+      if (found && nt >= 2u) adapter = __ldg(records + e.w + t).x;
+    }
+    if (!found) {
+      if (lane == 0) out[i] = pack_mpick(-1, (uint32_t)LIG_NO_MODEL, 255u);
+      if (kRows && lane < n_fallbacks) fallbacks[(size_t)i * (size_t)n_fallbacks + lane] = -1;
+      __syncwarp();
+      continue;
+    }
+    const uint32_t* Hrow = stage_adapter_row(s, (int)adapter, H, lane);
+    for (int w = lane; w < s.W; w += 32) {
+      if constexpr (kPool) {
+        T[w] = pool[w];
+      } else {
+        const int rem = s.P - w * 32;
+        T[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
+      }
+    }
+    __syncwarp();
+    if (ex >= 0 && ex < s.P) atomicAnd(T + (ex >> 5), ~(1u << (ex & 31)));
+    __syncwarp();
+    uint32_t n = 0;
+    for (int w = lane; w < s.W; w += 32) n += __popc(T[w]);
+    n = __reduce_add_sync(kFull, n);
+    EvalResult e;
+    if constexpr (kTree)
+      e = tree_walk_warp<kStaged, true>(f, tree.nodes, Hrow, critical != 0, s.P, s.W, T, X, lane, n);
+    else
+      e = tree_eval_warp<kStaged, true>(f, Hrow, critical != 0, thr, s.P, s.W, X, T, lane, n);
+    int pod = -1;
+    int16_t mine = -1;                         // kRows: row entry lane + 1
+    if (e.n > 0) {
+      if constexpr (kRows) {
+        uint32_t incl = 0;
+        const int groups = (s.W + 31) >> 5;
+        for (int g = 0; g < groups; ++g) {
+          const int w = g * 32 + lane;
+          const uint32_t cg = __reduce_add_sync(kFull, w < s.W ? __popc(e.mask[w]) : 0u);
+          if (lane == g) incl = cg;
+        }
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+          const uint32_t u = __shfl_up_sync(kFull, incl, d);
+          if (lane >= d) incl += u;
+        }
+        uint64_t state = seed ^ key;
+        uint32_t pos[LIG_MAX_FALLBACKS], val[LIG_MAX_FALLBACKS];
+        pos[0] = int31n_next(state, e.n);
+        val[0] = 0u;
+        pod = warp_select_survivor(e.mask, s.W, incl, pos[0], lane);
+        const uint32_t mm = e.status == (uint32_t)LIG_OK ? min(e.n, (uint32_t)n_fallbacks + 1u) : 0u;
+#pragma unroll
+        for (int j = 1; j <= LIG_MAX_FALLBACKS; ++j) {
+          if ((uint32_t)j >= mm) break;
+          const uint32_t rj = (uint32_t)j + int31n_next(state, e.n - (uint32_t)j);
+          uint32_t a = (uint32_t)j, b = rj;
+#pragma unroll
+          for (int k = 0; k < j; ++k) {
+            if (pos[k] == (uint32_t)j) a = val[k];
+            if (pos[k] == rj) b = val[k];
+          }
+          const int p = warp_select_survivor(e.mask, s.W, incl, b, lane);
+          if (lane == j - 1) mine = (int16_t)p;
+          if (j < LIG_MAX_FALLBACKS) {
+            pos[j] = rj;
+            val[j] = a;
+          }
+        }
+      } else {
+        uint32_t k = int31n(seed ^ key, e.n, max_accept_for(e.n));
+        for (int w = 0; w < s.W; ++w) {        // k-th survivor in pod order = pods[k]   scheduler.go:121
+          uint32_t word = e.mask[w];
+          uint32_t c = __popc(word);
+          if (k < c) { pod = w * 32 + (int)__fns(word, 0, (int)k + 1); break; }
+          k -= c;
+        }
+      }
+    }
+    if (lane == 0) {
+      out[i] = pack_mpick(pod, e.status, t);
+      if (kCount && pod >= 0) atomicAdd(hist + pod, 1);   // pod >= 0 only for LIG_OK
+    }
+    if (kRows && lane < n_fallbacks) fallbacks[(size_t)i * (size_t)n_fallbacks + lane] = mine;
+    __syncwarp();
+  }
+}
+
 }  // namespace lig

@@ -427,6 +427,141 @@ class Engine:
             self._ctx, epoch, seed, d_reqs or None, R, d_excluded or None, n_excluded, d_out or None, n,
             d_fallbacks or None, window, d_loads or None, stream or None))
 
+    # ---- model-id retries: keep the drawn target (an earlier model call's target_idx), resolve on the device ----
+    @staticmethod
+    def _model_retry_args(model_ids: np.ndarray, targets: np.ndarray, excluded: np.ndarray) -> int:
+        assert model_ids.dtype == np.uint32 and model_ids.flags.c_contiguous
+        assert targets.dtype == np.uint8 and targets.flags.c_contiguous
+        assert excluded.dtype == np.int16 and excluded.flags.c_contiguous and excluded.ndim == 2
+        R = int(model_ids.shape[0])
+        assert targets.shape == (R,) and excluded.shape[0] == R
+        return R
+
+    def schedule_models_batch_excluding(self, epoch: int, seed: int, model_ids: np.ndarray, targets: np.ndarray,
+                                        excluded: np.ndarray, first_index: int = 0) -> np.ndarray:
+        """lig_schedule_models_batch_excluding: request i is model_ids[i] at the fixed target targets[i]
+        (uint8, the target_idx an earlier model call returned; 255 = the model's own adapter), resolved
+        without a draw and scheduled as schedule_batch_excluding schedules its descriptor, rand_key
+        first_index + i."""
+        R = self._model_retry_args(model_ids, targets, excluded)
+        out = np.empty(R, dtype=MPICK_DTYPE)
+        N.check(self._lib.lig_schedule_models_batch_excluding(self._ctx, epoch, seed, first_index, _ptr(model_ids),
+                                                              _ptr(targets), R, _ptr(excluded),
+                                                              int(excluded.shape[1]), _ptr(out)))
+        return out
+
+    def schedule_models_batch_excluding_ptr(self, epoch: int, seed: int, first_index: int, h_ids: int, h_targets: int,
+                                            R: int, h_excluded: int, n_excluded: int, h_out: int) -> None:
+        N.check(self._lib.lig_schedule_models_batch_excluding(self._ctx, epoch, seed, first_index, h_ids or None,
+                                                              h_targets or None, R, h_excluded or None, n_excluded,
+                                                              h_out or None))
+
+    def schedule_models_batch_excluding_device(self, epoch: int, seed: int, first_index: int, d_ids: int,
+                                               d_targets: int, R: int, d_excluded: int, n_excluded: int, d_out: int,
+                                               stream: int = 0) -> None:
+        """Device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_models_batch_excluding_device(self._ctx, epoch, seed, first_index,
+                                                                     d_ids or None, d_targets or None, R,
+                                                                     d_excluded or None, n_excluded, d_out or None,
+                                                                     stream or None))
+
+    def schedule_models_batch_excluding_fallbacks(self, epoch: int, seed: int, model_ids: np.ndarray,
+                                                  targets: np.ndarray, excluded: np.ndarray, n: int,
+                                                  first_index: int = 0):
+        """lig_schedule_models_batch_excluding_fallbacks: (picks, int16 fallbacks (R, n)); the picks equal
+        schedule_models_batch_excluding's, the rows rank the reduced pool as
+        schedule_batch_excluding_fallbacks does."""
+        R = self._model_retry_args(model_ids, targets, excluded)
+        out = np.empty(R, dtype=MPICK_DTYPE)
+        rows = np.empty((R, max(n, 0)), dtype=np.int16)
+        N.check(self._lib.lig_schedule_models_batch_excluding_fallbacks(
+            self._ctx, epoch, seed, first_index, _ptr(model_ids), _ptr(targets), R, _ptr(excluded),
+            int(excluded.shape[1]), _ptr(out), n, _ptr(rows)))
+        return out, rows
+
+    def schedule_models_batch_excluding_fallbacks_ptr(self, epoch: int, seed: int, first_index: int, h_ids: int,
+                                                      h_targets: int, R: int, h_excluded: int, n_excluded: int,
+                                                      h_out: int, n: int, h_fallbacks: int) -> None:
+        N.check(self._lib.lig_schedule_models_batch_excluding_fallbacks(
+            self._ctx, epoch, seed, first_index, h_ids or None, h_targets or None, R, h_excluded or None, n_excluded,
+            h_out or None, n, h_fallbacks or None))
+
+    def schedule_models_batch_excluding_fallbacks_device(self, epoch: int, seed: int, first_index: int, d_ids: int,
+                                                         d_targets: int, R: int, d_excluded: int, n_excluded: int,
+                                                         d_out: int, n: int, d_fallbacks: int,
+                                                         stream: int = 0) -> None:
+        """Device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_models_batch_excluding_fallbacks_device(
+            self._ctx, epoch, seed, first_index, d_ids or None, d_targets or None, R, d_excluded or None, n_excluded,
+            d_out or None, n, d_fallbacks or None, stream or None))
+
+    def schedule_models_batch_feedback_chain_excluding(self, epoch: int, seed: int, model_ids: np.ndarray,
+                                                       targets: np.ndarray, excluded: np.ndarray, window: int,
+                                                       first_index: int = 0,
+                                                       loads: Optional[np.ndarray] = None) -> np.ndarray:
+        """lig_schedule_models_batch_feedback_chain_excluding: the model-id retry as a chain call, in the
+        chain's sequence and windows, on its load-adjusted copy.  `loads` as schedule_batch_feedback_chain's."""
+        R = self._model_retry_args(model_ids, targets, excluded)
+        out = np.empty(R, dtype=MPICK_DTYPE)
+        if loads is not None:
+            assert loads.dtype == np.int32 and loads.flags.c_contiguous
+        N.check(self._lib.lig_schedule_models_batch_feedback_chain_excluding(
+            self._ctx, epoch, seed, first_index, _ptr(model_ids), _ptr(targets), R, _ptr(excluded),
+            int(excluded.shape[1]), _ptr(out), window, _ptr(loads) if loads is not None else None))
+        return out
+
+    def schedule_models_batch_feedback_chain_excluding_ptr(self, epoch: int, seed: int, first_index: int, h_ids: int,
+                                                           h_targets: int, R: int, h_excluded: int, n_excluded: int,
+                                                           h_out: int, window: int, h_loads: int = 0) -> None:
+        N.check(self._lib.lig_schedule_models_batch_feedback_chain_excluding(
+            self._ctx, epoch, seed, first_index, h_ids or None, h_targets or None, R, h_excluded or None, n_excluded,
+            h_out or None, window, h_loads or None))
+
+    def schedule_models_batch_feedback_chain_excluding_device(self, epoch: int, seed: int, first_index: int,
+                                                              d_ids: int, d_targets: int, R: int, d_excluded: int,
+                                                              n_excluded: int, d_out: int, window: int,
+                                                              d_loads: int = 0, stream: int = 0) -> None:
+        """Device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_models_batch_feedback_chain_excluding_device(
+            self._ctx, epoch, seed, first_index, d_ids or None, d_targets or None, R, d_excluded or None, n_excluded,
+            d_out or None, window, d_loads or None, stream or None))
+
+    def schedule_models_batch_feedback_chain_excluding_fallbacks(self, epoch: int, seed: int, model_ids: np.ndarray,
+                                                                 targets: np.ndarray, excluded: np.ndarray, n: int,
+                                                                 window: int, first_index: int = 0,
+                                                                 loads: Optional[np.ndarray] = None):
+        """lig_schedule_models_batch_feedback_chain_excluding_fallbacks: (picks, int16 fallbacks (R, n)); the
+        picks and loads are schedule_models_batch_feedback_chain_excluding's."""
+        R = self._model_retry_args(model_ids, targets, excluded)
+        out = np.empty(R, dtype=MPICK_DTYPE)
+        rows = np.empty((R, max(n, 0)), dtype=np.int16)
+        if loads is not None:
+            assert loads.dtype == np.int32 and loads.flags.c_contiguous
+        N.check(self._lib.lig_schedule_models_batch_feedback_chain_excluding_fallbacks(
+            self._ctx, epoch, seed, first_index, _ptr(model_ids), _ptr(targets), R, _ptr(excluded),
+            int(excluded.shape[1]), _ptr(out), n, _ptr(rows), window, _ptr(loads) if loads is not None else None))
+        return out, rows
+
+    def schedule_models_batch_feedback_chain_excluding_fallbacks_ptr(self, epoch: int, seed: int, first_index: int,
+                                                                     h_ids: int, h_targets: int, R: int,
+                                                                     h_excluded: int, n_excluded: int, h_out: int,
+                                                                     n: int, h_fallbacks: int, window: int,
+                                                                     h_loads: int = 0) -> None:
+        N.check(self._lib.lig_schedule_models_batch_feedback_chain_excluding_fallbacks(
+            self._ctx, epoch, seed, first_index, h_ids or None, h_targets or None, R, h_excluded or None, n_excluded,
+            h_out or None, n, h_fallbacks or None, window, h_loads or None))
+
+    def schedule_models_batch_feedback_chain_excluding_fallbacks_device(self, epoch: int, seed: int,
+                                                                        first_index: int, d_ids: int, d_targets: int,
+                                                                        R: int, d_excluded: int, n_excluded: int,
+                                                                        d_out: int, n: int, d_fallbacks: int,
+                                                                        window: int, d_loads: int = 0,
+                                                                        stream: int = 0) -> None:
+        """Device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_models_batch_feedback_chain_excluding_fallbacks_device(
+            self._ctx, epoch, seed, first_index, d_ids or None, d_targets or None, R, d_excluded or None, n_excluded,
+            d_out or None, n, d_fallbacks or None, window, d_loads or None, stream or None))
+
     def schedule_models_batch_fallbacks(self, epoch: int, seed: int, model_ids: np.ndarray, n: int,
                                         first_index: int = 0):
         """lig_schedule_models_batch_fallbacks: (picks, int16 fallbacks (R, n)), the picks those of

@@ -30,6 +30,7 @@ EXPORTED_SYMBOLS = (
     "ligh_scheduler_set_models", "ligh_schedule_model_device", "ligh_model_stats", "ligh_schedule_models_concurrent",
     "ligh_filter", "ligh_schedule_with_fallbacks", "ligh_fallback_scheduled", "ligh_schedule_model_with_fallbacks",
     "ligh_schedule_retry", "ligh_retry_scheduled", "ligh_schedule_retry_with_fallbacks",
+    "ligh_schedule_model_retry", "ligh_schedule_model_retry_with_fallbacks",
     "ligh_eject_pods", "ligh_eject_stats",
 )
 
@@ -90,6 +91,10 @@ def load() -> C.CDLL:
     lib.ligh_schedule_retry_with_fallbacks.argtypes = [vp, C.c_char_p, i32, cpp, cpp, i32, i32, C.c_char_p, i32,
                                                        C.POINTER(i32), C.c_char_p, i32]
     lib.ligh_retry_scheduled.argtypes = [vp]
+    lib.ligh_schedule_model_retry.argtypes = [vp, C.c_char_p, C.c_char_p, cpp, cpp, i32, C.c_char_p, i32, C.c_char_p,
+                                              i32, C.c_char_p, i32]
+    lib.ligh_schedule_model_retry_with_fallbacks.argtypes = [vp, C.c_char_p, C.c_char_p, cpp, cpp, i32, i32,
+                                                             C.c_char_p, i32, C.POINTER(i32), C.c_char_p, i32]
     lib.ligh_eject_pods.argtypes = [vp, cpp, cpp, i32, C.c_char_p, i32]
     lib.ligh_eject_stats.argtypes = [vp, vp]
     lib.ligh_eject_stats.restype = None
@@ -244,6 +249,32 @@ class HostScheduler:
                                                             _strs([p.Name for p in tried]),
                                                             _strs([p.Address for p in tried]), len(tried), n, names,
                                                             cap, C.byref(k), err, 512)
+        pods = names.value.decode().split("\n") if k.value else []
+        return code, pods, err.value.decode("utf-8", "replace") if code != GRPC_OK else ""
+
+    def ScheduleModelRetry(self, model: str, resolved: str, tried: Sequence[Pod]
+                           ) -> Tuple[int, Optional[Pod], str]:  # noqa: N802
+        """Scheduler::ScheduleModelRetry: the retry of a model request at the target it drew (`resolved`, the
+        name ScheduleModel returned), without the pods in `tried`: (gRPC code, pod, error)."""
+        name, addr = C.create_string_buffer(256), C.create_string_buffer(256)
+        err = C.create_string_buffer(512)
+        code = self._lib.ligh_schedule_model_retry(self._s, model.encode(), resolved.encode(),
+                                                   _strs([p.Name for p in tried]), _strs([p.Address for p in tried]),
+                                                   len(tried), name, 256, addr, 256, err, 512)
+        if code == GRPC_OK:
+            return code, Pod(name.value.decode(), addr.value.decode()), ""
+        return code, None, err.value.decode("utf-8", "replace")
+
+    def ScheduleModelRetryWithFallbacks(self, model: str, resolved: str, tried: Sequence[Pod], n: int
+                                        ) -> Tuple[int, List[str], str]:  # noqa: N802
+        """Scheduler::ScheduleModelRetryWithFallbacks: ScheduleModelRetry plus up to n fallback pods of the
+        same reduced pool: (gRPC code, pod names [pick, fallbacks in retry order], error)."""
+        cap = 64 * 1024
+        names, err, k = C.create_string_buffer(cap), C.create_string_buffer(512), C.c_int(0)
+        code = self._lib.ligh_schedule_model_retry_with_fallbacks(self._s, model.encode(), resolved.encode(),
+                                                                  _strs([p.Name for p in tried]),
+                                                                  _strs([p.Address for p in tried]), len(tried), n,
+                                                                  names, cap, C.byref(k), err, 512)
         pods = names.value.decode().split("\n") if k.value else []
         return code, pods, err.value.decode("utf-8", "replace") if code != GRPC_OK else ""
 

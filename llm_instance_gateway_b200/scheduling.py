@@ -551,6 +551,137 @@ class Scheduler:
             raise err
         return pods
 
+    # ---- model-id retries: the retry of a model request at the target its first attempt drew ----
+    def _model_retry_batch(self, names: Sequence[str], resolved: Sequence[str],
+                           tried_lists: Sequence[Sequence[Pod]], empty):
+        """(snapshot, results, model ids, target indices, excluded rows, slots) of a model-retry batch.  Each
+        name is mapped to its model id and its resolved target to the first TargetModels entry of that
+        name (255 for a model without TargetModels whose own name it is); names the host answers get
+        (empty, resolved, error) in results and no row."""
+        if not len(names) == len(resolved) == len(tried_lists):
+            raise ValueError(f"{len(names)} names, {len(resolved)} resolved targets, {len(tried_lists)} tried lists")
+        for tried in tried_lists:
+            if len(tried) > N.LIG_MAX_EXCLUDED:
+                raise ValueError(f"{len(tried)} tried pods (at most {N.LIG_MAX_EXCLUDED})")
+        snap = self._current()
+        pm = self._packed_models
+        where: Dict[Pod, List[int]] = {}
+        for p, pod in enumerate(snap.pods):
+            where.setdefault(pod, []).append(p)
+        out: list = [None] * len(names)
+        ids, targets, rows, slots = [], [], [], []
+        for i, (name, res) in enumerate(zip(names, resolved)):
+            m = pm.model_ids.get(name) if pm is not None else None
+            if m is None:                                                       # request.go:42-45
+                out[i] = (empty, res, StatusError(
+                    "Unknown", f"error finding a model object in InferenceModel for input {name}"))
+                continue
+            if not pm.present[m]:                                               # request.go:48-51
+                out[i] = (empty, res, StatusError("Unknown", f"error getting target model name for model {name}"))
+                continue
+            tgt = pm.target_names[m]
+            t = (255 if res == name else None) if not tgt else next((j for j, x in enumerate(tgt) if x == res), None)
+            if t is None:
+                out[i] = (empty, res, StatusError("InvalidArgument", f"{res} is not a target model of {name}"))
+                continue
+            row = [p for pod in tried_lists[i] for p in where.get(pod, ())]
+            if len(row) > N.LIG_MAX_EXCLUDED:
+                raise ValueError(f"the tried pods match {len(row)} pods of the snapshot (at most "
+                                 f"{N.LIG_MAX_EXCLUDED})")
+            ids.append(m)
+            targets.append(t)
+            rows.append(row)
+            slots.append(i)
+        excluded = np.full((len(ids), max([1] + [len(r) for r in rows])), -1, dtype=np.int16)
+        for k, r in enumerate(rows):
+            excluded[k, :len(r)] = r
+        return snap, out, np.array(ids, dtype=np.uint32), np.array(targets, dtype=np.uint8), excluded, slots
+
+    def ScheduleModelBatchRetry(self, names: Sequence[str], resolved: Sequence[str],
+                                tried_lists: Sequence[Sequence[Pod]]
+                                ) -> List[Tuple[Optional[Pod], str, Optional[StatusError]]]:
+        """The retry of ScheduleModelBatch requests without the pods they tried, keeping the targets they
+        drew (resolved[i], the name ScheduleModelBatch returned): (pod, resolved target model, error) per
+        name, as lig_schedule_models_batch_excluding returns it; no second draw.  Names the host answers
+        from the list alone take no rand_key: unknown models and models whose weights sum to <= 0 with
+        ScheduleModelBatch's errors, a resolved name that is not a target of the model with
+        InvalidArgument.  Requests sent to the device take rand_keys from ScheduleModelBatch's sequence.
+        Tried pods are matched by value as in ScheduleBatchRetry.  Under load_feedback_window the call is
+        a chain call (lig_schedule_models_batch_feedback_chain_excluding) when the scheduler was built
+        with feedback_retries=True, and raises ValueError otherwise."""
+        if self._window and not self._feedback_retries:
+            raise ValueError("retries are not defined under load_feedback_window: the picks come from the feedback "
+                             "chain's load-adjusted copy of the snapshot, a retry would not")
+        snap, out, ids, targets, excluded, slots = self._model_retry_batch(names, resolved, tried_lists, None)
+        if not len(ids):
+            return out
+        if self._window:
+            picks = self._engine.schedule_models_batch_feedback_chain_excluding(
+                self._epoch, self._seed, ids, targets, excluded, self._window, first_index=self._model_index)
+        else:
+            picks = self._engine.schedule_models_batch_excluding(self._epoch, self._seed, ids, targets, excluded,
+                                                                 first_index=self._model_index)
+        self._model_index += len(ids)
+        for i, m, pk in zip(slots, ids, picks):
+            st = int(pk["status"])
+            if st == N.LIG_OK:
+                out[i] = (snap.pods[int(pk["pod_idx"])], resolved[i], None)
+            elif st == N.LIG_NO_MODEL:       # absent models and targets never reach the device
+                out[i] = (None, resolved[i], StatusError("Internal", _no_model_entry(int(m), names[i])))
+            else:
+                err = _schedule_error(st)
+                out[i] = (None, resolved[i], StatusError(err.code, _POD_PREFIX + str(err)))
+        return out
+
+    def ScheduleModelRetry(self, name: str, resolved: str, tried: Sequence[Pod]) -> Pod:
+        """The retry of one ScheduleModel request at its resolved target; raises like ScheduleModel."""
+        pod, _, err = self.ScheduleModelBatchRetry([name], [resolved], [tried])[0]
+        if err is not None:
+            raise err
+        return pod
+
+    def ScheduleModelBatchRetryWithFallbacks(self, names: Sequence[str], resolved: Sequence[str],
+                                             tried_lists: Sequence[Sequence[Pod]], n: int
+                                             ) -> List[Tuple[List[Pod], str, Optional[StatusError]]]:
+        """ScheduleModelBatchRetry plus up to n fallback pods of the same reduced pool per request
+        (lig_schedule_models_batch_excluding_fallbacks): (pods, resolved target model, error), pods[0] the
+        pod ScheduleModelBatchRetry would have returned.  ValueError for n outside [1, LIG_MAX_FALLBACKS];
+        under load_feedback_window it needs both feedback_retries=True and feedback_fallbacks=True."""
+        if self._window and not (self._feedback_retries and self._feedback_fallbacks):
+            raise ValueError("retries with fallbacks are not defined under load_feedback_window without "
+                             "feedback_retries and feedback_fallbacks: the picks come from the feedback chain's "
+                             "load-adjusted copy of the snapshot, these would not")
+        if not 1 <= n <= N.LIG_MAX_FALLBACKS:
+            raise ValueError(f"n must be in [1, {N.LIG_MAX_FALLBACKS}], got {n}")
+        snap, out, ids, targets, excluded, slots = self._model_retry_batch(names, resolved, tried_lists, [])
+        if not len(ids):
+            return out
+        if self._window:
+            picks, rows = self._engine.schedule_models_batch_feedback_chain_excluding_fallbacks(
+                self._epoch, self._seed, ids, targets, excluded, n, self._window, first_index=self._model_index)
+        else:
+            picks, rows = self._engine.schedule_models_batch_excluding_fallbacks(
+                self._epoch, self._seed, ids, targets, excluded, n, first_index=self._model_index)
+        self._model_index += len(ids)
+        for i, m, pk, row in zip(slots, ids, picks, rows):
+            st = int(pk["status"])
+            if st == N.LIG_OK:
+                out[i] = ([snap.pods[int(pk["pod_idx"])]] + [snap.pods[int(p)] for p in row if p >= 0], resolved[i],
+                          None)
+            elif st == N.LIG_NO_MODEL:
+                out[i] = ([], resolved[i], StatusError("Internal", _no_model_entry(int(m), names[i])))
+            else:
+                err = _schedule_error(st)
+                out[i] = ([], resolved[i], StatusError(err.code, _POD_PREFIX + str(err)))
+        return out
+
+    def ScheduleModelRetryWithFallbacks(self, name: str, resolved: str, tried: Sequence[Pod], n: int) -> List[Pod]:
+        """ScheduleModelRetry plus up to n fallback pods: [pick, fallback 1, ...]; raises like ScheduleModel."""
+        pods, _, err = self.ScheduleModelBatchRetryWithFallbacks([name], [resolved], [tried], n)[0]
+        if err is not None:
+            raise err
+        return pods
+
     # Filter-level view (the GPU analogue of Filter.Filter, filter.go:12-15): survivor slice.
     def Filter(self, req: LLMRequest) -> Tuple[List[Pod], Optional[StatusError]]:
         """The survivors of `req` against the scraped snapshot.  With load_feedback_window set this
