@@ -954,12 +954,12 @@ void abort_write(lig_ctx* c, SnapshotWrite*) { c->upload_mu.unlock(); }
 
 }  // namespace ligi
 
-// The dynamic shared-memory limit of every form of the model-id retry kernel: form I has kStaged = bit 0,
-// kTree = bit 1, kPool = bit 2, kRows = bit 3, kCount = bit 4.
+// The dynamic shared-memory limit of every form of the retry kernel: form I has kModels = bit 0,
+// kStaged = bit 1, kTree = bit 2, kPool = bit 3, kRows = bit 4, kCount = bit 5.
 template <size_t... I>
-static int set_models_excluding_smem(int bytes, std::index_sequence<I...>) {
-  const void* forms[] = {(const void*)lig_schedule_models_excluding_kernel<(I & 1) != 0, (I & 2) != 0, (I & 4) != 0,
-                                                                           (I & 8) != 0, (I & 16) != 0>...};
+static int set_excluding_smem(int bytes, std::index_sequence<I...>) {
+  const void* forms[] = {(const void*)lig_schedule_excluding_kernel<(I & 1) != 0, (I & 2) != 0, (I & 4) != 0,
+                                                                    (I & 8) != 0, (I & 16) != 0, (I & 32) != 0>...};
   for (const void* fn : forms) CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
   return 0;
 }
@@ -1086,34 +1086,7 @@ static int create_impl(lig_ctx* c, int device, int max_pods, int max_adapters, i
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, v));
   CUDA_TRY(cudaFuncSetAttribute(lig_scan_kernel<false>,
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_count_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_count_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_count_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_count_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_count_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_count_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_count_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  CUDA_TRY(cudaFuncSetAttribute(lig_schedule_excluding_fallback_count_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  const void* pool_forms[] = {   // the pool forms of the four retry kernels, every (staged, tree)
-      (const void*)lig_schedule_excluding_kernel<true, false, true>, (const void*)lig_schedule_excluding_kernel<false, false, true>,
-      (const void*)lig_schedule_excluding_kernel<true, true, true>, (const void*)lig_schedule_excluding_kernel<false, true, true>,
-      (const void*)lig_schedule_excluding_count_kernel<true, false, true>, (const void*)lig_schedule_excluding_count_kernel<false, false, true>,
-      (const void*)lig_schedule_excluding_count_kernel<true, true, true>, (const void*)lig_schedule_excluding_count_kernel<false, true, true>,
-      (const void*)lig_schedule_excluding_fallback_kernel<true, false, true>, (const void*)lig_schedule_excluding_fallback_kernel<false, false, true>,
-      (const void*)lig_schedule_excluding_fallback_kernel<true, true, true>, (const void*)lig_schedule_excluding_fallback_kernel<false, true, true>,
-      (const void*)lig_schedule_excluding_fallback_count_kernel<true, false, true>, (const void*)lig_schedule_excluding_fallback_count_kernel<false, false, true>,
-      (const void*)lig_schedule_excluding_fallback_count_kernel<true, true, true>, (const void*)lig_schedule_excluding_fallback_count_kernel<false, true, true>,
-  };
-  for (const void* fn : pool_forms) CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
-  if (int rc = set_models_excluding_smem(v, std::make_index_sequence<32>{})) return rc;
+  if (int rc = set_excluding_smem(v, std::make_index_sequence<64>{})) return rc;
   const size_t need = scratch_bytes(words_for(max_pods)) > build_fixed_bytes(words_for(max_pods))
                           ? scratch_bytes(words_for(max_pods)) : build_fixed_bytes(words_for(max_pods));
   if (need > c->smem_optin)
@@ -1226,7 +1199,8 @@ static int create_impl(lig_ctx* c, int device, int max_pods, int max_adapters, i
     CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&c->d_delta), cap));
     c->delta_capacity = cap;
   }
-  // (b) every kernel a tick or a batch can launch is loaded now
+  // (b) every kernel a tick or a batch can launch is loaded now; a lazy load while the resident
+  // doorbell kernel runs can wait for that kernel, which waits for the host: a hang
   {
     cudaFuncAttributes fa;
     const void* fns[] = {
@@ -1238,7 +1212,9 @@ static int create_impl(lig_ctx* c, int device, int max_pods, int max_adapters, i
         (const void*)lig_pick_models_stream_kernel, (const void*)lig_apply_delta_kernel,
         (const void*)lig_pick_count_kernel,      (const void*)lig_apply_feedback_kernel,
         (const void*)lig_feedback_loads_kernel,  (const void*)lig_pick_models_count_kernel,
-        (const void*)lig_pick_fallback_count_kernel<false>, (const void*)lig_pick_fallback_count_kernel<true>,
+        (const void*)lig_pick_fallback_kernel<false, false>, (const void*)lig_pick_fallback_kernel<true, false>,
+        (const void*)lig_pick_fallback_kernel<false, true>, (const void*)lig_pick_fallback_kernel<true, true>,
+        (const void*)lig_filter_kernel<false>,   (const void*)lig_filter_kernel<true>,
     };
     for (const void* fn : fns) CUDA_TRY(cudaFuncGetAttributes(&fa, fn));
   }
@@ -2213,12 +2189,12 @@ static int enqueue_fallbacks(lig_ctx* c, Slot& s, const FallbackCall& f, cudaStr
   const int blocks = (f.R + kFallbackThreads - 1) / kFallbackThreads;
   const uint4* cls = reinterpret_cast<const uint4*>(s.d_cls);
   if (f.models)
-    lig_pick_fallback_kernel<true><<<blocks, kFallbackThreads, 0, st>>>(
+    lig_pick_fallback_kernel<true, false><<<blocks, kFallbackThreads, 0, st>>>(
         f.in, f.out, f.fallbacks, f.R, f.n_fallbacks, cls, s.d_lists, s.A, s.d_ctab, s.d_mtab, s.n_models, f.seed,
-        f.first_index);
+        f.first_index, nullptr);
   else
-    lig_pick_fallback_kernel<false><<<blocks, kFallbackThreads, 0, st>>>(
-        f.in, f.out, f.fallbacks, f.R, f.n_fallbacks, cls, s.d_lists, s.A, s.d_ctab, nullptr, 0u, f.seed, 0);
+    lig_pick_fallback_kernel<false, false><<<blocks, kFallbackThreads, 0, st>>>(
+        f.in, f.out, f.fallbacks, f.R, f.n_fallbacks, cls, s.d_lists, s.A, s.d_ctab, nullptr, 0u, f.seed, 0, nullptr);
   CUDA_TRY(cudaGetLastError());
   c->launches++;
   return note_reader(s, st);
@@ -2319,10 +2295,11 @@ int lig_schedule_models_batch_fallbacks_device(lig_ctx* c, uint64_t epoch, uint6
                          stream);
 }
 
-// ---- retry scheduling (lig_schedule_[models_]batch_excluding) -----------------------------------------
+// ---- retry scheduling (lig_schedule_[models_]batch_excluding[_fallbacks]) -----------------------------
 // One retry call: descriptors in, lig_pick out; or (models) model ids in at the fixed targets
 // targets[i], lig_mpick out, request i with rand_key = first_index + i, resolved against the model
-// table mtab of n_models entries (set where the call is enqueued).
+// table mtab of n_models entries (set where the call is enqueued).  With n_fallbacks > 0, a row of
+// n_fallbacks int16 per request as well; every retry rule applies.
 struct ExcludingCall {
   uint64_t seed;
   const void* in;                        // lig_req[R] or uint32_t[R]
@@ -2330,6 +2307,8 @@ struct ExcludingCall {
   void* out;                             // lig_pick[R] or lig_mpick[R]
   int n_excluded;
   const int16_t* excluded;
+  int n_fallbacks = 0;                   // 0: no rows
+  int16_t* fallbacks = nullptr;
   bool models = false;
   uint64_t first_index = 0;
   const uint8_t* targets = nullptr;
@@ -2341,19 +2320,24 @@ struct ExcludingCall {
 };
 
 static ExcludingCall model_retry(uint64_t seed, uint64_t first_index, const uint32_t* ids, const uint8_t* targets,
-                                 int R, const int16_t* excluded, int n_excluded, lig_mpick* out) {
-  ExcludingCall x{seed, ids, R, out, n_excluded, excluded};
+                                 int R, const int16_t* excluded, int n_excluded, lig_mpick* out,
+                                 int n_fallbacks = 0, int16_t* fallbacks = nullptr) {
+  ExcludingCall x{seed, ids, R, out, n_excluded, excluded, n_fallbacks, fallbacks};
   x.models = true;
   x.first_index = first_index;
   x.targets = targets;
   return x;
 }
 
-static int excluding_check(const lig_ctx* c, const char* fn, const ExcludingCall& x) {
+// `rows`: the entry point takes fallback rows, so x.n_fallbacks must be in [1, LIG_MAX_FALLBACKS].
+static int excluding_check(const lig_ctx* c, const char* fn, const ExcludingCall& x, bool rows) {
   if (!c || x.R < 0 || (x.R > 0 && (!x.in || !x.out || !x.excluded || (x.models && !x.targets))))
     return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
   if (x.n_excluded < 1 || x.n_excluded > LIG_MAX_EXCLUDED)
     return fail(LIG_ERR_INVALID, "%s: n_excluded=%d outside [1, %d]", fn, x.n_excluded, LIG_MAX_EXCLUDED);
+  if (rows && x.R > 0 && !x.fallbacks) return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
+  if (rows && (x.n_fallbacks < 1 || x.n_fallbacks > LIG_MAX_FALLBACKS))
+    return fail(LIG_ERR_INVALID, "%s: n_fallbacks=%d outside [1, %d]", fn, x.n_fallbacks, LIG_MAX_FALLBACKS);
   return 0;
 }
 
@@ -2361,102 +2345,55 @@ static int excluding_slot(lig_ctx* c, const ExcludingCall& x, uint64_t epoch, Sl
   return x.models ? resolve_models_slot(c, epoch, s) : resolve_slot(c, epoch, s);
 }
 
-// Launch the retry walk for x (descriptors; R >= 1, device-visible, aligned pointers) over slot s on
-// st, with the scan's launch shape: `tree` (null = the built-in tree with `thr`); `hist` non-null
-// counts each LIG_OK pick into it (the feedback chain's segment).  The caller checks the launch.
+// Launch the retry kernel for x (R >= 1, device-visible, aligned pointers, x.mtab set for model ids)
+// over slot s on st, with the scan's launch shape: `tree` (null = the built-in tree with `thr`); the
+// pool of an ejected epoch; a row per request when x.n_fallbacks > 0; `hist` non-null counts each
+// LIG_OK pick into it (the feedback chain's segment).  The caller checks the launch.
 static void launch_excluding(const lig_ctx* c, const Slot& s, const Thr& thr, const FilterTree* tree,
                              const ExcludingCall& x, int* hist, cudaStream_t st) {
   static const FilterTree kNoTree{};
   const ScanShape sh = scan_shape(c, s, x.R);
   const SnapView v = view_of(s);
   const FilterTree& t = tree ? *tree : kNoTree;
-  const int4* in = static_cast<const int4*>(x.in);
-  int2* out = static_cast<int2*>(x.out);
-  auto launch = [&](auto staged, auto caller_tree) {
-    constexpr bool kS = decltype(staged)::value, kT = decltype(caller_tree)::value;
-    if (hist && s.n_ejected > 0)
-      lig_schedule_excluding_count_kernel<kS, kT, true><<<sh.grid, kCtaThreads, sh.smem, st>>>(
-          v, thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, hist, s.d_pool);
-    else if (hist)
-      lig_schedule_excluding_count_kernel<kS, kT><<<sh.grid, kCtaThreads, sh.smem, st>>>(
-          v, thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, hist);
-    else if (s.n_ejected > 0)
-      lig_schedule_excluding_kernel<kS, kT, true><<<sh.grid, kCtaThreads, sh.smem, st>>>(
-          v, thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, s.d_pool);
-    else
-      lig_schedule_excluding_kernel<kS, kT><<<sh.grid, kCtaThreads, sh.smem, st>>>(
-          v, thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed);
-  };
-  using Y = std::true_type;
-  using N = std::false_type;
-  if (tree) {
-    if (sh.staged) launch(Y{}, Y{});
-    else launch(N{}, Y{});
-  } else {
-    if (sh.staged) launch(Y{}, N{});
-    else launch(N{}, N{});
-  }
-}
-
-// Launch the model-id retry walk for x (models; R >= 1, device-visible, aligned pointers, x.mtab set)
-// over slot s on st, with the scan's launch shape: `tree` as above; a row of n_fallbacks per request
-// when n_fallbacks > 0; `hist` non-null counts each LIG_OK pick into it.  The caller checks the launch.
-static void launch_models_excluding(const lig_ctx* c, const Slot& s, const Thr& thr, const FilterTree* tree,
-                                    const ExcludingCall& x, int n_fallbacks, int16_t* fallbacks, int* hist,
-                                    cudaStream_t st) {
-  static const FilterTree kNoTree{};
-  const ScanShape sh = scan_shape(c, s, x.R);
-  const SnapView v = view_of(s);
-  const FilterTree& t = tree ? *tree : kNoTree;
   const uint32_t* pool = s.n_ejected > 0 ? s.d_pool : nullptr;
-  auto launch = [&](auto staged, auto caller_tree, auto ejected, auto rows, auto count) {
-    lig_schedule_models_excluding_kernel<decltype(staged)::value, decltype(caller_tree)::value,
-                                         decltype(ejected)::value, decltype(rows)::value, decltype(count)::value>
-        <<<sh.grid, kCtaThreads, sh.smem, st>>>(v, thr, t, static_cast<const uint32_t*>(x.in), x.targets, x.excluded,
-                                                x.n_excluded, static_cast<uint32_t*>(x.out), x.R, x.seed,
-                                                x.first_index, x.mtab, x.n_models, n_fallbacks, fallbacks, hist,
-                                                pool);
+  auto launch = [&](auto... form) {
+    lig_schedule_excluding_kernel<decltype(form)::value...><<<sh.grid, kCtaThreads, sh.smem, st>>>(
+        v, thr, t, x.in, x.targets, x.excluded, x.n_excluded, x.out, x.R, x.seed, x.first_index, x.mtab, x.n_models,
+        x.n_fallbacks, x.fallbacks, hist, pool);
   };
   using Y = std::true_type;
   using N = std::false_type;
   auto with_count = [&](auto... f) { if (hist) launch(f..., Y{}); else launch(f..., N{}); };
-  auto with_rows = [&](auto... f) { if (n_fallbacks > 0) with_count(f..., Y{}); else with_count(f..., N{}); };
+  auto with_rows = [&](auto... f) { if (x.n_fallbacks > 0) with_count(f..., Y{}); else with_count(f..., N{}); };
   auto with_pool = [&](auto... f) { if (pool) with_rows(f..., Y{}); else with_rows(f..., N{}); };
   auto with_tree = [&](auto... f) { if (tree) with_pool(f..., Y{}); else with_pool(f..., N{}); };
-  if (sh.staged) with_tree(Y{});
-  else with_tree(N{});
-}
-
-// The model-id form of x against slot s: ordered behind the slot's model table on st, reading it.
-// Caller holds c->mu.
-static int with_model_table(Slot& s, ExcludingCall* x, cudaStream_t st) {
-  CUDA_TRY(cudaStreamWaitEvent(st, s.models_ready, 0));
-  x->mtab = s.d_mtab;
-  x->n_models = s.n_models;
-  return 0;
+  auto with_staged = [&](auto... f) { if (sh.staged) with_tree(f..., Y{}); else with_tree(f..., N{}); };
+  if (x.models) with_staged(Y{});
+  else with_staged(N{});
 }
 
 // Enqueue the retry kernel for x (R >= 1, device-visible, aligned pointers) against slot s on st,
-// behind the slot's tables, and register st as a reader of the slot.  The walk is the tree that
-// built the slot's tables.  Caller holds c->mu.
+// behind the slot's tables (and model table), and register st as a reader of the slot.  The walk is
+// the tree that built the slot's tables.  Caller holds c->mu.
 static int enqueue_excluding(lig_ctx* c, Slot& s, const ExcludingCall& x, cudaStream_t st) {
   CUDA_TRY(cudaStreamWaitEvent(st, s.ready, 0));
+  ExcludingCall m = x;
   if (x.models) {
-    ExcludingCall m = x;
-    if (int rc = with_model_table(s, &m, st)) return rc;
-    launch_models_excluding(c, s, thr_of(c), s.caller_tree ? &s.tree : nullptr, m, 0, nullptr, nullptr, st);
-  } else {
-    launch_excluding(c, s, thr_of(c), s.caller_tree ? &s.tree : nullptr, x, nullptr, st);
+    CUDA_TRY(cudaStreamWaitEvent(st, s.models_ready, 0));
+    m.mtab = s.d_mtab;
+    m.n_models = s.n_models;
   }
+  launch_excluding(c, s, thr_of(c), s.caller_tree ? &s.tree : nullptr, m, nullptr, st);
   CUDA_TRY(cudaGetLastError());
   c->launches++;
   return note_reader(s, st);
 }
 
-static int excluding_device(lig_ctx* c, const char* fn, uint64_t epoch, const ExcludingCall& x, void* stream) {
-  if (int rc = excluding_check(c, fn, x)) return rc;
+static int excluding_device(lig_ctx* c, const char* fn, uint64_t epoch, const ExcludingCall& x, bool rows,
+                            void* stream) {
+  if (int rc = excluding_check(c, fn, x, rows)) return rc;
   if (x.R > 0 && (misaligned(x.in, x.in_bytes()) || misaligned(x.out, x.out_bytes()) ||
-                  misaligned(x.excluded, sizeof(int16_t))))
+                  misaligned(x.excluded, sizeof(int16_t)) || (rows && misaligned(x.fallbacks, sizeof(int16_t)))))
     return fail(LIG_ERR_INVALID, "%s: a device buffer is not aligned to its element", fn);
   std::lock_guard<std::mutex> lk(c->mu);
   Slot* s = nullptr;
@@ -2469,7 +2406,7 @@ static int excluding_device(lig_ctx* c, const char* fn, uint64_t epoch, const Ex
 int lig_schedule_batch_excluding_device(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* d_reqs, int R,
                                         const int16_t* d_excluded, int n_excluded, lig_pick* d_out, void* stream) {
   return excluding_device(c, "lig_schedule_batch_excluding_device", epoch,
-                          ExcludingCall{seed, d_reqs, R, d_out, n_excluded, d_excluded}, stream);
+                          ExcludingCall{seed, d_reqs, R, d_out, n_excluded, d_excluded}, false, stream);
 }
 
 int lig_schedule_models_batch_excluding_device(lig_ctx* c, uint64_t epoch, uint64_t seed, uint64_t first_index,
@@ -2478,85 +2415,15 @@ int lig_schedule_models_batch_excluding_device(lig_ctx* c, uint64_t epoch, uint6
                                                void* stream) {
   return excluding_device(c, "lig_schedule_models_batch_excluding_device", epoch,
                           model_retry(seed, first_index, d_model_ids, d_targets, R, d_excluded, n_excluded, d_out),
-                          stream);
-}
-
-// ---- retry scheduling with fallback rows (lig_schedule_[models_]batch_excluding_fallbacks) ------------
-// The retry call's arguments plus a row of n_fallbacks int16 per request; every retry rule applies.
-static int excluding_fallbacks_check(const lig_ctx* c, const char* fn, const ExcludingCall& x, int n_fallbacks,
-                                     const int16_t* fallbacks) {
-  if (int rc = excluding_check(c, fn, x)) return rc;
-  if (x.R > 0 && !fallbacks) return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
-  if (n_fallbacks < 1 || n_fallbacks > LIG_MAX_FALLBACKS)
-    return fail(LIG_ERR_INVALID, "%s: n_fallbacks=%d outside [1, %d]", fn, n_fallbacks, LIG_MAX_FALLBACKS);
-  return 0;
-}
-
-// Enqueue the retry-with-rows kernel for x (R >= 1, device-visible, aligned pointers) against slot s on
-// st, behind the slot's tables, with the scan's launch shape and the tree that built the slot's
-// tables, and register st as a reader of the slot.  Caller holds c->mu.
-static int enqueue_excluding_fallbacks(lig_ctx* c, Slot& s, const ExcludingCall& x, int n_fallbacks,
-                                       int16_t* fallbacks, cudaStream_t st) {
-  static const FilterTree kNoTree{};
-  CUDA_TRY(cudaStreamWaitEvent(st, s.ready, 0));
-  if (x.models) {
-    ExcludingCall m = x;
-    if (int rc = with_model_table(s, &m, st)) return rc;
-    launch_models_excluding(c, s, thr_of(c), s.caller_tree ? &s.tree : nullptr, m, n_fallbacks, fallbacks, nullptr,
-                            st);
-    CUDA_TRY(cudaGetLastError());
-    c->launches++;
-    return note_reader(s, st);
-  }
-  const ScanShape sh = scan_shape(c, s, x.R);
-  const SnapView v = view_of(s);
-  const FilterTree& t = s.caller_tree ? s.tree : kNoTree;
-  const Thr thr = thr_of(c);
-  const int4* in = static_cast<const int4*>(x.in);
-  int2* out = static_cast<int2*>(x.out);
-  auto launch = [&](auto staged, auto caller_tree) {
-    constexpr bool kS = decltype(staged)::value, kT = decltype(caller_tree)::value;
-    if (s.n_ejected > 0)
-      lig_schedule_excluding_fallback_kernel<kS, kT, true><<<sh.grid, kCtaThreads, sh.smem, st>>>(
-          v, thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, n_fallbacks, fallbacks, s.d_pool);
-    else
-      lig_schedule_excluding_fallback_kernel<kS, kT><<<sh.grid, kCtaThreads, sh.smem, st>>>(
-          v, thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, n_fallbacks, fallbacks);
-  };
-  using Y = std::true_type;
-  using N = std::false_type;
-  if (s.caller_tree) {
-    if (sh.staged) launch(Y{}, Y{});
-    else launch(N{}, Y{});
-  } else {
-    if (sh.staged) launch(Y{}, N{});
-    else launch(N{}, N{});
-  }
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return note_reader(s, st);
-}
-
-static int excluding_fallbacks_device(lig_ctx* c, const char* fn, uint64_t epoch, const ExcludingCall& x,
-                                      int n_fallbacks, int16_t* d_fallbacks, void* stream) {
-  if (int rc = excluding_fallbacks_check(c, fn, x, n_fallbacks, d_fallbacks)) return rc;
-  if (x.R > 0 && (misaligned(x.in, x.in_bytes()) || misaligned(x.out, x.out_bytes()) ||
-                  misaligned(x.excluded, sizeof(int16_t)) || misaligned(d_fallbacks, sizeof(int16_t))))
-    return fail(LIG_ERR_INVALID, "%s: a device buffer is not aligned to its element", fn);
-  std::lock_guard<std::mutex> lk(c->mu);
-  Slot* s = nullptr;
-  if (int rc = excluding_slot(c, x, epoch, &s)) return rc;
-  if (x.R == 0) return 0;
-  CUDA_TRY(cudaSetDevice(c->device));
-  return enqueue_excluding_fallbacks(c, *s, x, n_fallbacks, d_fallbacks, static_cast<cudaStream_t>(stream));
+                          false, stream);
 }
 
 int lig_schedule_batch_excluding_fallbacks_device(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* d_reqs,
                                                   int R, const int16_t* d_excluded, int n_excluded, lig_pick* d_out,
                                                   int n_fallbacks, int16_t* d_fallbacks, void* stream) {
-  return excluding_fallbacks_device(c, "lig_schedule_batch_excluding_fallbacks_device", epoch,
-                                    ExcludingCall{seed, d_reqs, R, d_out, n_excluded, d_excluded}, n_fallbacks,
-                                    d_fallbacks, stream);
+  return excluding_device(c, "lig_schedule_batch_excluding_fallbacks_device", epoch,
+                          ExcludingCall{seed, d_reqs, R, d_out, n_excluded, d_excluded, n_fallbacks, d_fallbacks},
+                          true, stream);
 }
 
 int lig_schedule_models_batch_excluding_fallbacks_device(lig_ctx* c, uint64_t epoch, uint64_t seed,
@@ -2564,34 +2431,34 @@ int lig_schedule_models_batch_excluding_fallbacks_device(lig_ctx* c, uint64_t ep
                                                          const uint8_t* d_targets, int R, const int16_t* d_excluded,
                                                          int n_excluded, lig_mpick* d_out, int n_fallbacks,
                                                          int16_t* d_fallbacks, void* stream) {
-  return excluding_fallbacks_device(
-      c, "lig_schedule_models_batch_excluding_fallbacks_device", epoch,
-      model_retry(seed, first_index, d_model_ids, d_targets, R, d_excluded, n_excluded, d_out), n_fallbacks,
-      d_fallbacks, stream);
+  return excluding_device(c, "lig_schedule_models_batch_excluding_fallbacks_device", epoch,
+                          model_retry(seed, first_index, d_model_ids, d_targets, R, d_excluded, n_excluded, d_out,
+                                      n_fallbacks, d_fallbacks),
+                          true, stream);
 }
 
-// The host buffers of a retry call (with rows when n_fallbacks > 0): page-locked, aligned ones are
+// The host buffers of a retry call (with rows when x.n_fallbacks > 0): page-locked, aligned ones are
 // read and written by the kernel in place; the others are staged in stream-ordered HBM and copied on
 // the call's lane.  Blocks until the picks (and rows) are back.
-static int excluding_host(lig_ctx* c, const char* fn, uint64_t epoch, const ExcludingCall& x, int n_fallbacks,
-                          int16_t* fallbacks) {
+static int excluding_host(lig_ctx* c, const char* fn, uint64_t epoch, const ExcludingCall& x, bool rows) {
+  if (int rc = excluding_check(c, fn, x, rows)) return rc;
   const int R = x.R;
   if (R > c->max_batch) return fail(LIG_ERR_INVALID, "%s: R=%d exceeds max_batch=%d", fn, R, c->max_batch);
   ExcludingCall d = x;    // the same call with device-visible pointers
   const size_t in_b = (size_t)R * x.in_bytes(), out_b = (size_t)R * x.out_bytes();
-  const size_t rows_b = (size_t)R * x.row_bytes(), fb_b = (size_t)R * (size_t)n_fallbacks * sizeof(int16_t);
+  const size_t rows_b = (size_t)R * x.row_bytes(), fb_b = (size_t)R * (size_t)x.n_fallbacks * sizeof(int16_t);
   const size_t tg_b = x.models ? (size_t)R : 0;
   d.in = R ? mapped_device_pointer(x.in) : nullptr;
   d.out = R ? mapped_device_pointer(x.out) : nullptr;
   d.excluded = R ? mapped_device_pointer(x.excluded) : nullptr;
   d.targets = R && x.models ? mapped_device_pointer(x.targets) : nullptr;
-  int16_t* d_fb = R && n_fallbacks ? mapped_device_pointer(fallbacks) : nullptr;
+  d.fallbacks = R && x.n_fallbacks ? mapped_device_pointer(x.fallbacks) : nullptr;
   // the kernels read a descriptor with one 16-byte load and store every pick whole
   const bool st_in = R && (!d.in || misaligned(d.in, x.in_bytes()));
   const bool st_out = R && (!d.out || misaligned(d.out, x.out_bytes()));
   const bool st_rows = R && (!d.excluded || misaligned(d.excluded, sizeof(int16_t)));
   const bool st_tg = R && x.models && !d.targets;
-  const bool st_fb = R && n_fallbacks && (!d_fb || misaligned(d_fb, sizeof(int16_t)));
+  const bool st_fb = R && x.n_fallbacks && (!d.fallbacks || misaligned(d.fallbacks, sizeof(int16_t)));
   cudaStream_t st = nullptr;
   unsigned char* stage = nullptr;
   {
@@ -2615,7 +2482,7 @@ static int excluding_host(lig_ctx* c, const char* fn, uint64_t epoch, const Excl
       if (st_out) d.out = stage + o_out;
       if (st_rows) d.excluded = reinterpret_cast<const int16_t*>(stage + o_rows);
       if (st_tg) d.targets = stage + o_tg;
-      if (st_fb) d_fb = reinterpret_cast<int16_t*>(stage + o_fb);
+      if (st_fb) d.fallbacks = reinterpret_cast<int16_t*>(stage + o_fb);
     }
     int rc = 0;
     if (st_in && cudaMemcpyAsync(const_cast<void*>(d.in), x.in, in_b, cudaMemcpyHostToDevice, st) != cudaSuccess)
@@ -2626,7 +2493,7 @@ static int excluding_host(lig_ctx* c, const char* fn, uint64_t epoch, const Excl
     if (!rc && st_tg &&
         cudaMemcpyAsync(const_cast<uint8_t*>(d.targets), x.targets, tg_b, cudaMemcpyHostToDevice, st) != cudaSuccess)
       rc = fail(LIG_ERR_CUDA, "%s: staging the targets failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
-    if (!rc) rc = n_fallbacks ? enqueue_excluding_fallbacks(c, *s, d, n_fallbacks, d_fb, st) : enqueue_excluding(c, *s, d, st);
+    if (!rc) rc = enqueue_excluding(c, *s, d, st);
     if (rc) {
       if (stage) cudaFreeAsync(stage, st);
       return rc;
@@ -2635,7 +2502,7 @@ static int excluding_host(lig_ctx* c, const char* fn, uint64_t epoch, const Excl
   // the copies back wait for the kernel on the lane; they may block, so not under c->mu
   cudaError_t e = cudaSuccess;
   if (st_out) e = cudaMemcpyAsync(x.out, d.out, out_b, cudaMemcpyDeviceToHost, st);
-  if (st_fb && e == cudaSuccess) e = cudaMemcpyAsync(fallbacks, d_fb, fb_b, cudaMemcpyDeviceToHost, st);
+  if (st_fb && e == cudaSuccess) e = cudaMemcpyAsync(x.fallbacks, d.fallbacks, fb_b, cudaMemcpyDeviceToHost, st);
   if (stage) cudaFreeAsync(stage, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   if (e != cudaSuccess) return fail(LIG_ERR_CUDA, "%s failed on the device: %s", fn, cudaGetErrorString(e));
@@ -2644,38 +2511,32 @@ static int excluding_host(lig_ctx* c, const char* fn, uint64_t epoch, const Excl
 
 int lig_schedule_batch_excluding(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
                                  const int16_t* excluded, int n_excluded, lig_pick* out) {
-  static const char fn[] = "lig_schedule_batch_excluding";
-  const ExcludingCall x{seed, reqs, R, out, n_excluded, excluded};
-  if (int rc = excluding_check(c, fn, x)) return rc;
-  return excluding_host(c, fn, epoch, x, 0, nullptr);
+  return excluding_host(c, "lig_schedule_batch_excluding", epoch,
+                        ExcludingCall{seed, reqs, R, out, n_excluded, excluded}, false);
 }
 
 int lig_schedule_models_batch_excluding(lig_ctx* c, uint64_t epoch, uint64_t seed, uint64_t first_index,
                                         const uint32_t* model_ids, const uint8_t* targets, int R,
                                         const int16_t* excluded, int n_excluded, lig_mpick* out) {
-  static const char fn[] = "lig_schedule_models_batch_excluding";
-  const ExcludingCall x = model_retry(seed, first_index, model_ids, targets, R, excluded, n_excluded, out);
-  if (int rc = excluding_check(c, fn, x)) return rc;
-  return excluding_host(c, fn, epoch, x, 0, nullptr);
+  return excluding_host(c, "lig_schedule_models_batch_excluding", epoch,
+                        model_retry(seed, first_index, model_ids, targets, R, excluded, n_excluded, out), false);
 }
 
 int lig_schedule_batch_excluding_fallbacks(lig_ctx* c, uint64_t epoch, uint64_t seed, const lig_req* reqs, int R,
                                            const int16_t* excluded, int n_excluded, lig_pick* out,
                                            int n_fallbacks, int16_t* fallbacks) {
-  static const char fn[] = "lig_schedule_batch_excluding_fallbacks";
-  const ExcludingCall x{seed, reqs, R, out, n_excluded, excluded};
-  if (int rc = excluding_fallbacks_check(c, fn, x, n_fallbacks, fallbacks)) return rc;
-  return excluding_host(c, fn, epoch, x, n_fallbacks, fallbacks);
+  return excluding_host(c, "lig_schedule_batch_excluding_fallbacks", epoch,
+                        ExcludingCall{seed, reqs, R, out, n_excluded, excluded, n_fallbacks, fallbacks}, true);
 }
 
 int lig_schedule_models_batch_excluding_fallbacks(lig_ctx* c, uint64_t epoch, uint64_t seed, uint64_t first_index,
                                                   const uint32_t* model_ids, const uint8_t* targets, int R,
                                                   const int16_t* excluded, int n_excluded, lig_mpick* out,
                                                   int n_fallbacks, int16_t* fallbacks) {
-  static const char fn[] = "lig_schedule_models_batch_excluding_fallbacks";
-  const ExcludingCall x = model_retry(seed, first_index, model_ids, targets, R, excluded, n_excluded, out);
-  if (int rc = excluding_fallbacks_check(c, fn, x, n_fallbacks, fallbacks)) return rc;
-  return excluding_host(c, fn, epoch, x, n_fallbacks, fallbacks);
+  return excluding_host(c, "lig_schedule_models_batch_excluding_fallbacks", epoch,
+                        model_retry(seed, first_index, model_ids, targets, R, excluded, n_excluded, out, n_fallbacks,
+                                    fallbacks),
+                        true);
 }
 
 int lig_pick_kernel_info(lig_ctx* c, uint64_t epoch, char* name, int name_len, int* grid, int* threads,
@@ -2790,39 +2651,6 @@ struct FbReqs {
   size_t out_bytes() const { return models ? sizeof(lig_mpick) : sizeof(lig_pick); }
 };
 
-// Launch the chain segment of a retry call with fallback rows: x (R >= 1, device-visible, aligned
-// pointers) over the chain's scratch slot fs on st, with the scan's launch shape and the chain's tree
-// and thresholds; each LIG_OK pick is counted into the open window.  The caller checks the launch.
-static void launch_excluding_fallback_count(const lig_ctx* c, const Slot& fs, const FbRun& run,
-                                            const ExcludingCall& x, int n_fallbacks, int16_t* fallbacks,
-                                            cudaStream_t st) {
-  static const FilterTree kNoTree{};
-  const ScanShape sh = scan_shape(c, fs, x.R);
-  const SnapView v = view_of(fs);
-  const FilterTree& t = run.tree ? *run.tree : kNoTree;
-  const int4* in = static_cast<const int4*>(x.in);
-  int2* out = static_cast<int2*>(x.out);
-  auto launch = [&](auto staged, auto caller_tree) {
-    constexpr bool kS = decltype(staged)::value, kT = decltype(caller_tree)::value;
-    if (fs.n_ejected > 0)
-      lig_schedule_excluding_fallback_count_kernel<kS, kT, true><<<sh.grid, kCtaThreads, sh.smem, st>>>(
-          v, run.thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, n_fallbacks, fallbacks, c->d_fb_hist,
-          fs.d_pool);
-    else
-      lig_schedule_excluding_fallback_count_kernel<kS, kT><<<sh.grid, kCtaThreads, sh.smem, st>>>(
-          v, run.thr, t, in, x.excluded, x.n_excluded, out, x.R, x.seed, n_fallbacks, fallbacks, c->d_fb_hist);
-  };
-  using Y = std::true_type;
-  using N = std::false_type;
-  if (run.tree) {
-    if (sh.staged) launch(Y{}, Y{});
-    else launch(N{}, Y{});
-  } else {
-    if (sh.staged) launch(Y{}, N{});
-    else launch(N{}, N{});
-  }
-}
-
 // Schedule R requests through the window sequence: each segment is the rest of the open window or
 // of the call, whichever is shorter; one fused pick + count launch per segment (pick + row + count
 // when the call asked for rows); a filled window is closed at once, its tables are rebuilt only
@@ -2846,33 +2674,30 @@ static int fb_schedule(lig_ctx* c, FbRun& run, uint64_t seed, const FbReqs& rq, 
     void* out = static_cast<unsigned char*>(rq.out) + (size_t)pos * rq.out_bytes();
     const int grid = (n + kPickThreads * kCountPerThread - 1) / (kPickThreads * kCountPerThread);
     const uint4* fcls = reinterpret_cast<const uint4*>(fs.d_cls);
-    if (rq.retry && rq.models) {
+    if (rq.retry) {
       ExcludingCall x{seed, in, n, out, rq.n_excluded, rq.excluded + (size_t)pos * (size_t)rq.n_excluded};
-      x.models = true;
-      x.first_index = rq.first_index + (uint64_t)pos;
-      x.targets = rq.targets + pos;
-      x.mtab = rq.mtab;
-      x.n_models = rq.n_models;
-      launch_models_excluding(c, fs, run.thr, run.tree, x, rq.rows ? rq.n_fallbacks : 0,
-                              rq.rows ? rq.fallbacks + (size_t)pos * (size_t)rq.n_fallbacks : nullptr, c->d_fb_hist,
-                              st);
-    } else if (rq.retry && rq.rows) {
-      const ExcludingCall x{seed, in, n, out, rq.n_excluded, rq.excluded + (size_t)pos * (size_t)rq.n_excluded};
-      launch_excluding_fallback_count(c, fs, run, x, rq.n_fallbacks,
-                                      rq.fallbacks + (size_t)pos * (size_t)rq.n_fallbacks, st);
-    } else if (rq.retry) {
-      const ExcludingCall x{seed, in, n, out, rq.n_excluded, rq.excluded + (size_t)pos * (size_t)rq.n_excluded};
+      if (rq.rows) {
+        x.n_fallbacks = rq.n_fallbacks;
+        x.fallbacks = rq.fallbacks + (size_t)pos * (size_t)rq.n_fallbacks;
+      }
+      if (rq.models) {
+        x.models = true;
+        x.first_index = rq.first_index + (uint64_t)pos;
+        x.targets = rq.targets + pos;
+        x.mtab = rq.mtab;
+        x.n_models = rq.n_models;
+      }
       launch_excluding(c, fs, run.thr, run.tree, x, c->d_fb_hist, st);
     } else if (rq.rows) {
       int16_t* rows = rq.fallbacks + (size_t)pos * (size_t)rq.n_fallbacks;
       const int blocks = (n + kFallbackThreads - 1) / kFallbackThreads;
       if (rq.models)
-        lig_pick_fallback_count_kernel<true><<<blocks, kFallbackThreads, 0, st>>>(
-            in, out, rows, n, rq.n_fallbacks, fcls, fs.d_lists, fs.A, rq.mtab, rq.n_models, seed,
+        lig_pick_fallback_kernel<true, true><<<blocks, kFallbackThreads, 0, st>>>(
+            in, out, rows, n, rq.n_fallbacks, fcls, fs.d_lists, fs.A, nullptr, rq.mtab, rq.n_models, seed,
             rq.first_index + (uint64_t)pos, c->d_fb_hist);
       else
-        lig_pick_fallback_count_kernel<false><<<blocks, kFallbackThreads, 0, st>>>(
-            in, out, rows, n, rq.n_fallbacks, fcls, fs.d_lists, fs.A, nullptr, 0u, seed, 0, c->d_fb_hist);
+        lig_pick_fallback_kernel<false, true><<<blocks, kFallbackThreads, 0, st>>>(
+            in, out, rows, n, rq.n_fallbacks, fcls, fs.d_lists, fs.A, nullptr, nullptr, 0u, seed, 0, c->d_fb_hist);
     } else if (rq.models)
       lig_pick_models_count_kernel<<<grid, kPickThreads, 0, st>>>(
           static_cast<const uint32_t*>(in), static_cast<uint32_t*>(out), n, reinterpret_cast<const uint4*>(fs.d_cls),

@@ -2584,7 +2584,6 @@ __device__ __forceinline__ uint32_t int31n_next(uint64_t& state, uint32_t n) {
 
 // Ranked entries 1 .. m-1 of a request's fallback row, then -1 to the end of the row: `state` is
 // the pick's stream (seed ^ rand_key), `e` the class entry the pick used, `ok` whether it is LIG_OK.
-// Shared by the resident-epoch kernel and the feedback chain's.
 __device__ __forceinline__ void write_fallback_row(uint64_t state, const uint4 e, bool ok, int n_fallbacks,
                                                    const uint16_t* __restrict__ glists, int16_t* __restrict__ row) {
   const uint32_t n = ok ? e.x >> 16 : 0u;
@@ -2617,57 +2616,28 @@ __device__ __forceinline__ void write_fallback_row(uint64_t state, const uint4 e
   }
 }
 
-template <bool kModels>
+// kCount: the chain segment of lig_schedule_[models_]batch_feedback_chain_fallbacks.  The same pick
+// and row on the chain's private tables (always the strided rows, as the count kernels read them),
+// and the pick counted into the open window like lig_pick_[models_]count_kernel.  Row entries are
+// not counted.  A lane past the end still reaches the full-warp match with pod -1.
+template <bool kModels, bool kCount>
 __global__ void __launch_bounds__(kFallbackThreads)
 lig_pick_fallback_kernel(const void* __restrict__ in, void* __restrict__ out, int16_t* __restrict__ fallbacks,
                          int R, int n_fallbacks, const uint4* __restrict__ cls, const uint16_t* __restrict__ lists,
                          int A, const unsigned char* __restrict__ ctab, const unsigned char* __restrict__ mtab,
-                         uint32_t n_models, uint64_t seed, uint64_t first_index) {
+                         uint32_t n_models, uint64_t seed, uint64_t first_index, int* __restrict__ hist) {
   const int i = (int)blockIdx.x * kFallbackThreads + (int)threadIdx.x;
-  if (i >= R) return;
-  const CompactHeader hdr = *reinterpret_cast<const CompactHeader*>(ctab);
-  const uint32_t n_classes = 2u * ((uint32_t)A + 1u);
+  if (!kCount && i >= R) return;
   const uint4* gcls = cls;
   const uint16_t* glists = lists;
-  if (hdr.bytes != 0u && hdr.n_classes == n_classes) {
-    gcls = reinterpret_cast<const uint4*>(ctab + sizeof(CompactHeader));
-    glists = reinterpret_cast<const uint16_t*>(ctab + sizeof(CompactHeader) + (size_t)n_classes * sizeof(ClassEntry));
+  if constexpr (!kCount) {
+    const CompactHeader hdr = *reinterpret_cast<const CompactHeader*>(ctab);
+    const uint32_t n_classes = 2u * ((uint32_t)A + 1u);
+    if (hdr.bytes != 0u && hdr.n_classes == n_classes) {
+      gcls = reinterpret_cast<const uint4*>(ctab + sizeof(CompactHeader));
+      glists = reinterpret_cast<const uint16_t*>(ctab + sizeof(CompactHeader) + (size_t)n_classes * sizeof(ClassEntry));
+    }
   }
-  uint4 e = make_uint4(0u, 0u, 0u, 0u);
-  uint64_t key;
-  bool ok;
-  if constexpr (kModels) {
-    ModelTables mt;
-    mt.entries = reinterpret_cast<const uint4*>(mtab + sizeof(ModelHeader));
-    mt.targets = reinterpret_cast<const uint2*>(mt.entries + n_models);
-    mt.n_models = n_models;
-    key = first_index + (uint64_t)i;
-    const uint32_t v = pick_model<Ld::kLdg>(__ldg(static_cast<const uint32_t*>(in) + i), key, mt, gcls, glists,
-                                            (uint32_t)A, seed, &e);
-    static_cast<uint32_t*>(out)[i] = v;
-    ok = ((v >> 16) & 0xffu) == (uint32_t)LIG_OK;
-  } else {
-    const int4 r = ld_stream_int4(static_cast<const int4*>(in) + i);
-    key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
-    const int2 p = pick_one(r, gcls, glists, (uint32_t)A, seed, &e);
-    st_stream_int2(static_cast<int2*>(out) + i, p);
-    ok = ((uint32_t)p.y & 7u) == (uint32_t)LIG_OK;
-  }
-  write_fallback_row(seed ^ key, e, ok, n_fallbacks, glists, fallbacks + (size_t)i * (size_t)n_fallbacks);
-}
-
-// The chain segment of lig_schedule_[models_]batch_feedback_chain_fallbacks: the pick and row of
-// lig_pick_fallback_kernel on the chain's private tables (always the strided rows, as the count
-// kernels read them), and the pick counted into the open window like lig_pick_[models_]count_kernel.
-// Row entries are not counted.  One request per thread; a lane past the end still reaches the
-// full-warp match with pod -1.
-template <bool kModels>
-__global__ void __launch_bounds__(kFallbackThreads)
-lig_pick_fallback_count_kernel(const void* __restrict__ in, void* __restrict__ out, int16_t* __restrict__ fallbacks,
-                               int R, int n_fallbacks, const uint4* __restrict__ cls,
-                               const uint16_t* __restrict__ lists, int A, const unsigned char* __restrict__ mtab,
-                               uint32_t n_models, uint64_t seed, uint64_t first_index, int* __restrict__ hist) {
-  const int i = (int)blockIdx.x * kFallbackThreads + (int)threadIdx.x;
   int pod = -1;
   if (i < R) {
     uint4 e = make_uint4(0u, 0u, 0u, 0u);
@@ -2679,7 +2649,7 @@ lig_pick_fallback_count_kernel(const void* __restrict__ in, void* __restrict__ o
       mt.targets = reinterpret_cast<const uint2*>(mt.entries + n_models);
       mt.n_models = n_models;
       key = first_index + (uint64_t)i;
-      const uint32_t v = pick_model<Ld::kLdg>(__ldg(static_cast<const uint32_t*>(in) + i), key, mt, cls, lists,
+      const uint32_t v = pick_model<Ld::kLdg>(__ldg(static_cast<const uint32_t*>(in) + i), key, mt, gcls, glists,
                                               (uint32_t)A, seed, &e);
       static_cast<uint32_t*>(out)[i] = v;
       ok = ((v >> 16) & 0xffu) == (uint32_t)LIG_OK;
@@ -2687,14 +2657,14 @@ lig_pick_fallback_count_kernel(const void* __restrict__ in, void* __restrict__ o
     } else {
       const int4 r = ld_stream_int4(static_cast<const int4*>(in) + i);
       key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
-      const int2 p = pick_one(r, cls, lists, (uint32_t)A, seed, &e);
+      const int2 p = pick_one(r, gcls, glists, (uint32_t)A, seed, &e);
       st_stream_int2(static_cast<int2*>(out) + i, p);
       ok = ((uint32_t)p.y & 7u) == (uint32_t)LIG_OK;
       pod = p.x;
     }
-    write_fallback_row(seed ^ key, e, ok, n_fallbacks, lists, fallbacks + (size_t)i * (size_t)n_fallbacks);
+    write_fallback_row(seed ^ key, e, ok, n_fallbacks, glists, fallbacks + (size_t)i * (size_t)n_fallbacks);
   }
-  count_window_picks(pod, (int)threadIdx.x & 31, hist);
+  if constexpr (kCount) count_window_picks(pod, (int)threadIdx.x & 31, hist);
 }
 
 // loads[p] = picks of the closed windows + picks of the open one (the chain's per-pod loads).
@@ -2870,135 +2840,6 @@ lig_scan_kernel(SnapView s, Thr thr, const int4* __restrict__ reqs, int2* __rest
 }
 
 // ---- retry scheduling: the tree over each request's pool without the pods it excludes --------------
-// The scan's launch shape (one warp per request, columns staged when they fit).  Lanes 0 .. n_excluded-1
-// each take one entry of the request's row and clear that pod's bit in the warp's root mask: a
-// shared-memory atomicAnd, so a duplicate clears nothing twice, and entries outside [0, P) clear
-// nothing.  The walk starts from that mask: the built-in tree, or (kTree) the caller tree that built
-// the epoch.  Requests and rows are read with plain loads: they may be page-locked host memory.
-// kPool (an epoch derived by lig_eject_pods, here and in the three kernels below): the mask starts from
-// the epoch's pool words instead of every pod.  The pool pointer of the two resident kernels is not
-// __restrict__: with it, ptxas allocated the registers of their kPool = false forms differently.
-template <bool kStaged, bool kTree, bool kPool = false>
-__global__ void __launch_bounds__(kCtaThreads)
-lig_schedule_excluding_kernel(SnapView s, Thr thr, const __grid_constant__ FilterTree tree, const int4* reqs,
-                              const int16_t* excluded, int n_excluded, int2* out, int R, uint64_t seed,
-                              const uint32_t* pool = nullptr) {
-  extern __shared__ __align__(16) unsigned char smem[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint32_t* X = reinterpret_cast<uint32_t*>(smem) + (size_t)warp * 3 * s.W;
-  uint32_t* T = X + s.W;       // the root mask: the built-in walk's second scratch mask, a tree walk's `in`
-  uint32_t* H = T + s.W;
-  Fields f{s.kv, s.q, s.n_active, s.max_active};
-  if constexpr (kStaged) {
-    f = stage_fields(s, smem + scratch_bytes(s.W));
-    __syncthreads();
-  }
-  for (int i = blockIdx.x * kWarpsPerCta + warp; i < R; i += gridDim.x * kWarpsPerCta) {
-    const int4 r = reqs[i];    // whole warp reads the same 16 bytes (broadcast)
-    const int ex = lane < n_excluded ? excluded[(size_t)i * n_excluded + lane] : -1;
-    const bool critical = ((uint32_t)r.y & LIG_REQ_CRITICAL) != 0;
-    const uint64_t key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
-    const uint32_t* Hrow = stage_adapter_row(s, r.x, H, lane);
-    for (int w = lane; w < s.W; w += 32) {   // the request's pool: every pod (kPool: of the epoch's pool) ...
-      if constexpr (kPool) {
-        T[w] = pool[w];
-      } else {
-        const int rem = s.P - w * 32;
-        T[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
-      }
-    }
-    __syncwarp();
-    if (ex >= 0 && ex < s.P) atomicAnd(T + (ex >> 5), ~(1u << (ex & 31)));   // ... but the excluded
-    __syncwarp();
-    uint32_t n = 0;
-    for (int w = lane; w < s.W; w += 32) n += __popc(T[w]);
-    n = __reduce_add_sync(kFull, n);
-    EvalResult e;
-    if constexpr (kTree)
-      e = tree_walk_warp<kStaged, true>(f, tree.nodes, Hrow, critical, s.P, s.W, T, X, lane, n);
-    else
-      e = tree_eval_warp<kStaged, true>(f, Hrow, critical, thr, s.P, s.W, X, T, lane, n);
-    int pod = -1;
-    if (e.n > 0) {
-      uint32_t k = int31n(seed ^ key, e.n, max_accept_for(e.n));
-      for (int w = 0; w < s.W; ++w) {  // k-th survivor in pod order = pods[k]   scheduler.go:121
-        uint32_t word = e.mask[w];
-        uint32_t c = __popc(word);
-        if (k < c) { pod = w * 32 + (int)__fns(word, 0, (int)k + 1); break; }
-        k -= c;
-      }
-    }
-    if (lane == 0) out[i] = make_int2(pod, (int)(e.status | (e.n << 16)));
-    __syncwarp();
-  }
-}
-
-// The chain segment of lig_schedule_batch_feedback_chain_excluding: lig_schedule_excluding_kernel's
-// walk, step for step, on the chain's private copy (its q column has grown by every closed window)
-// with the tree and thresholds the chain started with, plus the count: lane 0 adds each LIG_OK pick
-// to the open window's histogram, one atomic per request (one warp per request: no cross-lane match
-// as in count_window_picks).  A separate body, not a shared __forceinline__ one or a template flag
-// on the resident kernel: both of those change ptxas's register allocation of the resident
-// caller-tree forms (a 16-byte stack frame appears in the staged one).
-template <bool kStaged, bool kTree, bool kPool = false>
-__global__ void __launch_bounds__(kCtaThreads)
-lig_schedule_excluding_count_kernel(SnapView s, Thr thr, const __grid_constant__ FilterTree tree, const int4* reqs,
-                                    const int16_t* excluded, int n_excluded, int2* out, int R, uint64_t seed,
-                                    int* __restrict__ hist, const uint32_t* __restrict__ pool = nullptr) {
-  extern __shared__ __align__(16) unsigned char smem[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint32_t* X = reinterpret_cast<uint32_t*>(smem) + (size_t)warp * 3 * s.W;
-  uint32_t* T = X + s.W;
-  uint32_t* H = T + s.W;
-  Fields f{s.kv, s.q, s.n_active, s.max_active};
-  if constexpr (kStaged) {
-    f = stage_fields(s, smem + scratch_bytes(s.W));
-    __syncthreads();
-  }
-  for (int i = blockIdx.x * kWarpsPerCta + warp; i < R; i += gridDim.x * kWarpsPerCta) {
-    const int4 r = reqs[i];
-    const int ex = lane < n_excluded ? excluded[(size_t)i * n_excluded + lane] : -1;
-    const bool critical = ((uint32_t)r.y & LIG_REQ_CRITICAL) != 0;
-    const uint64_t key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
-    const uint32_t* Hrow = stage_adapter_row(s, r.x, H, lane);
-    for (int w = lane; w < s.W; w += 32) {
-      if constexpr (kPool) {
-        T[w] = pool[w];
-      } else {
-        const int rem = s.P - w * 32;
-        T[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
-      }
-    }
-    __syncwarp();
-    if (ex >= 0 && ex < s.P) atomicAnd(T + (ex >> 5), ~(1u << (ex & 31)));
-    __syncwarp();
-    uint32_t n = 0;
-    for (int w = lane; w < s.W; w += 32) n += __popc(T[w]);
-    n = __reduce_add_sync(kFull, n);
-    EvalResult e;
-    if constexpr (kTree)
-      e = tree_walk_warp<kStaged, true>(f, tree.nodes, Hrow, critical, s.P, s.W, T, X, lane, n);
-    else
-      e = tree_eval_warp<kStaged, true>(f, Hrow, critical, thr, s.P, s.W, X, T, lane, n);
-    int pod = -1;
-    if (e.n > 0) {
-      uint32_t k = int31n(seed ^ key, e.n, max_accept_for(e.n));
-      for (int w = 0; w < s.W; ++w) {
-        uint32_t word = e.mask[w];
-        uint32_t c = __popc(word);
-        if (k < c) { pod = w * 32 + (int)__fns(word, 0, (int)k + 1); break; }
-        k -= c;
-      }
-    }
-    if (lane == 0) {
-      out[i] = make_int2(pod, (int)(e.status | (e.n << 16)));
-      if (pod >= 0) atomicAdd(hist + pod, 1);   // pod >= 0 only for LIG_OK
-    }
-    __syncwarp();
-  }
-}
-
-// ---- retry scheduling with fallback rows (lig_schedule_batch_excluding_fallbacks) ----------------------
 // The p-th set bit of the W-word survivor mask M (p < the mask's popcount), warp-cooperatively.
 // Survivors are counted per group of 32 words: lane g holds the inclusive prefix `incl` of the
 // groups' counts (zero past the last group).  A ballot finds the group that holds position p, lane t
@@ -3024,217 +2865,44 @@ __device__ __forceinline__ int warp_select_survivor(const uint32_t* M, int W, ui
   return __shfl_sync(kFull, pod, t);
 }
 
-// lig_schedule_excluding_kernel's walk, step for step, then the pick and the fallback row of the
-// reduced survivor set: the pick is the resident retry's (the same Int31n(n') draws on seed ^
-// rand_key, continued here rather than on a copy), and entries 1 .. m-1 rank that set as
-// write_fallback_row ranks a class's list, with the same (position, value) record of the partial
-// Fisher-Yates shuffle.  Entry j is the perm[j]-th set bit of the survivor mask, selected by the
-// whole warp (warp_select_survivor) rather than by the retry's serial W-word loop.  Lane j-1 keeps
-// entry j and the row is stored by lanes 0 .. n_fallbacks-1.  A separate body, for the reason given
-// at lig_schedule_excluding_count_kernel.
-template <bool kStaged, bool kTree, bool kPool = false>
+// Every retry call (lig_schedule_[models_]batch[_feedback_chain]_excluding[_fallbacks]), with the
+// scan's launch shape: one warp per request, columns staged when they fit (kStaged).
+//
+// Request i is a lig_req descriptor, or (kModels) model ids[i] at the fixed target targets[i] (the
+// target_idx an earlier model call returned) with rand_key = first_index + i.  The warp resolves a
+// model id without a draw: one broadcast 16-byte gather of the model entry, plus one target record
+// when the model has >= 2 targets.  The request is LIG_NO_MODEL for an id past the table, an absent
+// model, a model without TargetModels and t != 255, or a model with TargetModels and t >= their
+// count; it writes that result (and a row of -1) and adds no load.  The model table is read through
+// the read-only path: every launch is ordered behind the table's upload.
+//
+// The walk: lanes 0 .. n_excluded-1 each take one entry of the request's row and clear that pod's bit
+// in the warp's root mask, which starts from every pod (kPool: the pool words of an epoch derived by
+// lig_eject_pods).  A shared-memory atomicAnd, so a duplicate clears nothing twice, and entries
+// outside [0, P) clear nothing.  The walk starts from that mask: the built-in tree, or (kTree) the
+// caller tree that built the epoch (under the chain, the tree and thresholds the chain started with,
+// on its private copy).  Requests and rows are read with plain loads: they may be page-locked host
+// memory.
+//
+// The pick is the k-th survivor in pod order.  kRows adds the fallback row of the reduced survivor
+// set: the pick is the same (the same Int31n(n') draws on seed ^ rand_key, continued here rather than
+// on a copy), and entries 1 .. m-1 rank that set as write_fallback_row ranks a class's list, with the
+// same (position, value) record of the partial Fisher-Yates shuffle.  Entry j is the perm[j]-th set
+// bit of the survivor mask, selected by the whole warp (warp_select_survivor).  Lane j-1 keeps entry j
+// and the row is stored by lanes 0 .. n_fallbacks-1.  kCount (the chain's segment): lane 0 adds each
+// LIG_OK pick to the open window's histogram, one atomic per request (one warp per request: no
+// cross-lane match as in count_window_picks); row entries add no load.
+template <bool kModels, bool kStaged, bool kTree, bool kPool, bool kRows, bool kCount>
 __global__ void __launch_bounds__(kCtaThreads)
-lig_schedule_excluding_fallback_kernel(SnapView s, Thr thr, const __grid_constant__ FilterTree tree, const int4* reqs,
-                                       const int16_t* excluded, int n_excluded, int2* out, int R, uint64_t seed,
-                                       int n_fallbacks, int16_t* fallbacks, const uint32_t* pool = nullptr) {
+lig_schedule_excluding_kernel(SnapView s, Thr thr, const __grid_constant__ FilterTree tree, const void* in,
+                              const uint8_t* targets, const int16_t* excluded, int n_excluded, void* out, int R,
+                              uint64_t seed, uint64_t first_index, const unsigned char* __restrict__ mtab,
+                              uint32_t n_models, int n_fallbacks, int16_t* fallbacks, int* __restrict__ hist,
+                              const uint32_t* __restrict__ pool) {
   extern __shared__ __align__(16) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint32_t* X = reinterpret_cast<uint32_t*>(smem) + (size_t)warp * 3 * s.W;
-  uint32_t* T = X + s.W;
-  uint32_t* H = T + s.W;
-  Fields f{s.kv, s.q, s.n_active, s.max_active};
-  if constexpr (kStaged) {
-    f = stage_fields(s, smem + scratch_bytes(s.W));
-    __syncthreads();
-  }
-  for (int i = blockIdx.x * kWarpsPerCta + warp; i < R; i += gridDim.x * kWarpsPerCta) {
-    const int4 r = reqs[i];
-    const int ex = lane < n_excluded ? excluded[(size_t)i * n_excluded + lane] : -1;
-    const bool critical = ((uint32_t)r.y & LIG_REQ_CRITICAL) != 0;
-    const uint64_t key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
-    const uint32_t* Hrow = stage_adapter_row(s, r.x, H, lane);
-    for (int w = lane; w < s.W; w += 32) {
-      if constexpr (kPool) {
-        T[w] = pool[w];
-      } else {
-        const int rem = s.P - w * 32;
-        T[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
-      }
-    }
-    __syncwarp();
-    if (ex >= 0 && ex < s.P) atomicAnd(T + (ex >> 5), ~(1u << (ex & 31)));
-    __syncwarp();
-    uint32_t n = 0;
-    for (int w = lane; w < s.W; w += 32) n += __popc(T[w]);
-    n = __reduce_add_sync(kFull, n);
-    EvalResult e;
-    if constexpr (kTree)
-      e = tree_walk_warp<kStaged, true>(f, tree.nodes, Hrow, critical, s.P, s.W, T, X, lane, n);
-    else
-      e = tree_eval_warp<kStaged, true>(f, Hrow, critical, thr, s.P, s.W, X, T, lane, n);
-    int pod = -1;
-    int16_t mine = -1;                 // row entry lane + 1
-    if (e.n > 0) {
-      // survivors per group of 32 words: group g's count on lane g, then the inclusive prefix
-      uint32_t incl = 0;
-      const int groups = (s.W + 31) >> 5;
-      for (int g = 0; g < groups; ++g) {
-        const int w = g * 32 + lane;
-        const uint32_t cg = __reduce_add_sync(kFull, w < s.W ? __popc(e.mask[w]) : 0u);
-        if (lane == g) incl = cg;
-      }
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) {
-        const uint32_t t = __shfl_up_sync(kFull, incl, d);
-        if (lane >= d) incl += t;
-      }
-      uint64_t state = seed ^ key;
-      uint32_t pos[LIG_MAX_FALLBACKS], val[LIG_MAX_FALLBACKS];
-      pos[0] = int31n_next(state, e.n);   // step 0: the pick's own draws, perm[r0] = 0
-      val[0] = 0u;
-      pod = warp_select_survivor(e.mask, s.W, incl, pos[0], lane);
-      const uint32_t m = e.status == (uint32_t)LIG_OK ? min(e.n, (uint32_t)n_fallbacks + 1u) : 0u;
-#pragma unroll
-      for (int j = 1; j <= LIG_MAX_FALLBACKS; ++j) {
-        if ((uint32_t)j >= m) break;
-        const uint32_t rj = (uint32_t)j + int31n_next(state, e.n - (uint32_t)j);
-        uint32_t a = (uint32_t)j, b = rj;   // perm[j], perm[r_j]: the latest record wins
-#pragma unroll
-        for (int k = 0; k < j; ++k) {
-          if (pos[k] == (uint32_t)j) a = val[k];
-          if (pos[k] == rj) b = val[k];
-        }
-        const int p = warp_select_survivor(e.mask, s.W, incl, b, lane);
-        if (lane == j - 1) mine = (int16_t)p;
-        if (j < LIG_MAX_FALLBACKS) {
-          pos[j] = rj;
-          val[j] = a;
-        }
-      }
-    }
-    if (lane == 0) out[i] = make_int2(pod, (int)(e.status | (e.n << 16)));
-    if (lane < n_fallbacks) fallbacks[(size_t)i * (size_t)n_fallbacks + lane] = mine;
-    __syncwarp();
-  }
-}
-
-// The chain segment of lig_schedule_batch_feedback_chain_excluding_fallbacks:
-// lig_schedule_excluding_fallback_kernel's walk, pick and row, step for step, on the chain's private
-// copy with the tree and thresholds the chain started with, plus lig_schedule_excluding_count_kernel's
-// count: lane 0 adds each LIG_OK pick to the open window's histogram (row entries add no load).  A
-// separate body, for the reason given at lig_schedule_excluding_count_kernel.
-template <bool kStaged, bool kTree, bool kPool = false>
-__global__ void __launch_bounds__(kCtaThreads)
-lig_schedule_excluding_fallback_count_kernel(SnapView s, Thr thr, const __grid_constant__ FilterTree tree,
-                                             const int4* reqs, const int16_t* excluded, int n_excluded, int2* out,
-                                             int R, uint64_t seed, int n_fallbacks, int16_t* fallbacks,
-                                             int* __restrict__ hist, const uint32_t* __restrict__ pool = nullptr) {
-  extern __shared__ __align__(16) unsigned char smem[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint32_t* X = reinterpret_cast<uint32_t*>(smem) + (size_t)warp * 3 * s.W;
-  uint32_t* T = X + s.W;
-  uint32_t* H = T + s.W;
-  Fields f{s.kv, s.q, s.n_active, s.max_active};
-  if constexpr (kStaged) {
-    f = stage_fields(s, smem + scratch_bytes(s.W));
-    __syncthreads();
-  }
-  for (int i = blockIdx.x * kWarpsPerCta + warp; i < R; i += gridDim.x * kWarpsPerCta) {
-    const int4 r = reqs[i];
-    const int ex = lane < n_excluded ? excluded[(size_t)i * n_excluded + lane] : -1;
-    const bool critical = ((uint32_t)r.y & LIG_REQ_CRITICAL) != 0;
-    const uint64_t key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
-    const uint32_t* Hrow = stage_adapter_row(s, r.x, H, lane);
-    for (int w = lane; w < s.W; w += 32) {
-      if constexpr (kPool) {
-        T[w] = pool[w];
-      } else {
-        const int rem = s.P - w * 32;
-        T[w] = rem >= 32 ? kFull : ((1u << rem) - 1u);
-      }
-    }
-    __syncwarp();
-    if (ex >= 0 && ex < s.P) atomicAnd(T + (ex >> 5), ~(1u << (ex & 31)));
-    __syncwarp();
-    uint32_t n = 0;
-    for (int w = lane; w < s.W; w += 32) n += __popc(T[w]);
-    n = __reduce_add_sync(kFull, n);
-    EvalResult e;
-    if constexpr (kTree)
-      e = tree_walk_warp<kStaged, true>(f, tree.nodes, Hrow, critical, s.P, s.W, T, X, lane, n);
-    else
-      e = tree_eval_warp<kStaged, true>(f, Hrow, critical, thr, s.P, s.W, X, T, lane, n);
-    int pod = -1;
-    int16_t mine = -1;                 // row entry lane + 1
-    if (e.n > 0) {
-      uint32_t incl = 0;
-      const int groups = (s.W + 31) >> 5;
-      for (int g = 0; g < groups; ++g) {
-        const int w = g * 32 + lane;
-        const uint32_t cg = __reduce_add_sync(kFull, w < s.W ? __popc(e.mask[w]) : 0u);
-        if (lane == g) incl = cg;
-      }
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) {
-        const uint32_t t = __shfl_up_sync(kFull, incl, d);
-        if (lane >= d) incl += t;
-      }
-      uint64_t state = seed ^ key;
-      uint32_t pos[LIG_MAX_FALLBACKS], val[LIG_MAX_FALLBACKS];
-      pos[0] = int31n_next(state, e.n);
-      val[0] = 0u;
-      pod = warp_select_survivor(e.mask, s.W, incl, pos[0], lane);
-      const uint32_t m = e.status == (uint32_t)LIG_OK ? min(e.n, (uint32_t)n_fallbacks + 1u) : 0u;
-#pragma unroll
-      for (int j = 1; j <= LIG_MAX_FALLBACKS; ++j) {
-        if ((uint32_t)j >= m) break;
-        const uint32_t rj = (uint32_t)j + int31n_next(state, e.n - (uint32_t)j);
-        uint32_t a = (uint32_t)j, b = rj;
-#pragma unroll
-        for (int k = 0; k < j; ++k) {
-          if (pos[k] == (uint32_t)j) a = val[k];
-          if (pos[k] == rj) b = val[k];
-        }
-        const int p = warp_select_survivor(e.mask, s.W, incl, b, lane);
-        if (lane == j - 1) mine = (int16_t)p;
-        if (j < LIG_MAX_FALLBACKS) {
-          pos[j] = rj;
-          val[j] = a;
-        }
-      }
-    }
-    if (lane == 0) {
-      out[i] = make_int2(pod, (int)(e.status | (e.n << 16)));
-      if (pod >= 0) atomicAdd(hist + pod, 1);   // pod >= 0 only for LIG_OK
-    }
-    if (lane < n_fallbacks) fallbacks[(size_t)i * (size_t)n_fallbacks + lane] = mine;
-    __syncwarp();
-  }
-}
-
-// ---- model-id retries (lig_schedule_models_batch[_feedback_chain]_excluding[_fallbacks]) ------------
-// Request i is model ids[i] at the fixed target targets[i] (the target_idx an earlier model call
-// returned), with rand_key = first_index + i.  The warp resolves it without a draw: one broadcast
-// 16-byte gather of the model entry, plus one target record when the model has >= 2 targets.  The
-// request is LIG_NO_MODEL for an id past the table, an absent model, a model without TargetModels
-// and t != 255, or a model with TargetModels and t >= their count.  Otherwise the descriptor
-// {adapter, Critical, rand_key} goes through the walk of lig_schedule_excluding_kernel, step for
-// step; kRows adds the row of lig_schedule_excluding_fallback_kernel, kCount the chain count of
-// lig_schedule_excluding_count_kernel (a LIG_NO_MODEL request writes its result and adds no load).
-// The pick is packed as a lig_mpick with target_idx = t.  The model table is read through the
-// read-only path: every launch is ordered behind the table's upload.  A body of its own, for the
-// reason given at lig_schedule_excluding_count_kernel.
-template <bool kStaged, bool kTree, bool kPool, bool kRows, bool kCount>
-__global__ void __launch_bounds__(kCtaThreads)
-lig_schedule_models_excluding_kernel(SnapView s, Thr thr, const __grid_constant__ FilterTree tree,
-                                     const uint32_t* ids, const uint8_t* targets, const int16_t* excluded,
-                                     int n_excluded, uint32_t* out, int R, uint64_t seed, uint64_t first_index,
-                                     const unsigned char* __restrict__ mtab, uint32_t n_models, int n_fallbacks,
-                                     int16_t* fallbacks, int* __restrict__ hist, const uint32_t* __restrict__ pool) {
-  extern __shared__ __align__(16) unsigned char smem[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint32_t* X = reinterpret_cast<uint32_t*>(smem) + (size_t)warp * 3 * s.W;
-  uint32_t* T = X + s.W;
+  uint32_t* T = X + s.W;       // the root mask: the built-in walk's second scratch mask, a tree walk's `in`
   uint32_t* H = T + s.W;
   const uint4* entries = reinterpret_cast<const uint4*>(mtab + sizeof(ModelHeader));
   const uint2* records = reinterpret_cast<const uint2*>(entries + n_models);
@@ -3244,28 +2912,43 @@ lig_schedule_models_excluding_kernel(SnapView s, Thr thr, const __grid_constant_
     __syncthreads();
   }
   for (int i = blockIdx.x * kWarpsPerCta + warp; i < R; i += gridDim.x * kWarpsPerCta) {
-    const uint32_t m = ids[i];                 // whole warp reads the same id and target (broadcast)
-    const uint32_t t = targets[i];
+    // ptxas's register allocation depends on the order of the statements below; this one gives the
+    // figures of DESIGN §3.
+    int4 r;                                    // whole warp reads the same request (broadcast)
+    uint32_t m = 0, t = 0;
+    if constexpr (kModels) {
+      m = static_cast<const uint32_t*>(in)[i];
+      t = targets[i];
+    } else {
+      r = static_cast<const int4*>(in)[i];
+    }
     const int ex = lane < n_excluded ? excluded[(size_t)i * n_excluded + lane] : -1;
-    const uint64_t key = first_index + (uint64_t)i;
+    uint64_t key;
     bool found = false;
     uint32_t adapter = 0, critical = 0;
-    if (m < n_models) {
-      const uint4 e = __ldg(entries + m);
-      const uint32_t nt = e.x & 0xffu;
-      found = (e.x & kModelPresent) && (nt == 0 ? t == 255u : t < nt);
-      critical = (e.x >> 8) & 1u;
-      adapter = e.w;                           // the own id (nt == 0) or the single target (nt == 1)
-      if (found && nt >= 2u) adapter = __ldg(records + e.w + t).x;
-    }
-    if (!found) {
-      if (lane == 0) out[i] = pack_mpick(-1, (uint32_t)LIG_NO_MODEL, 255u);
-      if (kRows && lane < n_fallbacks) fallbacks[(size_t)i * (size_t)n_fallbacks + lane] = -1;
-      __syncwarp();
-      continue;
+    if constexpr (kModels) {
+      key = first_index + (uint64_t)i;
+      if (m < n_models) {
+        const uint4 e = __ldg(entries + m);
+        const uint32_t nt = e.x & 0xffu;
+        found = (e.x & kModelPresent) && (nt == 0 ? t == 255u : t < nt);
+        critical = (e.x >> 8) & 1u;
+        adapter = e.w;                         // the own id (nt == 0) or the single target (nt == 1)
+        if (found && nt >= 2u) adapter = __ldg(records + e.w + t).x;
+      }
+      if (!found) {
+        if (lane == 0) static_cast<uint32_t*>(out)[i] = pack_mpick(-1, (uint32_t)LIG_NO_MODEL, 255u);
+        if (kRows && lane < n_fallbacks) fallbacks[(size_t)i * (size_t)n_fallbacks + lane] = -1;
+        __syncwarp();
+        continue;
+      }
+    } else {
+      critical = ((uint32_t)r.y & LIG_REQ_CRITICAL) != 0;
+      key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
+      adapter = (uint32_t)r.x;
     }
     const uint32_t* Hrow = stage_adapter_row(s, (int)adapter, H, lane);
-    for (int w = lane; w < s.W; w += 32) {
+    for (int w = lane; w < s.W; w += 32) {   // the request's pool: every pod (kPool: of the epoch's pool) ...
       if constexpr (kPool) {
         T[w] = pool[w];
       } else {
@@ -3274,7 +2957,7 @@ lig_schedule_models_excluding_kernel(SnapView s, Thr thr, const __grid_constant_
       }
     }
     __syncwarp();
-    if (ex >= 0 && ex < s.P) atomicAnd(T + (ex >> 5), ~(1u << (ex & 31)));
+    if (ex >= 0 && ex < s.P) atomicAnd(T + (ex >> 5), ~(1u << (ex & 31)));   // ... but the excluded
     __syncwarp();
     uint32_t n = 0;
     for (int w = lane; w < s.W; w += 32) n += __popc(T[w]);
@@ -3288,6 +2971,7 @@ lig_schedule_models_excluding_kernel(SnapView s, Thr thr, const __grid_constant_
     int16_t mine = -1;                         // kRows: row entry lane + 1
     if (e.n > 0) {
       if constexpr (kRows) {
+        // survivors per group of 32 words: group g's count on lane g, then the inclusive prefix
         uint32_t incl = 0;
         const int groups = (s.W + 31) >> 5;
         for (int g = 0; g < groups; ++g) {
@@ -3302,7 +2986,7 @@ lig_schedule_models_excluding_kernel(SnapView s, Thr thr, const __grid_constant_
         }
         uint64_t state = seed ^ key;
         uint32_t pos[LIG_MAX_FALLBACKS], val[LIG_MAX_FALLBACKS];
-        pos[0] = int31n_next(state, e.n);
+        pos[0] = int31n_next(state, e.n);     // step 0: the pick's own draws, perm[r0] = 0
         val[0] = 0u;
         pod = warp_select_survivor(e.mask, s.W, incl, pos[0], lane);
         const uint32_t mm = e.status == (uint32_t)LIG_OK ? min(e.n, (uint32_t)n_fallbacks + 1u) : 0u;
@@ -3310,7 +2994,7 @@ lig_schedule_models_excluding_kernel(SnapView s, Thr thr, const __grid_constant_
         for (int j = 1; j <= LIG_MAX_FALLBACKS; ++j) {
           if ((uint32_t)j >= mm) break;
           const uint32_t rj = (uint32_t)j + int31n_next(state, e.n - (uint32_t)j);
-          uint32_t a = (uint32_t)j, b = rj;
+          uint32_t a = (uint32_t)j, b = rj;   // perm[j], perm[r_j]: the latest record wins
 #pragma unroll
           for (int k = 0; k < j; ++k) {
             if (pos[k] == (uint32_t)j) a = val[k];
@@ -3334,7 +3018,10 @@ lig_schedule_models_excluding_kernel(SnapView s, Thr thr, const __grid_constant_
       }
     }
     if (lane == 0) {
-      out[i] = pack_mpick(pod, e.status, t);
+      if constexpr (kModels)
+        static_cast<uint32_t*>(out)[i] = pack_mpick(pod, e.status, t);
+      else
+        static_cast<int2*>(out)[i] = make_int2(pod, (int)(e.status | (e.n << 16)));
       if (kCount && pod >= 0) atomicAdd(hist + pod, 1);   // pod >= 0 only for LIG_OK
     }
     if (kRows && lane < n_fallbacks) fallbacks[(size_t)i * (size_t)n_fallbacks + lane] = mine;

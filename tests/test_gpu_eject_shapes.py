@@ -1,8 +1,8 @@
 """Ejected epochs (lig_eject_pods) at the shapes where the pool forms of the kernels differ, against the
 definition (eject_ref.py), byte for byte.
 
-* Every pool retry kernel with a non-empty pool: lig_schedule_excluding_kernel, ..._fallback_kernel,
-  ..._count_kernel and ..._fallback_count_kernel, staged (P <= 12224) and unstaged, under the
+* Every descriptor pool form of lig_schedule_excluding_kernel with a non-empty pool: with and without
+  rows, with and without the chain's count, staged (P <= 12224) and unstaged, under the
   built-in tree and caller trees, at P in {33, 4096, 5000, 13000, 32768}.  The ejected sets are hot
   pods, the last pod with pods of the last word, one whole 32-pod word, one whole 1024-pod group in
   the middle (so a warp-cooperative select skips an empty group) and every pod but one.  Rows name
