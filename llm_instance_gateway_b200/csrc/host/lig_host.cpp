@@ -36,6 +36,18 @@ Status PickError(uint16_t status) {
   return Errorf(Unknown, "failed to apply filter, resulted 0 pods, this should never happen: %!w(<nil>)");
 }
 
+// A model request's error for a device pick that is not LIG_OK: Schedule's, prefixed as
+// request.go:73-75 wraps it.
+constexpr const char* kModelPrefix = "failed to find target pod: ";
+Status ModelPickError(uint16_t status, int64_t model_id, const std::string& model) {
+  if (status == LIG_NO_MODEL)   // absent models and targets are answered on the host and never sent
+    return Errorf(Internal, std::string(kModelPrefix) + "rpc error: code = Internal desc = model id " +
+                                std::to_string(model_id) + " (" + model + ") has no model entry on the device");
+  Status st = PickError(status);
+  st.message = kModelPrefix + st.message;
+  return st;
+}
+
 inline uint64_t splitmix_next(uint64_t& s) {
   uint64_t z = (s += 0x9E3779B97F4A7C15ull);
   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
@@ -45,6 +57,12 @@ inline uint64_t splitmix_next(uint64_t& s) {
 
 // A stale epoch is re-resolved and tried again up to this many attempts in all (AwaitPublication).
 constexpr int kStaleAttempts = 4;
+
+double ThreadCpuUs() {
+  timespec ts;
+  clock_gettime(CLOCK_THREAD_CPUTIME_ID, &ts);
+  return (double)ts.tv_sec * 1e6 + (double)ts.tv_nsec * 1e-3;
+}
 
 template <class F>
 struct OnExit {
@@ -467,26 +485,39 @@ Status Scheduler::Schedule(const LLMRequest& req, backend::Pod* targetPod) {
   return w.status;
 }
 
-Status Scheduler::CheckFallbacks(const char* fn, int n) const {
-  if (n < 1 || n > LIG_MAX_FALLBACKS)
-    return Errorf(InvalidArgument, std::string(fn) + ": n=" + std::to_string(n) + " outside [1, " +
+// The refusals of the Schedule* calls that ask for more than Schedule: fallback rows (w.pods), a retry
+// (w.tried) or both, checked in this order before the waiter is queued.
+Status Scheduler::CheckRequest(const char* fn, const Waiter& w) const {
+  const bool rows = w.pods != nullptr, retry = w.tried != nullptr;
+  if (rows && (w.fallbacks < 1 || w.fallbacks > LIG_MAX_FALLBACKS))
+    return Errorf(InvalidArgument, std::string(fn) + ": n=" + std::to_string(w.fallbacks) + " outside [1, " +
                                        std::to_string(LIG_MAX_FALLBACKS) + "]");
-  if (opt_.load_feedback_window > 0 && !opt_.feedback_fallbacks)
-    return Errorf(InvalidArgument, std::string(fn) + ": not defined under load_feedback_window (the picks come "
-                                   "from the feedback chain's copy of the snapshot, the fallbacks would not)");
+  if (retry && w.tried->size() > (size_t)LIG_MAX_EXCLUDED)
+    return Errorf(InvalidArgument, std::string(fn) + ": " + std::to_string(w.tried->size()) + " tried pods (at most " +
+                                       std::to_string(LIG_MAX_EXCLUDED) + ")");
+  if (opt_.load_feedback_window > 0 && ((retry && !opt_.feedback_retries) || (rows && !opt_.feedback_fallbacks))) {
+    const char* needs = retry && rows ? "feedback_retries and feedback_fallbacks"
+                        : retry       ? "feedback_retries"
+                                      : "feedback_fallbacks";
+    const char* these = retry && rows ? "these" : retry ? "a retry" : "the fallbacks";
+    return Errorf(InvalidArgument, std::string(fn) + ": not defined under load_feedback_window without " + needs +
+                                       " (the picks come from the feedback chain's copy of the snapshot, " + these +
+                                       " would not)");
+  }
   if (group_)
-    return Errorf(InvalidArgument, std::string(fn) + ": a scheduler over several devices has no fallback call");
+    return Errorf(InvalidArgument, std::string(fn) + ": a scheduler over several devices has no " +
+                                       (retry ? "retry" : "fallback") + " call");
   return Status{};
 }
 
 Status Scheduler::ScheduleWithFallbacks(const LLMRequest& req, int n, std::vector<backend::Pod>* pods) {
   if (pods) pods->clear();
-  if (Status st = CheckFallbacks("ScheduleWithFallbacks", n); !st.ok()) return st;
   std::vector<backend::Pod> ranked;
   Waiter w;
   w.req = &req;
   w.fallbacks = n;
   w.pods = &ranked;
+  if (Status st = CheckRequest("ScheduleWithFallbacks", w); !st.ok()) return st;
   Submit(w);
   if (w.status.ok() && pods) *pods = std::move(ranked);
   return w.status;
@@ -494,17 +525,10 @@ Status Scheduler::ScheduleWithFallbacks(const LLMRequest& req, int n, std::vecto
 
 Status Scheduler::ScheduleRetry(const LLMRequest& req, const std::vector<backend::Pod>& tried,
                                 backend::Pod* targetPod) {
-  if (tried.size() > (size_t)LIG_MAX_EXCLUDED)
-    return Errorf(InvalidArgument, "ScheduleRetry: " + std::to_string(tried.size()) + " tried pods (at most " +
-                                       std::to_string(LIG_MAX_EXCLUDED) + ")");
-  if (opt_.load_feedback_window > 0 && !opt_.feedback_retries)
-    return Errorf(InvalidArgument, "ScheduleRetry: not defined under load_feedback_window (the picks come from the "
-                                   "feedback chain's copy of the snapshot, a retry would not)");
-  if (group_)
-    return Errorf(InvalidArgument, "ScheduleRetry: a scheduler over several devices has no retry call");
   Waiter w;
   w.req = &req;
   w.tried = &tried;
+  if (Status st = CheckRequest("ScheduleRetry", w); !st.ok()) return st;
   Submit(w);
   if (w.status.ok() && targetPod) *targetPod = std::move(w.pod);
   return w.status;
@@ -513,24 +537,13 @@ Status Scheduler::ScheduleRetry(const LLMRequest& req, const std::vector<backend
 Status Scheduler::ScheduleRetryWithFallbacks(const LLMRequest& req, const std::vector<backend::Pod>& tried, int n,
                                              std::vector<backend::Pod>* pods) {
   if (pods) pods->clear();
-  if (n < 1 || n > LIG_MAX_FALLBACKS)
-    return Errorf(InvalidArgument, "ScheduleRetryWithFallbacks: n=" + std::to_string(n) + " outside [1, " +
-                                       std::to_string(LIG_MAX_FALLBACKS) + "]");
-  if (tried.size() > (size_t)LIG_MAX_EXCLUDED)
-    return Errorf(InvalidArgument, "ScheduleRetryWithFallbacks: " + std::to_string(tried.size()) +
-                                       " tried pods (at most " + std::to_string(LIG_MAX_EXCLUDED) + ")");
-  if (opt_.load_feedback_window > 0 && !(opt_.feedback_retries && opt_.feedback_fallbacks))
-    return Errorf(InvalidArgument, "ScheduleRetryWithFallbacks: not defined under load_feedback_window without "
-                                   "feedback_retries and feedback_fallbacks (the picks come from the feedback "
-                                   "chain's copy of the snapshot, these would not)");
-  if (group_)
-    return Errorf(InvalidArgument, "ScheduleRetryWithFallbacks: a scheduler over several devices has no retry call");
   std::vector<backend::Pod> ranked;
   Waiter w;
   w.req = &req;
   w.tried = &tried;
   w.fallbacks = n;
   w.pods = &ranked;
+  if (Status st = CheckRequest("ScheduleRetryWithFallbacks", w); !st.ok()) return st;
   Submit(w);
   if (w.status.ok() && pods) *pods = std::move(ranked);
   return w.status;
@@ -548,12 +561,12 @@ Status Scheduler::ScheduleModel(const std::string& model, std::string* resolvedT
 Status Scheduler::ScheduleModelWithFallbacks(const std::string& model, int n, std::string* resolvedTargetModel,
                                              std::vector<backend::Pod>* pods) {
   if (pods) pods->clear();
-  if (Status st = CheckFallbacks("ScheduleModelWithFallbacks", n); !st.ok()) return st;
   std::vector<backend::Pod> ranked;
   Waiter w;
   w.model = &model;
   w.fallbacks = n;
   w.pods = &ranked;
+  if (Status st = CheckRequest("ScheduleModelWithFallbacks", w); !st.ok()) return st;
   Submit(w);
   if (w.status.ok() && pods) *pods = std::move(ranked);
   if (resolvedTargetModel) *resolvedTargetModel = std::move(w.resolved);
@@ -562,19 +575,11 @@ Status Scheduler::ScheduleModelWithFallbacks(const std::string& model, int n, st
 
 Status Scheduler::ScheduleModelRetry(const std::string& model, const std::string& resolvedTargetModel,
                                      const std::vector<backend::Pod>& tried, backend::Pod* targetPod) {
-  if (tried.size() > (size_t)LIG_MAX_EXCLUDED)
-    return Errorf(InvalidArgument, "ScheduleModelRetry: " + std::to_string(tried.size()) + " tried pods (at most " +
-                                       std::to_string(LIG_MAX_EXCLUDED) + ")");
-  if (opt_.load_feedback_window > 0 && !opt_.feedback_retries)
-    return Errorf(InvalidArgument, "ScheduleModelRetry: not defined under load_feedback_window without "
-                                   "feedback_retries (the picks come from the feedback chain's copy of the "
-                                   "snapshot, a retry would not)");
-  if (group_)
-    return Errorf(InvalidArgument, "ScheduleModelRetry: a scheduler over several devices has no retry call");
   Waiter w;
   w.model = &model;
   w.target = &resolvedTargetModel;
   w.tried = &tried;
+  if (Status st = CheckRequest("ScheduleModelRetry", w); !st.ok()) return st;
   Submit(w);
   if (w.status.ok() && targetPod) *targetPod = std::move(w.pod);
   return w.status;
@@ -584,19 +589,6 @@ Status Scheduler::ScheduleModelRetryWithFallbacks(const std::string& model, cons
                                                   const std::vector<backend::Pod>& tried, int n,
                                                   std::vector<backend::Pod>* pods) {
   if (pods) pods->clear();
-  if (n < 1 || n > LIG_MAX_FALLBACKS)
-    return Errorf(InvalidArgument, "ScheduleModelRetryWithFallbacks: n=" + std::to_string(n) + " outside [1, " +
-                                       std::to_string(LIG_MAX_FALLBACKS) + "]");
-  if (tried.size() > (size_t)LIG_MAX_EXCLUDED)
-    return Errorf(InvalidArgument, "ScheduleModelRetryWithFallbacks: " + std::to_string(tried.size()) +
-                                       " tried pods (at most " + std::to_string(LIG_MAX_EXCLUDED) + ")");
-  if (opt_.load_feedback_window > 0 && !(opt_.feedback_retries && opt_.feedback_fallbacks))
-    return Errorf(InvalidArgument, "ScheduleModelRetryWithFallbacks: not defined under load_feedback_window without "
-                                   "feedback_retries and feedback_fallbacks (the picks come from the feedback "
-                                   "chain's copy of the snapshot, these would not)");
-  if (group_)
-    return Errorf(InvalidArgument,
-                  "ScheduleModelRetryWithFallbacks: a scheduler over several devices has no retry call");
   std::vector<backend::Pod> ranked;
   Waiter w;
   w.model = &model;
@@ -604,6 +596,7 @@ Status Scheduler::ScheduleModelRetryWithFallbacks(const std::string& model, cons
   w.tried = &tried;
   w.fallbacks = n;
   w.pods = &ranked;
+  if (Status st = CheckRequest("ScheduleModelRetryWithFallbacks", w); !st.ok()) return st;
   Submit(w);
   if (w.status.ok() && pods) *pods = std::move(ranked);
   return w.status;
@@ -757,110 +750,18 @@ void Scheduler::CountFeedback(uint64_t epoch, int n) {
   fb_filled_ = (int)((fb_filled_ + (int64_t)n) % W);
 }
 
-// A flush that holds both kinds makes the descriptor calls first, then the model-id calls.
+// A flush makes its calls lane by lane: descriptors, retries, model ids, model-id retries.
 void Scheduler::Flush(std::vector<Waiter*>& all) {
-  desc_lane_.clear();
-  model_lane_.clear();
-  retry_lane_.clear();
-  model_retry_lane_.clear();
-  for (Waiter* w : all)
-    (w->model ? (w->tried ? model_retry_lane_ : model_lane_) : w->tried ? retry_lane_ : desc_lane_).push_back(w);
-  std::vector<Waiter*>& batch = desc_lane_;
-  size_t done = 0;
+  for (std::vector<Waiter*>& lane : lanes_) lane.clear();
+  for (Waiter* w : all) lanes_[(w->model ? 2 : 0) + (w->tried ? 1 : 0)].push_back(w);
   const auto flush_t0 = std::chrono::steady_clock::now();
-  double device_us = 0, device_cpu_us = 0;
-  auto thread_cpu_us = [] {
-    timespec ts;
-    clock_gettime(CLOCK_THREAD_CPUTIME_ID, &ts);
-    return (double)ts.tv_sec * 1e6 + (double)ts.tv_nsec * 1e-3;
-  };
-  while (done < batch.size()) {
-    const int n = (int)std::min(batch.size() - done, (size_t)opt_.max_batch);
-    // any ScheduleWithFallbacks caller in this call: one lig_schedule_batch_fallbacks call with the
-    // largest n asked (rows are prefixes of longer rows, picks are lig_schedule_batch's)
-    int nf = 0;
-    for (int i = 0; i < n; ++i) nf = std::max(nf, batch[done + i]->fallbacks);
-    std::shared_ptr<const Snapshot> snap;
-    Status failure;
-    int rc = 0;
-    uint64_t writes_seen = 0;
-  for (int attempt = 0; attempt < kStaleAttempts; ++attempt) {
-      {
-        std::lock_guard<std::mutex> lk(snap_mu_);
-        snap = snap_;
-        writes_seen = writes_done_;
-      }
-      for (int i = 0; i < n; ++i) {
-        const LLMRequest& r = *batch[done + i]->req;
-        auto it = snap->adapter_ids->find(r.ResolvedTargetModel);
-        // a model in no pod's ActiveModels: id A matches no pod, like a Go map miss (filter.go:170).
-        // An id interned after this snapshot was packed (>= A) is equally "in no pod" for it.
-        h_reqs_[i].adapter_id = (it == snap->adapter_ids->end() || it->second >= snap->A) ? snap->A : it->second;
-        h_reqs_[i].flags = r.Critical ? LIG_REQ_CRITICAL : 0u;
-        h_reqs_[i].rand_key = splitmix_next(rng_state_);
-      }
-      const auto call_t0 = std::chrono::steady_clock::now();
-      const double cpu_t0 = thread_cpu_us();
-      const int W = opt_.load_feedback_window;
-      rc = nf > 0 && W > 0
-               ? lig_schedule_batch_feedback_chain_fallbacks(ctx_, snap->epoch, seed_, h_reqs_, n, h_picks_, nf,
-                                                             h_fallbacks_, W, nullptr)
-           : nf > 0 ? lig_schedule_batch_fallbacks(ctx_, snap->epoch, seed_, h_reqs_, n, h_picks_, nf, h_fallbacks_)
-           : group_ ? lig_group_schedule_batch(group_, snap->epoch, seed_, h_reqs_, n, h_picks_)
-           : W > 0 ? lig_schedule_batch_feedback_chain(ctx_, snap->epoch, seed_, h_reqs_, n, h_picks_, W, nullptr)
-           : (opt_.use_doorbell && n <= lig_stream_capacity())
-               ? lig_stream_submit(ctx_, snap->epoch, seed_, h_reqs_, n, h_picks_)
-               : lig_schedule_batch(ctx_, snap->epoch, seed_, h_reqs_, n, h_picks_);
-      if (rc == 0 && W > 0) CountFeedback(snap->epoch, n);
-      const double call_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - call_t0).count();
-      if (call_us > device_us) {
-        device_us = call_us;
-        device_cpu_us = thread_cpu_us() - cpu_t0;
-      }
-      if (!AwaitPublication(rc, writes_seen, attempt)) break;
-    }
-    if (rc != 0)
-      failure = LigFailure(nf > 0 && opt_.load_feedback_window > 0 ? "lig_schedule_batch_feedback_chain_fallbacks"
-                           : nf > 0                         ? "lig_schedule_batch_fallbacks"
-                           : opt_.load_feedback_window > 0 ? "lig_schedule_batch_feedback_chain" : "lig_schedule_batch");
-    for (int i = 0; i < n; ++i) {
-      Waiter* w = batch[done + i];
-      if (rc != 0) {
-        w->status = failure;
-      } else if (h_picks_[i].status == LIG_OK) {
-        w->pod = snap->pods[(size_t)h_picks_[i].pod_idx];          // pods[i].Pod  scheduler.go:121
-        if (w->fallbacks > 0) {
-          w->pods->push_back(w->pod);
-          const int16_t* row = h_fallbacks_ + (size_t)i * (size_t)nf;
-          for (int j = 0; j < w->fallbacks && row[j] >= 0; ++j) w->pods->push_back(snap->pods[(size_t)row[j]]);
-        }
-      } else {
-        w->status = PickError(h_picks_[i].status);
-      }
-    }
-    {
-      std::lock_guard<std::mutex> sk(stats_mu_);
-      stats_.scheduled += (uint64_t)n;
-      for (int i = 0; i < n; ++i) stats_.fallback_scheduled += batch[done + i]->fallbacks > 0 ? 1 : 0;
-      stats_.batches++;
-      stats_.max_batch = std::max<uint64_t>(stats_.max_batch, (uint64_t)n);
-    }
-    for (int i = 0; i < n; ++i) {
-      Waiter* w = batch[done + i];
-      w->done.store(1, std::memory_order_release);
-      w->done.notify_one();
-      w->done.store(2, std::memory_order_release);   // last access: the caller may now destroy *w
-    }
-    done += (size_t)n;
-  }
-  FlushRetries(retry_lane_);
-  FlushModels(model_lane_);
-  FlushModelRetries(model_retry_lane_);
+  CallTime slowest;   // the descriptor lane's slowest device call
+  for (int l = 0; l < 4; ++l) FlushLane(lanes_[l], l == 0 ? &slowest : nullptr);
   const double flush_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - flush_t0).count();
   std::lock_guard<std::mutex> sk(stats_mu_);
-  if (device_us > stats_.max_device_call_us) {
-    stats_.max_device_call_us = device_us;
-    stats_.slowest_call_cpu_us = device_cpu_us;
+  if (slowest.us > stats_.max_device_call_us) {
+    stats_.max_device_call_us = slowest.us;
+    stats_.slowest_call_cpu_us = slowest.cpu_us;
     stats_.slowest_call_batch = stats_.batches ? stats_.batches - 1 : 0;
   }
   stats_.max_flush_us = std::max(stats_.max_flush_us, flush_us);
@@ -883,357 +784,224 @@ void Scheduler::TriedRows(const Snapshot& snap, Waiter* const* batch, int n, std
   }
 }
 
-// The retry lane: one lig_schedule_batch_excluding call per max_batch waiters (under
-// load_feedback_window, lig_schedule_batch_feedback_chain_excluding; with a ScheduleRetryWithFallbacks
-// caller among them, lig_schedule_batch_[feedback_chain_]excluding_fallbacks at the largest n asked,
-// whose picks, and under the chain whose windows, are the same).  Each waiter's tried pods are
-// matched by value against the captured snapshot; its row holds their indices, -1 padded to the
-// widest row of the call.  Every waiter takes a rand_key; under the chain a waiter refused on the
-// host is left out of the call, since its pick would load a pod and shift every later window.
-void Scheduler::FlushRetries(std::vector<Waiter*>& batch) {
-  if (batch.empty()) return;
-  Status failure;
-  if (!h_excluded_) {
+// A model waiter's id in the captured epoch's list and, for a retry, the index of its resolved target
+// among the model's TargetModels (the first of that name; 255 for a model without TargetModels whose
+// own name it is).  A waiter the list alone answers gets the error it is answered with.
+Status Scheduler::MapModel(const Snapshot& snap, Waiter* w, int* target) {
+  w->model_id = -1;
+  const ModelList* list = snap.models.get();
+  auto it = list ? list->ids.find(*w->model) : decltype(list->ids)::const_iterator{};
+  if (!list || it == list->ids.end())                                                   // request.go:42-45
+    return Errorf(Unknown, "error finding a model object in InferenceModel for input " + *w->model);
+  const backend::InferenceModel& im = *list->models[it->second];
+  if (!list->present[it->second])                                                       // request.go:48-51
+    return Errorf(Unknown, "error getting target model name for model " + im.ModelName);
+  if (w->target) {
+    *target = -1;
+    if (im.TargetModels.empty()) {
+      if (*w->target == *w->model) *target = 255;                                       // request.go:47
+    } else {
+      for (size_t j = 0; j < im.TargetModels.size() && *target < 0; ++j)
+        if (im.TargetModels[j].Name == *w->target) *target = (int)j;
+    }
+    if (*target < 0)
+      return Errorf(InvalidArgument, "ScheduleModelRetry: " + *w->target + " is not a target model of " + *w->model);
+  }
+  w->model_id = it->second;
+  return Status{};
+}
+
+// The library call for k mapped requests of one lane.  *call receives the name LigFailure reports: the
+// entry point's own, except that the group and the doorbell report as lig_schedule_batch.
+#define LIG_LANE_CALL(fn, ...) (*call = #fn, fn(__VA_ARGS__))
+int Scheduler::LaneCall(uint64_t epoch, bool models, bool retry, int k, int nf, int width, const char** call) {
+  const int W = opt_.load_feedback_window;
+  const uint64_t first = model_index_;
+  const uint8_t* targets = model_targets_.data();
+  if (models && retry) {
+    if (nf > 0 && W > 0)
+      return LIG_LANE_CALL(lig_schedule_models_batch_feedback_chain_excluding_fallbacks, ctx_, epoch, seed_, first,
+                           h_model_ids_, targets, k, h_excluded_, width, h_mpicks_, nf, h_fallbacks_, W, nullptr);
+    if (nf > 0)
+      return LIG_LANE_CALL(lig_schedule_models_batch_excluding_fallbacks, ctx_, epoch, seed_, first, h_model_ids_,
+                           targets, k, h_excluded_, width, h_mpicks_, nf, h_fallbacks_);
+    if (W > 0)
+      return LIG_LANE_CALL(lig_schedule_models_batch_feedback_chain_excluding, ctx_, epoch, seed_, first, h_model_ids_,
+                           targets, k, h_excluded_, width, h_mpicks_, W, nullptr);
+    return LIG_LANE_CALL(lig_schedule_models_batch_excluding, ctx_, epoch, seed_, first, h_model_ids_, targets, k,
+                         h_excluded_, width, h_mpicks_);
+  }
+  if (models) {
+    if (nf > 0 && W > 0)
+      return LIG_LANE_CALL(lig_schedule_models_batch_feedback_chain_fallbacks, ctx_, epoch, seed_, first, h_model_ids_,
+                           k, h_mpicks_, nf, h_fallbacks_, W, nullptr);
+    if (nf > 0)
+      return LIG_LANE_CALL(lig_schedule_models_batch_fallbacks, ctx_, epoch, seed_, first, h_model_ids_, k, h_mpicks_,
+                           nf, h_fallbacks_);
+    if (W > 0)
+      return LIG_LANE_CALL(lig_schedule_models_batch_feedback_chain, ctx_, epoch, seed_, first, h_model_ids_, k,
+                           h_mpicks_, W, nullptr);
+    if (opt_.use_doorbell && k <= lig_stream_capacity())
+      return LIG_LANE_CALL(lig_stream_submit_models, ctx_, epoch, seed_, first, h_model_ids_, k, h_mpicks_);
+    return LIG_LANE_CALL(lig_schedule_models_batch, ctx_, epoch, seed_, first, h_model_ids_, k, h_mpicks_);
+  }
+  if (retry) {
+    if (nf > 0 && W > 0)
+      return LIG_LANE_CALL(lig_schedule_batch_feedback_chain_excluding_fallbacks, ctx_, epoch, seed_, h_reqs_, k,
+                           h_excluded_, width, h_picks_, nf, h_fallbacks_, W, nullptr);
+    if (nf > 0)
+      return LIG_LANE_CALL(lig_schedule_batch_excluding_fallbacks, ctx_, epoch, seed_, h_reqs_, k, h_excluded_, width,
+                           h_picks_, nf, h_fallbacks_);
+    if (W > 0)
+      return LIG_LANE_CALL(lig_schedule_batch_feedback_chain_excluding, ctx_, epoch, seed_, h_reqs_, k, h_excluded_,
+                           width, h_picks_, W, nullptr);
+    return LIG_LANE_CALL(lig_schedule_batch_excluding, ctx_, epoch, seed_, h_reqs_, k, h_excluded_, width, h_picks_);
+  }
+  if (nf > 0 && W > 0)
+    return LIG_LANE_CALL(lig_schedule_batch_feedback_chain_fallbacks, ctx_, epoch, seed_, h_reqs_, k, h_picks_, nf,
+                         h_fallbacks_, W, nullptr);
+  if (nf > 0)
+    return LIG_LANE_CALL(lig_schedule_batch_fallbacks, ctx_, epoch, seed_, h_reqs_, k, h_picks_, nf, h_fallbacks_);
+  *call = "lig_schedule_batch";
+  if (group_) return lig_group_schedule_batch(group_, epoch, seed_, h_reqs_, k, h_picks_);
+  if (W > 0)
+    return LIG_LANE_CALL(lig_schedule_batch_feedback_chain, ctx_, epoch, seed_, h_reqs_, k, h_picks_, W, nullptr);
+  if (opt_.use_doorbell && k <= lig_stream_capacity()) return lig_stream_submit(ctx_, epoch, seed_, h_reqs_, k, h_picks_);
+  return lig_schedule_batch(ctx_, epoch, seed_, h_reqs_, k, h_picks_);
+}
+#undef LIG_LANE_CALL
+
+// One lane of a flush: its waiters are all of one kind, a descriptor (req) or a model name (model),
+// a first attempt or a retry (tried).  Each chunk of at most max_batch waiters captures the epoch, maps
+// every waiter to a device request or to the answer the host gives it, makes one library call
+// (LaneCall) for the mapped requests, maps again on a stale epoch (AwaitPublication), then answers,
+// counts and wakes its waiters.  A retry's tried pods become a row of their indices, -1 padded to the
+// widest row of the call; one that matches more than LIG_MAX_EXCLUDED pods is answered on the host.
+// Fallback rows are asked at the largest n of the lane's waiters (rows are prefixes of longer rows, the
+// picks are the plain call's).  rand_keys: each descriptor waiter, sent or not, takes the next splitmix
+// key on every attempt; the k model requests sent have rand_key = model_index_ + k on every attempt,
+// and model_index_ moves past them once per chunk.  Host-answered model waiters take no key.
+void Scheduler::FlushLane(std::vector<Waiter*>& lane, CallTime* timing) {
+  if (lane.empty()) return;
+  const bool models = lane[0]->model != nullptr, retry = lane[0]->tried != nullptr;
+  const int W = opt_.load_feedback_window;
+  Status failure;   // a retry lane's failure also answers its later chunks, which make no call
+  if (retry && !h_excluded_) {
     h_excluded_ = static_cast<int16_t*>(lig_host_alloc((size_t)opt_.max_batch * LIG_MAX_EXCLUDED * sizeof(int16_t)));
     if (!h_excluded_) failure = LigFailure("lig_host_alloc");
   }
+  if (models && retry) model_targets_.resize((size_t)opt_.max_batch);
   std::vector<std::vector<int16_t>> rows;
-  std::vector<int> slot;   // waiter i's request in the call, -1 when left out
-  const int W = opt_.load_feedback_window;
-  size_t done = 0;
-  while (done < batch.size()) {
-    const int n = (int)std::min(batch.size() - done, (size_t)opt_.max_batch);
-    int nf = 0;   // ScheduleRetryWithFallbacks callers: the largest n asked
-    for (int i = 0; i < n; ++i) nf = std::max(nf, batch[done + i]->fallbacks);
-    std::shared_ptr<const Snapshot> snap;
-    int rc = 0, width = 1, k = 0;
-    uint64_t writes_seen = 0;
-    for (int attempt = 0; failure.ok() && attempt < kStaleAttempts; ++attempt) {
-      {
-        std::lock_guard<std::mutex> lk(snap_mu_);
-        snap = snap_;
-        writes_seen = writes_done_;
-      }
-      TriedRows(*snap, batch.data() + done, n, &rows, &width);
-      slot.assign((size_t)n, -1);
-      k = 0;
-      for (int i = 0; i < n; ++i) {
-        const LLMRequest& r = *batch[done + i]->req;
-        const uint64_t key = splitmix_next(rng_state_);
-        const std::vector<int16_t>& ex = rows[(size_t)i];
-        if (W > 0 && ex.size() > (size_t)LIG_MAX_EXCLUDED) continue;
-        slot[(size_t)i] = k;
-        auto it = snap->adapter_ids->find(r.ResolvedTargetModel);   // interned as in Flush
-        h_reqs_[k].adapter_id = (it == snap->adapter_ids->end() || it->second >= snap->A) ? snap->A : it->second;
-        h_reqs_[k].flags = r.Critical ? LIG_REQ_CRITICAL : 0u;
-        h_reqs_[k].rand_key = key;
-        int16_t* row = h_excluded_ + (size_t)k * (size_t)width;
-        const int m = (int)ex.size() <= width ? (int)ex.size() : 0;
-        for (int j = 0; j < width; ++j) row[j] = j < m ? ex[(size_t)j] : (int16_t)-1;
-        ++k;
-      }
-      if (W > 0) {
-        rc = k == 0   ? 0
-             : nf > 0 ? lig_schedule_batch_feedback_chain_excluding_fallbacks(ctx_, snap->epoch, seed_, h_reqs_, k,
-                                                                              h_excluded_, width, h_picks_, nf,
-                                                                              h_fallbacks_, W, nullptr)
-                      : lig_schedule_batch_feedback_chain_excluding(ctx_, snap->epoch, seed_, h_reqs_, k, h_excluded_,
-                                                                    width, h_picks_, W, nullptr);
-        if (rc == 0) CountFeedback(snap->epoch, k);
-      } else if (nf > 0) {
-        rc = lig_schedule_batch_excluding_fallbacks(ctx_, snap->epoch, seed_, h_reqs_, n, h_excluded_, width, h_picks_,
-                                                    nf, h_fallbacks_);
-      } else {
-        rc = lig_schedule_batch_excluding(ctx_, snap->epoch, seed_, h_reqs_, n, h_excluded_, width, h_picks_);
-      }
-      if (!AwaitPublication(rc, writes_seen, attempt)) break;
-    }
-    if (failure.ok() && rc != 0)
-      failure = LigFailure(W > 0 && nf > 0 ? "lig_schedule_batch_feedback_chain_excluding_fallbacks"
-                           : W > 0         ? "lig_schedule_batch_feedback_chain_excluding"
-                           : nf > 0        ? "lig_schedule_batch_excluding_fallbacks"
-                                           : "lig_schedule_batch_excluding");
-    for (int i = 0; i < n; ++i) {
-      Waiter* w = batch[done + i];
-      const lig_pick* pk = failure.ok() && slot[(size_t)i] >= 0 ? &h_picks_[slot[(size_t)i]] : nullptr;
-      if (!failure.ok()) w->status = failure;
-      else if (rows[(size_t)i].size() > (size_t)LIG_MAX_EXCLUDED)
-        w->status = Errorf(InvalidArgument, "ScheduleRetry: the tried pods match more than " +
-                                                std::to_string(LIG_MAX_EXCLUDED) + " pods of the snapshot");
-      else if (pk->status == LIG_OK) {
-        w->pod = snap->pods[(size_t)pk->pod_idx];
-        if (w->fallbacks > 0) {
-          w->pods->push_back(w->pod);
-          const int16_t* row = h_fallbacks_ + (size_t)slot[(size_t)i] * (size_t)nf;
-          for (int j = 0; j < w->fallbacks && row[j] >= 0; ++j) w->pods->push_back(snap->pods[(size_t)row[j]]);
-        }
-      } else {
-        w->status = PickError(pk->status);
-      }
-    }
-    {
-      std::lock_guard<std::mutex> sk(stats_mu_);
-      stats_.scheduled += (uint64_t)n;
-      stats_.retry_scheduled += (uint64_t)n;
-      stats_.batches++;
-      stats_.max_batch = std::max<uint64_t>(stats_.max_batch, (uint64_t)n);
-    }
-    for (int i = 0; i < n; ++i) {
-      Waiter* w = batch[done + i];
-      w->done.store(1, std::memory_order_release);
-      w->done.notify_one();
-      w->done.store(2, std::memory_order_release);   // last access: the caller may now destroy *w
-    }
-    done += (size_t)n;
-  }
-}
-
-// A model request's result from its device pick (and row), with ScheduleModel's errors.
-static constexpr const char* kModelPrefix = "failed to find target pod: ";            // request.go:73-75
-
-template <class Snap, class W>
-static void ModelPickResult(const Snap& snap, const backend::InferenceModel& im, const lig_mpick& pk, const int16_t* row,
-                            W* w) {
-  const std::string prefix = kModelPrefix;
-  if (pk.status == LIG_OK) {
-    w->pod = snap.pods[(size_t)pk.pod_idx];
-    if (w->fallbacks > 0) {
-      w->pods->push_back(w->pod);
-      for (int f = 0; f < w->fallbacks && row[f] >= 0; ++f) w->pods->push_back(snap.pods[(size_t)row[f]]);
-    }
-  } else if (pk.status == LIG_DROP) {
-    w->status = Errorf(ResourceExhausted, prefix + "failed to apply filter, resulted 0 pods, this should never "
-                                                   "happen: " + kDropInner);
-  } else if (pk.status == LIG_NO_PODS_LEFT) {
-    w->status = Errorf(Unknown, prefix + "failed to apply filter, resulted 0 pods, this should never happen: "
-                                         "no pods left");
-  } else if (pk.status == LIG_EMPTY) {
-    w->status = Errorf(Unknown, prefix + "failed to apply filter, resulted 0 pods, this should never happen: "
-                                         "%!w(<nil>)");
-  } else {   // LIG_NO_MODEL: absent models and targets are answered on the host and never sent
-    w->status = Errorf(Internal, prefix + "rpc error: code = Internal desc = model id " +
-                                     std::to_string(w->model_id) + " (" + im.ModelName +
-                                     ") has no model entry on the device");
-  }
-}
-
-// The model-id lane: names are mapped to ids against the captured epoch's list; names the host can
-// answer from that list alone never reach the device.  Request k that reaches the device has
-// rand_key = model_index_ + k; a stale-epoch retry maps again and reuses the same first_index.
-void Scheduler::FlushModels(std::vector<Waiter*>& batch) {
-  size_t done = 0;
-  while (done < batch.size()) {
-    const int n = (int)std::min(batch.size() - done, (size_t)opt_.max_batch);
-    std::shared_ptr<const Snapshot> snap;
-    int rc = 0, k = 0, nf = 0;
-    const char* call = "lig_schedule_models_batch";
-    uint64_t writes_seen = 0;
-  for (int attempt = 0; attempt < kStaleAttempts; ++attempt) {
-      {
-        std::lock_guard<std::mutex> lk(snap_mu_);
-        snap = snap_;
-        writes_seen = writes_done_;
-      }
-      const ModelList* list = snap->models.get();
-      k = 0;
-      nf = 0;
-      for (int i = 0; i < n; ++i) {
-        Waiter* w = batch[done + i];
-        auto it = list ? list->ids.find(*w->model) : decltype(list->ids)::const_iterator{};
-        if (!list || it == list->ids.end()) {                                       // request.go:42-45
-          w->model_id = -1;
-          w->status = Errorf(Unknown, "error finding a model object in InferenceModel for input " + *w->model);
-        } else if (!list->present[it->second]) {                                     // request.go:48-51
-          w->model_id = -1;
-          w->status = Errorf(Unknown, "error getting target model name for model " +
-                                          list->models[it->second]->ModelName);
-        } else {
-          w->model_id = it->second;
-          w->status = Status{};   // a retry may map a name the previous epoch answered on the host
-          h_model_ids_[k++] = it->second;
-          nf = std::max(nf, w->fallbacks);   // rows only for the requests the device sees
-        }
-      }
-      if (k == 0) break;
-      const int W = opt_.load_feedback_window;
-      // any ScheduleModelWithFallbacks caller among them: one fallback call at the largest n asked
-      // (rows are prefixes of longer rows, picks are the plain call's); never the doorbell
-      if (nf > 0 && W > 0) {
-        call = "lig_schedule_models_batch_feedback_chain_fallbacks";
-        rc = lig_schedule_models_batch_feedback_chain_fallbacks(ctx_, snap->epoch, seed_, model_index_, h_model_ids_,
-                                                                k, h_mpicks_, nf, h_fallbacks_, W, nullptr);
-      } else if (nf > 0) {
-        call = "lig_schedule_models_batch_fallbacks";
-        rc = lig_schedule_models_batch_fallbacks(ctx_, snap->epoch, seed_, model_index_, h_model_ids_, k, h_mpicks_,
-                                                 nf, h_fallbacks_);
-      } else if (W > 0) {
-        call = "lig_schedule_models_batch_feedback_chain";
-        rc = lig_schedule_models_batch_feedback_chain(ctx_, snap->epoch, seed_, model_index_, h_model_ids_, k,
-                                                      h_mpicks_, W, nullptr);
-      } else if (opt_.use_doorbell && k <= lig_stream_capacity()) {
-        call = "lig_stream_submit_models";
-        rc = lig_stream_submit_models(ctx_, snap->epoch, seed_, model_index_, h_model_ids_, k, h_mpicks_);
-      } else {
-        rc = lig_schedule_models_batch(ctx_, snap->epoch, seed_, model_index_, h_model_ids_, k, h_mpicks_);
-      }
-      if (rc == 0 && W > 0) CountFeedback(snap->epoch, k);
-      if (!AwaitPublication(rc, writes_seen, attempt)) break;
-    }
-    if (k > 0) model_index_ += (uint64_t)k;
-    const Status failure = rc != 0 ? LigFailure(call) : Status{};
-    const std::string prefix = kModelPrefix;
-    for (int i = 0, j = 0; i < n; ++i) {
-      Waiter* w = batch[done + i];
-      if (w->model_id < 0) continue;
-      const int16_t* row = h_fallbacks_ + (size_t)j * (size_t)nf;
-      const lig_mpick& pk = h_mpicks_[j++];
-      if (rc != 0) {
-        w->status = failure;
-        w->status.message = prefix + w->status.message;
-        continue;
-      }
-      const backend::InferenceModel& im = *snap->models->models[(size_t)w->model_id];
-      // 255: TargetModels is empty and the requested name passes through (request.go:47)
-      w->resolved = pk.target_idx == 255 ? *w->model : im.TargetModels[pk.target_idx].Name;
-      ModelPickResult(*snap, im, pk, row, w);
-    }
-    {
-      std::lock_guard<std::mutex> sk(stats_mu_);
-      stats_.model_scheduled += (uint64_t)n;
-      for (int i = 0; i < n; ++i) stats_.fallback_scheduled += batch[done + i]->fallbacks > 0 ? 1 : 0;
-      stats_.model_batches += k > 0 ? 1 : 0;
-    }
-    for (int i = 0; i < n; ++i) {
-      Waiter* w = batch[done + i];
-      w->done.store(1, std::memory_order_release);
-      w->done.notify_one();
-      w->done.store(2, std::memory_order_release);   // last access: the caller may now destroy *w
-    }
-    done += (size_t)n;
-  }
-}
-
-// The model-retry lane: per max_batch waiters, names are mapped against the captured epoch's list (the
-// model to its id, the resolved target to its index, 255 for a model without TargetModels), tried pods
-// to their indices; waiters the host can answer never reach the device and take no rand_key.  Request k
-// that reaches the device has rand_key = model_index_ + k.  One lig_schedule_models_batch_excluding call
-// (with fallback rows at the largest n asked when any caller wants them; under load_feedback_window the
-// chain forms); a stale-epoch retry maps again and reuses the same first_index.
-void Scheduler::FlushModelRetries(std::vector<Waiter*>& batch) {
-  if (batch.empty()) return;
-  Status failure;
-  if (!h_excluded_) {
-    h_excluded_ = static_cast<int16_t*>(lig_host_alloc((size_t)opt_.max_batch * LIG_MAX_EXCLUDED * sizeof(int16_t)));
-    if (!h_excluded_) failure = LigFailure("lig_host_alloc");
-  }
-  model_targets_.resize((size_t)opt_.max_batch);
-  std::vector<std::vector<int16_t>> rows;
-  const int W = opt_.load_feedback_window;
-  size_t done = 0;
-  while (done < batch.size()) {
-    const int n = (int)std::min(batch.size() - done, (size_t)opt_.max_batch);
+  std::vector<int> slot;   // waiter i's request in the call, -1 when answered on the host
+  for (size_t done = 0; done < lane.size();) {
+    Waiter* const* batch = lane.data() + done;
+    const int n = (int)std::min(lane.size() - done, (size_t)opt_.max_batch);
+    if (!retry) failure = Status{};
     std::shared_ptr<const Snapshot> snap;
     int rc = 0, k = 0, nf = 0, width = 1;
-    bool mapped = false;   // the waiters were mapped against a snapshot (host answers are in place)
-    const char* call = "lig_schedule_models_batch_excluding";
+    const char* call = "";
     uint64_t writes_seen = 0;
+    slot.assign((size_t)n, -1);
     for (int attempt = 0; failure.ok() && attempt < kStaleAttempts; ++attempt) {
       {
         std::lock_guard<std::mutex> lk(snap_mu_);
         snap = snap_;
         writes_seen = writes_done_;
       }
-      const ModelList* list = snap->models.get();
-      TriedRows(*snap, batch.data() + done, n, &rows, &width);
-      mapped = true;
+      if (retry) TriedRows(*snap, batch, n, &rows, &width);
       k = 0;
       nf = 0;
       for (int i = 0; i < n; ++i) {
-        Waiter* w = batch[done + i];
-        w->model_id = -1;
-        auto it = list ? list->ids.find(*w->model) : decltype(list->ids)::const_iterator{};
-        if (!list || it == list->ids.end()) {                                       // request.go:42-45
-          w->status = Errorf(Unknown, "error finding a model object in InferenceModel for input " + *w->model);
-          continue;
-        }
-        if (!list->present[it->second]) {                                           // request.go:48-51
-          w->status = Errorf(Unknown, "error getting target model name for model " +
-                                          list->models[it->second]->ModelName);
-          continue;
-        }
-        const backend::InferenceModel& im = *list->models[it->second];
-        int t = -1;
-        if (im.TargetModels.empty()) {
-          if (*w->target == *w->model) t = 255;                                      // request.go:47
+        Waiter* w = batch[i];
+        uint64_t key = 0;
+        int target = 0;
+        if (w->model) {
+          w->status = MapModel(*snap, w, &target);
         } else {
-          for (size_t j = 0; j < im.TargetModels.size() && t < 0; ++j)
-            if (im.TargetModels[j].Name == *w->target) t = (int)j;
+          key = splitmix_next(rng_state_);
+          nf = std::max(nf, w->fallbacks);   // every descriptor waiter's n counts, sent or not
+          w->status = Status{};
         }
-        if (t < 0) {
-          w->status = Errorf(InvalidArgument, "ScheduleModelRetry: " + *w->target + " is not a target model of " +
-                                                  *w->model);
-          continue;
-        }
-        const std::vector<int16_t>& ex = rows[(size_t)i];
-        if (ex.size() > (size_t)LIG_MAX_EXCLUDED) {
-          w->status = Errorf(InvalidArgument, "ScheduleModelRetry: the tried pods match more than " +
+        if (w->status.ok() && retry && rows[(size_t)i].size() > (size_t)LIG_MAX_EXCLUDED)
+          w->status = Errorf(InvalidArgument, std::string(models ? "ScheduleModelRetry" : "ScheduleRetry") +
+                                                  ": the tried pods match more than " +
                                                   std::to_string(LIG_MAX_EXCLUDED) + " pods of the snapshot");
-          continue;
+        slot[(size_t)i] = w->status.ok() ? k : -1;
+        if (!w->status.ok()) continue;
+        if (w->model) {
+          h_model_ids_[k] = (uint32_t)w->model_id;
+          if (retry) model_targets_[(size_t)k] = (uint8_t)target;
+          nf = std::max(nf, w->fallbacks);   // model rows only for the requests the device sees
+        } else {
+          auto it = snap->adapter_ids->find(w->req->ResolvedTargetModel);
+          // a model in no pod's ActiveModels: id A matches no pod, like a Go map miss (filter.go:170).
+          // An id interned after this snapshot was packed (>= A) is equally "in no pod" for it.
+          h_reqs_[k].adapter_id = (it == snap->adapter_ids->end() || it->second >= snap->A) ? snap->A : it->second;
+          h_reqs_[k].flags = w->req->Critical ? LIG_REQ_CRITICAL : 0u;
+          h_reqs_[k].rand_key = key;
         }
-        w->model_id = it->second;
-        w->status = Status{};   // a retry may map a name the previous epoch answered on the host
-        w->resolved = *w->target;
-        h_model_ids_[k] = it->second;
-        model_targets_[(size_t)k] = (uint8_t)t;
-        int16_t* row = h_excluded_ + (size_t)k * (size_t)width;
-        for (int j = 0; j < width; ++j) row[j] = j < (int)ex.size() ? ex[(size_t)j] : (int16_t)-1;
-        nf = std::max(nf, w->fallbacks);   // rows only for the requests the device sees
+        if (retry) {
+          const std::vector<int16_t>& ex = rows[(size_t)i];
+          int16_t* row = h_excluded_ + (size_t)k * (size_t)width;
+          for (int j = 0; j < width; ++j) row[j] = j < (int)ex.size() ? ex[(size_t)j] : (int16_t)-1;
+        }
         ++k;
       }
-      if (k == 0) break;
-      if (nf > 0 && W > 0) {
-        call = "lig_schedule_models_batch_feedback_chain_excluding_fallbacks";
-        rc = lig_schedule_models_batch_feedback_chain_excluding_fallbacks(
-            ctx_, snap->epoch, seed_, model_index_, h_model_ids_, model_targets_.data(), k, h_excluded_, width,
-            h_mpicks_, nf, h_fallbacks_, W, nullptr);
-      } else if (nf > 0) {
-        call = "lig_schedule_models_batch_excluding_fallbacks";
-        rc = lig_schedule_models_batch_excluding_fallbacks(ctx_, snap->epoch, seed_, model_index_, h_model_ids_,
-                                                           model_targets_.data(), k, h_excluded_, width, h_mpicks_, nf,
-                                                           h_fallbacks_);
-      } else if (W > 0) {
-        call = "lig_schedule_models_batch_feedback_chain_excluding";
-        rc = lig_schedule_models_batch_feedback_chain_excluding(ctx_, snap->epoch, seed_, model_index_, h_model_ids_,
-                                                                model_targets_.data(), k, h_excluded_, width,
-                                                                h_mpicks_, W, nullptr);
-      } else {
-        rc = lig_schedule_models_batch_excluding(ctx_, snap->epoch, seed_, model_index_, h_model_ids_,
-                                                 model_targets_.data(), k, h_excluded_, width, h_mpicks_);
+      const auto call_t0 = std::chrono::steady_clock::now();
+      const double cpu_t0 = timing ? ThreadCpuUs() : 0;
+      rc = k > 0 ? LaneCall(snap->epoch, models, retry, k, nf, width, &call) : 0;
+      // a descriptor retry chunk refused on the host as a whole still moves the chain to its epoch
+      if (rc == 0 && W > 0 && (k > 0 || !models)) CountFeedback(snap->epoch, k);
+      if (timing) {
+        const double us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - call_t0).count();
+        if (us > timing->us) *timing = CallTime{us, ThreadCpuUs() - cpu_t0};
       }
-      if (rc == 0 && W > 0) CountFeedback(snap->epoch, k);
       if (!AwaitPublication(rc, writes_seen, attempt)) break;
     }
-    if (k > 0) model_index_ += (uint64_t)k;
+    if (models) model_index_ += (uint64_t)k;
     if (failure.ok() && rc != 0) failure = LigFailure(call);
-    for (int i = 0, j = 0; i < n; ++i) {
-      Waiter* w = batch[done + i];
-      if (mapped && w->model_id < 0) continue;
+    for (int i = 0; i < n; ++i) {
+      Waiter* w = batch[i];
+      const int s = slot[(size_t)i];
       if (!failure.ok()) {
+        if (w->model && !w->status.ok()) continue;   // a model answered on the host keeps that answer
         w->status = failure;
-        if (w->model_id >= 0) w->status.message = kModelPrefix + w->status.message;
+        if (w->model && s >= 0) w->status.message = kModelPrefix + w->status.message;
         continue;
       }
-      const int16_t* row = h_fallbacks_ + (size_t)j * (size_t)nf;
-      const lig_mpick& pk = h_mpicks_[j++];
-      ModelPickResult(*snap, *snap->models->models[(size_t)w->model_id], pk, row, w);
+      if (s < 0) continue;
+      const uint16_t status = models ? h_mpicks_[s].status : h_picks_[s].status;
+      if (models && !retry) {
+        const lig_mpick& pk = h_mpicks_[s];   // 255: TargetModels is empty and the name passes through (request.go:47)
+        w->resolved = pk.target_idx == 255 ? *w->model
+                                           : snap->models->models[(size_t)w->model_id]->TargetModels[pk.target_idx].Name;
+      }
+      if (status != LIG_OK) {
+        w->status = models ? ModelPickError(status, w->model_id, *w->model) : PickError(status);
+        continue;
+      }
+      w->pod = snap->pods[(size_t)(models ? h_mpicks_[s].pod_idx : h_picks_[s].pod_idx)];   // scheduler.go:121
+      if (w->fallbacks > 0) {
+        w->pods->push_back(w->pod);
+        const int16_t* row = h_fallbacks_ + (size_t)s * (size_t)nf;
+        for (int j = 0; j < w->fallbacks && row[j] >= 0; ++j) w->pods->push_back(snap->pods[(size_t)row[j]]);
+      }
     }
     {
       std::lock_guard<std::mutex> sk(stats_mu_);
-      stats_.retry_scheduled += (uint64_t)n;
-      stats_.model_batches += k > 0 ? 1 : 0;
+      if (!models) {
+        stats_.scheduled += (uint64_t)n;
+        stats_.batches++;
+        stats_.max_batch = std::max<uint64_t>(stats_.max_batch, (uint64_t)n);
+      }
+      if (retry) stats_.retry_scheduled += (uint64_t)n;
+      if (models && !retry) stats_.model_scheduled += (uint64_t)n;
+      if (!retry)
+        for (int i = 0; i < n; ++i) stats_.fallback_scheduled += batch[i]->fallbacks > 0 ? 1 : 0;
+      if (models) stats_.model_batches += k > 0 ? 1 : 0;
     }
     for (int i = 0; i < n; ++i) {
-      Waiter* w = batch[done + i];
+      Waiter* w = batch[i];
       w->done.store(1, std::memory_order_release);
       w->done.notify_one();
       w->done.store(2, std::memory_order_release);   // last access: the caller may now destroy *w

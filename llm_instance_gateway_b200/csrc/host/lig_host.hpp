@@ -427,10 +427,14 @@ class Scheduler {
   void BatcherLoop();
   void RefresherLoop();
   void Submit(Waiter& w);
+  struct CallTime {
+    double us = 0, cpu_us = 0;   // wall time of a device call, and the batcher thread's CPU time inside it
+  };
   void Flush(std::vector<Waiter*>& batch);
-  void FlushModels(std::vector<Waiter*>& batch);
-  void FlushRetries(std::vector<Waiter*>& batch);
-  void FlushModelRetries(std::vector<Waiter*>& batch);
+  // one lane of a flush; `timing` (may be null) keeps its slowest device call
+  void FlushLane(std::vector<Waiter*>& lane, CallTime* timing);
+  int LaneCall(uint64_t epoch, bool models, bool retry, int k, int nf, int width, const char** call);
+  Status MapModel(const Snapshot& snap, Waiter* w, int* target);
   // The tried pods of batch[0 .. n) as indices into snap.pods, matched by value; *width is the widest
   // row of at most LIG_MAX_EXCLUDED entries (at least 1)
   static void TriedRows(const Snapshot& snap, Waiter* const* batch, int n, std::vector<std::vector<int16_t>>* rows,
@@ -438,7 +442,7 @@ class Scheduler {
   void CountFeedback(uint64_t epoch, int n);
   bool AwaitPublication(int rc, uint64_t writes_seen, int attempt);
   void FinishWrite();
-  Status CheckFallbacks(const char* fn, int n) const;
+  Status CheckRequest(const char* fn, const Waiter& w) const;
 
   std::shared_ptr<PodMetricsProvider> pmp_;
   Options opt_;
@@ -450,8 +454,8 @@ class Scheduler {
   uint32_t* h_model_ids_ = nullptr;   // pinned, max_batch entries each: the model-id lane
   lig_mpick* h_mpicks_ = nullptr;
   uint64_t model_index_ = 0;          // first_index of the next model-id device call
-  std::vector<Waiter*> desc_lane_, model_lane_, retry_lane_, model_retry_lane_;   // a flush split by kind
-                                                                                  // (batcher thread only)
+  // a flush split by kind: descriptors, retries, model ids, model-id retries (batcher thread only)
+  std::vector<Waiter*> lanes_[4];
   std::vector<uint8_t> model_targets_;   // the model-retry lane's target indices (batcher thread only)
   int16_t* h_excluded_ = nullptr;     // pinned, max_batch x LIG_MAX_EXCLUDED rows (first retry flush)
   uint64_t seed_ = 0;

@@ -175,6 +175,32 @@ def _no_model_entry(model_id: int, name: str) -> str:
     return f"{_POD_PREFIX}rpc error: code = Internal desc = model id {model_id} ({name}) has no model entry on the device"
 
 
+# What a call under load_feedback_window is refused with when the scheduler was not built for its form,
+# by (retry, fallback rows).
+_FEEDBACK_REFUSALS = {
+    (False, True): "fallback endpoints are not defined under load_feedback_window: the picks come from the "
+                   "feedback chain's copy of the snapshot, the fallbacks would not",
+    (True, False): "retries are not defined under load_feedback_window: the picks come from the feedback "
+                   "chain's load-adjusted copy of the snapshot, a retry would not",
+    (True, True): "retries with fallbacks are not defined under load_feedback_window without "
+                  "feedback_retries and feedback_fallbacks: the picks come from the feedback chain's "
+                  "load-adjusted copy of the snapshot, these would not",
+}
+
+
+def _rows_array(rows: Sequence[Sequence[int]]) -> np.ndarray:
+    """Excluded rows as the excluding calls take them: -1 padded to the widest row (at least 1)."""
+    out = np.full((len(rows), max([1] + [len(r) for r in rows])), -1, dtype=np.int16)
+    for i, r in enumerate(rows):
+        out[i, :len(r)] = r
+    return out
+
+
+def _picks(results: list) -> list:
+    """Results of a batch body with the pick alone in place of the pod list (None on error)."""
+    return [(pods[0] if pods else None, *rest) for pods, *rest in results]
+
+
 def _check_models(models: Sequence[InferenceModel]) -> None:
     """What lig_upload_models refuses with LIG_ERR_RANGE, named by model.  A model whose weights sum
     to <= 0 is not refused: pack_models packs it as absent."""
@@ -303,64 +329,139 @@ class Scheduler:
             return self.Refresh()
         return self._snap
 
-    def ScheduleBatch(self, reqs: Sequence[LLMRequest]) -> List[Tuple[Optional[Pod], Optional[StatusError]]]:
+    # ---- the two batch bodies: descriptor requests and model names, each plain, with fallback rows, as a
+    # retry without the pods already tried, or both ----
+    def _check_form(self, n: Optional[int], tried_lists: Optional[Sequence[Sequence[Pod]]] = None,
+                    mismatch: Optional[str] = None) -> None:
+        """The refusals of a call with fallback rows (n) or a retry (tried_lists), in this order.
+        `mismatch` is the message for argument lists of different lengths, if they differ."""
+        retry, rows = tried_lists is not None, n is not None
+        if self._window and ((retry and not self._feedback_retries) or (rows and not self._feedback_fallbacks)):
+            raise ValueError(_FEEDBACK_REFUSALS[retry, rows])
+        if rows and not 1 <= n <= N.LIG_MAX_FALLBACKS:
+            raise ValueError(f"n must be in [1, {N.LIG_MAX_FALLBACKS}], got {n}")
+        if mismatch:
+            raise ValueError(mismatch)
+        for tried in tried_lists or ():
+            if len(tried) > N.LIG_MAX_EXCLUDED:
+                raise ValueError(f"{len(tried)} tried pods (at most {N.LIG_MAX_EXCLUDED})")
+
+    @staticmethod
+    def _tried_rows(snap: PackedSnapshot, tried_lists: Sequence[Sequence[Pod]]) -> List[List[int]]:
+        """Each list's tried pods as indices into the snapshot, matched by value; pods no longer in it
+        are ignored."""
+        where: Dict[Pod, List[int]] = {}
+        for p, pod in enumerate(snap.pods):
+            where.setdefault(pod, []).append(p)
+        return [[p for pod in tried for p in where.get(pod, ())] for tried in tried_lists]
+
+    def _call(self, kind: str, arr: np.ndarray, excluded: tuple, n: Optional[int], **kw):
+        """The Engine call of a batch: ``schedule_<kind>`` (kind "batch" or "models_batch"), as a chain
+        call under load_feedback_window, an excluding call for a retry (`excluded` holds the retry's
+        arrays), a fallback call for n rows.  Returns (picks, rows); without n every row is empty."""
+        name = ("schedule_" + kind + ("_feedback_chain" if self._window else "") + ("_excluding" if excluded else "")
+                + ("_fallbacks" if n is not None else ""))
+        args = (self._epoch, self._seed, arr, *excluded) + ((n,) if n is not None else ()) + \
+            ((self._window,) if self._window else ())
+        out = getattr(self._engine, name)(*args, **kw)
+        return out if n is not None else (out, [()] * len(out))
+
+    def _batch(self, reqs: Sequence[LLMRequest], tried_lists: Optional[Sequence[Sequence[Pod]]] = None,
+               n: Optional[int] = None) -> List[Tuple[List[Pod], Optional[StatusError]]]:
+        """(pods, error) per request: pods the pick and then its fallback row, [] on error.  One rand_key
+        per request, in order, from ScheduleBatch's sequence."""
+        self._check_form(n, tried_lists, None if tried_lists is None or len(tried_lists) == len(reqs)
+                         else f"{len(reqs)} requests but {len(tried_lists)} tried lists")
         snap = self._current()
+        excluded: tuple = ()
+        if tried_lists is not None:
+            rows = self._tried_rows(snap, tried_lists)
+            width = max([1] + [len(r) for r in rows])
+            if width > N.LIG_MAX_EXCLUDED:
+                raise ValueError(f"the tried pods match {width} pods of the snapshot (at most {N.LIG_MAX_EXCLUDED})")
+            excluded = (_rows_array(rows),)
         arr = np.zeros(len(reqs), dtype=REQ_DTYPE)
         for i, r in enumerate(reqs):
             arr[i] = (snap.adapter_id(r.ResolvedTargetModel), N.LIG_REQ_CRITICAL if r.Critical else 0,
                       self._rng.getrandbits(64))
-        if self._window:
-            # the feedback chain: each window of `_window` requests, across calls, adds its picks to
-            # the pods' WaitingQueueSize until the next refresh uploads a new epoch
-            picks = self._engine.schedule_batch_feedback_chain(self._epoch, self._seed, arr, self._window)
-        else:
-            picks = self._engine.schedule_batch(self._epoch, self._seed, arr)
-        out = []
-        for pk in picks:
-            if pk["status"] == N.LIG_OK:
-                out.append((snap.pods[int(pk["pod_idx"])], None))
+        # under load_feedback_window each window of `_window` requests, across calls, adds its picks to
+        # the pods' WaitingQueueSize until the next refresh uploads a new epoch
+        picks, rows = self._call("batch", arr, excluded, n)
+        return [([snap.pods[int(pk["pod_idx"])]] + [snap.pods[int(p)] for p in row if p >= 0], None)
+                if pk["status"] == N.LIG_OK else ([], _schedule_error(int(pk["status"])))
+                for pk, row in zip(picks, rows)]
+
+    def _map_models(self, names: Sequence[str], resolved: Optional[Sequence[str]] = None,
+                    rows: Optional[List[List[int]]] = None):
+        """(errors, model ids, target indices, slots): the names the device is sent, in order, as model
+        ids at positions `slots`, and for a retry (resolved) each resolved target as the first
+        TargetModels entry of that name (255 for a model without TargetModels whose own name it is).
+        A name the list alone answers gets its error instead."""
+        pm = self._packed_models
+        errors: List[Optional[StatusError]] = [None] * len(names)
+        ids, targets, slots = [], [], []
+        for i, name in enumerate(names):
+            m = pm.model_ids.get(name) if pm is not None else None
+            if m is None:                                                       # request.go:42-45
+                errors[i] = StatusError("Unknown", f"error finding a model object in InferenceModel for input {name}")
+                continue
+            if not pm.present[m]:                                               # request.go:48-51
+                errors[i] = StatusError("Unknown", f"error getting target model name for model {name}")
+                continue
+            if resolved is not None:
+                res, tgt = resolved[i], pm.target_names[m]
+                t = (255 if res == name else None) if not tgt else next((j for j, x in enumerate(tgt) if x == res), None)
+                if t is None:
+                    errors[i] = StatusError("InvalidArgument", f"{res} is not a target model of {name}")
+                    continue
+                if len(rows[i]) > N.LIG_MAX_EXCLUDED:
+                    raise ValueError(f"the tried pods match {len(rows[i])} pods of the snapshot (at most "
+                                     f"{N.LIG_MAX_EXCLUDED})")
+                targets.append(t)
+            ids.append(m)
+            slots.append(i)
+        return errors, ids, targets, slots
+
+    def _model_batch(self, names: Sequence[str], resolved: Optional[Sequence[str]] = None,
+                     tried_lists: Optional[Sequence[Sequence[Pod]]] = None, n: Optional[int] = None
+                     ) -> List[Tuple[List[Pod], str, Optional[StatusError]]]:
+        """(pods, resolved target model, error) per name: pods the pick and then its fallback row, [] on
+        error.  A retry (resolved, tried_lists) keeps the target the first attempt drew.  Names the host
+        answers take no rand_key; request k sent to the device has rand_key = _model_index + k."""
+        retry = tried_lists is not None
+        self._check_form(n, tried_lists, None if not retry or len(names) == len(resolved) == len(tried_lists)
+                         else f"{len(names)} names, {len(resolved)} resolved targets, {len(tried_lists)} tried lists")
+        snap = self._current()
+        rows = self._tried_rows(snap, tried_lists) if retry else None
+        errors, ids, targets, slots = self._map_models(names, resolved if retry else None, rows)
+        out = [([], resolved[i] if retry else "", err) for i, err in enumerate(errors)]
+        if not ids:
+            return out
+        excluded = (np.array(targets, dtype=np.uint8), _rows_array([rows[i] for i in slots])) if retry else ()
+        picks, fbs = self._call("models_batch", np.array(ids, dtype=np.uint32), excluded, n,
+                                first_index=self._model_index)
+        self._model_index += len(ids)
+        pm = self._packed_models
+        for i, m, pk, row in zip(slots, ids, picks, fbs):
+            t, st = int(pk["target_idx"]), int(pk["status"])
+            res = resolved[i] if retry else names[i] if t == 255 else pm.target_names[m][t]   # 255: request.go:47
+            if st == N.LIG_OK:
+                out[i] = ([snap.pods[int(pk["pod_idx"])]] + [snap.pods[int(p)] for p in row if p >= 0], res, None)
+            elif st == N.LIG_NO_MODEL:       # absent models and targets never reach the device
+                out[i] = ([], res, StatusError("Internal", _no_model_entry(m, names[i])))
             else:
-                out.append((None, _schedule_error(int(pk["status"]))))
+                err = _schedule_error(st)
+                out[i] = ([], res, StatusError(err.code, _POD_PREFIX + str(err)))
         return out
+
+    def ScheduleBatch(self, reqs: Sequence[LLMRequest]) -> List[Tuple[Optional[Pod], Optional[StatusError]]]:
+        return _picks(self._batch(reqs))
 
     def ScheduleModelBatch(self, names: Sequence[str]) -> List[Tuple[Optional[Pod], str, Optional[StatusError]]]:
         """The resolve step and the pick on the device, one call per batch: (pod, resolved target
         model, error) per name.  Names the host answers from the list alone (unknown, or weights
         summing to <= 0) take no rand_key; request k sent to the device has rand_key = k."""
-        snap = self._current()
-        pm = self._packed_models
-        out: List[Tuple[Optional[Pod], str, Optional[StatusError]]] = [None] * len(names)  # type: ignore
-        ids, slots = [], []
-        for i, name in enumerate(names):
-            m = pm.model_ids.get(name) if pm is not None else None
-            if m is None:                                                       # request.go:42-45
-                out[i] = (None, "", StatusError(
-                    "Unknown", f"error finding a model object in InferenceModel for input {name}"))
-            elif not pm.present[m]:                                             # request.go:48-51
-                out[i] = (None, "", StatusError("Unknown", f"error getting target model name for model {name}"))
-            else:
-                ids.append(m)
-                slots.append(i)
-        if not ids:
-            return out
-        arr = np.array(ids, dtype=np.uint32)
-        if self._window:
-            picks = self._engine.schedule_models_batch_feedback_chain(self._epoch, self._seed, arr, self._window,
-                                                                      first_index=self._model_index)
-        else:
-            picks = self._engine.schedule_models_batch(self._epoch, self._seed, arr, first_index=self._model_index)
-        self._model_index += len(ids)
-        for i, m, pk in zip(slots, ids, picks):
-            t, st = int(pk["target_idx"]), int(pk["status"])
-            resolved = names[i] if t == 255 else pm.target_names[m][t]         # 255: request.go:47
-            if st == N.LIG_OK:
-                out[i] = (snap.pods[int(pk["pod_idx"])], resolved, None)
-            elif st == N.LIG_NO_MODEL:       # absent models never reach the device
-                out[i] = (None, resolved, StatusError("Internal", _no_model_entry(m, names[i])))
-            else:
-                err = _schedule_error(st)
-                out[i] = (None, resolved, StatusError(err.code, _POD_PREFIX + str(err)))
-        return out
+        return _picks(self._model_batch(names))
 
     def ScheduleModel(self, name: str) -> Tuple[str, Pod]:
         """HandleRequestBody's resolve step and Schedule for one request: (resolved target model,
@@ -377,13 +478,6 @@ class Scheduler:
         return pod
 
     # ---- fallback endpoints: the pick, then up to n more distinct survivors in retry order ----
-    def _check_fallbacks(self, n: int) -> None:
-        if self._window and not self._feedback_fallbacks:
-            raise ValueError("fallback endpoints are not defined under load_feedback_window: the picks come from "
-                             "the feedback chain's copy of the snapshot, the fallbacks would not")
-        if not 1 <= n <= N.LIG_MAX_FALLBACKS:
-            raise ValueError(f"n must be in [1, {N.LIG_MAX_FALLBACKS}], got {n}")
-
     def ScheduleBatchWithFallbacks(self, reqs: Sequence[LLMRequest], n: int
                                    ) -> List[Tuple[List[Pod], Optional[StatusError]]]:
         """ScheduleBatch plus up to n fallback pods per request (lig_schedule_batch_fallbacks):
@@ -392,24 +486,7 @@ class Scheduler:
         sequence as ScheduleBatch.  Under load_feedback_window the call is a feedback-chain call
         (lig_schedule_batch_feedback_chain_fallbacks) when the scheduler was built with
         feedback_fallbacks=True, and raises ValueError otherwise."""
-        self._check_fallbacks(n)
-        snap = self._current()
-        arr = np.zeros(len(reqs), dtype=REQ_DTYPE)
-        for i, r in enumerate(reqs):
-            arr[i] = (snap.adapter_id(r.ResolvedTargetModel), N.LIG_REQ_CRITICAL if r.Critical else 0,
-                      self._rng.getrandbits(64))
-        if self._window:
-            picks, rows = self._engine.schedule_batch_feedback_chain_fallbacks(self._epoch, self._seed, arr, n,
-                                                                               self._window)
-        else:
-            picks, rows = self._engine.schedule_batch_fallbacks(self._epoch, self._seed, arr, n)
-        out: List[Tuple[List[Pod], Optional[StatusError]]] = []
-        for pk, row in zip(picks, rows):
-            if pk["status"] == N.LIG_OK:
-                out.append(([snap.pods[int(pk["pod_idx"])]] + [snap.pods[int(p)] for p in row if p >= 0], None))
-            else:
-                out.append(([], _schedule_error(int(pk["status"]))))
-        return out
+        return self._batch(reqs, n=n)
 
     def ScheduleWithFallbacks(self, req: LLMRequest, n: int) -> List[Pod]:
         """Schedule plus up to n fallback pods: [pick, fallback 1, ...]; raises like Schedule."""
@@ -424,70 +501,9 @@ class Scheduler:
         error) per name, pods[0] the pod ScheduleModelBatch would have returned.  Host-answered errors
         and the rand_key sequence (_model_index) as ScheduleModelBatch.  Under load_feedback_window
         as ScheduleBatchWithFallbacks: a chain call with feedback_fallbacks=True, else ValueError."""
-        self._check_fallbacks(n)
-        snap = self._current()
-        pm = self._packed_models
-        out: List[Tuple[List[Pod], str, Optional[StatusError]]] = [None] * len(names)  # type: ignore
-        ids, slots = [], []
-        for i, name in enumerate(names):
-            m = pm.model_ids.get(name) if pm is not None else None
-            if m is None:                                                       # request.go:42-45
-                out[i] = ([], "", StatusError(
-                    "Unknown", f"error finding a model object in InferenceModel for input {name}"))
-            elif not pm.present[m]:                                             # request.go:48-51
-                out[i] = ([], "", StatusError("Unknown", f"error getting target model name for model {name}"))
-            else:
-                ids.append(m)
-                slots.append(i)
-        if not ids:
-            return out
-        arr = np.array(ids, dtype=np.uint32)
-        if self._window:
-            picks, rows = self._engine.schedule_models_batch_feedback_chain_fallbacks(
-                self._epoch, self._seed, arr, n, self._window, first_index=self._model_index)
-        else:
-            picks, rows = self._engine.schedule_models_batch_fallbacks(self._epoch, self._seed, arr, n,
-                                                                       first_index=self._model_index)
-        self._model_index += len(ids)
-        for i, m, pk, row in zip(slots, ids, picks, rows):
-            t, st = int(pk["target_idx"]), int(pk["status"])
-            resolved = names[i] if t == 255 else pm.target_names[m][t]         # 255: request.go:47
-            if st == N.LIG_OK:
-                pods = [snap.pods[int(pk["pod_idx"])]] + [snap.pods[int(p)] for p in row if p >= 0]
-                out[i] = (pods, resolved, None)
-            elif st == N.LIG_NO_MODEL:       # absent models never reach the device
-                out[i] = ([], resolved, StatusError("Internal", _no_model_entry(m, names[i])))
-            else:
-                err = _schedule_error(st)
-                out[i] = ([], resolved, StatusError(err.code, _POD_PREFIX + str(err)))
-        return out
+        return self._model_batch(names, n=n)
 
     # ---- retry scheduling: Schedule again over the pool without the pods already tried ----
-    def _retry_batch(self, reqs: Sequence[LLMRequest], tried_lists: Sequence[Sequence[Pod]]):
-        """(snapshot, descriptors, excluded rows) of a retry batch: tried pods matched by value against the
-        current snapshot, one rand_key per request from ScheduleBatch's sequence."""
-        if len(tried_lists) != len(reqs):
-            raise ValueError(f"{len(reqs)} requests but {len(tried_lists)} tried lists")
-        for tried in tried_lists:
-            if len(tried) > N.LIG_MAX_EXCLUDED:
-                raise ValueError(f"{len(tried)} tried pods (at most {N.LIG_MAX_EXCLUDED})")
-        snap = self._current()
-        where: Dict[Pod, List[int]] = {}
-        for p, pod in enumerate(snap.pods):
-            where.setdefault(pod, []).append(p)
-        rows = [[p for pod in tried for p in where.get(pod, ())] for tried in tried_lists]
-        width = max([1] + [len(r) for r in rows])
-        if width > N.LIG_MAX_EXCLUDED:
-            raise ValueError(f"the tried pods match {width} pods of the snapshot (at most {N.LIG_MAX_EXCLUDED})")
-        excluded = np.full((len(reqs), width), -1, dtype=np.int16)
-        for i, r in enumerate(rows):
-            excluded[i, :len(r)] = r
-        arr = np.zeros(len(reqs), dtype=REQ_DTYPE)
-        for i, r in enumerate(reqs):
-            arr[i] = (snap.adapter_id(r.ResolvedTargetModel), N.LIG_REQ_CRITICAL if r.Critical else 0,
-                      self._rng.getrandbits(64))
-        return snap, arr, excluded
-
     def ScheduleBatchRetry(self, reqs: Sequence[LLMRequest], tried_lists: Sequence[Sequence[Pod]]
                            ) -> List[Tuple[Optional[Pod], Optional[StatusError]]]:
         """ScheduleBatch with request i scheduled over the current snapshot's pods without the pods of
@@ -498,17 +514,7 @@ class Scheduler:
         load_feedback_window the call is a feedback-chain call (lig_schedule_batch_feedback_chain_excluding:
         the pool is the chain's load-adjusted copy, and each pick counts toward the chain's windows)
         when the scheduler was built with feedback_retries=True, and raises ValueError otherwise."""
-        if self._window and not self._feedback_retries:
-            raise ValueError("retries are not defined under load_feedback_window: the picks come from the feedback "
-                             "chain's load-adjusted copy of the snapshot, a retry would not")
-        snap, arr, excluded = self._retry_batch(reqs, tried_lists)
-        if self._window:
-            picks = self._engine.schedule_batch_feedback_chain_excluding(self._epoch, self._seed, arr, excluded,
-                                                                         self._window)
-        else:
-            picks = self._engine.schedule_batch_excluding(self._epoch, self._seed, arr, excluded)
-        return [(snap.pods[int(pk["pod_idx"])], None) if pk["status"] == N.LIG_OK
-                else (None, _schedule_error(int(pk["status"]))) for pk in picks]
+        return _picks(self._batch(reqs, tried_lists))
 
     def ScheduleRetry(self, req: LLMRequest, tried: Sequence[Pod]) -> Pod:
         """Schedule over the pool without the pods in `tried`; raises like Schedule."""
@@ -528,21 +534,7 @@ class Scheduler:
         loads are ScheduleBatchRetry's chain call's, the rows rank the reduced pool of the chain's
         load-adjusted copy) when the scheduler was built with both feedback_retries=True and
         feedback_fallbacks=True, and raises ValueError otherwise."""
-        if self._window and not (self._feedback_retries and self._feedback_fallbacks):
-            raise ValueError("retries with fallbacks are not defined under load_feedback_window without "
-                             "feedback_retries and feedback_fallbacks: the picks come from the feedback chain's "
-                             "load-adjusted copy of the snapshot, these would not")
-        if not 1 <= n <= N.LIG_MAX_FALLBACKS:
-            raise ValueError(f"n must be in [1, {N.LIG_MAX_FALLBACKS}], got {n}")
-        snap, arr, excluded = self._retry_batch(reqs, tried_lists)
-        if self._window:
-            picks, rows = self._engine.schedule_batch_feedback_chain_excluding_fallbacks(
-                self._epoch, self._seed, arr, excluded, n, self._window)
-        else:
-            picks, rows = self._engine.schedule_batch_excluding_fallbacks(self._epoch, self._seed, arr, excluded, n)
-        return [([snap.pods[int(pk["pod_idx"])]] + [snap.pods[int(p)] for p in row if p >= 0], None)
-                if pk["status"] == N.LIG_OK else ([], _schedule_error(int(pk["status"])))
-                for pk, row in zip(picks, rows)]
+        return self._batch(reqs, tried_lists, n)
 
     def ScheduleRetryWithFallbacks(self, req: LLMRequest, tried: Sequence[Pod], n: int) -> List[Pod]:
         """ScheduleRetry plus up to n fallback pods: [pick, fallback 1, ...]; raises like Schedule."""
@@ -552,51 +544,6 @@ class Scheduler:
         return pods
 
     # ---- model-id retries: the retry of a model request at the target its first attempt drew ----
-    def _model_retry_batch(self, names: Sequence[str], resolved: Sequence[str],
-                           tried_lists: Sequence[Sequence[Pod]], empty):
-        """(snapshot, results, model ids, target indices, excluded rows, slots) of a model-retry batch.  Each
-        name is mapped to its model id and its resolved target to the first TargetModels entry of that
-        name (255 for a model without TargetModels whose own name it is); names the host answers get
-        (empty, resolved, error) in results and no row."""
-        if not len(names) == len(resolved) == len(tried_lists):
-            raise ValueError(f"{len(names)} names, {len(resolved)} resolved targets, {len(tried_lists)} tried lists")
-        for tried in tried_lists:
-            if len(tried) > N.LIG_MAX_EXCLUDED:
-                raise ValueError(f"{len(tried)} tried pods (at most {N.LIG_MAX_EXCLUDED})")
-        snap = self._current()
-        pm = self._packed_models
-        where: Dict[Pod, List[int]] = {}
-        for p, pod in enumerate(snap.pods):
-            where.setdefault(pod, []).append(p)
-        out: list = [None] * len(names)
-        ids, targets, rows, slots = [], [], [], []
-        for i, (name, res) in enumerate(zip(names, resolved)):
-            m = pm.model_ids.get(name) if pm is not None else None
-            if m is None:                                                       # request.go:42-45
-                out[i] = (empty, res, StatusError(
-                    "Unknown", f"error finding a model object in InferenceModel for input {name}"))
-                continue
-            if not pm.present[m]:                                               # request.go:48-51
-                out[i] = (empty, res, StatusError("Unknown", f"error getting target model name for model {name}"))
-                continue
-            tgt = pm.target_names[m]
-            t = (255 if res == name else None) if not tgt else next((j for j, x in enumerate(tgt) if x == res), None)
-            if t is None:
-                out[i] = (empty, res, StatusError("InvalidArgument", f"{res} is not a target model of {name}"))
-                continue
-            row = [p for pod in tried_lists[i] for p in where.get(pod, ())]
-            if len(row) > N.LIG_MAX_EXCLUDED:
-                raise ValueError(f"the tried pods match {len(row)} pods of the snapshot (at most "
-                                 f"{N.LIG_MAX_EXCLUDED})")
-            ids.append(m)
-            targets.append(t)
-            rows.append(row)
-            slots.append(i)
-        excluded = np.full((len(ids), max([1] + [len(r) for r in rows])), -1, dtype=np.int16)
-        for k, r in enumerate(rows):
-            excluded[k, :len(r)] = r
-        return snap, out, np.array(ids, dtype=np.uint32), np.array(targets, dtype=np.uint8), excluded, slots
-
     def ScheduleModelBatchRetry(self, names: Sequence[str], resolved: Sequence[str],
                                 tried_lists: Sequence[Sequence[Pod]]
                                 ) -> List[Tuple[Optional[Pod], str, Optional[StatusError]]]:
@@ -609,29 +556,7 @@ class Scheduler:
         Tried pods are matched by value as in ScheduleBatchRetry.  Under load_feedback_window the call is
         a chain call (lig_schedule_models_batch_feedback_chain_excluding) when the scheduler was built
         with feedback_retries=True, and raises ValueError otherwise."""
-        if self._window and not self._feedback_retries:
-            raise ValueError("retries are not defined under load_feedback_window: the picks come from the feedback "
-                             "chain's load-adjusted copy of the snapshot, a retry would not")
-        snap, out, ids, targets, excluded, slots = self._model_retry_batch(names, resolved, tried_lists, None)
-        if not len(ids):
-            return out
-        if self._window:
-            picks = self._engine.schedule_models_batch_feedback_chain_excluding(
-                self._epoch, self._seed, ids, targets, excluded, self._window, first_index=self._model_index)
-        else:
-            picks = self._engine.schedule_models_batch_excluding(self._epoch, self._seed, ids, targets, excluded,
-                                                                 first_index=self._model_index)
-        self._model_index += len(ids)
-        for i, m, pk in zip(slots, ids, picks):
-            st = int(pk["status"])
-            if st == N.LIG_OK:
-                out[i] = (snap.pods[int(pk["pod_idx"])], resolved[i], None)
-            elif st == N.LIG_NO_MODEL:       # absent models and targets never reach the device
-                out[i] = (None, resolved[i], StatusError("Internal", _no_model_entry(int(m), names[i])))
-            else:
-                err = _schedule_error(st)
-                out[i] = (None, resolved[i], StatusError(err.code, _POD_PREFIX + str(err)))
-        return out
+        return _picks(self._model_batch(names, resolved, tried_lists))
 
     def ScheduleModelRetry(self, name: str, resolved: str, tried: Sequence[Pod]) -> Pod:
         """The retry of one ScheduleModel request at its resolved target; raises like ScheduleModel."""
@@ -647,33 +572,7 @@ class Scheduler:
         (lig_schedule_models_batch_excluding_fallbacks): (pods, resolved target model, error), pods[0] the
         pod ScheduleModelBatchRetry would have returned.  ValueError for n outside [1, LIG_MAX_FALLBACKS];
         under load_feedback_window it needs both feedback_retries=True and feedback_fallbacks=True."""
-        if self._window and not (self._feedback_retries and self._feedback_fallbacks):
-            raise ValueError("retries with fallbacks are not defined under load_feedback_window without "
-                             "feedback_retries and feedback_fallbacks: the picks come from the feedback chain's "
-                             "load-adjusted copy of the snapshot, these would not")
-        if not 1 <= n <= N.LIG_MAX_FALLBACKS:
-            raise ValueError(f"n must be in [1, {N.LIG_MAX_FALLBACKS}], got {n}")
-        snap, out, ids, targets, excluded, slots = self._model_retry_batch(names, resolved, tried_lists, [])
-        if not len(ids):
-            return out
-        if self._window:
-            picks, rows = self._engine.schedule_models_batch_feedback_chain_excluding_fallbacks(
-                self._epoch, self._seed, ids, targets, excluded, n, self._window, first_index=self._model_index)
-        else:
-            picks, rows = self._engine.schedule_models_batch_excluding_fallbacks(
-                self._epoch, self._seed, ids, targets, excluded, n, first_index=self._model_index)
-        self._model_index += len(ids)
-        for i, m, pk, row in zip(slots, ids, picks, rows):
-            st = int(pk["status"])
-            if st == N.LIG_OK:
-                out[i] = ([snap.pods[int(pk["pod_idx"])]] + [snap.pods[int(p)] for p in row if p >= 0], resolved[i],
-                          None)
-            elif st == N.LIG_NO_MODEL:
-                out[i] = ([], resolved[i], StatusError("Internal", _no_model_entry(int(m), names[i])))
-            else:
-                err = _schedule_error(st)
-                out[i] = ([], resolved[i], StatusError(err.code, _POD_PREFIX + str(err)))
-        return out
+        return self._model_batch(names, resolved, tried_lists, n)
 
     def ScheduleModelRetryWithFallbacks(self, name: str, resolved: str, tried: Sequence[Pod], n: int) -> List[Pod]:
         """ScheduleModelRetry plus up to n fallback pods: [pick, fallback 1, ...]; raises like ScheduleModel."""
@@ -731,18 +630,8 @@ class Scheduler:
         the host answers from the list alone get ScheduleModelBatch's errors.  The draws use
         ScheduleModelBatch's rand_key sequence without advancing it."""
         snap = self._current()
-        pm = self._packed_models
-        out: List[Tuple[List[Pod], Optional[StatusError]]] = [None] * len(names)  # type: ignore
-        ids, slots = [], []
-        for i, name in enumerate(names):
-            m = pm.model_ids.get(name) if pm is not None else None
-            if m is None:                                                       # request.go:42-45
-                out[i] = ([], StatusError("Unknown", f"error finding a model object in InferenceModel for input {name}"))
-            elif not pm.present[m]:                                             # request.go:48-51
-                out[i] = ([], StatusError("Unknown", f"error getting target model name for model {name}"))
-            else:
-                ids.append(m)
-                slots.append(i)
+        errors, ids, _, slots = self._map_models(names)
+        out = [([], err) for err in errors]
         if not ids:
             return out
         picks, offsets, pods = self._engine.filter_models_batch(self._epoch, self._seed, np.array(ids, dtype=np.uint32),
