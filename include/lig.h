@@ -532,6 +532,65 @@ int lig_schedule_models_batch_fallbacks_device(lig_ctx* ctx, uint64_t epoch, uin
                                                const uint32_t* d_model_ids, int R, lig_mpick* d_out,
                                                int n_fallbacks, int16_t* d_fallbacks, void* stream);
 
+/* ---- session affinity: requests that share a key go to the same surviving pod -----------------------
+ * Every other pick is a fresh draw, so two turns of one conversation rarely meet the pod that holds the
+ * conversation's KV cache.  These calls replace the draw by rendezvous (highest random weight) hashing
+ * on a caller key.  The reference picks with rand.Intn on an unseeded source (scheduler.go:120), so
+ * any survivor is a legal outcome; an affinity pick is a member of exactly the survivor set the plain
+ * call computes.
+ *
+ * Pod keys.  lig_upload_pod_keys gives epoch E a stable 64-bit identity per pod (pod_key[P], in E's
+ * pod order; the schedulers use FNV-1a 64 over Name, a zero byte, then Address).  With mix the
+ * SplitMix64 finalizer of the pick's stream, z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;
+ * z = (z ^ (z >> 27)) * 0x94D049BB133111EB; return z ^ (z >> 31), the device stores h_p = mix(pod_key[p]).
+ * The table belongs to E like its model table: the upload is staged through the slot's pinned memory,
+ * copied on the upload stream behind the slot's readers and recorded as an event every affinity call
+ * on E is ordered behind.  lig_set_thresholds / lig_set_filter_tree rebuilds keep it; every writer that
+ * makes a new epoch (full uploads, lig_update_snapshot, lig_eject_pods, lig_comm_*, the group upload)
+ * leaves that epoch without keys.  LIG_ERR_INVALID when P differs from E's P or keys is null with
+ * P > 0; a missing or stale epoch as every call reports it.  Refused uploads keep E's keys.
+ *
+ * The definition.  A request with affinity key k (lig_req.rand_key, or keys[i] for model ids) gives
+ * survivor p the score s(k, p) = mix(k ^ h_p).  mix and ^k are bijections of 64-bit words, so distinct
+ * pod keys give distinct scores, and the ranking is a strict order that does not depend on where a
+ * pod sits in the snapshot.  Equal pod keys tie; ties break to the lower pod index, and the order
+ * independence then holds only among distinct keys.
+ *   - class, status and n_survivors are the plain call's (same class entry); for a LIG_OK request
+ *     pod_idx is the member of its survivor list L with the highest score; otherwise -1.
+ *   - the row, fallbacks[i * n_fallbacks .. (i + 1) * n_fallbacks): with m = min(n, 1 + n_fallbacks),
+ *     entries 1 .. m-1 are the next members of L in descending score, then -1; a request that is not
+ *     LIG_OK gets a row of -1.  The row for k fallbacks is a prefix of the row for any k' > k.
+ *   - model ids resolve as in lig_schedule_models_batch, except that the target draw's state is
+ *     k ^ LIG_DRAW_DOMAIN (no seed, no first_index), so a session keeps its target while the model's
+ *     targets and weights stay the same.  target_idx is reported as there; a model that does not
+ *     resolve gives {-1, LIG_NO_MODEL, 255} and a row of -1.
+ *   - there is no seed and no counter: a request's output depends only on E's tables, its pod keys and
+ *     the request, not on its place in the batch, how a batch is split or which ctx answers.  Two
+ *     gateway replicas holding the same snapshot and keys agree.
+ * Consistency: when L shrinks and still holds a key's pod, the key keeps it; when that pod leaves,
+ * only its keys move.
+ *
+ * The calls read the resident epoch's tables, whichever build made them (built-in tree, caller tree,
+ * an ejected epoch's pool, compact or strided lists), never a feedback chain's copy; they neither end
+ * nor advance a chain.  n_fallbacks = 0 means no row (fallbacks may then be NULL).  Refused, with
+ * nothing written: LIG_ERR_INVALID for n_fallbacks outside [0, LIG_MAX_FALLBACKS], null buffers,
+ * R > max_batch on the host forms and device buffers not aligned to their element (requests 16
+ * bytes, picks 8 / 4, keys 8, rows 2); a stale epoch and a missing snapshot as lig_schedule_batch
+ * reports them; LIG_ERR_NO_SNAPSHOT when E has no pod keys, and for the model forms when E has no
+ * model table.  Host forms read and write page-locked buffers in place and stage pageable or
+ * misaligned ones, as the fallback calls do, and block.  Device forms are enqueued on `stream` (NULL
+ * = legacy default stream), not synchronised, and register as readers of the slot. */
+int lig_upload_pod_keys(lig_ctx* ctx, uint64_t epoch, int P, const uint64_t* keys);
+int lig_schedule_batch_affinity(lig_ctx* ctx, uint64_t epoch, const lig_req* reqs, int R, lig_pick* out,
+                                int n_fallbacks, int16_t* fallbacks);
+int lig_schedule_batch_affinity_device(lig_ctx* ctx, uint64_t epoch, const lig_req* d_reqs, int R, lig_pick* d_out,
+                                       int n_fallbacks, int16_t* d_fallbacks, void* stream);
+int lig_schedule_models_batch_affinity(lig_ctx* ctx, uint64_t epoch, const uint32_t* model_ids, const uint64_t* keys,
+                                       int R, lig_mpick* out, int n_fallbacks, int16_t* fallbacks);
+int lig_schedule_models_batch_affinity_device(lig_ctx* ctx, uint64_t epoch, const uint32_t* d_model_ids,
+                                              const uint64_t* d_keys, int R, lig_mpick* d_out, int n_fallbacks,
+                                              int16_t* d_fallbacks, void* stream);
+
 /* ---- retry scheduling: schedule again without the pods a request already tried ------------------------
  * A fallback row runs out within a class's few survivors.  When every pod a proxy tried refused, the
  * reference's answer is Scheduler.Schedule over AllPodMetrics() without those pods (what it schedules

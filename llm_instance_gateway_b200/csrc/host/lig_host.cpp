@@ -139,6 +139,7 @@ Scheduler::~Scheduler() {
   if (h_picks_) lig_host_free(h_picks_);
   if (h_fallbacks_) lig_host_free(h_fallbacks_);
   if (h_excluded_) lig_host_free(h_excluded_);
+  if (h_keys_) lig_host_free(h_keys_);
   if (h_model_ids_) lig_host_free(h_model_ids_);
   if (h_mpicks_) lig_host_free(h_mpicks_);
   if (ctx_) lig_destroy(ctx_);
@@ -308,8 +309,10 @@ Status Scheduler::RefreshImpl(const std::shared_ptr<const ModelList>& models) {
       derived = true;
     }
   }
-  // The model table goes into the published epoch before it is published, so a flush that captures
-  // the epoch always finds the table its names were mapped against.
+  // So do the pod keys (a delta or derived epoch starts without them) and the model table: a flush
+  // that captures the epoch always finds the keys and the table its requests were mapped against.
+  if (opt_.affinity && !group_)
+    if (Status st = UploadPodKeys(*snap); !st.ok()) return st;
   if (models)
     if (Status st = UploadModelTable(*snap, models); !st.ok()) return st;
   snap->models = models;
@@ -375,6 +378,24 @@ Status Scheduler::UploadModelTable(const Snapshot& snap, const std::shared_ptr<c
   return Status{};
 }
 
+uint64_t PodKey(const backend::Pod& pod) {
+  uint64_t h = 0xCBF29CE484222325ull;
+  auto feed = [&h](const std::string& s) {
+    for (unsigned char c : s) h = (h ^ c) * 0x100000001B3ull;
+  };
+  feed(pod.Name);
+  h = (h ^ 0u) * 0x100000001B3ull;
+  feed(pod.Address);
+  return h;
+}
+
+Status Scheduler::UploadPodKeys(const Snapshot& snap) {
+  std::vector<uint64_t> keys(snap.pods.size());
+  for (size_t p = 0; p < keys.size(); ++p) keys[p] = PodKey(snap.pods[p]);
+  if (lig_upload_pod_keys(ctx_, snap.epoch, (int)keys.size(), keys.data()) != 0) return LigFailure("lig_upload_pod_keys");
+  return Status{};
+}
+
 std::vector<int32_t> Scheduler::EjectedIndices(const std::vector<backend::Pod>& pods) const {
   std::vector<int32_t> idx;
   if (ejected_.empty()) return idx;
@@ -404,6 +425,8 @@ Status Scheduler::EjectPods(const std::vector<backend::Pod>& pods) {
     snap->epoch = next_epoch_++;
     if (lig_eject_pods(ctx_, snap->epoch, cur->epoch, want.data(), (int)want.size()) != 0)
       return LigFailure("lig_eject_pods");
+    if (opt_.affinity)
+      if (Status st = UploadPodKeys(*snap); !st.ok()) return st;
     if (snap->models)
       if (Status st = UploadModelTable(*snap, snap->models); !st.ok()) return st;
     snap->ejected = std::move(want);
@@ -492,6 +515,17 @@ Status Scheduler::CheckRequest(const char* fn, const Waiter& w) const {
   if (rows && (w.fallbacks < 1 || w.fallbacks > LIG_MAX_FALLBACKS))
     return Errorf(InvalidArgument, std::string(fn) + ": n=" + std::to_string(w.fallbacks) + " outside [1, " +
                                        std::to_string(LIG_MAX_FALLBACKS) + "]");
+  if (w.affinity) {
+    if (!opt_.affinity)
+      return Errorf(InvalidArgument, std::string(fn) + ": the scheduler was built without Options::affinity (it "
+                                                       "uploads the pods' keys)");
+    if (opt_.load_feedback_window > 0)
+      return Errorf(InvalidArgument, std::string(fn) + ": not defined under load_feedback_window (affinity picks "
+                                                       "would bypass the feedback chain's per-pod counts)");
+    if (group_)
+      return Errorf(InvalidArgument, std::string(fn) + ": a scheduler over several devices has no affinity call");
+    return Status{};
+  }
   if (retry && w.tried->size() > (size_t)LIG_MAX_EXCLUDED)
     return Errorf(InvalidArgument, std::string(fn) + ": " + std::to_string(w.tried->size()) + " tried pods (at most " +
                                        std::to_string(LIG_MAX_EXCLUDED) + ")");
@@ -599,6 +633,64 @@ Status Scheduler::ScheduleModelRetryWithFallbacks(const std::string& model, cons
   if (Status st = CheckRequest("ScheduleModelRetryWithFallbacks", w); !st.ok()) return st;
   Submit(w);
   if (w.status.ok() && pods) *pods = std::move(ranked);
+  return w.status;
+}
+
+Status Scheduler::ScheduleAffinity(const LLMRequest& req, uint64_t key, backend::Pod* targetPod) {
+  Waiter w;
+  w.req = &req;
+  w.affinity = true;
+  w.key = key;
+  if (Status st = CheckRequest("ScheduleAffinity", w); !st.ok()) return st;
+  Submit(w);
+  if (w.status.ok() && targetPod) *targetPod = std::move(w.pod);
+  return w.status;
+}
+
+Status Scheduler::ScheduleAffinityWithFallbacks(const LLMRequest& req, uint64_t key, int n,
+                                                std::vector<backend::Pod>* pods) {
+  if (pods) pods->clear();
+  std::vector<backend::Pod> ranked;
+  Waiter w;
+  w.req = &req;
+  w.affinity = true;
+  w.key = key;
+  w.fallbacks = n;
+  w.pods = &ranked;
+  if (Status st = CheckRequest("ScheduleAffinityWithFallbacks", w); !st.ok()) return st;
+  Submit(w);
+  if (w.status.ok() && pods) *pods = std::move(ranked);
+  return w.status;
+}
+
+Status Scheduler::ScheduleModelAffinity(const std::string& model, uint64_t key, std::string* resolvedTargetModel,
+                                        backend::Pod* targetPod) {
+  Waiter w;
+  w.model = &model;
+  w.affinity = true;
+  w.key = key;
+  if (Status st = CheckRequest("ScheduleModelAffinity", w); !st.ok()) return st;
+  Submit(w);
+  if (w.status.ok() && targetPod) *targetPod = std::move(w.pod);
+  if (resolvedTargetModel) *resolvedTargetModel = std::move(w.resolved);
+  return w.status;
+}
+
+Status Scheduler::ScheduleModelAffinityWithFallbacks(const std::string& model, uint64_t key, int n,
+                                                     std::string* resolvedTargetModel,
+                                                     std::vector<backend::Pod>* pods) {
+  if (pods) pods->clear();
+  std::vector<backend::Pod> ranked;
+  Waiter w;
+  w.model = &model;
+  w.affinity = true;
+  w.key = key;
+  w.fallbacks = n;
+  w.pods = &ranked;
+  if (Status st = CheckRequest("ScheduleModelAffinityWithFallbacks", w); !st.ok()) return st;
+  Submit(w);
+  if (w.status.ok() && pods) *pods = std::move(ranked);
+  if (resolvedTargetModel) *resolvedTargetModel = std::move(w.resolved);
   return w.status;
 }
 
@@ -750,13 +842,15 @@ void Scheduler::CountFeedback(uint64_t epoch, int n) {
   fb_filled_ = (int)((fb_filled_ + (int64_t)n) % W);
 }
 
-// A flush makes its calls lane by lane: descriptors, retries, model ids, model-id retries.
+// A flush makes its calls lane by lane: descriptors, retries, model ids, model-id retries, affinity
+// descriptors, affinity model ids.
 void Scheduler::Flush(std::vector<Waiter*>& all) {
   for (std::vector<Waiter*>& lane : lanes_) lane.clear();
-  for (Waiter* w : all) lanes_[(w->model ? 2 : 0) + (w->tried ? 1 : 0)].push_back(w);
+  for (Waiter* w : all)
+    lanes_[w->affinity ? (w->model ? 5 : 4) : (w->model ? 2 : 0) + (w->tried ? 1 : 0)].push_back(w);
   const auto flush_t0 = std::chrono::steady_clock::now();
   CallTime slowest;   // the descriptor lane's slowest device call
-  for (int l = 0; l < 4; ++l) FlushLane(lanes_[l], l == 0 ? &slowest : nullptr);
+  for (int l = 0; l < 6; ++l) FlushLane(lanes_[l], l == 0 ? &slowest : nullptr);
   const double flush_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - flush_t0).count();
   std::lock_guard<std::mutex> sk(stats_mu_);
   if (slowest.us > stats_.max_device_call_us) {
@@ -814,10 +908,16 @@ Status Scheduler::MapModel(const Snapshot& snap, Waiter* w, int* target) {
 // The library call for k mapped requests of one lane.  *call receives the name LigFailure reports: the
 // entry point's own, except that the group and the doorbell report as lig_schedule_batch.
 #define LIG_LANE_CALL(fn, ...) (*call = #fn, fn(__VA_ARGS__))
-int Scheduler::LaneCall(uint64_t epoch, bool models, bool retry, int k, int nf, int width, const char** call) {
+int Scheduler::LaneCall(uint64_t epoch, bool models, bool retry, bool affinity, int k, int nf, int width,
+                        const char** call) {
   const int W = opt_.load_feedback_window;
   const uint64_t first = model_index_;
   const uint8_t* targets = model_targets_.data();
+  if (affinity && models)
+    return LIG_LANE_CALL(lig_schedule_models_batch_affinity, ctx_, epoch, h_model_ids_, h_keys_, k, h_mpicks_, nf,
+                         h_fallbacks_);
+  if (affinity)
+    return LIG_LANE_CALL(lig_schedule_batch_affinity, ctx_, epoch, h_reqs_, k, h_picks_, nf, h_fallbacks_);
   if (models && retry) {
     if (nf > 0 && W > 0)
       return LIG_LANE_CALL(lig_schedule_models_batch_feedback_chain_excluding_fallbacks, ctx_, epoch, seed_, first,
@@ -880,15 +980,20 @@ int Scheduler::LaneCall(uint64_t epoch, bool models, bool retry, int k, int nf, 
 // Fallback rows are asked at the largest n of the lane's waiters (rows are prefixes of longer rows, the
 // picks are the plain call's).  rand_keys: each descriptor waiter, sent or not, takes the next splitmix
 // key on every attempt; the k model requests sent have rand_key = model_index_ + k on every attempt,
-// and model_index_ moves past them once per chunk.  Host-answered model waiters take no key.
+// and model_index_ moves past them once per chunk.  Host-answered model waiters take no key.  An
+// affinity lane takes no rand_key either: each request carries its waiter's key.
 void Scheduler::FlushLane(std::vector<Waiter*>& lane, CallTime* timing) {
   if (lane.empty()) return;
-  const bool models = lane[0]->model != nullptr, retry = lane[0]->tried != nullptr;
+  const bool models = lane[0]->model != nullptr, retry = lane[0]->tried != nullptr, affinity = lane[0]->affinity;
   const int W = opt_.load_feedback_window;
-  Status failure;   // a retry lane's failure also answers its later chunks, which make no call
+  Status failure;   // a retry or affinity lane's failure also answers its later chunks, which make no call
   if (retry && !h_excluded_) {
     h_excluded_ = static_cast<int16_t*>(lig_host_alloc((size_t)opt_.max_batch * LIG_MAX_EXCLUDED * sizeof(int16_t)));
     if (!h_excluded_) failure = LigFailure("lig_host_alloc");
+  }
+  if (affinity && models && !h_keys_) {
+    h_keys_ = static_cast<uint64_t*>(lig_host_alloc((size_t)opt_.max_batch * sizeof(uint64_t)));
+    if (!h_keys_) failure = LigFailure("lig_host_alloc");
   }
   if (models && retry) model_targets_.resize((size_t)opt_.max_batch);
   std::vector<std::vector<int16_t>> rows;
@@ -896,7 +1001,7 @@ void Scheduler::FlushLane(std::vector<Waiter*>& lane, CallTime* timing) {
   for (size_t done = 0; done < lane.size();) {
     Waiter* const* batch = lane.data() + done;
     const int n = (int)std::min(lane.size() - done, (size_t)opt_.max_batch);
-    if (!retry) failure = Status{};
+    if (!retry && !affinity) failure = Status{};
     std::shared_ptr<const Snapshot> snap;
     int rc = 0, k = 0, nf = 0, width = 1;
     const char* call = "";
@@ -918,7 +1023,7 @@ void Scheduler::FlushLane(std::vector<Waiter*>& lane, CallTime* timing) {
         if (w->model) {
           w->status = MapModel(*snap, w, &target);
         } else {
-          key = splitmix_next(rng_state_);
+          key = affinity ? w->key : splitmix_next(rng_state_);
           nf = std::max(nf, w->fallbacks);   // every descriptor waiter's n counts, sent or not
           w->status = Status{};
         }
@@ -931,6 +1036,7 @@ void Scheduler::FlushLane(std::vector<Waiter*>& lane, CallTime* timing) {
         if (w->model) {
           h_model_ids_[k] = (uint32_t)w->model_id;
           if (retry) model_targets_[(size_t)k] = (uint8_t)target;
+          if (affinity) h_keys_[k] = w->key;
           nf = std::max(nf, w->fallbacks);   // model rows only for the requests the device sees
         } else {
           auto it = snap->adapter_ids->find(w->req->ResolvedTargetModel);
@@ -949,7 +1055,7 @@ void Scheduler::FlushLane(std::vector<Waiter*>& lane, CallTime* timing) {
       }
       const auto call_t0 = std::chrono::steady_clock::now();
       const double cpu_t0 = timing ? ThreadCpuUs() : 0;
-      rc = k > 0 ? LaneCall(snap->epoch, models, retry, k, nf, width, &call) : 0;
+      rc = k > 0 ? LaneCall(snap->epoch, models, retry, affinity, k, nf, width, &call) : 0;
       // a descriptor retry chunk refused on the host as a whole still moves the chain to its epoch
       if (rc == 0 && W > 0 && (k > 0 || !models)) CountFeedback(snap->epoch, k);
       if (timing) {
@@ -958,7 +1064,7 @@ void Scheduler::FlushLane(std::vector<Waiter*>& lane, CallTime* timing) {
       }
       if (!AwaitPublication(rc, writes_seen, attempt)) break;
     }
-    if (models) model_index_ += (uint64_t)k;
+    if (models && !affinity) model_index_ += (uint64_t)k;
     if (failure.ok() && rc != 0) failure = LigFailure(call);
     for (int i = 0; i < n; ++i) {
       Waiter* w = batch[i];
@@ -989,16 +1095,18 @@ void Scheduler::FlushLane(std::vector<Waiter*>& lane, CallTime* timing) {
     }
     {
       std::lock_guard<std::mutex> sk(stats_mu_);
-      if (!models) {
+      if (affinity) {
+        stats_.affinity_scheduled += (uint64_t)n;
+      } else if (!models) {
         stats_.scheduled += (uint64_t)n;
         stats_.batches++;
         stats_.max_batch = std::max<uint64_t>(stats_.max_batch, (uint64_t)n);
       }
       if (retry) stats_.retry_scheduled += (uint64_t)n;
-      if (models && !retry) stats_.model_scheduled += (uint64_t)n;
-      if (!retry)
+      if (models && !retry && !affinity) stats_.model_scheduled += (uint64_t)n;
+      if (!retry && !affinity)
         for (int i = 0; i < n; ++i) stats_.fallback_scheduled += batch[i]->fallbacks > 0 ? 1 : 0;
-      if (models) stats_.model_batches += k > 0 ? 1 : 0;
+      if (models && !affinity) stats_.model_batches += k > 0 ? 1 : 0;
     }
     for (int i = 0; i < n; ++i) {
       Waiter* w = batch[i];

@@ -171,7 +171,15 @@ struct Options {
   // without it, it still is.  No effect without load_feedback_window.  Together with
   // feedback_fallbacks it also lets ScheduleRetryWithFallbacks run under the chain (see there).
   bool feedback_retries = false;
+  // Upload the pods' keys (PodKey) with every epoch the scheduler publishes (full, delta and ejected),
+  // so that ScheduleAffinity and its relatives can place requests by a caller key
+  // (lig_schedule_[models_]batch_affinity).  Off: those calls are refused and nothing else changes.
+  bool affinity = false;
 };
+
+// A pod's affinity identity: FNV-1a 64 over Name, a zero byte, then Address (the provider's own
+// identity of a pod, so a pod keeps its key whatever order the provider lists it in).
+uint64_t PodKey(const backend::Pod& pod);
 
 struct Stats {
   uint64_t scheduled = 0;      // Schedule calls completed
@@ -191,6 +199,7 @@ struct Stats {
   uint64_t retry_scheduled = 0;    // ScheduleRetry, ScheduleModelRetry and their WithFallbacks calls completed
   uint64_t ejected_pods = 0;       // pods of the current snapshot left out of the pool (EjectPods)
   uint64_t eject_publishes = 0;    // epochs derived with lig_eject_pods and published
+  uint64_t affinity_scheduled = 0; // ScheduleAffinity, ScheduleModelAffinity and their WithFallbacks calls completed
   double last_pack_us = 0;     // last Refresh: provider slice -> columns + bitmap (host)
   double last_upload_us = 0;   // last Refresh: lig_upload_snapshot (H2D + class tables)
   double max_device_call_us = 0;   // slowest single lig_schedule_batch call (launch + kernel + synchronise)
@@ -346,6 +355,26 @@ class Scheduler {
   // delta tick inherits the set, and after a full upload (or when the pods' positions moved) one more
   // epoch is derived and published.  Single device only (InvalidArgument otherwise).
   Status EjectPods(const std::vector<backend::Pod>& pods);
+
+  // Session affinity: Schedule with the random pick replaced by rendezvous hashing on `key`
+  // (lig_schedule_batch_affinity): of req's survivors, the pod with the highest score
+  // mix(key ^ mix(PodKey(pod))).  A key keeps its pod while that pod survives, and the answer does not
+  // depend on the provider's pod order, on flushes or on the seed.  Goes through the micro-batcher in a
+  // lane of its own and takes no rand_key; never through the doorbell; counted in
+  // Stats::affinity_scheduled.  Errors are Schedule's.  InvalidArgument without Options::affinity, with
+  // load_feedback_window > 0 (affinity picks would bypass the chain's per-pod counts) and with several
+  // devices.
+  Status ScheduleAffinity(const LLMRequest& req, uint64_t key, backend::Pod* targetPod);
+  // ScheduleAffinity plus up to n (1..LIG_MAX_FALLBACKS) more survivors in descending score: the
+  // session's retry order.  A flush asks the lane's largest n; rows are prefixes of longer rows.
+  Status ScheduleAffinityWithFallbacks(const LLMRequest& req, uint64_t key, int n, std::vector<backend::Pod>* pods);
+  // ScheduleModel(model, ...) placed by `key` (lig_schedule_models_batch_affinity): the target is drawn on
+  // key ^ LIG_DRAW_DOMAIN, so a session keeps its target while the model's targets and weights stay.
+  // Host-answered errors as ScheduleModel; takes no rand_key; refused like ScheduleAffinity.
+  Status ScheduleModelAffinity(const std::string& model, uint64_t key, std::string* resolvedTargetModel,
+                               backend::Pod* targetPod);
+  Status ScheduleModelAffinityWithFallbacks(const std::string& model, uint64_t key, int n,
+                                            std::string* resolvedTargetModel, std::vector<backend::Pod>* pods);
  private:
   struct ModelList;
   Status RefreshImpl(const std::shared_ptr<const ModelList>& models);
@@ -379,6 +408,8 @@ class Scheduler {
   std::vector<int32_t> EjectedIndices(const std::vector<backend::Pod>& pods) const;
   // pack (when the list or the adapter ids changed) and upload the model table into snap.epoch
   Status UploadModelTable(const Snapshot& snap, const std::shared_ptr<const ModelList>& models);
+  // lig_upload_pod_keys for snap.epoch (Options::affinity only)
+  Status UploadPodKeys(const Snapshot& snap);
   // The last model table packed for lig_upload_models, reused while neither the list nor the
   // adapter-id table changed (guarded by refresh_mu_).
   struct PackedModelTable {
@@ -417,6 +448,8 @@ class Scheduler {
     std::vector<backend::Pod>* pods = nullptr;   // *WithFallbacks: receives the pick and its row
     const std::vector<backend::Pod>* tried = nullptr;   // ScheduleRetry: the pods to leave out
     const std::string* target = nullptr;   // ScheduleModelRetry: the resolved target model to keep
+    bool affinity = false;       // Schedule[Model]Affinity*: placed by `key`, no rand_key
+    uint64_t key = 0;
     int64_t model_id = -1;       // flush-time id in the captured epoch's table; -1: answered on the host
     std::string resolved;        // model requests: the resolved target model
     Status status;
@@ -433,7 +466,7 @@ class Scheduler {
   void Flush(std::vector<Waiter*>& batch);
   // one lane of a flush; `timing` (may be null) keeps its slowest device call
   void FlushLane(std::vector<Waiter*>& lane, CallTime* timing);
-  int LaneCall(uint64_t epoch, bool models, bool retry, int k, int nf, int width, const char** call);
+  int LaneCall(uint64_t epoch, bool models, bool retry, bool affinity, int k, int nf, int width, const char** call);
   Status MapModel(const Snapshot& snap, Waiter* w, int* target);
   // The tried pods of batch[0 .. n) as indices into snap.pods, matched by value; *width is the widest
   // row of at most LIG_MAX_EXCLUDED entries (at least 1)
@@ -454,8 +487,10 @@ class Scheduler {
   uint32_t* h_model_ids_ = nullptr;   // pinned, max_batch entries each: the model-id lane
   lig_mpick* h_mpicks_ = nullptr;
   uint64_t model_index_ = 0;          // first_index of the next model-id device call
-  // a flush split by kind: descriptors, retries, model ids, model-id retries (batcher thread only)
-  std::vector<Waiter*> lanes_[4];
+  // a flush split by kind: descriptors, retries, model ids, model-id retries, affinity descriptors,
+  // affinity model ids (batcher thread only)
+  std::vector<Waiter*> lanes_[6];
+  uint64_t* h_keys_ = nullptr;        // pinned, max_batch affinity keys of the model-id affinity lane (first use)
   std::vector<uint8_t> model_targets_;   // the model-retry lane's target indices (batcher thread only)
   int16_t* h_excluded_ = nullptr;     // pinned, max_batch x LIG_MAX_EXCLUDED rows (first retry flush)
   uint64_t seed_ = 0;

@@ -230,7 +230,20 @@ ligh_scheduler* ligh_scheduler_new_feedback(ligh_provider* p, int device, const 
                                             int caller_spin_us, int use_doorbell, const lig_filter_node* nodes,
                                             int n_nodes, int load_feedback_window, int feedback_fallbacks,
                                             int feedback_retries, char* err, int err_cap) {
+  return ligh_scheduler_new_affinity(p, device, devices, n_devices, max_pods, max_adapters, max_batch, flush_size,
+                                     window_us, refresh_ms, seed, busy_poll, caller_spin_us, use_doorbell, nodes,
+                                     n_nodes, load_feedback_window, feedback_fallbacks, feedback_retries, 0, err,
+                                     err_cap);
+}
+
+ligh_scheduler* ligh_scheduler_new_affinity(ligh_provider* p, int device, const int* devices, int n_devices,
+                                            int max_pods, int max_adapters, int max_batch, int flush_size,
+                                            int window_us, int refresh_ms, uint64_t seed, int busy_poll,
+                                            int caller_spin_us, int use_doorbell, const lig_filter_node* nodes,
+                                            int n_nodes, int load_feedback_window, int feedback_fallbacks,
+                                            int feedback_retries, int affinity, char* err, int err_cap) {
   scheduling::Options o;
+  o.affinity = affinity != 0;
   o.load_feedback_window = load_feedback_window;
   o.feedback_fallbacks = feedback_fallbacks != 0;
   o.feedback_retries = feedback_retries != 0;
@@ -334,6 +347,46 @@ int ligh_schedule_retry_with_fallbacks(ligh_scheduler* s, const char* resolved, 
 }
 
 uint64_t ligh_retry_scheduled(ligh_scheduler* s) { return s->sched->stats().retry_scheduled; }
+
+int ligh_schedule_affinity(ligh_scheduler* s, const char* resolved, int critical, uint64_t key, int n, char* names,
+                           int names_cap, int* n_pods, char* err, int err_cap) {
+  scheduling::LLMRequest req;
+  req.ResolvedTargetModel = resolved ? resolved : "";
+  req.Critical = critical != 0;
+  std::vector<backend::Pod> pods(1);
+  scheduling::Status st = n == 0 ? s->sched->ScheduleAffinity(req, key, &pods[0])
+                                 : s->sched->ScheduleAffinityWithFallbacks(req, key, n, &pods);
+  if (!st.ok()) pods.clear();
+  std::string joined;
+  for (size_t i = 0; i < pods.size(); ++i) joined += (i ? "\n" : "") + pods[i].Name;
+  if (n_pods) *n_pods = (int)pods.size();
+  put(names, names_cap, joined);
+  if (!st.ok()) put(err, err_cap, st.message);
+  return st.code;
+}
+
+int ligh_schedule_model_affinity(ligh_scheduler* s, const char* model, uint64_t key, int n, char* resolved,
+                                 int resolved_cap, char* names, int names_cap, int* n_pods, char* err, int err_cap) {
+  std::string target;
+  std::vector<backend::Pod> pods(1);
+  const std::string m(model ? model : "");
+  scheduling::Status st = n == 0 ? s->sched->ScheduleModelAffinity(m, key, &target, &pods[0])
+                                 : s->sched->ScheduleModelAffinityWithFallbacks(m, key, n, &target, &pods);
+  if (!st.ok()) pods.clear();
+  put(resolved, resolved_cap, target);
+  std::string joined;
+  for (size_t i = 0; i < pods.size(); ++i) joined += (i ? "\n" : "") + pods[i].Name;
+  if (n_pods) *n_pods = (int)pods.size();
+  put(names, names_cap, joined);
+  if (!st.ok()) put(err, err_cap, st.message);
+  return st.code;
+}
+
+uint64_t ligh_affinity_scheduled(ligh_scheduler* s) { return s->sched->stats().affinity_scheduled; }
+
+uint64_t ligh_pod_key(const char* name, const char* address) {
+  return scheduling::PodKey(backend::Pod{name ? name : "", address ? address : ""});
+}
 
 int ligh_schedule_model_retry(ligh_scheduler* s, const char* model, const char* resolved,
                               const char* const* tried_names, const char* const* tried_addrs, int n_tried, char* name,

@@ -48,6 +48,15 @@ ligh_scheduler* ligh_scheduler_new_feedback(ligh_provider*, int device, const in
                                             int busy_poll, int caller_spin_us, int use_doorbell,
                                             const lig_filter_node* nodes, int n_nodes, int load_feedback_window,
                                             int feedback_fallbacks, int feedback_retries, char* err, int err_cap);
+/* ligh_scheduler_new_feedback plus Options::affinity (nonzero: every published epoch carries the pods'
+ * keys, and ligh_schedule_affinity / ligh_schedule_model_affinity are served). */
+ligh_scheduler* ligh_scheduler_new_affinity(ligh_provider*, int device, const int* devices, int n_devices,
+                                            int max_pods, int max_adapters, int max_batch, int flush_size,
+                                            int batch_window_us, int refresh_interval_ms, uint64_t seed,
+                                            int busy_poll, int caller_spin_us, int use_doorbell,
+                                            const lig_filter_node* nodes, int n_nodes, int load_feedback_window,
+                                            int feedback_fallbacks, int feedback_retries, int affinity, char* err,
+                                            int err_cap);
 void ligh_scheduler_free(ligh_scheduler*);
 /* Scheduler.Schedule: returns the gRPC code (0 OK, 8 ResourceExhausted, 2 Unknown, 13 Internal). */
 int ligh_schedule(ligh_scheduler*, const char* model, const char* resolved_target_model, int critical,
@@ -73,6 +82,16 @@ int ligh_schedule_retry_with_fallbacks(ligh_scheduler*, const char* resolved_tar
                                        const char* const* tried_names, const char* const* tried_addrs, int n_tried,
                                        int n, char* names, int names_cap, int* n_pods, char* err, int err_cap);
 uint64_t ligh_retry_scheduled(ligh_scheduler*);      /* Stats::retry_scheduled */
+/* Scheduler::ScheduleAffinity (n = 0) or ScheduleAffinityWithFallbacks (n fallbacks): returns the gRPC
+ * code; names receives the pick and then the row's pods' names joined by '\n' and *n_pods their count. */
+int ligh_schedule_affinity(ligh_scheduler*, const char* resolved_target_model, int critical, uint64_t key, int n,
+                           char* names, int names_cap, int* n_pods, char* err, int err_cap);
+/* Scheduler::ScheduleModelAffinity[WithFallbacks], as ligh_schedule_affinity; resolved receives the
+ * resolved target model. */
+int ligh_schedule_model_affinity(ligh_scheduler*, const char* model, uint64_t key, int n, char* resolved,
+                                 int resolved_cap, char* names, int names_cap, int* n_pods, char* err, int err_cap);
+uint64_t ligh_affinity_scheduled(ligh_scheduler*);   /* Stats::affinity_scheduled */
+uint64_t ligh_pod_key(const char* name, const char* address);   /* scheduling::PodKey */
 /* Scheduler::ScheduleModelRetry: returns the gRPC code; resolved_target_model is the name the model call
  * returned; the tried pods as ligh_schedule_retry's. */
 int ligh_schedule_model_retry(ligh_scheduler*, const char* model, const char* resolved_target_model,

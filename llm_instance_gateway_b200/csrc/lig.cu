@@ -99,6 +99,11 @@ struct Slot {
   uint32_t mtab_bytes = 0, n_models = 0;
   bool models_valid = false;
   cudaEvent_t models_ready = nullptr;
+  // pod keys of this epoch (lig_upload_pod_keys): h[p] = mix(pod_key[p]), max_pods entries
+  uint64_t* d_podkeys = nullptr;
+  uint64_t* h_podkeys = nullptr;    // pinned staging
+  bool keys_valid = false;
+  cudaEvent_t keys_ready = nullptr;
   cudaEvent_t ready = nullptr;      // class tables built
   // Batches that read this slot, possibly on different caller streams: a ring of events, one per
   // schedule call.  A writer (re-upload, threshold rebuild) waits on every event of the ring; when
@@ -893,6 +898,7 @@ int begin_write(lig_ctx* c, uint64_t epoch, int P, int A, cudaStream_t stream, b
     Slot& s = victim_slot(c, epoch);
     s.valid = false;                       // evicted: schedule calls on its old epoch now get STALE_EPOCH
     s.models_valid = false;                // the model table is interned against the old snapshot
+    s.keys_valid = false;                  // and the pod keys name the old snapshot's pods
     s.n_ejected = 0;                       // full uploads start with every pod; lig_update_snapshot and
                                            // lig_eject_pods set the set after begin_write
     rc = wait_readers(s, st);              // batches still reading the old content
@@ -1036,6 +1042,9 @@ static int alloc_slot(lig_ctx* c, Slot& s) {
   CUDA_TRY(cudaHostAlloc(&s.h_blob, l.total, cudaHostAllocDefault));
   CUDA_TRY(cudaEventCreateWithFlags(&s.ready, cudaEventDisableTiming));
   CUDA_TRY(cudaEventCreateWithFlags(&s.models_ready, cudaEventDisableTiming));
+  CUDA_TRY(cudaMalloc(&s.d_podkeys, (size_t)c->max_pods * sizeof(uint64_t)));
+  CUDA_TRY(cudaHostAlloc(&s.h_podkeys, (size_t)c->max_pods * sizeof(uint64_t), cudaHostAllocDefault));
+  CUDA_TRY(cudaEventCreateWithFlags(&s.keys_ready, cudaEventDisableTiming));
   for (auto& ev : s.readers) CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
   return 0;
 }
@@ -1050,6 +1059,9 @@ static void free_slot(Slot& s) {
   cudaFree(s.d_mtab);
   if (s.h_mtab) cudaFreeHost(s.h_mtab);
   if (s.models_ready) cudaEventDestroy(s.models_ready);
+  cudaFree(s.d_podkeys);
+  if (s.h_podkeys) cudaFreeHost(s.h_podkeys);
+  if (s.keys_ready) cudaEventDestroy(s.keys_ready);
   if (s.h_hdr) cudaFreeHost(s.h_hdr);
   cudaFreeHost(s.h_blob);
   if (s.ready) cudaEventDestroy(s.ready);
@@ -1215,6 +1227,7 @@ static int create_impl(lig_ctx* c, int device, int max_pods, int max_adapters, i
         (const void*)lig_pick_fallback_kernel<false, false>, (const void*)lig_pick_fallback_kernel<true, false>,
         (const void*)lig_pick_fallback_kernel<false, true>, (const void*)lig_pick_fallback_kernel<true, true>,
         (const void*)lig_filter_kernel<false>,   (const void*)lig_filter_kernel<true>,
+        (const void*)lig_pick_affinity_kernel<false>, (const void*)lig_pick_affinity_kernel<true>,
     };
     for (const void* fn : fns) CUDA_TRY(cudaFuncGetAttributes(&fa, fn));
   }
@@ -1892,6 +1905,38 @@ static int resolve_models_slot(lig_ctx* c, uint64_t epoch, Slot** out) {
   return 0;
 }
 
+int lig_upload_pod_keys(lig_ctx* c, uint64_t epoch, int P, const uint64_t* keys) {
+  if (!c) return fail(LIG_ERR_INVALID, "lig_upload_pod_keys: bad argument");
+  std::lock_guard<std::mutex> uk(c->upload_mu);
+  CUDA_TRY(cudaSetDevice(c->device));
+  Slot* s = nullptr;
+  {
+    std::lock_guard<std::mutex> lk(c->mu);
+    if (int rc = resolve_slot(c, epoch, &s)) return rc;
+    if (P != s->P)
+      return fail(LIG_ERR_INVALID, "lig_upload_pod_keys: P=%d, epoch %llu has P=%d", P, (unsigned long long)epoch,
+                  s->P);
+    if (P > 0 && !keys) return fail(LIG_ERR_INVALID, "lig_upload_pod_keys: keys is null with P=%d", P);
+    s->keys_valid = false;
+    if (int rc = wait_readers(*s, c->s_up)) return rc;      // batches still reading the old keys
+  }
+  CUDA_TRY(cudaEventSynchronize(s->keys_ready));   // an earlier upload may still read the staging copy
+  for (int p = 0; p < P; ++p) {
+    uint64_t z = keys[p];
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    s->h_podkeys[p] = z ^ (z >> 31);
+  }
+  if (P > 0)
+    CUDA_TRY(cudaMemcpyAsync(s->d_podkeys, s->h_podkeys, (size_t)P * sizeof(uint64_t), cudaMemcpyHostToDevice, c->s_up));
+  CUDA_TRY(cudaEventRecord(s->keys_ready, c->s_up));
+  {
+    std::lock_guard<std::mutex> lk(c->mu);
+    s->keys_valid = s->valid && s->epoch == epoch;
+  }
+  return 0;
+}
+
 int lig_schedule_models_batches_device(lig_ctx* c, uint64_t epoch, uint64_t seed, uint64_t first_index,
                                        const uint32_t* const* d_ids, int R, lig_mpick* const* d_out,
                                        int n_batches, void* stream) {
@@ -2158,6 +2203,7 @@ int lig_filter_models_batch_device(lig_ctx* c, uint64_t epoch, uint64_t seed, ui
 }
 
 // ---- fallback endpoints (lig_schedule_batch_fallbacks, lig_schedule_models_batch_fallbacks) ----------
+// and the session-affinity calls (lig_schedule_[models_]batch_affinity), which share their staging.
 struct FallbackCall {
   bool models;
   uint64_t seed, first_index;
@@ -2166,16 +2212,34 @@ struct FallbackCall {
   void* out;
   int n_fallbacks;
   int16_t* fallbacks;
+  // affinity: no seed, no first_index; keys (model ids only) are the requests' affinity keys, and
+  // n_fallbacks = 0 means no row (fallbacks may then be null)
+  bool affinity = false;
+  const uint64_t* keys = nullptr;
   size_t in_bytes() const { return models ? sizeof(uint32_t) : sizeof(lig_req); }
   size_t out_bytes() const { return models ? sizeof(lig_mpick) : sizeof(lig_pick); }
   size_t row_bytes() const { return (size_t)n_fallbacks * sizeof(int16_t); }
+  bool has_keys() const { return affinity && models; }
+  bool has_rows() const { return n_fallbacks > 0; }
 };
 
 static int fallback_check(const lig_ctx* c, const char* fn, const FallbackCall& f) {
-  if (!c || f.R < 0 || (f.R > 0 && (!f.in || !f.out || !f.fallbacks)))
+  if (!c || f.R < 0 ||
+      (f.R > 0 && (!f.in || !f.out || (!f.fallbacks && (!f.affinity || f.has_rows())) || (f.has_keys() && !f.keys))))
     return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
-  if (f.n_fallbacks < 1 || f.n_fallbacks > LIG_MAX_FALLBACKS)
-    return fail(LIG_ERR_INVALID, "%s: n_fallbacks=%d outside [1, %d]", fn, f.n_fallbacks, LIG_MAX_FALLBACKS);
+  const int lo = f.affinity ? 0 : 1;
+  if (f.n_fallbacks < lo || f.n_fallbacks > LIG_MAX_FALLBACKS)
+    return fail(LIG_ERR_INVALID, "%s: n_fallbacks=%d outside [%d, %d]", fn, f.n_fallbacks, lo, LIG_MAX_FALLBACKS);
+  return 0;
+}
+
+// The slot a fallback or affinity call reads: the model forms need the epoch's model table, the
+// affinity forms its pod keys.  Caller holds c->mu.
+static int fallback_slot(lig_ctx* c, uint64_t epoch, const FallbackCall& f, Slot** s) {
+  if (int rc = f.models ? resolve_models_slot(c, epoch, s) : resolve_slot(c, epoch, s)) return rc;
+  if (f.affinity && !(*s)->keys_valid)
+    return fail(LIG_ERR_NO_SNAPSHOT, "no pod keys uploaded for epoch %llu (lig_upload_pod_keys)",
+                (unsigned long long)epoch);
   return 0;
 }
 
@@ -2188,7 +2252,17 @@ static int enqueue_fallbacks(lig_ctx* c, Slot& s, const FallbackCall& f, cudaStr
   if (f.models) CUDA_TRY(cudaStreamWaitEvent(st, s.models_ready, 0));
   const int blocks = (f.R + kFallbackThreads - 1) / kFallbackThreads;
   const uint4* cls = reinterpret_cast<const uint4*>(s.d_cls);
-  if (f.models)
+  if (f.affinity) {
+    CUDA_TRY(cudaStreamWaitEvent(st, s.keys_ready, 0));
+    if (f.models)
+      lig_pick_affinity_kernel<true><<<blocks, kFallbackThreads, 0, st>>>(
+          f.in, f.keys, f.out, f.fallbacks, f.R, f.n_fallbacks, cls, s.d_lists, s.A, s.d_ctab, s.d_mtab, s.n_models,
+          s.d_podkeys);
+    else
+      lig_pick_affinity_kernel<false><<<blocks, kFallbackThreads, 0, st>>>(
+          f.in, nullptr, f.out, f.fallbacks, f.R, f.n_fallbacks, cls, s.d_lists, s.A, s.d_ctab, nullptr, 0u,
+          s.d_podkeys);
+  } else if (f.models)
     lig_pick_fallback_kernel<true, false><<<blocks, kFallbackThreads, 0, st>>>(
         f.in, f.out, f.fallbacks, f.R, f.n_fallbacks, cls, s.d_lists, s.A, s.d_ctab, s.d_mtab, s.n_models, f.seed,
         f.first_index, nullptr);
@@ -2203,11 +2277,11 @@ static int enqueue_fallbacks(lig_ctx* c, Slot& s, const FallbackCall& f, cudaStr
 static int fallback_device(lig_ctx* c, const char* fn, uint64_t epoch, const FallbackCall& f, void* stream) {
   if (int rc = fallback_check(c, fn, f)) return rc;
   if (f.R > 0 && (misaligned(f.in, f.in_bytes()) || misaligned(f.out, f.out_bytes()) ||
-                  misaligned(f.fallbacks, sizeof(int16_t))))
+                  misaligned(f.fallbacks, sizeof(int16_t)) || misaligned(f.keys, sizeof(uint64_t))))
     return fail(LIG_ERR_INVALID, "%s: a device buffer is not aligned to its element", fn);
   std::lock_guard<std::mutex> lk(c->mu);
   Slot* s = nullptr;
-  if (int rc = f.models ? resolve_models_slot(c, epoch, &s) : resolve_slot(c, epoch, &s)) return rc;
+  if (int rc = fallback_slot(c, epoch, f, &s)) return rc;
   if (f.R == 0) return 0;
   CUDA_TRY(cudaSetDevice(c->device));
   return enqueue_fallbacks(c, *s, f, static_cast<cudaStream_t>(stream));
@@ -2220,38 +2294,45 @@ static int fallback_host(lig_ctx* c, const char* fn, uint64_t epoch, const Fallb
   if (f.R > c->max_batch) return fail(LIG_ERR_INVALID, "%s: R=%d exceeds max_batch=%d", fn, f.R, c->max_batch);
   FallbackCall d = f;    // the same call with device-visible pointers
   const size_t in_b = (size_t)f.R * f.in_bytes(), out_b = (size_t)f.R * f.out_bytes();
-  const size_t rows_b = (size_t)f.R * f.row_bytes();
+  const size_t rows_b = (size_t)f.R * f.row_bytes(), keys_b = (size_t)f.R * sizeof(uint64_t);
   d.in = f.R ? mapped_device_pointer(f.in) : nullptr;
   d.out = f.R ? mapped_device_pointer(f.out) : nullptr;
-  d.fallbacks = f.R ? mapped_device_pointer(f.fallbacks) : nullptr;
+  d.fallbacks = f.R && f.has_rows() ? mapped_device_pointer(f.fallbacks) : nullptr;
+  d.keys = f.R && f.has_keys() ? mapped_device_pointer(f.keys) : nullptr;
   // the kernel reads a descriptor with one 16-byte load and stores every element whole
   const bool st_in = f.R && (!d.in || misaligned(d.in, f.in_bytes()));
   const bool st_out = f.R && (!d.out || misaligned(d.out, f.out_bytes()));
-  const bool st_rows = f.R && (!d.fallbacks || misaligned(d.fallbacks, sizeof(int16_t)));
+  const bool st_rows = f.R && f.has_rows() && (!d.fallbacks || misaligned(d.fallbacks, sizeof(int16_t)));
+  const bool st_keys = f.R && f.has_keys() && (!d.keys || misaligned(d.keys, sizeof(uint64_t)));
   cudaStream_t st = nullptr;
   unsigned char* stage = nullptr;
   {
     std::lock_guard<std::mutex> lk(c->mu);
     Slot* s = nullptr;
-    if (int rc = f.models ? resolve_models_slot(c, epoch, &s) : resolve_slot(c, epoch, &s)) return rc;
+    if (int rc = fallback_slot(c, epoch, f, &s)) return rc;
     if (f.R == 0) return 0;
     CUDA_TRY(cudaSetDevice(c->device));
     st = c->s_lane[c->next_lane];
     c->next_lane = (c->next_lane + 1) % kLanes;
-    size_t at = 0, o_in = 0, o_out = 0, o_rows = 0;
+    size_t at = 0, o_in = 0, o_out = 0, o_rows = 0, o_keys = 0;
     auto take = [&](bool on, size_t bytes, size_t* o) { if (on) { *o = at; at = (at + bytes + 255) & ~(size_t)255; } };
     take(st_in, in_b, &o_in);
     take(st_out, out_b, &o_out);
     take(st_rows, rows_b, &o_rows);
+    take(st_keys, keys_b, &o_keys);
     if (at) {
       CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&stage), at, st));
       if (st_in) d.in = stage + o_in;
       if (st_out) d.out = stage + o_out;
       if (st_rows) d.fallbacks = reinterpret_cast<int16_t*>(stage + o_rows);
+      if (st_keys) d.keys = reinterpret_cast<const uint64_t*>(stage + o_keys);
     }
     int rc = 0;
     if (st_in && cudaMemcpyAsync(const_cast<void*>(d.in), f.in, in_b, cudaMemcpyHostToDevice, st) != cudaSuccess)
       rc = fail(LIG_ERR_CUDA, "%s: staging the requests failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
+    if (!rc && st_keys &&
+        cudaMemcpyAsync(const_cast<uint64_t*>(d.keys), f.keys, keys_b, cudaMemcpyHostToDevice, st) != cudaSuccess)
+      rc = fail(LIG_ERR_CUDA, "%s: staging the keys failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
     if (!rc) rc = enqueue_fallbacks(c, *s, d, st);
     if (rc) {
       if (stage) cudaFreeAsync(stage, st);
@@ -2293,6 +2374,37 @@ int lig_schedule_models_batch_fallbacks_device(lig_ctx* c, uint64_t epoch, uint6
   return fallback_device(c, "lig_schedule_models_batch_fallbacks_device", epoch,
                          FallbackCall{true, seed, first_index, d_model_ids, R, d_out, n_fallbacks, d_fallbacks},
                          stream);
+}
+
+int lig_schedule_batch_affinity(lig_ctx* c, uint64_t epoch, const lig_req* reqs, int R, lig_pick* out,
+                                int n_fallbacks, int16_t* fallbacks) {
+  FallbackCall f{false, 0, 0, reqs, R, out, n_fallbacks, fallbacks};
+  f.affinity = true;
+  return fallback_host(c, "lig_schedule_batch_affinity", epoch, f);
+}
+
+int lig_schedule_batch_affinity_device(lig_ctx* c, uint64_t epoch, const lig_req* d_reqs, int R, lig_pick* d_out,
+                                       int n_fallbacks, int16_t* d_fallbacks, void* stream) {
+  FallbackCall f{false, 0, 0, d_reqs, R, d_out, n_fallbacks, d_fallbacks};
+  f.affinity = true;
+  return fallback_device(c, "lig_schedule_batch_affinity_device", epoch, f, stream);
+}
+
+int lig_schedule_models_batch_affinity(lig_ctx* c, uint64_t epoch, const uint32_t* model_ids, const uint64_t* keys,
+                                       int R, lig_mpick* out, int n_fallbacks, int16_t* fallbacks) {
+  FallbackCall f{true, 0, 0, model_ids, R, out, n_fallbacks, fallbacks};
+  f.affinity = true;
+  f.keys = keys;
+  return fallback_host(c, "lig_schedule_models_batch_affinity", epoch, f);
+}
+
+int lig_schedule_models_batch_affinity_device(lig_ctx* c, uint64_t epoch, const uint32_t* d_model_ids,
+                                              const uint64_t* d_keys, int R, lig_mpick* d_out, int n_fallbacks,
+                                              int16_t* d_fallbacks, void* stream) {
+  FallbackCall f{true, 0, 0, d_model_ids, R, d_out, n_fallbacks, d_fallbacks};
+  f.affinity = true;
+  f.keys = d_keys;
+  return fallback_device(c, "lig_schedule_models_batch_affinity_device", epoch, f, stream);
 }
 
 // ---- retry scheduling (lig_schedule_[models_]batch_excluding[_fallbacks]) -----------------------------

@@ -1464,16 +1464,21 @@ __global__ void lig_apply_delta_kernel(DeltaView d, double* __restrict__ kv, int
 // contiguous bytes and every store 256.  All loads of a thread are issued before the first use.
 constexpr int kPickThreads = 256;
 
+// The class entry {info, magic, q_limit, list_off} of descriptor r (the pick's class lookup).
+__device__ __forceinline__ uint4 class_entry(const int4 r, const uint4* __restrict__ cls, uint32_t A) {
+  const uint32_t critical = (uint32_t)r.y & LIG_REQ_CRITICAL;
+  const uint32_t a = min((uint32_t)r.x, A);          // ids outside [0, A) (negative too) -> A
+  const uint32_t c = critical * (A + 1u) + a;
+  return __ldg(cls + c);
+}
+
 // `entry` (nullable) receives the class entry the pick used: the survivor-list kernel copies the
 // class's list from it.  Every other caller passes nothing and compiles as without it.
 __device__ __forceinline__ int2 pick_one(const int4 r, const uint4* __restrict__ cls,
                                          const uint16_t* __restrict__ lists, uint32_t A,
                                          uint64_t seed, uint4* entry = nullptr) {
-  const uint32_t critical = (uint32_t)r.y & LIG_REQ_CRITICAL;
+  const uint4 e = class_entry(r, cls, A);
   const uint64_t key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
-  const uint32_t a = min((uint32_t)r.x, A);          // ids outside [0, A) (negative too) -> A
-  const uint32_t c = critical * (A + 1u) + a;
-  const uint4 e = __ldg(cls + c);                    // {info, magic, q_limit, list_off}
   if (entry) *entry = e;
   const uint32_t k = int31n_entry(seed ^ key, e);
   // n == 0: list_off is the pool's 0xffff sentinel -> -1
@@ -2616,6 +2621,17 @@ __device__ __forceinline__ void write_fallback_row(uint64_t state, const uint4 e
   }
 }
 
+// The compact pool when the build sealed one for this epoch's A, else the strided rows as given.
+__device__ __forceinline__ void sealed_tables(const unsigned char* __restrict__ ctab, int A, const uint4** gcls,
+                                              const uint16_t** glists) {
+  const CompactHeader hdr = *reinterpret_cast<const CompactHeader*>(ctab);
+  const uint32_t n_classes = 2u * ((uint32_t)A + 1u);
+  if (hdr.bytes != 0u && hdr.n_classes == n_classes) {
+    *gcls = reinterpret_cast<const uint4*>(ctab + sizeof(CompactHeader));
+    *glists = reinterpret_cast<const uint16_t*>(ctab + sizeof(CompactHeader) + (size_t)n_classes * sizeof(ClassEntry));
+  }
+}
+
 // kCount: the chain segment of lig_schedule_[models_]batch_feedback_chain_fallbacks.  The same pick
 // and row on the chain's private tables (always the strided rows, as the count kernels read them),
 // and the pick counted into the open window like lig_pick_[models_]count_kernel.  Row entries are
@@ -2630,14 +2646,7 @@ lig_pick_fallback_kernel(const void* __restrict__ in, void* __restrict__ out, in
   if (!kCount && i >= R) return;
   const uint4* gcls = cls;
   const uint16_t* glists = lists;
-  if constexpr (!kCount) {
-    const CompactHeader hdr = *reinterpret_cast<const CompactHeader*>(ctab);
-    const uint32_t n_classes = 2u * ((uint32_t)A + 1u);
-    if (hdr.bytes != 0u && hdr.n_classes == n_classes) {
-      gcls = reinterpret_cast<const uint4*>(ctab + sizeof(CompactHeader));
-      glists = reinterpret_cast<const uint16_t*>(ctab + sizeof(CompactHeader) + (size_t)n_classes * sizeof(ClassEntry));
-    }
-  }
+  if constexpr (!kCount) sealed_tables(ctab, A, &gcls, &glists);
   int pod = -1;
   if (i < R) {
     uint4 e = make_uint4(0u, 0u, 0u, 0u);
@@ -2665,6 +2674,136 @@ lig_pick_fallback_kernel(const void* __restrict__ in, void* __restrict__ out, in
     write_fallback_row(seed ^ key, e, ok, n_fallbacks, glists, fallbacks + (size_t)i * (size_t)n_fallbacks);
   }
   if constexpr (kCount) count_window_picks(pod, (int)threadIdx.x & 31, hist);
+}
+
+// ---- K2j: session affinity (lig_schedule_[models_]batch_affinity; definition in include/lig.h) -----
+// The class lookup and model resolve of the fallback kernel; only the selection differs.  A survivor
+// p of the request's list scores mix(key ^ h[p]), h[p] = mix(pod_key[p]) (the slot's key table), and
+// ranked entry j is the (j+1)-th in descending (score, ascending pod) order: pass j takes the largest
+// pair below pass j-1's, so a row needs no sort and no per-thread storage.  Lists of up to
+// kAffinityShortList pods are scored by their own thread; longer ones (caller trees of predicate
+// nodes, KV ties) are found with a ballot and served one at a time by the whole warp, strided scoring
+// and a __shfl_xor max-reduce per rank.  One thread per request, plain loads and stores (`in`, `keys`,
+// `out` and `fallbacks` may be page-locked host memory); `fallbacks` is null when n_fallbacks = 0.
+constexpr int kAffinityShortList = 32;
+
+__device__ __forceinline__ uint64_t affinity_mix(uint64_t z) {
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+// (s, p) ranks before (bs, bp): a higher score, or an equal score (equal pod keys) and a lower pod.
+__device__ __forceinline__ bool ranks_before(uint64_t s, int p, uint64_t bs, int bp) {
+  return s > bs || (s == bs && p < bp);
+}
+
+template <bool kModels>
+__global__ void __launch_bounds__(kFallbackThreads)
+lig_pick_affinity_kernel(const void* __restrict__ in, const uint64_t* __restrict__ keys, void* __restrict__ out,
+                         int16_t* __restrict__ fallbacks, int R, int n_fallbacks, const uint4* __restrict__ cls,
+                         const uint16_t* __restrict__ lists, int A, const unsigned char* __restrict__ ctab,
+                         const unsigned char* __restrict__ mtab, uint32_t n_models,
+                         const uint64_t* __restrict__ hkeys) {
+  const int i = (int)blockIdx.x * kFallbackThreads + (int)threadIdx.x;
+  const int lane = (int)threadIdx.x & 31;
+  const uint4* gcls = cls;
+  const uint16_t* glists = lists;
+  sealed_tables(ctab, A, &gcls, &glists);
+  uint4 e = make_uint4(0u, 0u, 0u, 0u);
+  uint64_t key = 0;
+  bool resolved = false;
+  uint32_t target = 255u;
+  if (i < R) {
+    if constexpr (kModels) {
+      ModelTables mt;
+      mt.entries = reinterpret_cast<const uint4*>(mtab + sizeof(ModelHeader));
+      mt.targets = reinterpret_cast<const uint2*>(mt.entries + n_models);
+      mt.n_models = n_models;
+      key = keys[i];
+      uint32_t adapter, critical;
+      // the draw state is seed ^ key ^ LIG_DRAW_DOMAIN with seed 0: key ^ LIG_DRAW_DOMAIN
+      resolved = resolve_model<Ld::kLdg>(static_cast<const uint32_t*>(in)[i], mt, 0, key, &adapter, &critical,
+                                         &target);
+      if (resolved) e = class_entry(make_int4((int)adapter, (int)critical, 0, 0), gcls, (uint32_t)A);
+    } else {
+      const int4 r = ld_stream_int4(static_cast<const int4*>(in) + i);
+      key = ((uint64_t)(uint32_t)r.w << 32) | (uint32_t)r.z;
+      e = class_entry(r, gcls, (uint32_t)A);
+      resolved = true;
+    }
+  }
+  const bool ok = resolved && (e.x & 7u) == (uint32_t)LIG_OK;
+  const uint32_t n = ok ? e.x >> 16 : 0u;
+  const uint32_t m = min(n, (uint32_t)n_fallbacks + 1u);   // ranked entries, the pick included
+  const uint16_t* list = glists + e.w;
+  int16_t* row = fallbacks ? fallbacks + (size_t)i * (size_t)n_fallbacks : nullptr;
+  int pod = -1;
+  if (n <= (uint32_t)kAffinityShortList) {
+    uint64_t ps = ~0ull;   // pass j-1's pair; (2^64-1, -1) ranks before every pair
+    int pp = -1;
+    for (uint32_t j = 0; j < m; ++j) {
+      uint64_t bs = 0;
+      int bp = 0x7fffffff;   // (0, INT_MAX) ranks after every pair
+      for (uint32_t t = 0; t < n; ++t) {
+        const int p = (int)__ldg(list + t);
+        const uint64_t s = affinity_mix(key ^ __ldg(hkeys + p));
+        if (ranks_before(ps, pp, s, p) && ranks_before(s, p, bs, bp)) {
+          bs = s;
+          bp = p;
+        }
+      }
+      if (j == 0) pod = bp; else row[j - 1] = (int16_t)bp;
+      ps = bs;
+      pp = bp;
+    }
+  }
+  // long lists: the warp serves each in turn (lanes past R take part with n = 0)
+  unsigned pending = __ballot_sync(0xffffffffu, n > (uint32_t)kAffinityShortList);
+  while (pending) {
+    const int src = __ffs(pending) - 1;
+    pending &= pending - 1u;
+    const uint64_t k = __shfl_sync(0xffffffffu, key, src);
+    const uint32_t off = __shfl_sync(0xffffffffu, e.w, src);
+    const uint32_t nn = __shfl_sync(0xffffffffu, n, src);
+    const uint32_t mm = __shfl_sync(0xffffffffu, m, src);
+    uint64_t ps = ~0ull;
+    int pp = -1;
+    for (uint32_t j = 0; j < mm; ++j) {
+      uint64_t bs = 0;
+      int bp = 0x7fffffff;
+      for (uint32_t t = (uint32_t)lane; t < nn; t += 32u) {
+        const int p = (int)__ldg(glists + off + t);
+        const uint64_t s = affinity_mix(k ^ __ldg(hkeys + p));
+        if (ranks_before(ps, pp, s, p) && ranks_before(s, p, bs, bp)) {
+          bs = s;
+          bp = p;
+        }
+      }
+#pragma unroll
+      for (int d = 16; d >= 1; d >>= 1) {
+        const uint64_t os = __shfl_xor_sync(0xffffffffu, bs, d);
+        const int op = __shfl_xor_sync(0xffffffffu, bp, d);
+        if (ranks_before(os, op, bs, bp)) {
+          bs = os;
+          bp = op;
+        }
+      }
+      if (lane == src) {
+        if (j == 0) pod = bp; else row[j - 1] = (int16_t)bp;
+      }
+      ps = bs;
+      pp = bp;
+    }
+  }
+  if (i >= R) return;
+  for (int j = (int)max(m, 1u); j <= n_fallbacks; ++j) row[j - 1] = -1;
+  if constexpr (kModels) {
+    const uint32_t status = resolved ? e.x & 7u : (uint32_t)LIG_NO_MODEL;
+    static_cast<uint32_t*>(out)[i] = pack_mpick(pod, status, resolved ? target : 255u);
+  } else {
+    st_stream_int2(static_cast<int2*>(out) + i, make_int2(pod, (int)(e.x & 0xffff0007u)));
+  }
 }
 
 // loads[p] = picks of the closed windows + picks of the open one (the chain's per-pod loads).

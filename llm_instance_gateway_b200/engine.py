@@ -301,6 +301,59 @@ class Engine:
         N.check(self._lib.lig_schedule_batch_fallbacks_device(self._ctx, epoch, seed, d_reqs or None, R,
                                                               d_out or None, n, d_fallbacks or None, stream or None))
 
+    # ---- session affinity: rendezvous hashing of a caller key over the survivors ----
+    def upload_pod_keys(self, epoch: int, keys) -> None:
+        """lig_upload_pod_keys: one stable uint64 identity per pod of `epoch`, in its pod order."""
+        k = np.ascontiguousarray(keys, dtype=np.uint64)
+        N.check(self._lib.lig_upload_pod_keys(self._ctx, epoch, len(k), _ptr(k)))
+
+    def schedule_batch_affinity(self, epoch: int, reqs: np.ndarray, n: int = 0):
+        """lig_schedule_batch_affinity: (picks, int16 fallbacks of shape (R, n)); rand_key is the affinity
+        key, status and n_survivors are schedule_batch's, pod_idx the survivor with the highest score."""
+        assert reqs.dtype == REQ_DTYPE and reqs.flags.c_contiguous
+        R = int(reqs.shape[0])
+        out = np.empty(R, dtype=PICK_DTYPE)
+        rows = np.empty((R, max(n, 0)), dtype=np.int16)
+        N.check(self._lib.lig_schedule_batch_affinity(self._ctx, epoch, _ptr(reqs), R, _ptr(out), n,
+                                                      _ptr(rows) if n > 0 else None))
+        return out, rows
+
+    def schedule_batch_affinity_ptr(self, epoch: int, h_reqs: int, R: int, h_out: int, n: int,
+                                    h_fallbacks: int) -> None:
+        N.check(self._lib.lig_schedule_batch_affinity(self._ctx, epoch, h_reqs or None, R, h_out or None, n,
+                                                      h_fallbacks or None))
+
+    def schedule_batch_affinity_device(self, epoch: int, d_reqs: int, R: int, d_out: int, n: int,
+                                       d_fallbacks: int, stream: int = 0) -> None:
+        """Device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_batch_affinity_device(self._ctx, epoch, d_reqs or None, R, d_out or None, n,
+                                                             d_fallbacks or None, stream or None))
+
+    def schedule_models_batch_affinity(self, epoch: int, model_ids: np.ndarray, keys: np.ndarray, n: int = 0):
+        """lig_schedule_models_batch_affinity: (picks, int16 fallbacks (R, n)); request i is model_ids[i]
+        with affinity key keys[i], its target drawn on the state keys[i] ^ LIG_DRAW_DOMAIN."""
+        assert model_ids.dtype == np.uint32 and model_ids.flags.c_contiguous
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        R = int(model_ids.shape[0])
+        assert keys.shape == (R,)
+        out = np.empty(R, dtype=MPICK_DTYPE)
+        rows = np.empty((R, max(n, 0)), dtype=np.int16)
+        N.check(self._lib.lig_schedule_models_batch_affinity(self._ctx, epoch, _ptr(model_ids), _ptr(keys), R,
+                                                             _ptr(out), n, _ptr(rows) if n > 0 else None))
+        return out, rows
+
+    def schedule_models_batch_affinity_ptr(self, epoch: int, h_ids: int, h_keys: int, R: int, h_out: int, n: int,
+                                           h_fallbacks: int) -> None:
+        N.check(self._lib.lig_schedule_models_batch_affinity(self._ctx, epoch, h_ids or None, h_keys or None, R,
+                                                             h_out or None, n, h_fallbacks or None))
+
+    def schedule_models_batch_affinity_device(self, epoch: int, d_ids: int, d_keys: int, R: int, d_out: int, n: int,
+                                              d_fallbacks: int, stream: int = 0) -> None:
+        """The model-id form with device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_models_batch_affinity_device(self._ctx, epoch, d_ids or None, d_keys or None,
+                                                                    R, d_out or None, n, d_fallbacks or None,
+                                                                    stream or None))
+
     # ---- retry scheduling: the tree again over each request's pool without the pods it excludes ----
     def schedule_batch_excluding(self, epoch: int, seed: int, reqs: np.ndarray, excluded: np.ndarray) -> np.ndarray:
         """lig_schedule_batch_excluding: excluded is an int16 array of shape (R, n_excluded) of pod indices

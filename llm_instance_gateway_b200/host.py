@@ -32,6 +32,8 @@ EXPORTED_SYMBOLS = (
     "ligh_schedule_retry", "ligh_retry_scheduled", "ligh_schedule_retry_with_fallbacks",
     "ligh_schedule_model_retry", "ligh_schedule_model_retry_with_fallbacks",
     "ligh_eject_pods", "ligh_eject_stats",
+    "ligh_scheduler_new_affinity", "ligh_schedule_affinity", "ligh_schedule_model_affinity", "ligh_affinity_scheduled",
+    "ligh_pod_key",
 )
 
 _lib = None
@@ -62,6 +64,17 @@ def load() -> C.CDLL:
     lib.ligh_scheduler_new_feedback.argtypes = [vp, i32, C.POINTER(i32), i32, i32, i32, i32, i32, i32, i32, u64, i32,
                                                 i32, i32, vp, i32, i32, i32, i32, C.c_char_p, i32]
     lib.ligh_scheduler_new_feedback.restype = vp
+    lib.ligh_scheduler_new_affinity.argtypes = [vp, i32, C.POINTER(i32), i32, i32, i32, i32, i32, i32, i32, u64, i32,
+                                                i32, i32, vp, i32, i32, i32, i32, i32, C.c_char_p, i32]
+    lib.ligh_scheduler_new_affinity.restype = vp
+    lib.ligh_schedule_affinity.argtypes = [vp, C.c_char_p, i32, u64, i32, C.c_char_p, i32, C.POINTER(i32),
+                                           C.c_char_p, i32]
+    lib.ligh_schedule_model_affinity.argtypes = [vp, C.c_char_p, u64, i32, C.c_char_p, i32, C.c_char_p, i32,
+                                                 C.POINTER(i32), C.c_char_p, i32]
+    lib.ligh_affinity_scheduled.argtypes = [vp]
+    lib.ligh_affinity_scheduled.restype = u64
+    lib.ligh_pod_key.argtypes = [C.c_char_p, C.c_char_p]
+    lib.ligh_pod_key.restype = u64
     lib.ligh_feedback_stats.argtypes = [vp, vp]
     lib.ligh_feedback_stats.restype = None
     lib.ligh_datastore_new.restype = vp
@@ -163,25 +176,26 @@ class HostScheduler:
                  batch_window_us: int = 50, refresh_interval_ms: int = 0, seed: int = 1,
                  busy_poll: bool = False, caller_spin_us: int = 0, use_doorbell: bool = False,
                  devices: Optional[Sequence[int]] = None, filter=None, load_feedback_window: int = 0,
-                 feedback_fallbacks: bool = False, feedback_retries: bool = False):
+                 feedback_fallbacks: bool = False, feedback_retries: bool = False, affinity: bool = False):
         self._lib = load()
         self.provider = provider
         err = C.create_string_buffer(512)
-        if filter is not None or load_feedback_window or feedback_fallbacks or feedback_retries:
+        if filter is not None or load_feedback_window or feedback_fallbacks or feedback_retries or affinity:
             # Options::filter (a scheduling.Filter chart or a node table),
             # Options::load_feedback_window (load feedback carried across flushes, 0 = off) and
             # Options::feedback_fallbacks / feedback_retries (the *WithFallbacks calls and ScheduleRetry
-            # under that feedback; with both, ScheduleRetryWithFallbacks too)
+            # under that feedback; with both, ScheduleRetryWithFallbacks too) and Options::affinity (the pods'
+            # keys with every published epoch, for ScheduleAffinity and its relatives)
             from .engine import _node_table
             nodes, n = _node_table(filter)
             devs = list(devices) if devices is not None else []
             arr = (C.c_int * max(len(devs), 1))(*devs)
-            self._s = self._lib.ligh_scheduler_new_feedback(provider._p, device, arr, len(devs), max_pods,
+            self._s = self._lib.ligh_scheduler_new_affinity(provider._p, device, arr, len(devs), max_pods,
                                                             max_adapters, max_batch, flush_size, batch_window_us,
                                                             refresh_interval_ms, seed, int(busy_poll), caller_spin_us,
                                                             int(use_doorbell), C.cast(nodes, C.c_void_p), n,
                                                             load_feedback_window, int(feedback_fallbacks),
-                                                            int(feedback_retries), err, 512)
+                                                            int(feedback_retries), int(affinity), err, 512)
         elif devices is not None and len(devices) > 1:
             arr = (C.c_int * len(devices))(*devices)
             self._s = self._lib.ligh_scheduler_new_devices(provider._p, arr, len(devices), max_pods, max_adapters,
@@ -289,6 +303,28 @@ class HostScheduler:
         pods = names.value.decode().split("\n") if k.value else []
         return code, resolved.value.decode(), pods, err.value.decode("utf-8", "replace") if code != GRPC_OK else ""
 
+    def ScheduleAffinity(self, resolved: str, critical: bool, key: int, n: int = 0
+                         ) -> Tuple[int, List[str], str]:  # noqa: N802
+        """Scheduler::ScheduleAffinity (n = 0) or ScheduleAffinityWithFallbacks (n fallbacks): (gRPC code, pod
+        names [pick, then the row in descending score], error)."""
+        cap = 64 * 1024
+        names, err, k = C.create_string_buffer(cap), C.create_string_buffer(512), C.c_int(0)
+        code = self._lib.ligh_schedule_affinity(self._s, resolved.encode(), int(critical), key & ((1 << 64) - 1), n,
+                                                names, cap, C.byref(k), err, 512)
+        pods = names.value.decode().split("\n") if k.value else []
+        return code, pods, err.value.decode("utf-8", "replace") if code != GRPC_OK else ""
+
+    def ScheduleModelAffinity(self, model: str, key: int, n: int = 0
+                              ) -> Tuple[int, str, List[str], str]:  # noqa: N802
+        """Scheduler::ScheduleModelAffinity[WithFallbacks]: (gRPC code, resolved target model, pod names, error)."""
+        cap = 64 * 1024
+        resolved, names = C.create_string_buffer(256), C.create_string_buffer(cap)
+        err, k = C.create_string_buffer(512), C.c_int(0)
+        code = self._lib.ligh_schedule_model_affinity(self._s, model.encode(), key & ((1 << 64) - 1), n, resolved, 256,
+                                                      names, cap, C.byref(k), err, 512)
+        pods = names.value.decode().split("\n") if k.value else []
+        return code, resolved.value.decode(), pods, err.value.decode("utf-8", "replace") if code != GRPC_OK else ""
+
     def EjectPods(self, pods: Sequence[Pod]) -> None:  # noqa: N802
         """Scheduler::EjectPods: schedule as if `pods` (the complete set, matched by value; empty = every
         pod back) had left the provider, from the return on and across refreshes."""
@@ -315,10 +351,10 @@ class HostScheduler:
         return dict(zip(("scheduled", "batches", "max_batch", "refreshes", "stale_retries", "failed_refreshes",
                          "excluded_pods", "delta_refreshes", "last_dirty_pods", "feedback_windows",
                          "feedback_restarts", "model_scheduled", "model_batches", "fallback_scheduled",
-                         "retry_scheduled", "ejected_pods", "eject_publishes"),
+                         "retry_scheduled", "ejected_pods", "eject_publishes", "affinity_scheduled"),
                         map(int, list(out) + list(fb) + list(ms) + [self._lib.ligh_fallback_scheduled(self._s),
                                                                     self._lib.ligh_retry_scheduled(self._s)] +
-                            list(ej))))
+                            list(ej) + [self._lib.ligh_affinity_scheduled(self._s)])))
 
     def ScheduleModel(self, datastore: "HostDataStore", model: str):  # noqa: N802
         """resolve (FetchModelData + RandomWeightedDraw + IsCritical) + Schedule: (code, resolved, pod, err)."""

@@ -25,7 +25,9 @@ schedule a request again without the pods it already tried, as Schedule would on
 feedback-chain calls.  ``ScheduleRetryWithFallbacks`` / ``ScheduleBatchRetryWithFallbacks`` return the retry's
 pick followed by up to n more distinct survivors of the reduced pool (lig_schedule_batch_excluding_fallbacks), so
 one call serves several attempts; under load_feedback_window they need both ``feedback_retries=True`` and
-``feedback_fallbacks=True`` and then run as feedback-chain calls whose rows rank the chain's reduced pool.  There is
+``feedback_fallbacks=True`` and then run as feedback-chain calls whose rows rank the chain's reduced pool.  ``NewScheduler(pmp, affinity=True)`` adds
+``ScheduleAffinity`` and its relatives: requests that share a key go to the same surviving pod, by rendezvous hashing
+over the survivors on the device (lig_schedule_batch_affinity).  There is
 no CPU path here: without liblig.so or without a CUDA device construction fails.
 """
 from __future__ import annotations
@@ -201,6 +203,18 @@ def _picks(results: list) -> list:
     return [(pods[0] if pods else None, *rest) for pods, *rest in results]
 
 
+_M64 = (1 << 64) - 1
+
+
+def pod_key(pod: Pod) -> int:
+    """A pod's affinity identity: FNV-1a 64 over Name, a zero byte, then Address (the provider's own
+    identity of a pod, so the key does not depend on where the pod is listed)."""
+    h = 0xCBF29CE484222325
+    for b in pod.Name.encode() + b"\0" + pod.Address.encode():
+        h = ((h ^ b) * 0x100000001B3) & _M64
+    return h
+
+
 def _check_models(models: Sequence[InferenceModel]) -> None:
     """What lig_upload_models refuses with LIG_ERR_RANGE, named by model.  A model whose weights sum
     to <= 0 is not refused: pack_models packs it as absent."""
@@ -221,7 +235,7 @@ class Scheduler:
     def __init__(self, podMetricsProvider: PodMetricsProvider, device: int = 0,
                  max_pods: int = 4096, max_adapters: int = 1024, max_batch: int = 1 << 16,
                  seed: Optional[int] = None, filter: Optional[Filter] = None, load_feedback_window: int = 0,
-                 feedback_fallbacks: bool = False, feedback_retries: bool = False):
+                 feedback_fallbacks: bool = False, feedback_retries: bool = False, affinity: bool = False):
         if load_feedback_window < 0:
             raise ValueError(f"load_feedback_window must be >= 0, got {load_feedback_window}")
         self.podMetricsProvider = podMetricsProvider
@@ -231,6 +245,9 @@ class Scheduler:
         self._feedback_fallbacks = bool(feedback_fallbacks)
         # retries under load_feedback_window run on the chain's copy and load it; opt-in for the same reason
         self._feedback_retries = bool(feedback_retries)
+        # every published epoch carries the pods' keys (lig_upload_pod_keys) only with affinity on
+        self._affinity = bool(affinity)
+        self._pod_keys: Optional[np.ndarray] = None
         self._engine = Engine(device, max_pods, max_adapters, max_batch)
         self._filter = filter                # None: the built-in defaultFilter
         if filter is not None:
@@ -262,6 +279,9 @@ class Scheduler:
         snap = pack_pod_metrics(list(self.podMetricsProvider.AllPodMetrics()))
         self._uploaded += 1
         self._engine.upload_snapshot(self._uploaded, snap)
+        if self._affinity:
+            self._pod_keys = np.array([pod_key(p) for p in snap.pods], dtype=np.uint64)
+            self._engine.upload_pod_keys(self._uploaded, self._pod_keys)
         packed = pack_models(models, snap) if models is not None else None
         self._epoch, self._snap, self._packed_models, self._ejected_idx = self._uploaded, snap, packed, []
         idx = self._ejected_indices()
@@ -281,6 +301,8 @@ class Scheduler:
         with the model table when a list is set."""
         self._uploaded += 1
         self._engine.eject_pods(self._uploaded, self._epoch, idx)
+        if self._affinity:                   # same pods in the same order: the same keys
+            self._engine.upload_pod_keys(self._uploaded, self._pod_keys)
         if self._packed_models is not None:
             self._engine.upload_models(self._uploaded, self._packed_models)
         self._epoch, self._ejected_idx = self._uploaded, idx
@@ -332,10 +354,15 @@ class Scheduler:
     # ---- the two batch bodies: descriptor requests and model names, each plain, with fallback rows, as a
     # retry without the pods already tried, or both ----
     def _check_form(self, n: Optional[int], tried_lists: Optional[Sequence[Sequence[Pod]]] = None,
-                    mismatch: Optional[str] = None) -> None:
-        """The refusals of a call with fallback rows (n) or a retry (tried_lists), in this order.
-        `mismatch` is the message for argument lists of different lengths, if they differ."""
+                    mismatch: Optional[str] = None, affinity: bool = False) -> None:
+        """The refusals of a call with fallback rows (n), a retry (tried_lists) or an affinity call, in
+        this order.  `mismatch` is the message for argument lists of different lengths, if they differ."""
         retry, rows = tried_lists is not None, n is not None
+        if affinity and not self._affinity:
+            raise ValueError("affinity calls need a scheduler built with affinity=True (it uploads the pods' keys)")
+        if affinity and self._window:
+            raise ValueError("affinity is not defined under load_feedback_window: affinity picks would bypass the "
+                             "feedback chain's per-pod counts")
         if self._window and ((retry and not self._feedback_retries) or (rows and not self._feedback_fallbacks)):
             raise ValueError(_FEEDBACK_REFUSALS[retry, rows])
         if rows and not 1 <= n <= N.LIG_MAX_FALLBACKS:
@@ -355,10 +382,16 @@ class Scheduler:
             where.setdefault(pod, []).append(p)
         return [[p for pod in tried for p in where.get(pod, ())] for tried in tried_lists]
 
-    def _call(self, kind: str, arr: np.ndarray, excluded: tuple, n: Optional[int], **kw):
+    def _call(self, kind: str, arr: np.ndarray, excluded: tuple, n: Optional[int],
+              keys: Optional[np.ndarray] = None, **kw):
         """The Engine call of a batch: ``schedule_<kind>`` (kind "batch" or "models_batch"), as a chain
         call under load_feedback_window, an excluding call for a retry (`excluded` holds the retry's
-        arrays), a fallback call for n rows.  Returns (picks, rows); without n every row is empty."""
+        arrays), a fallback call for n rows, an affinity call with `keys` (the descriptors carry theirs
+        as rand_key, model ids take them beside).  Returns (picks, rows); without n every row is empty."""
+        if keys is not None:
+            extra = (keys,) if kind == "models_batch" else ()
+            out, rows = getattr(self._engine, "schedule_" + kind + "_affinity")(self._epoch, arr, *extra, n or 0)
+            return (out, rows) if n is not None else (out, [()] * len(out))
         name = ("schedule_" + kind + ("_feedback_chain" if self._window else "") + ("_excluding" if excluded else "")
                 + ("_fallbacks" if n is not None else ""))
         args = (self._epoch, self._seed, arr, *excluded) + ((n,) if n is not None else ()) + \
@@ -367,11 +400,17 @@ class Scheduler:
         return out if n is not None else (out, [()] * len(out))
 
     def _batch(self, reqs: Sequence[LLMRequest], tried_lists: Optional[Sequence[Sequence[Pod]]] = None,
-               n: Optional[int] = None) -> List[Tuple[List[Pod], Optional[StatusError]]]:
+               n: Optional[int] = None, keys: Optional[Sequence[int]] = None
+               ) -> List[Tuple[List[Pod], Optional[StatusError]]]:
         """(pods, error) per request: pods the pick and then its fallback row, [] on error.  One rand_key
-        per request, in order, from ScheduleBatch's sequence."""
-        self._check_form(n, tried_lists, None if tried_lists is None or len(tried_lists) == len(reqs)
-                         else f"{len(reqs)} requests but {len(tried_lists)} tried lists")
+        per request, in order, from ScheduleBatch's sequence; an affinity call (keys) takes none."""
+        affinity = keys is not None
+        if affinity:
+            self._check_form(n, None, None if len(keys) == len(reqs) else f"{len(reqs)} requests but {len(keys)} keys",
+                             True)
+        else:
+            self._check_form(n, tried_lists, None if tried_lists is None or len(tried_lists) == len(reqs)
+                             else f"{len(reqs)} requests but {len(tried_lists)} tried lists")
         snap = self._current()
         excluded: tuple = ()
         if tried_lists is not None:
@@ -383,10 +422,10 @@ class Scheduler:
         arr = np.zeros(len(reqs), dtype=REQ_DTYPE)
         for i, r in enumerate(reqs):
             arr[i] = (snap.adapter_id(r.ResolvedTargetModel), N.LIG_REQ_CRITICAL if r.Critical else 0,
-                      self._rng.getrandbits(64))
+                      int(keys[i]) & _M64 if affinity else self._rng.getrandbits(64))
         # under load_feedback_window each window of `_window` requests, across calls, adds its picks to
         # the pods' WaitingQueueSize until the next refresh uploads a new epoch
-        picks, rows = self._call("batch", arr, excluded, n)
+        picks, rows = self._call("batch", arr, excluded, n, keys=arr["rand_key"] if affinity else None)
         return [([snap.pods[int(pk["pod_idx"])]] + [snap.pods[int(p)] for p in row if p >= 0], None)
                 if pk["status"] == N.LIG_OK else ([], _schedule_error(int(pk["status"])))
                 for pk, row in zip(picks, rows)]
@@ -423,14 +462,20 @@ class Scheduler:
         return errors, ids, targets, slots
 
     def _model_batch(self, names: Sequence[str], resolved: Optional[Sequence[str]] = None,
-                     tried_lists: Optional[Sequence[Sequence[Pod]]] = None, n: Optional[int] = None
-                     ) -> List[Tuple[List[Pod], str, Optional[StatusError]]]:
+                     tried_lists: Optional[Sequence[Sequence[Pod]]] = None, n: Optional[int] = None,
+                     keys: Optional[Sequence[int]] = None) -> List[Tuple[List[Pod], str, Optional[StatusError]]]:
         """(pods, resolved target model, error) per name: pods the pick and then its fallback row, [] on
         error.  A retry (resolved, tried_lists) keeps the target the first attempt drew.  Names the host
-        answers take no rand_key; request k sent to the device has rand_key = _model_index + k."""
-        retry = tried_lists is not None
-        self._check_form(n, tried_lists, None if not retry or len(names) == len(resolved) == len(tried_lists)
-                         else f"{len(names)} names, {len(resolved)} resolved targets, {len(tried_lists)} tried lists")
+        answers take no rand_key; request k sent to the device has rand_key = _model_index + k.  An
+        affinity call (keys) draws on its keys and leaves the sequence alone."""
+        retry, affinity = tried_lists is not None, keys is not None
+        if affinity:
+            self._check_form(n, None, None if len(keys) == len(names) else f"{len(names)} names but {len(keys)} keys",
+                             True)
+        else:
+            self._check_form(n, tried_lists, None if not retry or len(names) == len(resolved) == len(tried_lists)
+                             else f"{len(names)} names, {len(resolved)} resolved targets, {len(tried_lists)} tried "
+                                  "lists")
         snap = self._current()
         rows = self._tried_rows(snap, tried_lists) if retry else None
         errors, ids, targets, slots = self._map_models(names, resolved if retry else None, rows)
@@ -438,9 +483,13 @@ class Scheduler:
         if not ids:
             return out
         excluded = (np.array(targets, dtype=np.uint8), _rows_array([rows[i] for i in slots])) if retry else ()
-        picks, fbs = self._call("models_batch", np.array(ids, dtype=np.uint32), excluded, n,
-                                first_index=self._model_index)
-        self._model_index += len(ids)
+        if affinity:
+            picks, fbs = self._call("models_batch", np.array(ids, dtype=np.uint32), (), n,
+                                    keys=np.array([int(keys[i]) & _M64 for i in slots], dtype=np.uint64))
+        else:
+            picks, fbs = self._call("models_batch", np.array(ids, dtype=np.uint32), excluded, n,
+                                    first_index=self._model_index)
+            self._model_index += len(ids)
         pm = self._packed_models
         for i, m, pk, row in zip(slots, ids, picks, fbs):
             t, st = int(pk["target_idx"]), int(pk["status"])
@@ -581,6 +630,54 @@ class Scheduler:
             raise err
         return pods
 
+    # ---- session affinity: requests that share a key go to the same surviving pod ----
+    def ScheduleBatchAffinity(self, reqs: Sequence[LLMRequest], keys: Sequence[int], n: Optional[int] = None):
+        """ScheduleBatch with request i placed by its affinity key keys[i] (lig_schedule_batch_affinity):
+        the survivor with the highest rendezvous score mix(key ^ mix(pod_key(pod))), so a key keeps its
+        pod while that pod survives, whatever order the provider lists pods in.  (pod, error) per
+        request, or with n (1..LIG_MAX_FALLBACKS) (pods, error): the pick, then up to n more survivors in
+        descending score.  Takes no rand_key.  Errors as ScheduleBatch.  ValueError unless the scheduler
+        was built with affinity=True, and under load_feedback_window."""
+        results = self._batch(reqs, n=n, keys=keys)
+        return results if n is not None else _picks(results)
+
+    def ScheduleAffinity(self, req: LLMRequest, key: int) -> Pod:
+        """Schedule placed by the affinity key `key`; raises like Schedule."""
+        pod, err = self.ScheduleBatchAffinity([req], [key])[0]
+        if err is not None:
+            raise err
+        return pod
+
+    def ScheduleAffinityWithFallbacks(self, req: LLMRequest, key: int, n: int) -> List[Pod]:
+        """ScheduleAffinity plus up to n fallback pods in descending score; raises like Schedule."""
+        pods, err = self.ScheduleBatchAffinity([req], [key], n)[0]
+        if err is not None:
+            raise err
+        return pods
+
+    def ScheduleModelBatchAffinity(self, names: Sequence[str], keys: Sequence[int], n: Optional[int] = None):
+        """ScheduleModelBatch with name i placed by keys[i] (lig_schedule_models_batch_affinity): the target
+        is drawn on the key (so a session keeps its target while the model's targets and weights stay),
+        then the pick is ScheduleBatchAffinity's.  (pod, resolved target model, error) per name, or with n
+        (pods, resolved, error).  Names the host answers as ScheduleModelBatch; takes no rand_key."""
+        results = self._model_batch(names, n=n, keys=keys)
+        return results if n is not None else _picks(results)
+
+    def ScheduleModelAffinity(self, name: str, key: int) -> Tuple[str, Pod]:
+        """ScheduleModel placed by the affinity key `key`: (resolved target model, pod); raises like
+        ScheduleModel."""
+        pod, resolved, err = self.ScheduleModelBatchAffinity([name], [key])[0]
+        if err is not None:
+            raise err
+        return resolved, pod
+
+    def ScheduleModelAffinityWithFallbacks(self, name: str, key: int, n: int) -> Tuple[str, List[Pod]]:
+        """ScheduleModelAffinity plus up to n fallback pods: (resolved target model, [pick, ...])."""
+        pods, resolved, err = self.ScheduleModelBatchAffinity([name], [key], n)[0]
+        if err is not None:
+            raise err
+        return resolved, pods
+
     # Filter-level view (the GPU analogue of Filter.Filter, filter.go:12-15): survivor slice.
     def Filter(self, req: LLMRequest) -> Tuple[List[Pod], Optional[StatusError]]:
         """The survivors of `req` against the scraped snapshot.  With load_feedback_window set this
@@ -646,7 +743,7 @@ class Scheduler:
 
 
 def NewScheduler(pmp: PodMetricsProvider, filter: Optional[Filter] = None, load_feedback_window: int = 0,
-                 feedback_fallbacks: bool = False, feedback_retries: bool = False,
+                 feedback_fallbacks: bool = False, feedback_retries: bool = False, affinity: bool = False,
                  **kw) -> Scheduler:  # scheduler.go:93-99
     """filter: a caller flow chart (None = defaultFilter, the reference's only tree).
     load_feedback_window > 0: ScheduleBatch goes through the load-feedback chain (include/lig.h,
@@ -663,6 +760,10 @@ def NewScheduler(pmp: PodMetricsProvider, filter: Optional[Filter] = None, load_
     With both feedback_fallbacks and feedback_retries, ScheduleRetryWithFallbacks /
     ScheduleBatchRetryWithFallbacks run as chain calls too
     (lig_schedule_batch_feedback_chain_excluding_fallbacks); with either one alone they raise ValueError
-    under load_feedback_window."""
+    under load_feedback_window.
+    affinity: upload the pods' keys (pod_key) with every published epoch, so that ScheduleAffinity and its
+    relatives can place requests by a caller key (lig_schedule_batch_affinity); without it they raise
+    ValueError and nothing else changes."""
     return Scheduler(pmp, filter=filter, load_feedback_window=load_feedback_window,
-                     feedback_fallbacks=feedback_fallbacks, feedback_retries=feedback_retries, **kw)
+                     feedback_fallbacks=feedback_fallbacks, feedback_retries=feedback_retries, affinity=affinity,
+                     **kw)
