@@ -572,7 +572,8 @@ int lig_schedule_models_batch_fallbacks_device(lig_ctx* ctx, uint64_t epoch, uin
  *
  * The calls read the resident epoch's tables, whichever build made them (built-in tree, caller tree,
  * an ejected epoch's pool, compact or strided lists), never a feedback chain's copy; they neither end
- * nor advance a chain.  n_fallbacks = 0 means no row (fallbacks may then be NULL).  Refused, with
+ * nor advance a chain.  Under a chain, lig_schedule_[models_]batch_feedback_chain_affinity below ranks
+ * the chain's load-adjusted lists.  n_fallbacks = 0 means no row (fallbacks may then be NULL).  Refused, with
  * nothing written: LIG_ERR_INVALID for n_fallbacks outside [0, LIG_MAX_FALLBACKS], null buffers,
  * R > max_batch on the host forms and device buffers not aligned to their element (requests 16
  * bytes, picks 8 / 4, keys 8, rows 2); a stale epoch and a missing snapshot as lig_schedule_batch
@@ -828,6 +829,58 @@ int lig_schedule_models_batch_feedback_chain_fallbacks_device(lig_ctx* ctx, uint
                                                               int R, lig_mpick* d_out, int n_fallbacks,
                                                               int16_t* d_fallbacks, int window, int32_t* d_loads,
                                                               void* stream);
+/* Session affinity under the chain.  Affinity alone sends every turn of a hot session, and every
+ * key whose top pod is the same pod, to that pod for a whole scrape window.  Under the chain, the
+ * pod's counts grow, the least-queuing filters drop it from the load-adjusted survivor set, and by
+ * the consistency property of the ranking only the keys whose top was that pod move, each to its
+ * next-ranked pod; the next scrape starts a new chain and they come back (bounded-load consistent
+ * hashing).  A chain affinity call is a chain call in every respect except the choice among
+ * survivors:
+ *   1. Sequence and windows: the R requests join the ctx's one chain sequence and its windows
+ *      exactly as a plain chain call's would; descriptor and model-id calls, with or without rows,
+ *      of every chain kind (plain, fallback, retry, affinity), may alternate in one chain, and the
+ *      restart rules are unchanged.
+ *   2. The pick: request j takes the class entry of its class in the chain's private tables at its
+ *      position in the sequence (the table a plain chain request at that position reads); status and
+ *      n_survivors come from that entry.  For a LIG_OK request, pod_idx is the member of that list
+ *      with the highest mix(k ^ h_p), ties to the lower pod index: the ranking of
+ *      lig_schedule_batch_affinity applied to the load-adjusted list.  k is rand_key for descriptors
+ *      and keys[i] for model ids; h_p are E's pod keys, read from E's resident slot.
+ *   3. Counting: only the pick adds one to its pod in the open window; row entries add none.  DROP,
+ *      EMPTY, NO_PODS_LEFT and NO_MODEL count toward the window and add no pick.
+ *   4. Rows: n_fallbacks in [0, LIG_MAX_FALLBACKS], 0 = no row (fallbacks may then be NULL).  Entries
+ *      1 .. m-1 (m = min(n, 1 + n_fallbacks)) are the next members of the same load-adjusted list in
+ *      descending score, then -1; a request that is not LIG_OK gets a row of -1.  The row for k is a
+ *      prefix of the row for any k' > k.
+ *   5. Model ids resolve as in lig_schedule_models_batch_affinity (draw state k ^ LIG_DRAW_DOMAIN, no
+ *      seed, no first_index) against E's model table as it stands at the call.  Neither a model
+ *      upload nor a pod-key upload for E restarts the chain (loads belong to pods, and the keys to
+ *      the same pods); a later upload of either waits on the device for the chain calls that read the
+ *      old table.
+ * So while no window of the chain has closed, `out` and the rows are lig_schedule_[models_]batch_affinity's
+ * on E byte for byte; how requests are split into calls changes neither `out`, the rows nor `loads`;
+ * and, like the resident affinity calls, the calls take no seed.  Refused, with nothing written and
+ * the chain exactly as it was (not started, not restarted), for every reason a chain call is refused,
+ * n_fallbacks outside [0, LIG_MAX_FALLBACKS], null buffers when R > 0, device buffers not aligned to
+ * their element (requests 16 bytes, picks 8 / 4, keys 8, rows 2), and LIG_ERR_NO_SNAPSHOT when E has
+ * no pod keys (and, for the model forms, no model table).  Host forms: page-locked, aligned buffers
+ * are used in place; pageable or misaligned requests and picks bounce as for the plain chain call,
+ * rows are staged as for the chain fallback calls, keys in stream-ordered device memory; they block.
+ * Device forms: device pointers, enqueued on `stream`, not synchronised. */
+int lig_schedule_batch_feedback_chain_affinity(lig_ctx* ctx, uint64_t epoch, const lig_req* reqs, int R,
+                                               lig_pick* out, int n_fallbacks, int16_t* fallbacks, int window,
+                                               int32_t* loads);
+int lig_schedule_batch_feedback_chain_affinity_device(lig_ctx* ctx, uint64_t epoch, const lig_req* d_reqs, int R,
+                                                      lig_pick* d_out, int n_fallbacks, int16_t* d_fallbacks,
+                                                      int window, int32_t* d_loads, void* stream);
+int lig_schedule_models_batch_feedback_chain_affinity(lig_ctx* ctx, uint64_t epoch, const uint32_t* model_ids,
+                                                      const uint64_t* keys, int R, lig_mpick* out, int n_fallbacks,
+                                                      int16_t* fallbacks, int window, int32_t* loads);
+int lig_schedule_models_batch_feedback_chain_affinity_device(lig_ctx* ctx, uint64_t epoch,
+                                                             const uint32_t* d_model_ids, const uint64_t* d_keys,
+                                                             int R, lig_mpick* d_out, int n_fallbacks,
+                                                             int16_t* d_fallbacks, int window, int32_t* d_loads,
+                                                             void* stream);
 /* Retries under the chain.  A chain retry call is a descriptor chain call in every respect, plus a
  * row of excluded pods per request in the format of lig_schedule_batch_excluding (int16, n_excluded
  * in [1, LIG_MAX_EXCLUDED], entries outside [0, P), -1 included, exclude nothing):

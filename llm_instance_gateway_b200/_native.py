@@ -66,6 +66,8 @@ EXPORTED_SYMBOLS = (
     "lig_schedule_models_batch_feedback_chain_excluding_fallbacks_device",
     "lig_upload_pod_keys", "lig_schedule_batch_affinity", "lig_schedule_batch_affinity_device",
     "lig_schedule_models_batch_affinity", "lig_schedule_models_batch_affinity_device",
+    "lig_schedule_batch_feedback_chain_affinity", "lig_schedule_batch_feedback_chain_affinity_device",
+    "lig_schedule_models_batch_feedback_chain_affinity", "lig_schedule_models_batch_feedback_chain_affinity_device",
 )
 
 
@@ -222,6 +224,12 @@ def load() -> C.CDLL:
     lib.lig_schedule_batch_affinity_device.argtypes = [vp, u64, vp, i32, vp, i32, vp, vp]
     lib.lig_schedule_models_batch_affinity.argtypes = [vp, u64, vp, vp, i32, vp, i32, vp]
     lib.lig_schedule_models_batch_affinity_device.argtypes = [vp, u64, vp, vp, i32, vp, i32, vp, vp]
+    # ... and under the feedback chain: the chain fallback calls' arguments without seed or first_index
+    lib.lig_schedule_batch_feedback_chain_affinity.argtypes = [vp, u64, vp, i32, vp, i32, vp, i32, vp]
+    lib.lig_schedule_batch_feedback_chain_affinity_device.argtypes = [vp, u64, vp, i32, vp, i32, vp, i32, vp, vp]
+    lib.lig_schedule_models_batch_feedback_chain_affinity.argtypes = [vp, u64, vp, vp, i32, vp, i32, vp, i32, vp]
+    lib.lig_schedule_models_batch_feedback_chain_affinity_device.argtypes = [vp, u64, vp, vp, i32, vp, i32, vp, i32,
+                                                                             vp, vp]
     lib.lig_update_snapshot.argtypes = [vp, u64, u64, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.lig_eject_pods.argtypes = [vp, u64, u64, vp, i32]
     lib.lig_pick_kernel_info.argtypes = [vp, u64, C.c_char_p, i32, C.POINTER(i32), C.POINTER(i32),

@@ -519,7 +519,7 @@ Status Scheduler::CheckRequest(const char* fn, const Waiter& w) const {
     if (!opt_.affinity)
       return Errorf(InvalidArgument, std::string(fn) + ": the scheduler was built without Options::affinity (it "
                                                        "uploads the pods' keys)");
-    if (opt_.load_feedback_window > 0)
+    if (opt_.load_feedback_window > 0 && !opt_.feedback_affinity)
       return Errorf(InvalidArgument, std::string(fn) + ": not defined under load_feedback_window (affinity picks "
                                                        "would bypass the feedback chain's per-pod counts)");
     if (group_)
@@ -843,7 +843,8 @@ void Scheduler::CountFeedback(uint64_t epoch, int n) {
 }
 
 // A flush makes its calls lane by lane: descriptors, retries, model ids, model-id retries, affinity
-// descriptors, affinity model ids.
+// descriptors, affinity model ids.  Under load_feedback_window this is the order of the flush's
+// requests in the feedback chain.
 void Scheduler::Flush(std::vector<Waiter*>& all) {
   for (std::vector<Waiter*>& lane : lanes_) lane.clear();
   for (Waiter* w : all)
@@ -913,9 +914,15 @@ int Scheduler::LaneCall(uint64_t epoch, bool models, bool retry, bool affinity, 
   const int W = opt_.load_feedback_window;
   const uint64_t first = model_index_;
   const uint8_t* targets = model_targets_.data();
+  if (affinity && models && W > 0)
+    return LIG_LANE_CALL(lig_schedule_models_batch_feedback_chain_affinity, ctx_, epoch, h_model_ids_, h_keys_, k,
+                         h_mpicks_, nf, h_fallbacks_, W, nullptr);
   if (affinity && models)
     return LIG_LANE_CALL(lig_schedule_models_batch_affinity, ctx_, epoch, h_model_ids_, h_keys_, k, h_mpicks_, nf,
                          h_fallbacks_);
+  if (affinity && W > 0)
+    return LIG_LANE_CALL(lig_schedule_batch_feedback_chain_affinity, ctx_, epoch, h_reqs_, k, h_picks_, nf,
+                         h_fallbacks_, W, nullptr);
   if (affinity)
     return LIG_LANE_CALL(lig_schedule_batch_affinity, ctx_, epoch, h_reqs_, k, h_picks_, nf, h_fallbacks_);
   if (models && retry) {

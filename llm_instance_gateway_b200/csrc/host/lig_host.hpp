@@ -175,6 +175,13 @@ struct Options {
   // so that ScheduleAffinity and its relatives can place requests by a caller key
   // (lig_schedule_[models_]batch_affinity).  Off: those calls are refused and nothing else changes.
   bool affinity = false;
+  // With affinity and load_feedback_window > 0: let the affinity calls run as feedback-chain calls
+  // (lig_schedule_[models_]batch_feedback_chain_affinity): a request takes the top-scoring pod of the
+  // chain's load-adjusted survivors, and its pick counts toward the chain's windows like any other, so
+  // a hot key moves off a pod the chain has loaded out of the survivor set until the next refresh.  Off
+  // by default because those calls have always been refused under feedback with InvalidArgument;
+  // without it they still are.  No effect without load_feedback_window.
+  bool feedback_affinity = false;
 };
 
 // A pod's affinity identity: FNV-1a 64 over Name, a zero byte, then Address (the provider's own
@@ -362,8 +369,9 @@ class Scheduler {
   // depend on the provider's pod order, on flushes or on the seed.  Goes through the micro-batcher in a
   // lane of its own and takes no rand_key; never through the doorbell; counted in
   // Stats::affinity_scheduled.  Errors are Schedule's.  InvalidArgument without Options::affinity, with
-  // load_feedback_window > 0 (affinity picks would bypass the chain's per-pod counts) and with several
-  // devices.
+  // load_feedback_window > 0 unless Options::feedback_affinity is set (affinity picks would bypass the
+  // chain's per-pod counts; with it they are chain calls, counted in the feedback_* stats) and with
+  // several devices.
   Status ScheduleAffinity(const LLMRequest& req, uint64_t key, backend::Pod* targetPod);
   // ScheduleAffinity plus up to n (1..LIG_MAX_FALLBACKS) more survivors in descending score: the
   // session's retry order.  A flush asks the lane's largest n; rows are prefixes of longer rows.

@@ -242,8 +242,23 @@ ligh_scheduler* ligh_scheduler_new_affinity(ligh_provider* p, int device, const 
                                             int caller_spin_us, int use_doorbell, const lig_filter_node* nodes,
                                             int n_nodes, int load_feedback_window, int feedback_fallbacks,
                                             int feedback_retries, int affinity, char* err, int err_cap) {
+  return ligh_scheduler_new_feedback_affinity(p, device, devices, n_devices, max_pods, max_adapters, max_batch,
+                                              flush_size, window_us, refresh_ms, seed, busy_poll, caller_spin_us,
+                                              use_doorbell, nodes, n_nodes, load_feedback_window, feedback_fallbacks,
+                                              feedback_retries, affinity, 0, err, err_cap);
+}
+
+ligh_scheduler* ligh_scheduler_new_feedback_affinity(ligh_provider* p, int device, const int* devices,
+                                                     int n_devices, int max_pods, int max_adapters, int max_batch,
+                                                     int flush_size, int window_us, int refresh_ms, uint64_t seed,
+                                                     int busy_poll, int caller_spin_us, int use_doorbell,
+                                                     const lig_filter_node* nodes, int n_nodes,
+                                                     int load_feedback_window, int feedback_fallbacks,
+                                                     int feedback_retries, int affinity, int feedback_affinity,
+                                                     char* err, int err_cap) {
   scheduling::Options o;
   o.affinity = affinity != 0;
+  o.feedback_affinity = feedback_affinity != 0;
   o.load_feedback_window = load_feedback_window;
   o.feedback_fallbacks = feedback_fallbacks != 0;
   o.feedback_retries = feedback_retries != 0;

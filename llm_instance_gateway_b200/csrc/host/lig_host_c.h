@@ -57,6 +57,16 @@ ligh_scheduler* ligh_scheduler_new_affinity(ligh_provider*, int device, const in
                                             const lig_filter_node* nodes, int n_nodes, int load_feedback_window,
                                             int feedback_fallbacks, int feedback_retries, int affinity, char* err,
                                             int err_cap);
+/* ligh_scheduler_new_affinity plus Options::feedback_affinity (nonzero, with affinity and
+ * load_feedback_window: ligh_schedule_affinity / ligh_schedule_model_affinity run under the chain). */
+ligh_scheduler* ligh_scheduler_new_feedback_affinity(ligh_provider*, int device, const int* devices, int n_devices,
+                                                     int max_pods, int max_adapters, int max_batch, int flush_size,
+                                                     int batch_window_us, int refresh_interval_ms, uint64_t seed,
+                                                     int busy_poll, int caller_spin_us, int use_doorbell,
+                                                     const lig_filter_node* nodes, int n_nodes,
+                                                     int load_feedback_window, int feedback_fallbacks,
+                                                     int feedback_retries, int affinity, int feedback_affinity,
+                                                     char* err, int err_cap);
 void ligh_scheduler_free(ligh_scheduler*);
 /* Scheduler.Schedule: returns the gRPC code (0 OK, 8 ResourceExhausted, 2 Unknown, 13 Internal). */
 int ligh_schedule(ligh_scheduler*, const char* model, const char* resolved_target_model, int critical,

@@ -1227,7 +1227,8 @@ static int create_impl(lig_ctx* c, int device, int max_pods, int max_adapters, i
         (const void*)lig_pick_fallback_kernel<false, false>, (const void*)lig_pick_fallback_kernel<true, false>,
         (const void*)lig_pick_fallback_kernel<false, true>, (const void*)lig_pick_fallback_kernel<true, true>,
         (const void*)lig_filter_kernel<false>,   (const void*)lig_filter_kernel<true>,
-        (const void*)lig_pick_affinity_kernel<false>, (const void*)lig_pick_affinity_kernel<true>,
+        (const void*)lig_pick_affinity_kernel<false, false>, (const void*)lig_pick_affinity_kernel<true, false>,
+        (const void*)lig_pick_affinity_kernel<false, true>, (const void*)lig_pick_affinity_kernel<true, true>,
     };
     for (const void* fn : fns) CUDA_TRY(cudaFuncGetAttributes(&fa, fn));
   }
@@ -2255,13 +2256,13 @@ static int enqueue_fallbacks(lig_ctx* c, Slot& s, const FallbackCall& f, cudaStr
   if (f.affinity) {
     CUDA_TRY(cudaStreamWaitEvent(st, s.keys_ready, 0));
     if (f.models)
-      lig_pick_affinity_kernel<true><<<blocks, kFallbackThreads, 0, st>>>(
+      lig_pick_affinity_kernel<true, false><<<blocks, kFallbackThreads, 0, st>>>(
           f.in, f.keys, f.out, f.fallbacks, f.R, f.n_fallbacks, cls, s.d_lists, s.A, s.d_ctab, s.d_mtab, s.n_models,
-          s.d_podkeys);
+          s.d_podkeys, nullptr);
     else
-      lig_pick_affinity_kernel<false><<<blocks, kFallbackThreads, 0, st>>>(
+      lig_pick_affinity_kernel<false, false><<<blocks, kFallbackThreads, 0, st>>>(
           f.in, nullptr, f.out, f.fallbacks, f.R, f.n_fallbacks, cls, s.d_lists, s.A, s.d_ctab, nullptr, 0u,
-          s.d_podkeys);
+          s.d_podkeys, nullptr);
   } else if (f.models)
     lig_pick_fallback_kernel<true, false><<<blocks, kFallbackThreads, 0, st>>>(
         f.in, f.out, f.fallbacks, f.R, f.n_fallbacks, cls, s.d_lists, s.A, s.d_ctab, s.d_mtab, s.n_models, f.seed,
@@ -2759,16 +2760,19 @@ struct FbReqs {
   const int16_t* excluded = nullptr;     //   excluded + i * n_excluded (with rows: a chain retry
   int n_excluded = 0;                    //   call with fallback rows)
   const uint8_t* targets = nullptr;      // a model-id retry call: request i's fixed target
+  bool affinity = false;                 // a chain affinity call: no seed, no first_index; rows as
+  const uint64_t* keys = nullptr;        //   above when n_fallbacks > 0; model ids: request i's key
+  const uint64_t* hkeys = nullptr;       //   E's pod keys (set by chain_call)
   size_t in_bytes() const { return models ? sizeof(uint32_t) : sizeof(lig_req); }
   size_t out_bytes() const { return models ? sizeof(lig_mpick) : sizeof(lig_pick); }
 };
 
 // Schedule R requests through the window sequence: each segment is the rest of the open window or
 // of the call, whichever is shorter; one fused pick + count launch per segment (pick + row + count
-// when the call asked for rows); a filled window is closed at once, its tables are rebuilt only
-// when the next segment needs them.  A retry segment (with or without rows) walks the tree over the
-// scratch's pod columns and reads no class table: it leaves them stale, so a later table-reading
-// segment rebuilds once.
+// when the call asked for rows, the affinity ranking + row + count for an affinity call); a filled
+// window is closed at once, its tables are rebuilt only when the next segment needs them.  A retry
+// segment (with or without rows) walks the tree over the scratch's pod columns and reads no class
+// table: it leaves them stale, so a later table-reading segment rebuilds once.
 static int fb_schedule(lig_ctx* c, FbRun& run, uint64_t seed, const FbReqs& rq, int R, cudaStream_t st) {
   Slot& fs = c->fb_scratch;
   for (int pos = 0; pos < R;) {
@@ -2800,6 +2804,17 @@ static int fb_schedule(lig_ctx* c, FbRun& run, uint64_t seed, const FbReqs& rq, 
         x.n_models = rq.n_models;
       }
       launch_excluding(c, fs, run.thr, run.tree, x, c->d_fb_hist, st);
+    } else if (rq.affinity) {
+      int16_t* rows = rq.rows ? rq.fallbacks + (size_t)pos * (size_t)rq.n_fallbacks : nullptr;
+      const int blocks = (n + kFallbackThreads - 1) / kFallbackThreads;
+      if (rq.models)
+        lig_pick_affinity_kernel<true, true><<<blocks, kFallbackThreads, 0, st>>>(
+            in, rq.keys + pos, out, rows, n, rq.n_fallbacks, fcls, fs.d_lists, fs.A, nullptr, rq.mtab, rq.n_models,
+            rq.hkeys, c->d_fb_hist);
+      else
+        lig_pick_affinity_kernel<false, true><<<blocks, kFallbackThreads, 0, st>>>(
+            in, nullptr, out, rows, n, rq.n_fallbacks, fcls, fs.d_lists, fs.A, nullptr, nullptr, 0u, rq.hkeys,
+            c->d_fb_hist);
     } else if (rq.rows) {
       int16_t* rows = rq.fallbacks + (size_t)pos * (size_t)rq.n_fallbacks;
       const int blocks = (n + kFallbackThreads - 1) / kFallbackThreads;
@@ -2881,11 +2896,13 @@ int lig_schedule_batch_feedback_device(lig_ctx* c, uint64_t epoch, uint64_t seed
 // Model ids are resolved against E's resident model table, which the chain never copies: a model
 // upload does not restart the chain.  The call holds upload_mu until it is enqueued, so that no
 // upload replaces the table between the resolve and the last launch, and registers as a reader of
-// E's slot, so that a later upload waits for the launches before it overwrites the table.
+// E's slot, so that a later upload waits for the launches before it overwrites the table.  An
+// affinity call reads E's pod keys the same way: a pod-key upload does not restart the chain either.
 static int chain_call(lig_ctx* c, uint64_t epoch, uint64_t seed, FbReqs rq, int R, int window, int32_t* d_loads,
                       cudaStream_t st) {
   std::unique_lock<std::mutex> held(c->upload_mu, std::defer_lock);
-  if (rq.models) held.lock();
+  const bool reads_slot = rq.models || rq.affinity;             // E's model table or pod keys
+  if (reads_slot) held.lock();
   // A chain (re)starts when it is not live, on another epoch or another upload of it (the next
   // scrape supersedes the estimate), or with another window size.  The tree and thresholds in
   // force at the start rebuild every window of the chain.  The tree is read under upload_mu, which
@@ -2900,8 +2917,11 @@ static int chain_call(lig_ctx* c, uint64_t epoch, uint64_t seed, FbReqs rq, int 
     uint64_t stamp = 0;
     {
       std::lock_guard<std::mutex> lk(c->mu);
-      // refused (stale epoch, no model table): the chain is untouched
+      // refused (stale epoch, no model table, no pod keys): the chain is untouched
       if (int rc = rq.models ? resolve_models_slot(c, epoch, &s) : resolve_slot(c, epoch, &s)) return rc;
+      if (rq.affinity && !s->keys_valid)
+        return fail(LIG_ERR_NO_SNAPSHOT, "no pod keys uploaded for epoch %llu (lig_upload_pod_keys)",
+                    (unsigned long long)epoch);
       const bool restart = !c->chain_live || c->chain_epoch != epoch || c->chain_stamp != s->stamp ||
                            c->chain_window != window;
       if (!restart) {
@@ -2935,11 +2955,17 @@ static int chain_call(lig_ctx* c, uint64_t epoch, uint64_t seed, FbReqs rq, int 
     have_tree = true;
     tree_stamp = stamp;
   }
-  if (rq.models) {
+  if (reads_slot) {
     std::lock_guard<std::mutex> lk(c->mu);
-    CUDA_TRY(cudaStreamWaitEvent(st, s->models_ready, 0));
-    rq.mtab = s->d_mtab;
-    rq.n_models = s->n_models;
+    if (rq.models) {
+      CUDA_TRY(cudaStreamWaitEvent(st, s->models_ready, 0));
+      rq.mtab = s->d_mtab;
+      rq.n_models = s->n_models;
+    }
+    if (rq.affinity) {
+      CUDA_TRY(cudaStreamWaitEvent(st, s->keys_ready, 0));
+      rq.hkeys = s->d_podkeys;
+    }
   }
   FbRun run;
   run.window = window;
@@ -2949,7 +2975,7 @@ static int chain_call(lig_ctx* c, uint64_t epoch, uint64_t seed, FbReqs rq, int 
   run.thr = c->chain_thr;
   run.d_total = c->d_fb_total;
   if (int rc = fb_schedule(c, run, seed, rq, R, st)) return rc;
-  if (rq.models) {
+  if (reads_slot) {
     std::lock_guard<std::mutex> lk(c->mu);
     if (int rc = note_reader(*s, st)) return rc;
   }
@@ -2974,13 +3000,18 @@ static int chain_admit(lig_ctx* c, const char* fn) {
   return fb_alloc_scratch(c);
 }
 
-// The row arguments of a chain fallback or retry call, both sets for a retry call with fallback rows;
-// 0 for a plain chain call.
+// The row arguments of a chain fallback or retry call, both sets for a retry call with fallback rows,
+// and the rows and keys of a chain affinity call; 0 for a plain chain call.
 static int chain_rows_check(const char* fn, const FbReqs& rq, int R) {
   if (rq.retry) {
     if (rq.n_excluded < 1 || rq.n_excluded > LIG_MAX_EXCLUDED)
       return fail(LIG_ERR_INVALID, "%s: n_excluded=%d outside [1, %d]", fn, rq.n_excluded, LIG_MAX_EXCLUDED);
     if (R > 0 && (!rq.excluded || (rq.models && !rq.targets))) return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
+  }
+  if (rq.affinity) {                                          // n_fallbacks = 0: no row
+    if (rq.n_fallbacks < 0 || rq.n_fallbacks > LIG_MAX_FALLBACKS)
+      return fail(LIG_ERR_INVALID, "%s: n_fallbacks=%d outside [0, %d]", fn, rq.n_fallbacks, LIG_MAX_FALLBACKS);
+    if (R > 0 && rq.models && !rq.keys) return fail(LIG_ERR_INVALID, "%s: bad argument", fn);
   }
   if (!rq.rows) return 0;
   if (rq.n_fallbacks < 1 || rq.n_fallbacks > LIG_MAX_FALLBACKS)
@@ -2996,8 +3027,9 @@ static int chain_device(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t see
   if (int rc = chain_rows_check(fn, rq, R)) return rc;
   if (R > 0 && rq.rows && misaligned(rq.fallbacks, sizeof(int16_t)))
     return fail(LIG_ERR_INVALID, "%s: the row buffer is not 2-byte aligned", fn);
-  if (R > 0 && rq.retry && (misaligned(rq.in, rq.in_bytes()) || misaligned(rq.out, rq.out_bytes()) ||
-                            misaligned(rq.excluded, sizeof(int16_t))))
+  if (R > 0 && (rq.retry || rq.affinity) &&
+      (misaligned(rq.in, rq.in_bytes()) || misaligned(rq.out, rq.out_bytes()) ||
+       misaligned(rq.excluded, sizeof(int16_t)) || misaligned(rq.keys, sizeof(uint64_t))))
     return fail(LIG_ERR_INVALID, "%s: a device buffer is not aligned to its element", fn);
   std::lock_guard<std::mutex> fk(c->fb_mu);
   CUDA_TRY(cudaSetDevice(c->device));
@@ -3019,7 +3051,7 @@ static int chain_host(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t seed,
   rq.in = R ? mapped_device_pointer(in) : nullptr;
   rq.out = R ? mapped_device_pointer(out) : nullptr;
   const bool bounce = R > 0 && !(rq.in && rq.out && !(reinterpret_cast<uintptr_t>(rq.in) & (rq.in_bytes() - 1)) &&
-                                 !(rq.retry && misaligned(rq.out, rq.out_bytes())));
+                                 !((rq.retry || rq.affinity) && misaligned(rq.out, rq.out_bytes())));
   std::unique_lock<std::mutex> bk(c->bounce_mu, std::defer_lock);
   if (bounce) {
     bk.lock();
@@ -3083,9 +3115,27 @@ static int chain_host(lig_ctx* c, const char* fn, uint64_t epoch, uint64_t seed,
       rq.targets = stage_tg;
     }
   }
+  // affinity keys of model ids: page-locked, 8-byte aligned ones are read in place, the others staged
+  // in stream-ordered HBM like the retry rows
+  uint64_t* stage_keys = nullptr;
+  if (R > 0 && rq.affinity && rq.models) {
+    const uint64_t* keys = rq.keys;
+    rq.keys = mapped_device_pointer(keys);
+    if (!rq.keys || misaligned(rq.keys, sizeof(uint64_t))) {
+      const size_t keys_b = (size_t)R * sizeof(uint64_t);
+      cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&stage_keys), keys_b, c->s_fb);
+      if (e == cudaSuccess) e = cudaMemcpyAsync(stage_keys, keys, keys_b, cudaMemcpyHostToDevice, c->s_fb);
+      if (e != cudaSuccess) {
+        if (stage_keys) cudaFreeAsync(stage_keys, c->s_fb);
+        return fail(LIG_ERR_CUDA, "%s: staging the keys failed: %s", fn, cudaGetErrorString(e));
+      }
+      rq.keys = stage_keys;
+    }
+  }
   const int rc = chain_call(c, epoch, seed, rq, R, window, dev_loads, c->s_fb);
   if (stage) cudaFreeAsync(stage, c->s_fb);
   if (stage_tg) cudaFreeAsync(stage_tg, c->s_fb);
+  if (stage_keys) cudaFreeAsync(stage_keys, c->s_fb);
   if (rc) return rc;
   const cudaError_t e = cudaStreamSynchronize(c->s_fb);
   if (e != cudaSuccess) {
@@ -3179,6 +3229,45 @@ int lig_schedule_models_batch_feedback_chain_fallbacks_device(lig_ctx* c, uint64
                                                               void* stream) {
   return chain_device(c, "lig_schedule_models_batch_feedback_chain_fallbacks_device", epoch, seed,
                       with_rows(model_reqs(d_ids, d_out, first_index), n_fallbacks, d_fallbacks), R, window,
+                      d_loads, stream);
+}
+
+// n_fallbacks outside [0, LIG_MAX_FALLBACKS] is refused by chain_rows_check
+static FbReqs with_affinity(FbReqs rq, const uint64_t* keys, int n_fallbacks, int16_t* fallbacks) {
+  if (n_fallbacks != 0) rq = with_rows(rq, n_fallbacks, fallbacks);
+  rq.n_fallbacks = n_fallbacks;
+  rq.affinity = true;
+  rq.keys = keys;
+  return rq;
+}
+
+int lig_schedule_batch_feedback_chain_affinity(lig_ctx* c, uint64_t epoch, const lig_req* reqs, int R, lig_pick* out,
+                                               int n_fallbacks, int16_t* fallbacks, int window, int32_t* loads) {
+  return chain_host(c, "lig_schedule_batch_feedback_chain_affinity", epoch, 0,
+                    with_affinity(descriptor_reqs(reqs, out), nullptr, n_fallbacks, fallbacks), R, window, loads);
+}
+
+int lig_schedule_batch_feedback_chain_affinity_device(lig_ctx* c, uint64_t epoch, const lig_req* d_reqs, int R,
+                                                      lig_pick* d_out, int n_fallbacks, int16_t* d_fallbacks,
+                                                      int window, int32_t* d_loads, void* stream) {
+  return chain_device(c, "lig_schedule_batch_feedback_chain_affinity_device", epoch, 0,
+                      with_affinity(descriptor_reqs(d_reqs, d_out), nullptr, n_fallbacks, d_fallbacks), R, window,
+                      d_loads, stream);
+}
+
+int lig_schedule_models_batch_feedback_chain_affinity(lig_ctx* c, uint64_t epoch, const uint32_t* model_ids,
+                                                      const uint64_t* keys, int R, lig_mpick* out, int n_fallbacks,
+                                                      int16_t* fallbacks, int window, int32_t* loads) {
+  return chain_host(c, "lig_schedule_models_batch_feedback_chain_affinity", epoch, 0,
+                    with_affinity(model_reqs(model_ids, out, 0), keys, n_fallbacks, fallbacks), R, window, loads);
+}
+
+int lig_schedule_models_batch_feedback_chain_affinity_device(lig_ctx* c, uint64_t epoch, const uint32_t* d_model_ids,
+                                                             const uint64_t* d_keys, int R, lig_mpick* d_out,
+                                                             int n_fallbacks, int16_t* d_fallbacks, int window,
+                                                             int32_t* d_loads, void* stream) {
+  return chain_device(c, "lig_schedule_models_batch_feedback_chain_affinity_device", epoch, 0,
+                      with_affinity(model_reqs(d_model_ids, d_out, 0), d_keys, n_fallbacks, d_fallbacks), R, window,
                       d_loads, stream);
 }
 

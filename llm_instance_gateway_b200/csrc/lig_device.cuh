@@ -2685,6 +2685,9 @@ lig_pick_fallback_kernel(const void* __restrict__ in, void* __restrict__ out, in
 // nodes, KV ties) are found with a ballot and served one at a time by the whole warp, strided scoring
 // and a __shfl_xor max-reduce per rank.  One thread per request, plain loads and stores (`in`, `keys`,
 // `out` and `fallbacks` may be page-locked host memory); `fallbacks` is null when n_fallbacks = 0.
+// kCount: the chain segment of lig_schedule_[models_]batch_feedback_chain_affinity.  The same ranking
+// on the chain's private tables (always the strided rows, as the count kernels read them), and the
+// pick counted into the open window like lig_pick_[models_]count_kernel; row entries are not counted.
 constexpr int kAffinityShortList = 32;
 
 __device__ __forceinline__ uint64_t affinity_mix(uint64_t z) {
@@ -2698,18 +2701,18 @@ __device__ __forceinline__ bool ranks_before(uint64_t s, int p, uint64_t bs, int
   return s > bs || (s == bs && p < bp);
 }
 
-template <bool kModels>
+template <bool kModels, bool kCount>
 __global__ void __launch_bounds__(kFallbackThreads)
 lig_pick_affinity_kernel(const void* __restrict__ in, const uint64_t* __restrict__ keys, void* __restrict__ out,
                          int16_t* __restrict__ fallbacks, int R, int n_fallbacks, const uint4* __restrict__ cls,
                          const uint16_t* __restrict__ lists, int A, const unsigned char* __restrict__ ctab,
                          const unsigned char* __restrict__ mtab, uint32_t n_models,
-                         const uint64_t* __restrict__ hkeys) {
+                         const uint64_t* __restrict__ hkeys, int* __restrict__ hist) {
   const int i = (int)blockIdx.x * kFallbackThreads + (int)threadIdx.x;
   const int lane = (int)threadIdx.x & 31;
   const uint4* gcls = cls;
   const uint16_t* glists = lists;
-  sealed_tables(ctab, A, &gcls, &glists);
+  if constexpr (!kCount) sealed_tables(ctab, A, &gcls, &glists);
   uint4 e = make_uint4(0u, 0u, 0u, 0u);
   uint64_t key = 0;
   bool resolved = false;
@@ -2796,6 +2799,7 @@ lig_pick_affinity_kernel(const void* __restrict__ in, const uint64_t* __restrict
       pp = bp;
     }
   }
+  if constexpr (kCount) count_window_picks(pod, lane, hist);   // every lane, pod -1 past R
   if (i >= R) return;
   for (int j = (int)max(m, 1u); j <= n_fallbacks; ++j) row[j - 1] = -1;
   if constexpr (kModels) {

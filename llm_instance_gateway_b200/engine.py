@@ -702,6 +702,69 @@ class Engine:
             self._ctx, epoch, seed, first_index, d_ids or None, R, d_out or None, n, d_fallbacks or None, window,
             d_loads or None, stream or None))
 
+    # ---- session affinity under the feedback chain: the affinity ranking over the chain's tables ----
+    def schedule_batch_feedback_chain_affinity(self, epoch: int, reqs: np.ndarray, n: int, window: int,
+                                               loads: Optional[np.ndarray] = None):
+        """lig_schedule_batch_feedback_chain_affinity: (picks, int16 fallbacks (R, n)).  A chain call whose
+        pick and row rank the survivors of request i's class in the chain's tables at its position by
+        the affinity key rand_key; only the pick is counted into the chain's windows."""
+        assert reqs.dtype == REQ_DTYPE and reqs.flags.c_contiguous
+        R = int(reqs.shape[0])
+        out = np.empty(R, dtype=PICK_DTYPE)
+        rows = np.empty((R, max(n, 0)), dtype=np.int16)
+        if loads is not None:
+            assert loads.dtype == np.int32 and loads.flags.c_contiguous
+        N.check(self._lib.lig_schedule_batch_feedback_chain_affinity(
+            self._ctx, epoch, _ptr(reqs), R, _ptr(out), n, _ptr(rows) if n > 0 else None, window,
+            _ptr(loads) if loads is not None else None))
+        return out, rows
+
+    def schedule_batch_feedback_chain_affinity_ptr(self, epoch: int, h_reqs: int, R: int, h_out: int, n: int,
+                                                   h_fallbacks: int, window: int, h_loads: int = 0) -> None:
+        N.check(self._lib.lig_schedule_batch_feedback_chain_affinity(self._ctx, epoch, h_reqs or None, R,
+                                                                     h_out or None, n, h_fallbacks or None, window,
+                                                                     h_loads or None))
+
+    def schedule_batch_feedback_chain_affinity_device(self, epoch: int, d_reqs: int, R: int, d_out: int, n: int,
+                                                      d_fallbacks: int, window: int, d_loads: int = 0,
+                                                      stream: int = 0) -> None:
+        """Device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_batch_feedback_chain_affinity_device(
+            self._ctx, epoch, d_reqs or None, R, d_out or None, n, d_fallbacks or None, window, d_loads or None,
+            stream or None))
+
+    def schedule_models_batch_feedback_chain_affinity(self, epoch: int, model_ids: np.ndarray, keys: np.ndarray,
+                                                      n: int, window: int, loads: Optional[np.ndarray] = None):
+        """lig_schedule_models_batch_feedback_chain_affinity: (picks, int16 fallbacks (R, n)); request i is
+        model_ids[i] with affinity key keys[i], resolved as schedule_models_batch_affinity resolves it."""
+        assert model_ids.dtype == np.uint32 and model_ids.flags.c_contiguous
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        R = int(model_ids.shape[0])
+        assert keys.shape == (R,)
+        out = np.empty(R, dtype=MPICK_DTYPE)
+        rows = np.empty((R, max(n, 0)), dtype=np.int16)
+        if loads is not None:
+            assert loads.dtype == np.int32 and loads.flags.c_contiguous
+        N.check(self._lib.lig_schedule_models_batch_feedback_chain_affinity(
+            self._ctx, epoch, _ptr(model_ids), _ptr(keys), R, _ptr(out), n, _ptr(rows) if n > 0 else None, window,
+            _ptr(loads) if loads is not None else None))
+        return out, rows
+
+    def schedule_models_batch_feedback_chain_affinity_ptr(self, epoch: int, h_ids: int, h_keys: int, R: int,
+                                                          h_out: int, n: int, h_fallbacks: int, window: int,
+                                                          h_loads: int = 0) -> None:
+        N.check(self._lib.lig_schedule_models_batch_feedback_chain_affinity(
+            self._ctx, epoch, h_ids or None, h_keys or None, R, h_out or None, n, h_fallbacks or None, window,
+            h_loads or None))
+
+    def schedule_models_batch_feedback_chain_affinity_device(self, epoch: int, d_ids: int, d_keys: int, R: int,
+                                                             d_out: int, n: int, d_fallbacks: int, window: int,
+                                                             d_loads: int = 0, stream: int = 0) -> None:
+        """The model-id form with device pointers, enqueued on `stream` (not synchronised)."""
+        N.check(self._lib.lig_schedule_models_batch_feedback_chain_affinity_device(
+            self._ctx, epoch, d_ids or None, d_keys or None, R, d_out or None, n, d_fallbacks or None, window,
+            d_loads or None, stream or None))
+
     def pick_kernel_info(self, epoch: int) -> dict:
         name = C.create_string_buffer(64)
         grid, threads, tb, in_smem = C.c_int(), C.c_int(), C.c_int(), C.c_int()

@@ -33,7 +33,7 @@ EXPORTED_SYMBOLS = (
     "ligh_schedule_model_retry", "ligh_schedule_model_retry_with_fallbacks",
     "ligh_eject_pods", "ligh_eject_stats",
     "ligh_scheduler_new_affinity", "ligh_schedule_affinity", "ligh_schedule_model_affinity", "ligh_affinity_scheduled",
-    "ligh_pod_key",
+    "ligh_pod_key", "ligh_scheduler_new_feedback_affinity",
 )
 
 _lib = None
@@ -67,6 +67,10 @@ def load() -> C.CDLL:
     lib.ligh_scheduler_new_affinity.argtypes = [vp, i32, C.POINTER(i32), i32, i32, i32, i32, i32, i32, i32, u64, i32,
                                                 i32, i32, vp, i32, i32, i32, i32, i32, C.c_char_p, i32]
     lib.ligh_scheduler_new_affinity.restype = vp
+    lib.ligh_scheduler_new_feedback_affinity.argtypes = [vp, i32, C.POINTER(i32), i32, i32, i32, i32, i32, i32, i32,
+                                                         u64, i32, i32, i32, vp, i32, i32, i32, i32, i32, i32,
+                                                         C.c_char_p, i32]
+    lib.ligh_scheduler_new_feedback_affinity.restype = vp
     lib.ligh_schedule_affinity.argtypes = [vp, C.c_char_p, i32, u64, i32, C.c_char_p, i32, C.POINTER(i32),
                                            C.c_char_p, i32]
     lib.ligh_schedule_model_affinity.argtypes = [vp, C.c_char_p, u64, i32, C.c_char_p, i32, C.c_char_p, i32,
@@ -176,26 +180,28 @@ class HostScheduler:
                  batch_window_us: int = 50, refresh_interval_ms: int = 0, seed: int = 1,
                  busy_poll: bool = False, caller_spin_us: int = 0, use_doorbell: bool = False,
                  devices: Optional[Sequence[int]] = None, filter=None, load_feedback_window: int = 0,
-                 feedback_fallbacks: bool = False, feedback_retries: bool = False, affinity: bool = False):
+                 feedback_fallbacks: bool = False, feedback_retries: bool = False, affinity: bool = False,
+                 feedback_affinity: bool = False):
         self._lib = load()
         self.provider = provider
         err = C.create_string_buffer(512)
-        if filter is not None or load_feedback_window or feedback_fallbacks or feedback_retries or affinity:
+        if (filter is not None or load_feedback_window or feedback_fallbacks or feedback_retries or affinity
+                or feedback_affinity):
             # Options::filter (a scheduling.Filter chart or a node table),
             # Options::load_feedback_window (load feedback carried across flushes, 0 = off) and
             # Options::feedback_fallbacks / feedback_retries (the *WithFallbacks calls and ScheduleRetry
             # under that feedback; with both, ScheduleRetryWithFallbacks too) and Options::affinity (the pods'
-            # keys with every published epoch, for ScheduleAffinity and its relatives)
+            # keys with every published epoch, for ScheduleAffinity and its relatives; with
+            # Options::feedback_affinity those run as chain calls under load_feedback_window)
             from .engine import _node_table
             nodes, n = _node_table(filter)
             devs = list(devices) if devices is not None else []
             arr = (C.c_int * max(len(devs), 1))(*devs)
-            self._s = self._lib.ligh_scheduler_new_affinity(provider._p, device, arr, len(devs), max_pods,
-                                                            max_adapters, max_batch, flush_size, batch_window_us,
-                                                            refresh_interval_ms, seed, int(busy_poll), caller_spin_us,
-                                                            int(use_doorbell), C.cast(nodes, C.c_void_p), n,
-                                                            load_feedback_window, int(feedback_fallbacks),
-                                                            int(feedback_retries), int(affinity), err, 512)
+            self._s = self._lib.ligh_scheduler_new_feedback_affinity(
+                provider._p, device, arr, len(devs), max_pods, max_adapters, max_batch, flush_size, batch_window_us,
+                refresh_interval_ms, seed, int(busy_poll), caller_spin_us, int(use_doorbell), C.cast(nodes, C.c_void_p),
+                n, load_feedback_window, int(feedback_fallbacks), int(feedback_retries), int(affinity),
+                int(feedback_affinity), err, 512)
         elif devices is not None and len(devices) > 1:
             arr = (C.c_int * len(devices))(*devices)
             self._s = self._lib.ligh_scheduler_new_devices(provider._p, arr, len(devices), max_pods, max_adapters,

@@ -27,7 +27,8 @@ pick followed by up to n more distinct survivors of the reduced pool (lig_schedu
 one call serves several attempts; under load_feedback_window they need both ``feedback_retries=True`` and
 ``feedback_fallbacks=True`` and then run as feedback-chain calls whose rows rank the chain's reduced pool.  ``NewScheduler(pmp, affinity=True)`` adds
 ``ScheduleAffinity`` and its relatives: requests that share a key go to the same surviving pod, by rendezvous hashing
-over the survivors on the device (lig_schedule_batch_affinity).  There is
+over the survivors on the device (lig_schedule_batch_affinity); under load_feedback_window they need
+``feedback_affinity=True`` and then rank the feedback chain's load-adjusted survivors.  There is
 no CPU path here: without liblig.so or without a CUDA device construction fails.
 """
 from __future__ import annotations
@@ -235,7 +236,8 @@ class Scheduler:
     def __init__(self, podMetricsProvider: PodMetricsProvider, device: int = 0,
                  max_pods: int = 4096, max_adapters: int = 1024, max_batch: int = 1 << 16,
                  seed: Optional[int] = None, filter: Optional[Filter] = None, load_feedback_window: int = 0,
-                 feedback_fallbacks: bool = False, feedback_retries: bool = False, affinity: bool = False):
+                 feedback_fallbacks: bool = False, feedback_retries: bool = False, affinity: bool = False,
+                 feedback_affinity: bool = False):
         if load_feedback_window < 0:
             raise ValueError(f"load_feedback_window must be >= 0, got {load_feedback_window}")
         self.podMetricsProvider = podMetricsProvider
@@ -247,6 +249,8 @@ class Scheduler:
         self._feedback_retries = bool(feedback_retries)
         # every published epoch carries the pods' keys (lig_upload_pod_keys) only with affinity on
         self._affinity = bool(affinity)
+        # affinity under load_feedback_window ranks the chain's tables and loads it; opt-in for the same reason
+        self._feedback_affinity = bool(feedback_affinity)
         self._pod_keys: Optional[np.ndarray] = None
         self._engine = Engine(device, max_pods, max_adapters, max_batch)
         self._filter = filter                # None: the built-in defaultFilter
@@ -360,10 +364,10 @@ class Scheduler:
         retry, rows = tried_lists is not None, n is not None
         if affinity and not self._affinity:
             raise ValueError("affinity calls need a scheduler built with affinity=True (it uploads the pods' keys)")
-        if affinity and self._window:
+        if affinity and self._window and not self._feedback_affinity:
             raise ValueError("affinity is not defined under load_feedback_window: affinity picks would bypass the "
                              "feedback chain's per-pod counts")
-        if self._window and ((retry and not self._feedback_retries) or (rows and not self._feedback_fallbacks)):
+        if self._window and not affinity and ((retry and not self._feedback_retries) or (rows and not self._feedback_fallbacks)):
             raise ValueError(_FEEDBACK_REFUSALS[retry, rows])
         if rows and not 1 <= n <= N.LIG_MAX_FALLBACKS:
             raise ValueError(f"n must be in [1, {N.LIG_MAX_FALLBACKS}], got {n}")
@@ -390,7 +394,9 @@ class Scheduler:
         as rand_key, model ids take them beside).  Returns (picks, rows); without n every row is empty."""
         if keys is not None:
             extra = (keys,) if kind == "models_batch" else ()
-            out, rows = getattr(self._engine, "schedule_" + kind + "_affinity")(self._epoch, arr, *extra, n or 0)
+            chain = ("_feedback_chain", (self._window,)) if self._window else ("", ())
+            out, rows = getattr(self._engine, "schedule_" + kind + chain[0] + "_affinity")(self._epoch, arr, *extra,
+                                                                                         n or 0, *chain[1])
             return (out, rows) if n is not None else (out, [()] * len(out))
         name = ("schedule_" + kind + ("_feedback_chain" if self._window else "") + ("_excluding" if excluded else "")
                 + ("_fallbacks" if n is not None else ""))
@@ -637,7 +643,9 @@ class Scheduler:
         pod while that pod survives, whatever order the provider lists pods in.  (pod, error) per
         request, or with n (1..LIG_MAX_FALLBACKS) (pods, error): the pick, then up to n more survivors in
         descending score.  Takes no rand_key.  Errors as ScheduleBatch.  ValueError unless the scheduler
-        was built with affinity=True, and under load_feedback_window."""
+        was built with affinity=True, and under load_feedback_window unless it was built with
+        feedback_affinity=True: then the call is a chain call (lig_schedule_batch_feedback_chain_affinity)
+        that ranks the chain's load-adjusted survivors and loads the chain with its picks."""
         results = self._batch(reqs, n=n, keys=keys)
         return results if n is not None else _picks(results)
 
@@ -744,7 +752,7 @@ class Scheduler:
 
 def NewScheduler(pmp: PodMetricsProvider, filter: Optional[Filter] = None, load_feedback_window: int = 0,
                  feedback_fallbacks: bool = False, feedback_retries: bool = False, affinity: bool = False,
-                 **kw) -> Scheduler:  # scheduler.go:93-99
+                 feedback_affinity: bool = False, **kw) -> Scheduler:  # scheduler.go:93-99
     """filter: a caller flow chart (None = defaultFilter, the reference's only tree).
     load_feedback_window > 0: ScheduleBatch goes through the load-feedback chain (include/lig.h,
     lig_schedule_batch_feedback_chain): every window of that many requests, counted across calls,
@@ -763,7 +771,12 @@ def NewScheduler(pmp: PodMetricsProvider, filter: Optional[Filter] = None, load_
     under load_feedback_window.
     affinity: upload the pods' keys (pod_key) with every published epoch, so that ScheduleAffinity and its
     relatives can place requests by a caller key (lig_schedule_batch_affinity); without it they raise
-    ValueError and nothing else changes."""
+    ValueError and nothing else changes.
+    feedback_affinity: with affinity, under load_feedback_window, let the affinity calls run as chain calls
+    (lig_schedule_batch_feedback_chain_affinity): each request takes the top-scoring pod of the chain's
+    load-adjusted survivors, and its pick loads the chain like any other, so a hot key moves off a pod
+    the chain has loaded out of the survivor set; without it they raise ValueError there, as they
+    always have.  Without load_feedback_window it has no effect."""
     return Scheduler(pmp, filter=filter, load_feedback_window=load_feedback_window,
                      feedback_fallbacks=feedback_fallbacks, feedback_retries=feedback_retries, affinity=affinity,
-                     **kw)
+                     feedback_affinity=feedback_affinity, **kw)
